@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Contract benchmark: audio samples/sec (fwd+bwd) of the dasp hot path on B200.
+"""Benchmark: audio samples/sec (fwd+bwd) of the dasp hot path on one or more H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W]                    # this repo's CUDA path
+    python bench.py --steps K --dump-outputs DIR                           # ... and save the last timed step's results
     python bench.py --impl reference [--gpus N] [--steps K] [--warmup W]   # the reference's own CPU path
     python bench.py --impl reference-cuda                                  # the reference's own PyTorch-CUDA path (1 GPU)
 
@@ -21,6 +22,11 @@ noise on every replay).  The JSON line carries: value (inputs resident in HBM), 
 loss + parameter gradients read back, every step), roofline of the dominant stage (algorithmic bytes / CUDA-event time
 / measured HBM peak; per-stage events come from an eager pass of the same step), per-config sub-results (BASELINE
 configs 2-4), reference_gpu (the reference's own CUDA path on this GPU), cpu_baseline, clocks.
+
+--dump-outputs DIR writes, after the timed replays, what the last timed step computed as float32 .npy files: loss,
+p_grad (bs, 49) and drive_grad (bs * 2) in full, and y / x_grad for a fixed seeded sample of DUMP_ITEMS items (the full
+(bs, 2, 48000) tensors are far above 64 MB).  Inputs, the reverb noise key and hence the outputs depend only on the
+arguments, so two builds run with the same arguments can be compared file by file.
 """
 from __future__ import annotations
 
@@ -47,13 +53,17 @@ UNIT = "samples/s"
 GLOBAL_BATCH = 1024
 
 
+DUMP_ITEMS = 16          # items of y / x_grad kept by --dump-outputs (2 x 16 x 2 x 48000 x 4 B = 12 MB)
+DUMP_SEED = 20240
+
+
 def measured_peak_gbs():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 # ------------------------------------------------------------------------------------------
@@ -329,7 +339,7 @@ def make_config(bs_global, world, scaling, chunk, graph=True):
             "global_batch": per * world, "per_gpu_batch": per,
             "parallelism": f"dp{world} (contiguous item shards, no data-path collective)",
             "l2": "inputs (>= 49 MB/tensor/GPU, 393 MB at N=1) and the reverb's 4.7 MB/item intermediates exceed the "
-                  "126 MB L2 within a step: no flush needed", "reverb_chunk_items": chunk,
+                  "50 MB L2 within a step: no flush needed", "reverb_chunk_items": chunk,
             "timed_region": "replays of one CUDA graph of the whole step (fwd+bwd)"}
     if not graph:
         cfg["timed_region"] = "one eager fwd+bwd per step on a bounded sample of the batch (see cpu_baseline.sample)"
@@ -355,6 +365,7 @@ class Step:
         self.d = self.host[2].to(dev).requires_grad_(True)
         self.graph = None
         self.loss = None
+        self.y = None
         self.pool = pool
 
     def eager(self):
@@ -363,6 +374,7 @@ class Step:
         y = chain(self.D, self.x, self.p, self.d)
         loss = y.pow(2).mean()
         loss.backward()
+        self.y = y.detach()
         return loss
 
     def capture(self, warm=3):
@@ -383,6 +395,16 @@ class Step:
 
     def replay(self):
         self.graph.replay()
+
+    def outputs(self, n_items):
+        """what a caller of the step receives, as float32 numpy arrays: y and x_grad for a fixed seeded sample of
+        items, loss and the parameter / drive gradients in full"""
+        torch = self.torch
+        idx = torch.randperm(self.bs, generator=torch.Generator().manual_seed(DUMP_SEED))[:n_items].sort().values
+        idx = idx.to(self.dev)
+        out = {"loss": self.loss.detach().reshape(1), "y": self.y[idx], "x_grad": self.x.grad[idx],
+               "p_grad": self.p.grad, "drive_grad": self.d.grad}
+        return {k: v.float().cpu().numpy() for k, v in out.items()}
 
 
 def own_launches_per_step(bs, chunk_items):
@@ -470,6 +492,8 @@ def main():
                                                                    "under weak scaling (BASELINE config: 1024)")
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"])
     ap.add_argument("--no-extras", action="store_true", help="skip sub-configs / reference_gpu / cpu_baseline / edges")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy "
+                                                          "(float32; y and x_grad for a seeded sample of items)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -524,6 +548,7 @@ def main():
 
     sampler = ClockSampler(local_rank)
     sampler.start()
+    torch.manual_seed(1000 + rank)          # the reverb's device noise key: same arguments, same outputs
     step = Step(D, dev, bs, seed=1000 + rank)
     for _ in range(args.warmup):
         step.eager()
@@ -563,6 +588,11 @@ def main():
     clocks = sampler.stop(wall0, wall1)
     value = samples_per_step * args.steps / (ms_max * 1e-3)
     loss_val = float(step.loss.item())
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in step.outputs(min(DUMP_ITEMS, bs)).items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
 
     # ---- end-to-end: pinned host inputs -> H2D -> graph replay -> D2H of loss and parameter gradients ----
     # Every step uploads ITS inputs from pinned host memory into a staging set on a copy stream (overlapping the
@@ -728,18 +758,6 @@ def main():
                               "cuFFT C2C(8192) x1 (IR partitions)",
                 "reverb_bwd": "reverb bwd pipeline: g_fft_kernel, partition_mac_kernel x2, ifft_dx_kernel, "
                               "ifft_irgrad_kernel (all on the own in-shared-memory FFT), reverb_param_grad_kernel"}
-        # DRAM bytes actually moved by the two reverb pipelines (dram__bytes_read.sum + dram__bytes_write.sum summed
-        # over their kernels, one `ncu --set full` capture of a chunk at this geometry): read from the committed
-        # summary that tools/summarize_profiles.py writes, never typed in here
-        traffic_item = {}
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as f:
-                tj = json.load(f)
-            if tj.get("geometry") == [N_SAMPLES, IR_LEN, TAPS]:
-                traffic_item = {k: float(v) for k, v in tj["dram_bytes_per_item"].items()}
-                traffic_src = tj.get("source")
-        except Exception:
-            traffic_src = None
         breakdown = {}
         for name, v in stages.items():
             m = statistics.mean(v)
@@ -750,8 +768,7 @@ def main():
         if dom:
             roofline = {"bound": "hbm", "kernel": kern[dom], "achieved": breakdown[dom]["alg_GBps"], "peak": peak,
                         "unit": "GB/s", "frac": breakdown[dom]["frac"],
-                        "traffic": traffic_item[dom] * bs if dom in traffic_item else None,
-                        "traffic_source": traffic_src if dom in traffic_item else None, "peak_source": peak_src,
+                        "peak_source": peak_src,
                         "algorithmic_bytes_per_launch": alg[dom], "ms_per_launch": breakdown[dom]["ms"],
                         "note": "stage = one C-ABI call, timed with CUDA events around it in an eager pass of the same step"}
         if roofline and dom in ("reverb_fwd", "reverb_bwd"):
@@ -762,7 +779,7 @@ def main():
             nfft = (12 * R + J + 2 * I) if dom == "reverb_fwd" else (2 * I + J)
             flops = nfft * 5 * 8192 * 13 * bs
             props = torch.cuda.get_device_properties(dev)
-            fp32_peak = props.multi_processor_count * 128 * 2 * (clocks.get("sm_max_mhz") or 1965.0) * 1e6 / 1e12
+            fp32_peak = props.multi_processor_count * 128 * 2 * (clocks.get("sm_max_mhz") or 1980.0) * 1e6 / 1e12
             roofline["fft_context"] = {
                 "transforms_per_item": nfft, "fft_TFLOPs": round(flops / (breakdown[dom]["ms"] * 1e-3) / 1e12, 2),
                 "fp32_peak_TFLOPs": round(fp32_peak, 1),

@@ -1,4 +1,4 @@
-"""dasp_pytorch_b200: B200-native (sm_100a) kernels behind dasp_pytorch's functional audio processors.
+"""dasp_pytorch_b200: H100-native (sm_90a) kernels behind dasp_pytorch's functional audio processors.
 
 Drop-in surface: the same names the reference package exports (``dasp_pytorch/__init__.py``) for the hot
 path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_shaped_reverberation`` and the

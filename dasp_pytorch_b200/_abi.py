@@ -86,7 +86,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -m dasp_pytorch_b200.build` "
-            "(nvcc, sm_100a).  dasp_pytorch_b200 has no CPU / PyTorch fallback."
+            "(nvcc, sm_90a).  dasp_pytorch_b200 has no CPU / PyTorch fallback."
         )
     handle = ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_GLOBAL)
     for name, (res, args) in _SIGNATURES.items():
@@ -119,7 +119,7 @@ def require_cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
     (no silent host fallback)."""
     if not t.is_cuda:
         raise DaspError(
-            f"{name}: dasp_pytorch_b200 runs on CUDA (B200) tensors only, got device {t.device}; "
+            f"{name}: dasp_pytorch_b200 runs on CUDA (H100) tensors only, got device {t.device}; "
             "there is no CPU path"
         )
     if t.dtype != torch.float32:

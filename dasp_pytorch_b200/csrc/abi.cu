@@ -20,10 +20,10 @@ int sm_count() {
   static thread_local int cached_dev = -1;
   static thread_local int cached_sms = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev != cached_dev) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached_dev = dev;
     cached_sms = n;
   }
@@ -63,7 +63,7 @@ extern "C" {
 
 int dasp_abi_version(void) { return DASP_ABI_VERSION; }
 const char* dasp_last_error(void) { return dasp::g_err; }
-int dasp_compiled_arch(void) { return 1000; }
+int dasp_compiled_arch(void) { return 900; }
 void dasp_shutdown(void) { dasp::reverb_shutdown(); }
 void dasp_debug_force_warps(int warps) { dasp::g_forced_warps = (warps == 1 || warps == 2 || warps == 3 || warps == 4 || warps == 8 || warps == 16) ? warps : 0; }
 

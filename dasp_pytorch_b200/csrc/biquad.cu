@@ -18,11 +18,11 @@
 // measured against the fp64 reference this is 100-1000x more accurate than the reference's own
 // fp32 path (DESIGN.md, numerics table).  Coefficients and all matrix powers are designed in fp64.
 //
-// Parallelisation (round 2: "row pairs on FFMA2, warps decoupled along time").
+// Parallelisation ("row pairs, warps decoupled along time").
 //   * Two rows (the left/right channel of an item when C = 2; any two consecutive rows otherwise) are the two
-//     lanes of Blackwell's packed fp32x2 instructions (FFMA2 / FMUL2 / FADD2): one issue slot, two FMAs.  The
-//     kernels are instruction-issue bound (about 100 fp32 instructions per sample in the scalar round-1 form,
-//     at the fp32 ridge of the chip), so this halves the cost per sample.  All tables hold (row A, row B) pairs.
+//     lanes of one thread's value pairs: the table loads, shuffles and scan control flow of a step serve both rows,
+//     and when both rows belong to one item a coefficient register serves both FMAs.  All tables hold (row A, row B)
+//     pairs.
 //   * One CTA per row pair, W warps.  The row is cut into tiles of 32*E samples; warp w owns tiles w, w+W, ...
 //     and runs the WHOLE cascade on a tile with the data in registers: per section a zero-state local pass over
 //     the lane's E samples, a Kogge-Stone shuffle scan of the lanes' end states with the precomputed powers
@@ -145,22 +145,10 @@ __device__ inline M2d mpow(double sg, double q, unsigned n) {
 }
 
 // ------------------------------------------------------------------ arithmetic on row pairs (x = row A, y = row B)
-// DASP_EQ_PACKED = 1 (default) issues Blackwell's packed FFMA2/FMUL2/FADD2 where both operands are row pairs; 0 issues
-// two scalar instructions per pair.  Measured on B200 (profiles/r02_ffma2_probe.md, profiles/r02_eq_variants.md): in a
-// micro-benchmark an FFMA2 with three distinct register-pair operands occupies the FMA pipe ~4.3 cycles per warp
-// (two scalar FFMAs: ~2.4), but inside these kernels the packed form still wins (forward 0.39 vs 0.45 ms): operand
-// reuse between neighbouring instructions is high and the halved issue count matters more.
-#ifndef DASP_EQ_PACKED
-#define DASP_EQ_PACKED 1
-#endif
+// Both rows of a pair go through the same instruction stream as two scalar fp32 operations.
 typedef float2 f2;
-#if DASP_EQ_PACKED
-__device__ __forceinline__ f2 ffma2(f2 a, f2 b, f2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ f2 fmul2(f2 a, f2 b) { return __fmul2_rn(a, b); }
-#else
 __device__ __forceinline__ f2 ffma2(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ f2 fmul2(f2 a, f2 b) { return make_float2(a.x * b.x, a.y * b.y); }
-#endif
 __device__ __forceinline__ f2 zero2() { return make_float2(0.f, 0.f); }
 __device__ __forceinline__ f2 shfl_up2(f2 v, int d) {
   return make_float2(__shfl_up_sync(0xffffffffu, v.x, d), __shfl_up_sync(0xffffffffu, v.y, d));
@@ -175,10 +163,9 @@ __device__ __forceinline__ f2 shfl2(f2 v, int l) {
 // Coefficient type C of the per-pair tables:
 //   float : both rows of the pair belong to the SAME item (every pair when the channel count is even -- stereo), so
 //           one scalar coefficient serves both rows: half the table bytes, a whole 2x2 matrix per 128-bit load, and
-//           the coefficient register is shared by the two scalar FMAs of the pair.  The first packed version of these
-//           kernels ran with the shared-memory / shuffle pipe 68 % busy (ncu: l1tex__data_pipe_lsu_wavefronts, 762
-//           wavefronts per tile, most of them broadcast 128-bit table loads); this halves that traffic.
-//   f2    : the rows belong to different items (odd channel counts): (row A, row B) coefficient pairs, packed FFMA2.
+//           the coefficient register is shared by the two scalar FMAs of the pair.  Most shared-memory wavefronts of a
+//           tile are broadcast 128-bit table loads; this halves that traffic.
+//   f2    : the rows belong to different items (odd channel counts): (row A, row B) coefficient pairs.
 __device__ __forceinline__ f2 cfma(float c, f2 v, f2 a) { return make_float2(fmaf(c, v.x, a.x), fmaf(c, v.y, a.y)); }
 __device__ __forceinline__ f2 cfma(f2 c, f2 v, f2 a) { return ffma2(c, v, a); }
 __device__ __forceinline__ f2 dup(float c) { return make_float2(c, c); }
@@ -285,7 +272,7 @@ __device__ void build_tables(Tables<C>& tb, const float* params, int64_t ia, int
   __syncthreads();
 }
 
-// the five section coefficients, expanded to row pairs for the (packed) local passes
+// the five section coefficients, expanded to row pairs for the local passes
 struct Cf { f2 sg, q, be1, B2, b0; };
 __device__ __forceinline__ Cf load_cf(const Tables<float>& tb, int k) {
   const float4 a = *reinterpret_cast<const float4*>(&tb.cf[k][0]);
@@ -307,7 +294,7 @@ __device__ __forceinline__ void load_fix(const Tables<f2>& tb, int k, int j, f2&
 }
 
 // zero-state local pass of section k over the lane's E samples (in place); returns the end state.
-// Two dependent packed operations per sample on the (s1, s2) recurrence.
+// Two dependent pair operations per sample on the (s1, s2) recurrence.
 __device__ __forceinline__ St local_pass(f2 (&v)[kE], const Cf& c) {
   f2 s1 = zero2(), s2 = zero2();
 #pragma unroll
@@ -834,10 +821,10 @@ int tune_bwd_s() {
 // force the general (pair-coefficient) tables even when every pair lies inside one item: test hook via the env
 int tune_force_pair_tables() { static const int v = env_int("DASP_EQ_PAIR_TABLES"); return v; }
 
-// Warps per row pair (W in {1, 2, 3, 4, 8}, forward also 16; 0 / other = automatic).  Measured on B200 at 1024 pairs x 48000 samples
-// (profiles/r02_eq_variants.md): forward W=4 with two load stages beats W=2 and the single-wave choices; small batches
-// want W=8 to fill the SMs at all.  The backward holds 255 registers per thread, i.e. 8 warps per SM whatever the
-// split: W=8 with one stage (one CTA per SM, least shared memory per warp) measured best.
+// Warps per row pair (W in {1, 2, 3, 4, 8}, forward also 16; 0 / other = automatic).  The automatic choice: forward W=4
+// with two load stages at large batches; small batches want W=8 to fill the SMs at all.  The backward holds 255
+// registers per thread, i.e. 8 warps per SM whatever the split: W=8 with one stage (one CTA per SM, least shared memory
+// per warp).
 bool valid_w(int w) { return w == 1 || w == 2 || w == 3 || w == 4 || w == 8; }
 // The forward also has W = 16 (512 threads, 80 registers): when there is at most one row pair per SM (e.g. 1024 stereo
 // items split over 8 GPUs) a pair's CTA is alone on its SM, and sixteen warps walk its tiles twice as fast as eight.

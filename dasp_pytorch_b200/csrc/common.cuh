@@ -1,4 +1,4 @@
-// Shared device/host helpers for the dasp_b200 kernels (sm_100a only).
+// Shared device/host helpers for the dasp_b200 kernels (sm_90a only).
 //
 //  * error plumbing for the C ABI (thread-local last-error string, no exceptions cross the ABI)
 //  * 1-D TMA ("bulk async copy") + mbarrier wrappers: the recurrence kernels stage contiguous
@@ -13,8 +13,8 @@
 
 #include "../../include/dasp_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "dasp_b200 kernels are written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "dasp_b200 kernels are written for sm_90a (H100) only"
 #endif
 
 namespace dasp {

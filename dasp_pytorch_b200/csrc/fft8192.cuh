@@ -13,9 +13,8 @@
 //   P4  DFT16 over n4 (contiguous)                                              Y (B) -> registers
 // Thread t of P4 ends with X[t + 512 k4], k4 = 0..15.
 //
-// Every thread processes TWO adjacent sub-transforms at once in the two lanes of a packed fp32x2 value
-// (Blackwell FADD2/FMUL2/FFMA2 take one issue slot for two flops): with planar storage a 64-bit shared load
-// of two neighbouring floats IS the packed operand, so there is no pack/unpack traffic.  P4 uses the lanes for
+// Every thread processes TWO adjacent sub-transforms at once as the two lanes of a value pair: with planar
+// storage one 64-bit shared load of two neighbouring floats fetches both lanes' operands.  P4 uses the lanes for
 // the even / odd halves of its 16-point transform and finishes with one scalar radix-2 stage.
 //
 // Layouts (floats, per plane): linear = n;  A(k1,k2,n3,n4) = 1152 k1 + 144 k2 + 16 n3 + n4;
@@ -24,7 +23,7 @@
 //
 // The arithmetic is written against a small lane-vector interface so that the SAME code runs in a host
 // emulation (tests/test_fft8192_host.py drives tools/probe/fft8192_host_check.cpp: threads looped over
-// sequentially, packed lanes emulated) and pins the index mathematics without a GPU.
+// sequentially) and pins the index mathematics without a GPU.
 #pragma once
 
 #ifdef __CUDACC__
@@ -42,35 +41,14 @@ constexpr int kPlaneG = 8192;          // floats per plane of the linear buffer
 constexpr int kPlaneY = 9216;          // floats per plane of the padded buffer (layouts A and B)
 constexpr int kTabFloats = 2 * (2 * 64) + 2 * (2 * 512) + 2 * 1024 + 2 * 128;   // see Tables
 
-// ---- packed lane pair ------------------------------------------------------------------------------
-// DASP_FFT_PACKED = 1 (default): the lane pair is one packed fp32x2 register pair (FADD2/FMUL2/FFMA2); 0: the same
-// two lanes as two scalar instructions.  A/B on B200 (profiles/r02_eq_variants.md): although a micro-benchmark shows
-// FFMA2 with three distinct register pairs at half the FMA-pipe throughput of two scalar FFMAs (FADD2 is at parity),
-// the packed FFT kernels are 1-6 % FASTER end to end (reverb forward 6.11 vs 6.47 ms), so packed stays.
-#ifndef DASP_FFT_PACKED
-#define DASP_FFT_PACKED 1
-#endif
+// ---- lane pair ------------------------------------------------------------------------------------
 // DASP_FFT_TWIDDLE_RECURRENCE = 1 (default): the seven twiddles a thread needs in a pass are successive powers of one
 // table entry, formed by complex multiplication in registers instead of being fetched one by one -- the FFT kernels are
-// bound by the shared-memory pipe (data exchange + twiddle fetches), not by the FMA pipe (profiles/r02_reverb_*.md).
+// bound by the shared-memory pipe (data exchange + twiddle fetches), not by the FMA pipe.
 #ifndef DASP_FFT_TWIDDLE_RECURRENCE
 #define DASP_FFT_TWIDDLE_RECURRENCE 1
 #endif
-#if defined(__CUDA_ARCH__) && DASP_FFT_PACKED
-struct V2 { float2 v; };
-DASP_HD V2 v2(float a, float b) { V2 r; r.v = make_float2(a, b); return r; }
-DASP_HD V2 bc(float a) { return v2(a, a); }
-DASP_HD V2 operator+(V2 a, V2 b) { V2 r; r.v = __fadd2_rn(a.v, b.v); return r; }
-DASP_HD V2 operator-(V2 a, V2 b) { V2 r; r.v = __ffma2_rn(b.v, make_float2(-1.f, -1.f), a.v); return r; }
-DASP_HD V2 operator*(V2 a, V2 b) { V2 r; r.v = __fmul2_rn(a.v, b.v); return r; }
-DASP_HD V2 fma2(V2 a, V2 b, V2 c) { V2 r; r.v = __ffma2_rn(a.v, b.v, c.v); return r; }            // a b + c
-DASP_HD V2 fnma2(V2 a, V2 b, V2 c) { V2 r; r.v = __ffma2_rn(make_float2(-a.v.x, -a.v.y), b.v, c.v); return r; }   // c - a b
-DASP_HD V2 neg(V2 a) { return v2(-a.v.x, -a.v.y); }
-DASP_HD float lane0(V2 a) { return a.v.x; }
-DASP_HD float lane1(V2 a) { return a.v.y; }
-DASP_HD V2 ld2(const float* p) { V2 r; r.v = *reinterpret_cast<const float2*>(p); return r; }
-DASP_HD void st2(float* p, V2 a) { *reinterpret_cast<float2*>(p) = a.v; }
-#elif defined(__CUDA_ARCH__)
+#if defined(__CUDA_ARCH__)
 struct V2 { float x, y; };
 DASP_HD V2 v2(float a, float b) { V2 r; r.x = a; r.y = b; return r; }
 DASP_HD V2 bc(float a) { return v2(a, a); }
@@ -127,7 +105,7 @@ DASP_HD void table_entry(int e, int& c_off, int& s_off, int& dup, double& turns)
 }
 constexpr int kTabEntries = 64 + 512 + 1024 + 128;
 
-// ---- packed 8-point DFT, natural order in and out --------------------------------------------------
+// ---- lane-pair 8-point DFT, natural order in and out --------------------------------------------------
 // s = +1: X[k] = sum_j x[j] e^{+2 pi i j k / 8};  s = -1: the conjugate kernel
 template <bool INV>
 DASP_HD void mul_i(V2& r, V2& i) {            // (r + i i) * (s i)

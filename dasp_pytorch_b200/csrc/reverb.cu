@@ -6,8 +6,8 @@
 // exponential envelope and a gain (:561-567), then convolves the audio with it by a second
 // time-domain conv1d with an L-tap kernel (:570-572).  >99.9 % of its time is those two direct
 // convolutions.  Here both are FFT convolutions (SURVEY.md Appendix A.5) built from ONE transform shape,
-// the 8192-point batched C2C that cuFFT runs as a single shared-memory kernel (~4.5 TB/s effective on
-// B200; its long transforms reach 0.3-1.5 TB/s), with everything between the transforms fused:
+// the 8192-point batched C2C that cuFFT runs as a single shared-memory kernel (long transforms take several
+// passes over HBM), with everything between the transforms fused:
 //
 //   * Only the first Leff = min(L, N) taps of the impulse response can reach the N output samples
 //     (y[n] = sum_{t<=n} IR[t] x[n-t], n < N), so only those are synthesised -- an exact saving.
@@ -225,14 +225,9 @@ __global__ void cmul_filter_pairs_kernel(float2* __restrict__ C, const float2* _
   }
 }
 
-// packed fp32x2 helpers of the generator's R-point DFT: scalar pairs unless DASP_FFT_PACKED (see fft8192.cuh)
-#if DASP_FFT_PACKED
-__device__ __forceinline__ float2 gen_ffma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ float2 gen_fmul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
-#else
+// lane-pair helpers of the generator's R-point DFT
 __device__ __forceinline__ float2 gen_ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float2 gen_fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
-#endif
 
 // ---- spectral synthesis (device-noise mode) ------------------------------------------------------
 // The band-filtered noise only has to be a stationary Gaussian process with the FIR's autocovariance on
@@ -319,7 +314,7 @@ __device__ __forceinline__ void spectral_unit(int j1, int nb, const float2* __re
     gb[R - 1 - j2] = m;          // mirror of bin j1 + nb j2 is bin (nb - j1) + nb (R-1-j2)
   }
   // The two residue classes (j1 and nb - j1) go through the SAME R-point DFT and twiddle ladder, so they are
-  // packed into the two lanes of Blackwell's fp32x2 instructions (FFMA2/FMUL2: one issue slot, two FMAs).
+  // carried as the two lanes of float2 values.
   float2 gx[R], gy[R];                       // (class A, class B) real parts / imaginary parts
 #pragma unroll
   for (int j2 = 0; j2 < R; ++j2) { gx[j2] = make_float2(ga[j2].x, gb[j2].x); gy[j2] = make_float2(ga[j2].y, gb[j2].y); }
@@ -339,7 +334,7 @@ __device__ __forceinline__ void spectral_unit(int j1, int nb, const float2* __re
   const float2 wx = make_float2(w1a.x, w1b.x), wy = make_float2(w1a.y, w1b.y), nwy = make_float2(-w1a.y, -w1b.y);
   float2 tx = make_float2(1.f, 1.f), ty = make_float2(0.f, 0.f);      // twiddle e^{2 pi i j b / n1}, both classes
   // S[b] = sum_{j2} g[j2] e^{+2 pi i j2 b / R}: generic O(R^2) form, or for R = 6 (IR 96000 on 48000 samples, the
-  // BASELINE geometry) radix 2 x 3 with literal constants -- 48 packed operations instead of 144
+  // BASELINE geometry) radix 2 x 3 with literal constants -- 48 pair operations instead of 144
   float2 Sre[R], Sim[R];
   if constexpr (R == 6) {
     const float2 hlf = make_float2(0.5f, 0.5f), nhlf = make_float2(-0.5f, -0.5f);

@@ -1,4 +1,4 @@
-"""B200-native drop-in for ``dasp_pytorch.functional``'s audio-processor hot path.
+"""H100-native drop-in for ``dasp_pytorch.functional``'s audio-processor hot path.
 
 Same function names, argument order, keyword names, defaults and
 ``(batch, channels, samples)`` tensor contract as the reference
@@ -6,7 +6,7 @@ Same function names, argument order, keyword names, defaults and
 ``Processor.process_normalized`` -> ``process_fn(x, sample_rate, **params)``
 (reference ``modules.py:45-49``) and direct calls keep working unchanged.  Every
 op is a ``torch.autograd.Function`` whose forward and backward call hand-written
-sm_100a kernels through the C ABI in ``include/dasp_b200.h``; there is no PyTorch,
+sm_90a kernels through the C ABI in ``include/dasp_b200.h``; there is no PyTorch,
 Triton or CPU fallback -- non-CUDA inputs raise ``DaspError``.
 
 Arithmetic is fp32 (coefficient design in fp64 inside the kernels).  Inputs in
@@ -45,7 +45,7 @@ def _audio(x: torch.Tensor, name: str = "x"):
         raise ValueError(f"{name} must be a tensor of shape (batch, channels, samples)")
     if not x.is_cuda:
         raise DaspError(
-            f"{name} is on {x.device}: dasp_pytorch_b200 only runs on CUDA (B200) tensors and has no CPU path"
+            f"{name} is on {x.device}: dasp_pytorch_b200 only runs on CUDA (H100) tensors and has no CPU path"
         )
     if not x.is_floating_point():
         raise DaspError(f"{name} must be a floating-point tensor, got {x.dtype}")
@@ -241,7 +241,7 @@ def _audio_nd(x, ndim, name="x"):
     if not torch.is_tensor(x) or x.dim() != ndim:
         raise ValueError(f"{name} must be a {ndim}-dimensional tensor")
     if not x.is_cuda:
-        raise DaspError(f"{name} is on {x.device}: dasp_pytorch_b200 only runs on CUDA (B200) tensors and has no CPU path")
+        raise DaspError(f"{name} is on {x.device}: dasp_pytorch_b200 only runs on CUDA (H100) tensors and has no CPU path")
     if not x.is_floating_point():
         raise DaspError(f"{name} must be a floating-point tensor, got {x.dtype}")
     return x.to(torch.float32).contiguous(), x.dtype
@@ -532,10 +532,10 @@ def parametric_eq_packed(x: torch.Tensor, sample_rate: float, params: torch.Tens
 
 import os as _os
 
-# Items per pass of the reverb pipeline (bounds the workspace).  Default: one item per SM of the device, so that the
-# one-CTA-per-SM FFT kernels run in whole waves (ifft_shape_kernel: R CTAs per item -> exactly R waves; the persistent
-# block-transform kernels: the same number of blocks per CTA).  Measured on B200 (148 SMs), chain step at batch 1024:
-# 74 -> 14.83 ms, 128 -> 14.61 ms, 148 -> 14.11 ms.  Override for experiments with DASP_REVERB_CHUNK.
+# Items per pass of the reverb pipeline (bounds the workspace).  Default: two items per SM of the device, so that the
+# one-CTA-per-SM FFT kernels run in whole waves (ifft_shape_kernel: R CTAs per item -> exactly 2 R waves; the persistent
+# block-transform kernels: the same number of blocks per CTA).  Measured on one H100 SXM (400 W), chain step at batch
+# 1024: 66 items 23.4 ms, 132 items 22.5 ms, 264 items 22.1 ms.  Override for experiments with DASP_REVERB_CHUNK.
 REVERB_CHUNK_ITEMS = int(_os.environ.get("DASP_REVERB_CHUNK", "0"))      # 0 = automatic
 
 
@@ -543,7 +543,7 @@ def reverb_chunk_items(device) -> int:
     """Items per pass of the reverb pipeline on ``device`` (see REVERB_CHUNK_ITEMS)."""
     if REVERB_CHUNK_ITEMS > 0:
         return REVERB_CHUNK_ITEMS
-    return int(torch.cuda.get_device_properties(device).multi_processor_count)
+    return 2 * int(torch.cuda.get_device_properties(device).multi_processor_count)
 
 
 def _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps):

@@ -1,4 +1,4 @@
-"""Normalised-parameter processors over the B200 kernels.
+"""Normalised-parameter processors over the H100 kernels.
 
 Same contract as the reference's ``dasp_pytorch/modules.py`` (@ c9ae0126): a ``Processor`` owns an ordered
 ``param_ranges`` dict, ``process_normalized(x, p)`` takes ``p`` in ``[0, 1]`` with shape

@@ -1,4 +1,4 @@
-/* dasp_b200.h -- C ABI of libdasp_b200.so: the B200 (sm_100a) kernels behind
+/* dasp_b200.h -- C ABI of libdasp_b200.so: the H100 (sm_90a) kernels behind
  * dasp_pytorch.functional's batched audio-processor hot path.
  *
  * The reference (csteinmetz1/dasp-pytorch @ c9ae0126) is pure Python and has no FFI of its
@@ -39,7 +39,7 @@ extern "C" {
 /* ---- library ---------------------------------------------------------------------- */
 int dasp_abi_version(void);
 const char* dasp_last_error(void);
-/* compiled-for architecture as an integer (1000 for sm_100a) */
+/* compiled-for architecture as an integer (900 for sm_90a) */
 int dasp_compiled_arch(void);
 /* frees cached cuFFT plans and device-side filter-bank spectra */
 void dasp_shutdown(void);

@@ -1,9 +1,9 @@
 """Generate tests/golden/*.npz by running the UNMODIFIED reference on CPU.
 
-Run in the authoring container only (needs /root/reference, which does not exist on
-the GPU box):
+Needs the unmodified reference package ``dasp_pytorch`` importable, either installed or
+from a checkout named by DASP_REFERENCE:
 
-    python oracle/make_golden.py
+    DASP_REFERENCE=/path/to/dasp-pytorch python oracle/make_golden.py
 
 Each fixture stores seeded inputs, the reference outputs in fp32 and fp64, and the
 reference's autograd gradients (loss = mean(y^2)) in fp64.  The oracle
@@ -20,8 +20,8 @@ import sys
 import numpy as np
 import torch
 
-REF = os.environ.get("DASP_REFERENCE", "/root/reference")
-sys.path.insert(0, REF)
+if os.environ.get("DASP_REFERENCE"):
+    sys.path.insert(0, os.environ["DASP_REFERENCE"])
 import dasp_pytorch  # noqa: E402  (the reference)
 import dasp_pytorch.functional as RF  # noqa: E402
 

@@ -26,11 +26,11 @@ def test_header_symbols_exported(lib):
     for name in sorted(declared):
         assert hasattr(lib, name), f"{name} declared in include/dasp_b200.h but not exported"
     assert declared == set(_abi.exported_symbols()), declared ^ set(_abi.exported_symbols())
-    assert lib.dasp_abi_version() == _abi.ABI_VERSION == 2 and lib.dasp_compiled_arch() == 1000
+    assert lib.dasp_abi_version() == _abi.ABI_VERSION == 2 and lib.dasp_compiled_arch() == 900
 
 
-def test_sm100a_sass_and_tma(lib):
-    """the shared library carries sm_100a SASS with TMA bulk copies (UBLKCP) in the recurrence kernels"""
+def test_sm90a_sass_and_tma(lib):
+    """the shared library carries sm_90a SASS with TMA bulk copies (UBLKCP) in the recurrence kernels"""
     import shutil
     import subprocess
     from dasp_pytorch_b200 import _abi
@@ -38,8 +38,8 @@ def test_sm100a_sass_and_tma(lib):
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-lelf", _abi.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert "sm_52" not in out and "sm_90" not in out          # sm_100a only: no multi-arch fat binary
+    assert "sm_90a" in out
+    assert "sm_52" not in out and "sm_100" not in out         # sm_90a only: no multi-arch fat binary
     sass = subprocess.run([cuobjdump, "-sass", _abi.LIB_PATH], capture_output=True, text=True).stdout
     assert "UBLKCP" in sass and "SYNCS" in sass               # cp.async.bulk + mbarrier in the scan kernels
 

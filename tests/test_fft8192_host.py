@@ -1,5 +1,5 @@
 """Host emulation of the in-shared-memory 8192-point FFT (csrc/fft8192.cuh): the same pass functions the fused
-reverb kernel runs, with the CTA's 512 threads looped over sequentially and the packed fp32x2 lanes emulated.
+reverb kernel runs, with the CTA's 512 threads looped over sequentially.
 Pins the index mathematics / twiddle tables of both transform directions without a GPU."""
 import os
 import subprocess

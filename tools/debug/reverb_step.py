@@ -6,7 +6,7 @@ sys.path.insert(0, ".")
 import dasp_pytorch_b200 as D
 
 dev = torch.device("cuda:0")
-bs, n, L = int(sys.argv[1]) if len(sys.argv) > 1 else 148, 48000, 96000
+bs, n, L = int(sys.argv[1]) if len(sys.argv) > 1 else 132, 48000, 96000
 x = torch.rand(bs, 2, n, device=dev, requires_grad=True)
 p = [torch.rand(bs, device=dev, requires_grad=True) for _ in range(25)]
 for _ in range(2):

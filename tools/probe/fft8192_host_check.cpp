@@ -1,5 +1,5 @@
 // Host emulation of csrc/fft8192.cuh: the 512 threads of the CTA are looped over sequentially between the
-// points where the kernel has a barrier, the packed fp32x2 lanes are emulated.  Checks both transform
+// points where the kernel has a barrier.  Checks both transform
 // directions against a double-precision O(N^2)-free reference (recursive radix-2) and prints the max error.
 //   g++ -O2 -std=c++17 -I dasp_pytorch_b200/csrc tools/probe/fft8192_host_check.cpp -o /tmp/fft8192_host_check
 #include <cmath>

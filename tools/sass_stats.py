@@ -3,8 +3,8 @@
 
     python tools/sass_stats.py dasp_pytorch_b200/libdasp_b200.so [--filter eq_] [--md]
 
-Used to check, without a GPU, what the compiler made of a kernel (packed FFMA2 vs scalar FFMA, shuffles, shared-memory
-and local-memory traffic, TMA bulk copies) and to produce the opcode table committed under profiles/.
+Used to check, without a GPU, what the compiler made of a kernel (FFMA / FMUL / FADD counts, shuffles, shared-memory
+and local-memory traffic, TMA bulk copies).
 """
 import collections
 import re

@@ -64,9 +64,10 @@ int debug_eq_bwd_stages();
 // Test hook (dasp_debug_reverb_path): IR synthesis of the device-noise reverb: 0 = automatic, 1 = generator / cuFFT /
 // shaping kernels, 2 = single cluster kernel
 int debug_reverb_path();
-// Test hook (dasp_debug_reverb_flat_filterbank): the spectral IR synthesis uses unit-impulse "filters", so the
-// band-filtered noise it keeps for the backward IS the periodic white sequence w_k the generator draws; the parity
-// test rebuilds the reference-style noise tensor from it and checks the default path against the oracle.
+// Test hook (dasp_debug_reverb_flat_filterbank): both IR syntheses use unit-impulse "filters", so the band-filtered
+// noise they keep for the backward IS the white noise they draw -- the periodic sequence w_k of the spectral
+// generator, or the time-domain blocks noise[b*hop + m] of the overlap-save path; the parity tests rebuild the
+// reference-style noise tensor from it and check the default path against the oracle.
 int debug_flat_filterbank();
 
 // ---------------------------------------------------------------- device helpers

@@ -1474,12 +1474,17 @@ __global__ void reverb_param_grad_kernel(const float* __restrict__ ir_part, cons
 int get_filterbank(const Geom& g, double sr, cudaStream_t st, const float2** out) {
   int dev = 0;
   DASP_CUDA_OK(cudaGetDevice(&dev));
-  FbKey key{dev, g.taps, g.nb, sr};
+  const bool flat = debug_flat_filterbank();        // test hook: H_k = 1 -> the blocks keep the white noise itself
+  FbKey key{dev, flat ? -g.taps : g.taps, g.nb, sr};
   auto it = g_fb.find(key);
   if (it != g_fb.end()) { *out = reinterpret_cast<const float2*>(it->second); return DASP_OK; }
   DASP_REQUIRE(sr / 2.0 > 18000.0, "sample_rate %.1f too low: the filter bank needs 18 kHz < sr/2 (signal.py:84)", sr);
   std::vector<float> taps;
   octave_filterbank((int)g.taps, sr, taps);
+  if (flat) {
+    taps.assign(taps.size(), 0.f);
+    for (int k = 0; k < kBands; ++k) taps[(size_t)k * g.taps] = 1.0f;      // unit impulse at lag 0
+  }
   std::vector<float2> padded((size_t)kBands * g.nb, make_float2(0.f, 0.f));
   const float inv = 1.0f / (float)g.nb;
   for (int k = 0; k < kBands; ++k)

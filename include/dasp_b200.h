@@ -58,8 +58,10 @@ void dasp_debug_reverb_path(int path);
    kernel, 2 = generator + fused FFT/shaping kernel */
 int dasp_debug_reverb_last_path(void);
 
-/* test hook: 1 = the spectral IR synthesis uses unit-impulse filters, so the f_save buffer of dasp_reverb_fwd
-   returns the periodic white sequences w_k themselves (used to rebuild a reference-style noise tensor) */
+/* test hook: 1 = the IR synthesis uses unit-impulse filters, so the f_save buffer of dasp_reverb_fwd returns the white
+   noise itself (used to rebuild a reference-style noise tensor): the periodic sequences w_k of the spectral generator
+   (polyphase layout), or, on the overlap-save path (caller's noise, or device noise with a polyphase factor > 16), the
+   noise blocks C[((item*12 + k)*nbk + b)*nb + m] = noise[b*hop + m] */
 void dasp_debug_reverb_flat_filterbank(int on);
 
 /* ---- Processor.denormalize_param_dict on the device      (reference modules.py:13-14, 70-91) ------

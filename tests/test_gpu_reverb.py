@@ -245,61 +245,3 @@ def test_reverb_chunking_is_invisible(cuda_device, monkeypatch):
         got = run(chunk)
         for a, b in zip(got, ref):              # (cuFFT may pick another kernel for another batch size: rounding only)
             assert float((a - b).abs().max() / b.abs().max()) < 2e-6, chunk
-
-
-@pytest.mark.parametrize("n,L,taps,want_r", [(6000, 4000, 255, 1), (48000, 48000, 1023, 6), (48000, 96000, 1023, 6),
-                                             (70000, 66000, 1023, 9)])
-def test_reverb_device_noise_path_pinned_to_oracle(cuda_device, n, L, taps, want_r):
-    """DETERMINISTIC parity of the DEFAULT (benchmarked) device-noise path -- spectral_gen_kernel -> ifft_shape_kernel
-    -> partitioned convolution, and its backward incl. ir_grad_pp_kernel -- against the fp64 oracle.
-
-    The generator draws, per (item, band, channel), a white PERIODIC sequence w of length n1 = R*8192 in the frequency
-    domain and filters it circularly: f[t] = sum_m h[m] w[(t-m) mod n1].  With the test hook
-    dasp_debug_reverb_flat_filterbank the filters are unit impulses, so the f buffer kept for the backward is w itself.
-    The reference-style noise tensor  noise[t'] = w[(t' - P) mod n1]  (P = taps-1, h symmetric) then makes the
-    reference's valid cross-correlation (functional.py:551-556) produce exactly the same f for every t < min(L, n)
-    (n1 >= min(L, n) + P: no wrap-around inside the window), so y, dL/dx and all 25 parameter gradients of the default
-    call must equal oracle.noise_shaped_reverberation(noise=...) to 1e-4 -- a wrong Hermitian pairing, twiddle,
-    s_half/s_full scaling or polyphase index anywhere in the benchmarked kernels fails this test."""
-    import dasp_pytorch_b200 as D
-    from dasp_pytorch_b200 import _abi
-    lib = _abi.lib()
-    bs, P, nb = 2, taps - 1, 8192
-    leff = min(L, n)
-    R = -(-(leff + P) // nb)
-    assert R == want_r
-    n1 = R * nb
-    g = torch.Generator().manual_seed(n + L)
-    x = (torch.rand(bs, 2, n, generator=g) * 2 - 1)
-    params = _params01(bs, 5 + want_r)
-    kw = dict(num_samples=L, num_bandpass_taps=taps)
-
-    # 1) the white sequences: same seed, unit-impulse filter bank, read f_save from the autograd node
-    lib.dasp_debug_reverb_flat_filterbank(1)
-    try:
-        torch.manual_seed(1234)
-        xq = x.to(cuda_device).requires_grad_(True)
-        yq = D.noise_shaped_reverberation(xq, SR, *[p.to(cuda_device) for p in params], **kw)
-        fsave = yq.grad_fn.saved_tensors[3]
-    finally:
-        lib.dasp_debug_reverb_flat_filterbank(0)
-    assert lib.dasp_debug_reverb_last_path() == 2                      # generator + fused FFT/shaping kernel
-    w = torch.view_as_complex(fsave[: bs * 12 * R * nb * 2].reshape(bs, 12, R, nb, 2).contiguous())   # [.., b, a] = w[R a + b]
-    w = w.permute(0, 1, 3, 2).reshape(bs, 12, n1).cpu()               # (item, band, t), real = left, imag = right
-    assert abs(float(w.real.std()) - 1.0) < 0.02 and abs(float(w.imag.std()) - 1.0) < 0.02      # white, unit variance
-    idx = (torch.arange(L + P) - P) % n1
-    noise = torch.stack([w.real[:, :, idx], w.imag[:, :, idx]], 1).reshape(bs * 2, 12, L + P).double()
-
-    # 2) the default call with the same seed vs the oracle fed that noise
-    def run_default(xx, p):
-        torch.manual_seed(1234)
-        return D.noise_shaped_reverberation(xx, SR, *p, **kw)
-
-    y, dx, dp = run_with_grads(run_default, x, params, torch.float32, cuda_device)
-    assert lib.dasp_debug_reverb_last_path() == 2
-    y64, dx64, dp64 = run_with_grads(
-        lambda xx, p: oracle.noise_shaped_reverberation(xx, SR, *p, noise=noise, method="fft", **kw),
-        x, params, torch.float64, "cpu")
-    assert peak_err(y, y64).max() < TOL, peak_err(y, y64)
-    assert peak_err(dx, dx64).max() < TOL, peak_err(dx, dx64)
-    assert param_grad_err(dp, dp64).max() < TOL, param_grad_err(dp, dp64)

@@ -29,7 +29,7 @@ class ReverbGeom(ctypes.Structure):
 
     _fields_ = [(name, c_int64) for name in (
         "nb", "hop", "nbk", "leff", "rpp", "conv_block", "x_blocks", "ir_partitions", "chunk_items",
-        "f_floats", "xspec_c64", "irspec_c64", "wet_floats", "fwd_workspace_bytes", "bwd_workspace_bytes")]
+        "f_floats", "xspec_c64", "irspec_c64", "fwd_workspace_bytes", "bwd_workspace_bytes")]
 
 P = c_void_p       # device pointer
 I64 = c_int64
@@ -64,8 +64,8 @@ _SIGNATURES = {
     "dasp_eq_fwd": (c_int, [P, P, P, P, I64, I64, I64, c_float, P]),
     "dasp_eq_bwd": (c_int, [P, P, P, P, P, P, P, I64, I64, I64, I64, c_float, P]),
     "dasp_reverb_geometry": (c_int, [I64, I64, I64, I64, I64, ctypes.POINTER(ReverbGeom)]),
-    "dasp_reverb_fwd": (c_int, [P, I64, P, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, c_float, P]),
-    "dasp_reverb_bwd": (c_int, [P, P, I64, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_reverb_fwd": (c_int, [P, I64, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, c_float, P]),
+    "dasp_reverb_bwd": (c_int, [P, P, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_reverb_filterbank": (c_int, [I64, c_double, ctypes.POINTER(c_float)]),
     "dasp_dynamics_tile_len": (I64, [I64, I64]),
     "dasp_dynamics_fwd": (c_int, [c_int, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),

@@ -19,13 +19,14 @@
 //   * IR synthesis, parity mode (caller's noise tensor): overlap-save blocks -> C2C -> cmul_filter_pairs ->
 //     inverse C2C -> shape_ir_pairs_kernel.
 //   * Audio convolution: uniformly partitioned overlap-save in the frequency domain: x_fft_kernel (window gather +
-//     FFT), partition_mac_kernel, ifft_mix_kernel (inverse FFT + crop + wet/dry mix), all on the own FFT; rows that
-//     are not 16-byte aligned use x_blocks_kernel, cuFFT C2C, mix_blocks_kernel.
+//     FFT, and the FFT of the IR partitions), partition_mac_kernel, ifft_mix_kernel (inverse FFT + crop + wet/dry mix),
+//     all on the own FFT; rows that are not 16-byte aligned use x_blocks_kernel, cuFFT C2C, mix_blocks_kernel.
 //   * Items are processed in chunks (chosen by the caller; the Python host uses one item per SM) to bound the workspace.
 //
-// Backward (A.5): g_blocks_kernel (+ dL/dmix partials), C2C, two correlation passes of partition_mac_kernel
-// against the saved block spectra (dL/dx windows, dL/dIR partitions), two inverse C2C, finish_dx_blocks_kernel,
-// ir_grad_*_kernel (dL/dIR * env * f reductions for the 24 band parameters; deterministic two-stage sums).
+// Backward (A.5): g_fft_kernel, two correlation passes of partition_mac_kernel against the saved block spectra (dL/dx
+// windows, dL/dIR partitions), ifft_dx_kernel (+ dL/dmix partials), ifft_irgrad_kernel (dL/dIR * env * f reductions for
+// the 24 band parameters; deterministic two-stage sums); the cuFFT variants are g_blocks_kernel, C2C,
+// finish_dx_blocks_kernel, inverse C2C, ir_grad_*_kernel.
 #include <cufft.h>
 #include <curand_kernel.h>
 #include <math.h>
@@ -425,7 +426,8 @@ __device__ __forceinline__ float time_axis32(int t, int L, float step) {
 }
 
 // IR[c][t] = (1/12) sum_k gain_k exp(-(10 decay_k + 1) tt(t)) f_c[k][t]  for t < leff, written as (left, right)
-// complex pairs into the zero-initialised partition layout of the audio convolution.
+// complex pairs into the partition layout of the audio convolution (first half of partition t / kB; every synthesis
+// variant writes these taps and nothing else).
 // grid = (nbk, items): CTA (b, item) produces samples [b*hop, (b+1)*hop).
 __global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params /* chunk x 25 */,
                                       float2* __restrict__ Hb, int64_t L, int64_t leff, int jb, int nbk, int nb,
@@ -627,18 +629,35 @@ __device__ __forceinline__ void fft8192_in_smem(float* gr, float* gi, const FftS
   fft8k::p4<INV>(s.Yr, s.Yi, t, xr, xi);
 }
 
-// Xb[(il*I + i)*kNbA + f] = FFT of the window (x_left + i x_right)[(i-1) kB + m], m < kNbA  (zero outside [0, n)):
-// x_blocks_kernel + forward C2C in one kernel.  Requires n % 4 == 0 and 16-byte aligned rows (bulk copies).
+// Both forward block transforms of the audio convolution, one persistent work list of nwin + items*J units:
+//   unit m < nwin = items*I:  Xb[(il*I + i)*kNbA + f] = FFT of the window (x_left + i x_right)[(i-1) kB + m], m < kNbA
+//                             (zero outside [0, n)): x_blocks_kernel + forward C2C in one kernel.
+//   unit nwin + il*J + j:     IR partition j of item il, in place in Hb: only the first kB (left, right) pairs of the slot
+//                             are read (the synthesis writes nothing else), taps >= leff and the second half are zeroed in
+//                             shared memory, so Hb needs no zero-fill and nobody reads the rest of the slot.
+// Requires n % 4 == 0 and 16-byte aligned rows (bulk copies).
 __global__ void __launch_bounds__(kFusedThreads, 1)
-x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, const float* __restrict__ twiddles, int64_t item0,
-             int I, int64_t n, int in_chs, int nblocks) {
+x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __restrict__ Hb,
+             const float* __restrict__ twiddles, int64_t item0, int I, int J, int64_t n, int64_t leff, int in_chs,
+             int nwin, int nunits) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
   const int t = threadIdx.x;
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
   auto fetch = [&](int it, int m) {                // all threads: zero padding; thread 0: the bulk copies
-    if (m >= nblocks) return;
+    if (m >= nunits) return;
+    if (m >= nwin) {                               // partition: its 32 KB of taps land in the im plane, see below
+      if (t == 0) {
+        float* im = s.G + (it & 1) * 2 * fft8k::kPlaneG + fft8k::kPlaneG;
+        const float* src = reinterpret_cast<const float*>(Hb + (int64_t)(m - nwin) * kNbA);
+        uint64_t* bar = &s.full[it & 1];
+        mbar_arrive_expect_tx(bar, 2u * kB * 4u);
+        tma_load_1d(im, src, 16384u, bar);
+        tma_load_1d(im + 4096, src + 4096, 16384u, bar);
+      }
+      return;
+    }
     const int64_t il = m / I;
     const int i = m - (int)il * I;
     float* re = s.G + (it & 1) * 2 * fft8k::kPlaneG;
@@ -665,12 +684,30 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, const float* 
   fetch(1, blockIdx.x + gridDim.x);
   __syncthreads();                                 // the zero padding of the first two buffers is in place
   int it = 0;
-  for (int m = blockIdx.x; m < nblocks; m += gridDim.x, ++it) {
+  for (int m = blockIdx.x; m < nunits; m += gridDim.x, ++it) {
     mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
     float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    float* gi = gr + fft8k::kPlaneG;
+    if (m >= nwin) {                               // deinterleave the partition's (left, right) pairs into the planes
+      const int64_t lim = leff - (int64_t)((m - nwin) % J) * kB;      // taps e < lim exist (lim > 0)
+      float2 v[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) v[q] = reinterpret_cast<const float2*>(gi)[t + 512 * q];
+      __syncthreads();
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const int e = t + 512 * q;
+        const bool tap = e < lim;                  // a select, not a product: the bytes past leff are never written
+        gr[e] = tap ? v[q].x : 0.f;
+        gi[e] = tap ? v[q].y : 0.f;
+        gr[kB + e] = 0.f;
+        gi[kB + e] = 0.f;
+      }
+      __syncthreads();
+    }
     float xr[16], xi[16];
-    fft8192_in_smem<false>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
-    float2* out = Xb + (int64_t)m * kNbA;
+    fft8192_in_smem<false>(gr, gi, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
+    float2* out = m < nwin ? Xb + (int64_t)m * kNbA : Hb + (int64_t)(m - nwin) * kNbA;
 #pragma unroll
     for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(xr[q], xi[q]);
   }
@@ -680,8 +717,8 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, const float* 
 // samples [i kB, (i+1) kB) as the second half of the transform; y = x + mix (wet - x).
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddles, const float* __restrict__ x,
-                const float* __restrict__ params, float* __restrict__ y, float* __restrict__ wet_save, int64_t item0,
-                int I, int64_t n, int in_chs, int nblocks) {
+                const float* __restrict__ params, float* __restrict__ y, int64_t item0, int I, int64_t n, int in_chs,
+                int nblocks) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
   const int t = threadIdx.x;
@@ -725,29 +762,32 @@ ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddle
       if (tg < n) {
         y[(b * 2 + 0) * n + tg] = fmaf(mix, xr[q] - a0[q - 8], a0[q - 8]);
         y[(b * 2 + 1) * n + tg] = fmaf(mix, xi[q] - a1[q - 8], a1[q - 8]);
-        if (wet_save) { wet_save[(b * 2 + 0) * n + tg] = xr[q]; wet_save[(b * 2 + 1) * n + tg] = xi[q]; }
       }
     }
   }
 }
 
 // ---- the backward's block transforms on the same in-shared-memory FFT --------------------------------------
-// g_fft_kernel     = g_blocks_kernel + forward C2C:  Gs[i] = FFT([0 .. 0 | mix g block i]),  + dL/dmix partials
+// g_fft_kernel     = g_blocks_kernel + forward C2C:  Gs[i] = FFT([0 .. 0 | g block i])  (not scaled by mix)
 // ifft_dx_kernel   = inverse C2C + finish_dx_blocks_kernel: one CTA walks the windows of an item in order and keeps
 //                    the second half of window i in registers until the first half of window i + 1 arrives, so the
-//                    overlap-add of the two windows that cover a sample needs no second pass and no atomics
+//                    overlap-add of the two windows that cover a sample needs no second pass and no atomics; it also
+//                    forms the dL/dmix partials (see there)
 // ifft_irgrad_kernel = inverse C2C of the dL/dIR partitions + ir_grad_pp_kernel: the 4096 taps of a partition go to
 //                    shared memory and are correlated with the filtered noise f read class by class (coalesced)
+//
+// Why G is not scaled: the inverse transforms of the dx windows then yield c(s) = sum_tau IR(tau) g(s + tau), the
+// gradient of the wet signal with respect to x, and since sum_t g(t) wet(t) = sum_s x(s) c(s),
+//   dL/dmix = sum over both channels of g (wet - x) = sum_s x (c - g)
+// needs x but not the wet signal, so the forward does not save it.  mix is applied to c in ifft_dx_kernel and to the
+// dL/dIR band sums in reverb_param_grad_kernel.
 
-// Gb[(il*I + i)*kNbA + f] = FFT of [zeros(kB) | mix (g_left + i g_right)[i kB + m], m < kB];
-// mix_part[il*I + i] = sum over the block and both channels of g (wet - x)
+// Gb[(il*I + i)*kNbA + f] = FFT of [zeros(kB) | (g_left + i g_right)[i kB + m], m < kB]
 __global__ void __launch_bounds__(kFusedThreads, 1)
-g_fft_kernel(const float* __restrict__ gy, const float* __restrict__ x, const float* __restrict__ wet,
-             const float* __restrict__ params, float2* __restrict__ Gb, float* __restrict__ mix_part,
-             const float* __restrict__ twiddles, int64_t item0, int I, int64_t n, int in_chs, int nblocks) {
+g_fft_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, const float* __restrict__ twiddles, int64_t item0,
+             int I, int64_t n, int nblocks) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
-  __shared__ float wp[kFusedThreads / 32];
   const int t = threadIdx.x;
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
@@ -777,52 +817,24 @@ g_fft_kernel(const float* __restrict__ gy, const float* __restrict__ x, const fl
   for (int m = blockIdx.x; m < nblocks; m += gridDim.x, ++it) {
     mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
     float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
-    const int64_t il = m / I, b = item0 + il;
-    const int i = m - (int)il * I;
-    const float mix = params[b * 25 + 24];
-    // dL/dmix partial: the block's g sits in shared memory (second half of the planes), wet and x come from HBM
-    float acc = 0.f;
-    {
-      const float* xl = x + (b * in_chs) * n;
-      const float* xr = in_chs == 1 ? xl : xl + n;
-      const float* wl = wet + (b * 2) * n;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int mm = t + 512 * q;
-        const int64_t tg = (int64_t)i * kB + mm;
-        if (tg < n) {
-          const float g0 = gr[kB + mm], g1 = gr[fft8k::kPlaneG + kB + mm];
-          acc = fmaf(g0, wl[tg] - xl[tg], fmaf(g1, wl[n + tg] - xr[tg], acc));
-        }
-      }
-    }
-    __syncthreads();                                 // pass 1 transforms the planes in place
     float xr_[16], xi_[16];
     fft8192_in_smem<false>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr_, xi_);
     float2* out = Gb + (int64_t)m * kNbA;
 #pragma unroll
-    for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(mix * xr_[q], mix * xi_[q]);
-    acc = warp_sum(acc);
-    if ((t & 31) == 0) wp[t >> 5] = acc;
-    __syncthreads();
-    if (t == 0) {
-      float sum = 0.f;
-#pragma unroll
-      for (int w = 0; w < kFusedThreads / 32; ++w) sum += wp[w];
-      mix_part[m] = sum;
-    }
-    // (wp is next written after the barriers inside the following transform)
+    for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(xr_[q], xi_[q]);
   }
 }
 
-// gx[t] = (1-mix) g[t] + D[q][kB + t - q kB] + D[q+1][t - q kB], q = t / kB, from the planar product spectra Dpl
-// (one CTA per item at a time; mono input receives the sum of both channel gradients)
+// gx[t] = (1-mix) g[t] + mix c[t],  c[t] = D[q][kB + t - q kB] + D[q+1][t - q kB], q = t / kB, from the planar product
+// spectra Dpl (one CTA per item at a time; mono input receives the sum of both channel gradients);
+// mix_part[il*I + q] = sum over block q and both channels of x (c - g)  (mono: x counted once per channel)
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles, const float* __restrict__ gy,
-               const float* __restrict__ params, float* __restrict__ gx, int64_t item0, int items, int I, int64_t n,
-               int in_chs) {
+               const float* __restrict__ x, const float* __restrict__ params, float* __restrict__ gx,
+               float* __restrict__ mix_part, int64_t item0, int items, int I, int64_t n, int in_chs) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
+  __shared__ float wp[2][kFusedThreads / 32];
   const int t = threadIdx.x;
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
@@ -850,26 +862,34 @@ ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles
     const int i = it % I;
     const float mix = params[b * 25 + 24];
     const float* g0p = gy + (b * 2) * n;
+    const float* xl = x + (b * in_chs) * n;
+    const float* xrr = in_chs == 1 ? xl : xl + n;
     // the block finished by this window is i - 1 (its first half); after the last window also block I - 1
-    float ga[8], gb[8];
+    float ga[8], gb[8], xa[8], xb[8];
     float xr[16], xi[16];
     fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2); },
                           [&] {
 #pragma unroll
                             for (int q = 0; q < 8; ++q) {
                               const int64_t t0 = (int64_t)(i - 1) * kB + (t + 512 * q);
-                              ga[q] = (i > 0 && t0 < n) ? g0p[t0] : 0.f;
-                              gb[q] = (i > 0 && t0 < n) ? g0p[n + t0] : 0.f;
+                              const bool in = i > 0 && t0 < n;
+                              ga[q] = in ? g0p[t0] : 0.f;
+                              gb[q] = in ? g0p[n + t0] : 0.f;
+                              xa[q] = in ? xl[t0] : 0.f;
+                              xb[q] = in ? xrr[t0] : 0.f;
                             }
                           },
                           xr, xi);
     const float om = 1.0f - mix;
+    float acc0 = 0.f, acc1 = 0.f;                    // dL/dmix partials of blocks i - 1 and (last window) I - 1
     if (i > 0) {
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         const int64_t tg = (int64_t)(i - 1) * kB + (t + 512 * q);
         if (tg < n) {
-          const float o0 = fmaf(om, ga[q], pr[q] + xr[q]), o1 = fmaf(om, gb[q], pi[q] + xi[q]);
+          const float c0 = pr[q] + xr[q], c1 = pi[q] + xi[q];
+          const float o0 = fmaf(om, ga[q], mix * c0), o1 = fmaf(om, gb[q], mix * c1);
+          acc0 = fmaf(xa[q], c0 - ga[q], fmaf(xb[q], c1 - gb[q], acc0));
           if (in_chs == 1) gx[b * n + tg] = o0 + o1;
           else { gx[(b * 2) * n + tg] = o0; gx[(b * 2 + 1) * n + tg] = o1; }
         }
@@ -882,11 +902,27 @@ ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles
       for (int q = 0; q < 8; ++q) {
         const int64_t tg = (int64_t)i * kB + (t + 512 * q);
         if (tg < n) {
-          const float o0 = fmaf(om, g0p[tg], pr[q]), o1 = fmaf(om, g0p[n + tg], pi[q]);
+          const float g0 = g0p[tg], g1 = g0p[n + tg];
+          const float o0 = fmaf(om, g0, mix * pr[q]), o1 = fmaf(om, g1, mix * pi[q]);
+          acc1 = fmaf(xl[tg], pr[q] - g0, fmaf(xrr[tg], pi[q] - g1, acc1));
           if (in_chs == 1) gx[b * n + tg] = o0 + o1;
           else { gx[(b * 2) * n + tg] = o0; gx[(b * 2 + 1) * n + tg] = o1; }
         }
       }
+    }
+    if (i > 0 || i == I - 1) {                       // uniform over the CTA
+      acc0 = warp_sum(acc0);
+      acc1 = warp_sum(acc1);
+      if ((t & 31) == 0) { wp[0][t >> 5] = acc0; wp[1][t >> 5] = acc1; }
+      __syncthreads();
+      if (t == 0) {
+        float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+        for (int w = 0; w < kFusedThreads / 32; ++w) { s0 += wp[0][w]; s1 += wp[1][w]; }
+        if (i > 0) mix_part[il * I + i - 1] = s0;
+        if (i == I - 1) mix_part[il * I + i] = s1;
+      }
+      // (wp is next written after the barriers inside the following transform)
     }
   }
 }
@@ -1321,10 +1357,10 @@ __global__ void __launch_bounds__(128) partition_mac_bwd_kernel(const float2* __
   }
 }
 
-// y = (1-mix) x + mix wet; wet[n] = Yt[(il*I + n/kB)*kNbA + kB + n%kB]; also saves wet for the backward
+// y = (1-mix) x + mix wet; wet[n] = Yt[(il*I + n/kB)*kNbA + kB + n%kB]
 __global__ void mix_blocks_kernel(const float* __restrict__ x, const float2* __restrict__ Yt,
-                                  const float* __restrict__ params, float* __restrict__ y, float* __restrict__ wet_save,
-                                  int64_t item0, int I, int64_t n, int in_chs) {
+                                  const float* __restrict__ params, float* __restrict__ y, int64_t item0, int I,
+                                  int64_t n, int in_chs) {
   const int i = blockIdx.x;
   const int64_t il = blockIdx.y, b = item0 + il;
   const float mix = params[b * 25 + 24];
@@ -1338,36 +1374,48 @@ __global__ void mix_blocks_kernel(const float* __restrict__ x, const float2* __r
     const float a0 = xl[t], a1 = xr[t];
     y[(b * 2 + 0) * n + t] = fmaf(mix, w.x - a0, a0);
     y[(b * 2 + 1) * n + t] = fmaf(mix, w.y - a1, a1);
-    if (wet_save) { wet_save[(b * 2 + 0) * n + t] = w.x; wet_save[(b * 2 + 1) * n + t] = w.y; }
   }
 }
 
-// backward: Gb[(il*I + i)*kNbA + kB + m] = mix (g_left, g_right)[i kB + m], first half zero;
-// mix_part[il*I + i] = sum over the block and both channels of g (wet - x)
-__global__ void g_blocks_kernel(const float* __restrict__ gy, const float* __restrict__ x, const float* __restrict__ wet,
-                                const float* __restrict__ params, float2* __restrict__ Gb, float* __restrict__ mix_part,
-                                int64_t item0, int I, int64_t n, int in_chs) {
+// backward: Gb[(il*I + i)*kNbA + kB + m] = (g_left, g_right)[i kB + m] (not scaled by mix), first half zero
+__global__ void g_blocks_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, int64_t item0, int I, int64_t n) {
+  const int i = blockIdx.x;
+  const int64_t il = blockIdx.y, b = item0 + il;
+  const float* gl = gy + (b * 2 + 0) * n;
+  const float* gr = gy + (b * 2 + 1) * n;
+  float2* out = Gb + (il * I + i) * (int64_t)kNbA;
+  for (int m = threadIdx.x; m < kB; m += blockDim.x) {
+    const int64_t t = (int64_t)i * kB + m;
+    out[m] = make_float2(0.f, 0.f);
+    out[kB + m] = t < n ? make_float2(gl[t], gr[t]) : make_float2(0.f, 0.f);
+  }
+}
+
+// gx[t] = (1-mix) g[t] + mix c[t],  c[t] = Dt[q][t - (q-1) kB] + Dt[q+1][t - q kB], q = t / kB (every sample sits in
+// two windows); mono input receives the sum of both channel gradients.
+// mix_part[il*I + i] = sum over block i and both channels of x (c - g)  (see g_fft_kernel)
+__global__ void finish_dx_blocks_kernel(const float* __restrict__ gy, const float* __restrict__ x,
+                                        const float2* __restrict__ Dt, const float* __restrict__ params,
+                                        float* __restrict__ gx, float* __restrict__ mix_part, int64_t item0, int I,
+                                        int64_t n, int in_chs) {
   const int i = blockIdx.x;
   const int64_t il = blockIdx.y, b = item0 + il;
   const float mix = params[b * 25 + 24];
   const float* xl = x + (b * in_chs) * n;
   const float* xr = in_chs == 1 ? xl : xl + n;
-  const float* gl = gy + (b * 2 + 0) * n;
-  const float* gr = gy + (b * 2 + 1) * n;
-  const float* wl = wet + (b * 2 + 0) * n;
-  const float* wr = wet + (b * 2 + 1) * n;
-  float2* out = Gb + (il * I + i) * (int64_t)kNbA;
+  const float2* d0 = Dt + (il * I + i) * (int64_t)kNbA + kB;
+  const float2* d1 = (i + 1 < I) ? Dt + (il * I + i + 1) * (int64_t)kNbA : nullptr;
   float acc = 0.f;
   for (int m = threadIdx.x; m < kB; m += blockDim.x) {
     const int64_t t = (int64_t)i * kB + m;
-    float2 v = make_float2(0.f, 0.f);
-    if (t < n) {
-      const float g0 = gl[t], g1 = gr[t];
-      v = make_float2(mix * g0, mix * g1);
-      acc = fmaf(g0, wl[t] - xl[t], fmaf(g1, wr[t] - xr[t], acc));
-    }
-    out[m] = make_float2(0.f, 0.f);
-    out[kB + m] = v;
+    if (t >= n) break;
+    float2 v = d0[m];
+    if (d1) { const float2 u = d1[m]; v.x += u.x; v.y += u.y; }
+    const float g0 = gy[(b * 2 + 0) * n + t], g1 = gy[(b * 2 + 1) * n + t];
+    const float o0 = fmaf(1.0f - mix, g0, mix * v.x), o1 = fmaf(1.0f - mix, g1, mix * v.y);
+    acc = fmaf(xl[t], v.x - g0, fmaf(xr[t], v.y - g1, acc));
+    if (in_chs == 1) gx[b * n + t] = o0 + o1;
+    else { gx[(b * 2 + 0) * n + t] = o0; gx[(b * 2 + 1) * n + t] = o1; }
   }
   __shared__ float wp[32];
   acc = warp_sum(acc);
@@ -1377,28 +1425,6 @@ __global__ void g_blocks_kernel(const float* __restrict__ gy, const float* __res
     float sum = 0.f;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) sum += wp[w];
     mix_part[il * I + i] = sum;
-  }
-}
-
-// gx[t] = (1-mix) g[t] + Dt[q][t - (q-1) kB] + Dt[q+1][t - q kB], q = t / kB (every sample sits in two windows);
-// mono input receives the sum of both channel gradients
-__global__ void finish_dx_blocks_kernel(const float* __restrict__ gy, const float2* __restrict__ Dt,
-                                        const float* __restrict__ params, float* __restrict__ gx, int64_t item0, int I,
-                                        int64_t n, int in_chs) {
-  const int i = blockIdx.x;
-  const int64_t il = blockIdx.y, b = item0 + il;
-  const float mix = params[b * 25 + 24];
-  const float2* d0 = Dt + (il * I + i) * (int64_t)kNbA + kB;
-  const float2* d1 = (i + 1 < I) ? Dt + (il * I + i + 1) * (int64_t)kNbA : nullptr;
-  for (int m = threadIdx.x; m < kB; m += blockDim.x) {
-    const int64_t t = (int64_t)i * kB + m;
-    if (t >= n) break;
-    float2 v = d0[m];
-    if (d1) { const float2 u = d1[m]; v.x += u.x; v.y += u.y; }
-    const float g0 = gy[(b * 2 + 0) * n + t], g1 = gy[(b * 2 + 1) * n + t];
-    const float o0 = fmaf(1.0f - mix, g0, v.x), o1 = fmaf(1.0f - mix, g1, v.y);
-    if (in_chs == 1) gx[b * n + t] = o0 + o1;
-    else { gx[(b * 2 + 0) * n + t] = o0; gx[(b * 2 + 1) * n + t] = o1; }
   }
 }
 
@@ -1447,7 +1473,8 @@ __global__ void ir_grad_pairs_kernel(const float2* __restrict__ Et, const float2
   }
 }
 
-// one thread per (item, param): gains (0..11), decays (12..23), mix (24)
+// one thread per (item, param): gains (0..11), decays (12..23), mix (24).  The dL/dIR partials come from gradient
+// spectra that are not scaled by mix (see g_fft_kernel), so the band sums take the factor here.
 __global__ void reverb_param_grad_kernel(const float* __restrict__ ir_part, const float* __restrict__ mix_part,
                                          const float* __restrict__ params, float* __restrict__ gparams, int64_t item0,
                                          int64_t items, int nbk, int mix_blocks) {
@@ -1461,6 +1488,7 @@ __global__ void reverb_param_grad_kernel(const float* __restrict__ ir_part, cons
     const int k = q % kBands;
     const float* pr = ir_part + (bl * nbk * kBands + k) * 2 + (q < kBands ? 0 : 1);
     for (int i = 0; i < nbk; ++i) s += (double)pr[(int64_t)i * kBands * 2];
+    s *= (double)pp[24];
     if (q < kBands) s *= (1.0 / kBands);
     else s *= (double)pp[k] * (-10.0 / kBands);
   } else {
@@ -1795,14 +1823,13 @@ int dasp_reverb_geometry(int64_t bs, int64_t n, int64_t num_samples, int64_t tap
   out->f_floats = bs * kBands * g.pair_c64() * 2;
   out->xspec_c64 = bs * g.ib * kNbA;
   out->irspec_c64 = bs * g.jb * kNbA;
-  out->wet_floats = bs * 2 * n;
   out->fwd_workspace_bytes = (int64_t)fw.total;
   out->bwd_workspace_bytes = (int64_t)bw.total;
   return DASP_OK;
 }
 
 int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const float* noise, const uint64_t* seed_dev, float* y,
-                    float* wet_save, float* f_save, void* xspec_save, void* irspec_save, void* workspace,
+                    float* f_save, void* xspec_save, void* irspec_save, void* workspace,
                     int64_t workspace_bytes, int64_t bs, int64_t n, int64_t num_samples, int64_t taps,
                     int64_t chunk_items, float sample_rate, void* stream) {
   Geom g;
@@ -1843,9 +1870,13 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? (float2*)irspec_save + item0 * J * (int64_t)kNbA : (float2*)(base + w.hsp);
     const dim3 gblk((unsigned)nbk, kBands, (unsigned)items);
+    // audio convolution: block transforms on the own FFT (fused with their pre/post kernels) when the rows allow bulk copies
+    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(x) && aligned16(hs);
 
-    // ---- IR synthesis: (left, right) taps land in the zero-initialised partition layout hs ----
-    DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
+    // ---- IR synthesis: taps t < leff land as (left, right) pairs in the first half of partition t / kB of hs ----
+    // x_fft_kernel reads nothing else of hs; the cuFFT transform of the partitions reads whole slots, so they are
+    // zero-filled first
+    if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
     // device-noise IR synthesis, three variants (same Philox stream, so they agree to transform rounding):
     //   2 = generator -> ifft_shape_kernel (own in-shared-memory FFT fused with the shaping; default for nb == 8192)
     //   1 = one thread-block cluster per item (generator + FFT + shaping in one kernel; dasp_debug_reverb_path(2))
@@ -1854,8 +1885,6 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
     if (own_fft && debug_reverb_path() == 2 && g.rpp <= kMaxFusedR) synth = 1;
     else if (own_fft && debug_reverb_path() != 1) synth = 2;
-    // audio convolution: block transforms on the own FFT (fused with their pre/post kernels) when the rows allow bulk copies
-    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(x);
     const float* tw = nullptr;
     if ((synth != 0 || own_conv) && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
     if (synth == 1) {
@@ -1901,20 +1930,24 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     // ---- audio convolution (partitioned, frequency domain) ----
     const int nblk = (int)(items * I);
     const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-    DASP_CUFFT_OK(cufftSetStream(pl.hj_c2c.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj_c2c.h, ws_cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.hj_c2c.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
     if (own_conv) {
       if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
-      x_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, I, n, (int)in_chs, nblk);
+      // one work list: the items*I audio windows, then the items*J IR partitions (transformed in place in hs)
+      const int nunits = (int)(items * (I + J));
+      const unsigned xh_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
+      x_fft_kernel<<<xh_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, n, g.leff, (int)in_chs, nblk,
+                                                                  nunits);
       DASP_LAUNCH_OK("x_fft_kernel");
       launch_mac<false, true>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
       DASP_LAUNCH_OK("partition_mac_kernel");
       ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ys), tw, x, params, y,
-                                                                     wet_save, item0, I, n, (int)in_chs, nblk);
+                                                                     item0, I, n, (int)in_chs, nblk);
       DASP_LAUNCH_OK("ifft_mix_kernel");
       continue;
     }
+    DASP_CUFFT_OK(cufftSetStream(pl.hj_c2c.h, st));
+    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj_c2c.h, ws_cufft));
+    DASP_CUFFT_OK(cufftExecC2C(pl.hj_c2c.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
     x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, n, (int)in_chs);
     DASP_LAUNCH_OK("x_blocks_kernel");
     DASP_CUFFT_OK(cufftSetStream(pl.xi_c2c.h, st));
@@ -1923,14 +1956,13 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     launch_mac<false>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
     DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_ys, (cufftComplex*)ws_ys, CUFFT_INVERSE));
-    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, params, y, wet_save, item0, I, n,
-                                                                        (int)in_chs);
+    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, params, y, item0, I, n, (int)in_chs);
     DASP_LAUNCH_OK("mix_blocks_kernel");
   }
   return DASP_OK;
 }
 
-int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float* params, const float* wet_save,
+int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float* params,
                     const float* f_save, const void* xspec_save, const void* irspec_save, float* gx, float* gparams,
                     void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t num_samples, int64_t taps,
                     int64_t chunk_items, int64_t device_noise, void* stream) {
@@ -1940,7 +1972,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
   DASP_REQUIRE(in_chs == 1 || in_chs == 2, "only mono/stereo signals are supported");
   if (bs == 0) return DASP_OK;
   const bool polyphase = device_noise != 0 && g.rpp <= kMaxSpectralR;   // layout the forward left in f_save
-  DASP_REQUIRE(gy && x && params && wet_save && f_save && xspec_save && irspec_save && gx && gparams && workspace,
+  DASP_REQUIRE(gy && x && params && f_save && xspec_save && irspec_save && gx && gparams && workspace,
                "reverb bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
@@ -1984,8 +2016,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
     const int mb = I > J ? I : J;
     const bool fused_mac = own_irgrad && mb <= 16;
     if (own_conv) {
-      g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, x, wet_save, params, ws_gs, ws_mixpart, tw, item0, I, n,
-                                                                   (int)in_chs, nblk);
+      g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, ws_gs, tw, item0, I, n, nblk);
       DASP_LAUNCH_OK("g_fft_kernel");
       if (fused_mac) {
         dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
@@ -1997,12 +2028,11 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
         DASP_LAUNCH_OK("partition_mac_kernel<corr>");
       }
       const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
-      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, params, gx,
-                                                                    item0, (int)items, I, n, (int)in_chs);
+      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, x, params,
+                                                                    gx, ws_mixpart, item0, (int)items, I, n, (int)in_chs);
       DASP_LAUNCH_OK("ifft_dx_kernel");
     } else {
-      g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, wet_save, params, ws_gs, ws_mixpart, item0,
-                                                                        I, n, (int)in_chs);
+      g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, ws_gs, item0, I, n);
       DASP_LAUNCH_OK("g_blocks_kernel");
       DASP_CUFFT_OK(cufftSetStream(pl.xi_c2c.h, st));
       DASP_CUFFT_OK(cufftSetWorkArea(pl.xi_c2c.h, ws_cufft));
@@ -2010,8 +2040,8 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
       launch_mac<true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);
       DASP_LAUNCH_OK("partition_mac_kernel<corr>");
       DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_ds, (cufftComplex*)ws_ds, CUFFT_INVERSE));
-      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, ws_ds, params, gx, item0, I, n,
-                                                                                (int)in_chs);
+      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ws_ds, params, gx, ws_mixpart, item0,
+                                                                                I, n, (int)in_chs);
       DASP_LAUNCH_OK("finish_dx_blocks_kernel");
     }
     int nparts;

@@ -576,25 +576,26 @@ class _ReverbFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             check(lib.dasp_reverb_geometry(bs, n, num_samples, taps, chunk, geom), "dasp_reverb_geometry")
             ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
-            wet = fsave = xspec = irspec = None
+            fsave = xspec = irspec = None
             if need_bwd:
-                wet = torch.empty(geom.wet_floats, dtype=torch.float32, device=dev)
                 fsave = torch.empty(geom.f_floats, dtype=torch.float32, device=dev)
                 xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
                 irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
             with _timed("reverb_fwd", dev):
-                check(lib.dasp_reverb_fwd(ptr(x), in_chs, ptr(params), ptr(noise), ptr(seed), ptr(y), ptr(wet),
-                                          ptr(fsave), ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n, num_samples,
-                                          taps, chunk, float(sample_rate), stream_ptr(dev)), "dasp_reverb_fwd")
+                check(lib.dasp_reverb_fwd(ptr(x), in_chs, ptr(params), ptr(noise), ptr(seed), ptr(y), ptr(fsave),
+                                          ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n, num_samples, taps, chunk,
+                                          float(sample_rate), stream_ptr(dev)), "dasp_reverb_fwd")
         if need_bwd:
-            ctx.save_for_backward(x, params, wet, fsave, xspec, irspec)
+            # slot 2 (the wet signal, which the backward no longer needs) stays empty so that callers that inspect
+            # grad_fn.saved_tensors keep the layout (x, params, -, f, X spectra, IR spectra)
+            ctx.save_for_backward(x, params, None, fsave, xspec, irspec)
         ctx.cfg = (num_samples, taps, chunk, geom.bwd_workspace_bytes, 1 if noise is None else 0)
         return y
 
     @staticmethod
     def backward(ctx, gy):
         lib = _abi.lib()
-        x, params, wet, fsave, xspec, irspec = ctx.saved_tensors
+        x, params, _, fsave, xspec, irspec = ctx.saved_tensors
         num_samples, taps, chunk, bwd_bytes, device_noise = ctx.cfg
         bs, in_chs, n = x.shape
         dev = x.device
@@ -603,9 +604,9 @@ class _ReverbFn(torch.autograd.Function):
         gp = torch.empty_like(params)
         ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev), _timed("reverb_bwd", dev):
-            check(lib.dasp_reverb_bwd(ptr(gy), ptr(x), in_chs, ptr(params), ptr(wet), ptr(fsave), ptr(xspec),
-                                      ptr(irspec), ptr(gx), ptr(gp), ptr(ws), ws.numel(), bs, n, num_samples, taps,
-                                      chunk, device_noise, stream_ptr(dev)), "dasp_reverb_bwd")
+            check(lib.dasp_reverb_bwd(ptr(gy), ptr(x), in_chs, ptr(params), ptr(fsave), ptr(xspec), ptr(irspec),
+                                      ptr(gx), ptr(gp), ptr(ws), ws.numel(), bs, n, num_samples, taps, chunk,
+                                      device_noise, stream_ptr(dev)), "dasp_reverb_bwd")
         return gx, gp, None, None, None, None, None, None
 
 

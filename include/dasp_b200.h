@@ -149,10 +149,10 @@ int dasp_eq_bwd(const float* gy, const float* x, const float* params, const floa
  *        replay as long as the caller's graph also refreshes that word, as torch's graph-safe generator does);
  *        else the (bs*2, 12, num_samples + taps - 1) tensor the reference would have drawn
  *        (functional.py:547-548) -- the parity-test entry.
- * Buffers kept for the backward (pass NULL for all four when no backward follows):
- *   wet_save  bs*2*n floats, f_save  geom.f_floats floats (band-filtered noise blocks, left/right
- *   channel interleaved as complex pairs),
+ * Buffers kept for the backward (pass NULL for all three when no backward follows):
+ *   f_save  geom.f_floats floats (band-filtered noise blocks, left/right channel interleaved as complex pairs),
  *   xspec_save  geom.xspec_c64 complex64, irspec_save  geom.irspec_c64 complex64 (block spectra).
+ *   The wet signal is not kept: the backward forms dL/dmix from x and the gradient it propagates to x.
  * workspace: geom.fwd_workspace_bytes / geom.bwd_workspace_bytes bytes of device memory. */
 typedef struct dasp_reverb_geom {
   int64_t nb, hop, nbk;       /* IR synthesis, overlap-save path: block length, hop, blocks per band signal */
@@ -162,17 +162,17 @@ typedef struct dasp_reverb_geom {
   int64_t x_blocks;           /* ceil(n / conv_block) */
   int64_t ir_partitions;      /* ceil(leff / conv_block) */
   int64_t chunk_items;        /* items processed per pass */
-  int64_t f_floats, xspec_c64, irspec_c64, wet_floats;      /* sizes of the buffers kept for the backward */
+  int64_t f_floats, xspec_c64, irspec_c64;  /* sizes of the buffers kept for the backward */
   int64_t fwd_workspace_bytes, bwd_workspace_bytes;
 } dasp_reverb_geom;
 int dasp_reverb_geometry(int64_t bs, int64_t n, int64_t num_samples, int64_t taps, int64_t chunk_items,
                          dasp_reverb_geom* out);
 int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const float* noise, const uint64_t* seed_dev,
-                    float* y, float* wet_save, float* f_save, void* xspec_save, void* irspec_save,
+                    float* y, float* f_save, void* xspec_save, void* irspec_save,
                     void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t num_samples,
                     int64_t taps, int64_t chunk_items, float sample_rate, void* stream);
 int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float* params,
-                    const float* wet_save, const float* f_save, const void* xspec_save,
+                    const float* f_save, const void* xspec_save,
                     const void* irspec_save, float* gx, float* gparams, void* workspace,
                     int64_t workspace_bytes, int64_t bs, int64_t n, int64_t num_samples, int64_t taps,
                     int64_t chunk_items, int64_t device_noise /* 1 iff the forward ran with noise == NULL */,

@@ -2,11 +2,13 @@
 
 Drop-in surface: the same names the reference package exports (``dasp_pytorch/__init__.py``) for the hot
 path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_shaped_reverberation`` and the
-``Processor`` classes, ``stereo_bus``, ``stereo_panner``, ``stereo_widener`` -- plus ``expander`` (stubbed upstream).
+``Processor`` classes, ``stereo_bus``, ``stereo_panner``, ``stereo_widener`` -- plus ``expander`` (stubbed upstream)
+and ``convolution_reverberation`` (the reverb's convolution with a caller-supplied impulse response).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
     compressor,
+    convolution_reverberation,
     distortion,
     expander,
     gain,

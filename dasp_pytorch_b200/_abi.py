@@ -31,6 +31,14 @@ class ReverbGeom(ctypes.Structure):
         "nb", "hop", "nbk", "leff", "rpp", "conv_block", "x_blocks", "ir_partitions", "chunk_items",
         "f_floats", "xspec_c64", "irspec_c64", "fwd_workspace_bytes", "bwd_workspace_bytes")]
 
+class ConvGeom(ctypes.Structure):
+    """mirror of ``dasp_conv_geom`` (include/dasp_b200.h)"""
+
+    _fields_ = [(name, c_int64) for name in (
+        "leff", "conv_block", "x_blocks", "ir_partitions", "chunk_items", "xspec_c64", "irspec_c64",
+        "fwd_workspace_bytes", "bwd_workspace_bytes")]
+
+
 P = c_void_p       # device pointer
 I64 = c_int64
 
@@ -67,6 +75,10 @@ _SIGNATURES = {
     "dasp_reverb_fwd": (c_int, [P, I64, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, c_float, P]),
     "dasp_reverb_bwd": (c_int, [P, P, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_reverb_filterbank": (c_int, [I64, c_double, ctypes.POINTER(c_float)]),
+    "dasp_conv_geometry": (c_int, [I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
+    "dasp_conv_fwd": (c_int, [P, I64, P, I64, I64, P, P, P, P, P, I64, I64, I64, I64, P]),
+    "dasp_conv_bwd": (c_int, [P, P, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, P]),
+    "dasp_debug_conv_last_path": (c_int, [c_int]),
     "dasp_dynamics_tile_len": (I64, [I64, I64]),
     "dasp_dynamics_fwd": (c_int, [c_int, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),
     "dasp_dynamics_bwd": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),

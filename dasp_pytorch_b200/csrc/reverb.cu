@@ -717,8 +717,8 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __res
 // samples [i kB, (i+1) kB) as the second half of the transform; y = x + mix (wet - x).
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddles, const float* __restrict__ x,
-                const float* __restrict__ params, float* __restrict__ y, int64_t item0, int I, int64_t n, int in_chs,
-                int nblocks) {
+                const float* __restrict__ mix_p, int mix_stride, float* __restrict__ y, int64_t item0, int I, int64_t n,
+                int in_chs, int nblocks) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
   const int t = threadIdx.x;
@@ -742,7 +742,7 @@ ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddle
     float xr[16], xi[16];
     const int64_t il = m / I, b = item0 + il;
     const int i = m - (int)il * I;
-    const float mix = params[b * 25 + 24];
+    const float mix = mix_p[b * mix_stride];
     const float* xl = x + (b * in_chs) * n;
     const float* xrr = in_chs == 1 ? xl : xl + n;
     float a0[8], a1[8];                            // the dry samples of this thread's 8 outputs
@@ -830,7 +830,7 @@ g_fft_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, const float*
 // mix_part[il*I + q] = sum over block q and both channels of x (c - g)  (mono: x counted once per channel)
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles, const float* __restrict__ gy,
-               const float* __restrict__ x, const float* __restrict__ params, float* __restrict__ gx,
+               const float* __restrict__ x, const float* __restrict__ mix_p, int mix_stride, float* __restrict__ gx,
                float* __restrict__ mix_part, int64_t item0, int items, int I, int64_t n, int in_chs) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
@@ -860,7 +860,7 @@ ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles
     float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
     const int64_t il = blockIdx.x + (int64_t)(it / I) * gridDim.x, b = item0 + il;
     const int i = it % I;
-    const float mix = params[b * 25 + 24];
+    const float mix = mix_p[b * mix_stride];
     const float* g0p = gy + (b * 2) * n;
     const float* xl = x + (b * in_chs) * n;
     const float* xrr = in_chs == 1 ? xl : xl + n;
@@ -1359,11 +1359,11 @@ __global__ void __launch_bounds__(128) partition_mac_bwd_kernel(const float2* __
 
 // y = (1-mix) x + mix wet; wet[n] = Yt[(il*I + n/kB)*kNbA + kB + n%kB]
 __global__ void mix_blocks_kernel(const float* __restrict__ x, const float2* __restrict__ Yt,
-                                  const float* __restrict__ params, float* __restrict__ y, int64_t item0, int I,
-                                  int64_t n, int in_chs) {
+                                  const float* __restrict__ mix_p, int mix_stride, float* __restrict__ y, int64_t item0,
+                                  int I, int64_t n, int in_chs) {
   const int i = blockIdx.x;
   const int64_t il = blockIdx.y, b = item0 + il;
-  const float mix = params[b * 25 + 24];
+  const float mix = mix_p[b * mix_stride];
   const float* xl = x + (b * in_chs) * n;
   const float* xr = in_chs == 1 ? xl : xl + n;
   const float2* yt = Yt + (il * I + i) * (int64_t)kNbA + kB;
@@ -1395,12 +1395,12 @@ __global__ void g_blocks_kernel(const float* __restrict__ gy, float2* __restrict
 // two windows); mono input receives the sum of both channel gradients.
 // mix_part[il*I + i] = sum over block i and both channels of x (c - g)  (see g_fft_kernel)
 __global__ void finish_dx_blocks_kernel(const float* __restrict__ gy, const float* __restrict__ x,
-                                        const float2* __restrict__ Dt, const float* __restrict__ params,
+                                        const float2* __restrict__ Dt, const float* __restrict__ mix_p, int mix_stride,
                                         float* __restrict__ gx, float* __restrict__ mix_part, int64_t item0, int I,
                                         int64_t n, int in_chs) {
   const int i = blockIdx.x;
   const int64_t il = blockIdx.y, b = item0 + il;
-  const float mix = params[b * 25 + 24];
+  const float mix = mix_p[b * mix_stride];
   const float* xl = x + (b * in_chs) * n;
   const float* xr = in_chs == 1 ? xl : xl + n;
   const float2* d0 = Dt + (il * I + i) * (int64_t)kNbA + kB;
@@ -1495,6 +1495,95 @@ __global__ void reverb_param_grad_kernel(const float* __restrict__ ir_part, cons
     for (int i = 0; i < mix_blocks; ++i) s += (double)mix_part[bl * mix_blocks + i];
   }
   gparams[(item0 + bl) * 25 + q] = (float)s;
+}
+
+// ---- convolution_reverberation: the audio convolution above with an impulse response supplied by the caller ----------
+// Forward: ir_pack_kernel puts the caller's taps where the IR synthesis puts its own; x_fft_kernel, partition_mac_kernel
+// and ifft_mix_kernel (or the cuFFT pipeline) then run unchanged.  Backward: g_fft_kernel, the correlations and
+// ifft_dx_kernel as in the reverb; dL/dIR partition j = mix * first half of IFFT(sum_p G[j+p] conj(X[p])), unpacked into
+// the caller's rows by ifft_irtaps_kernel (or irtaps_unpack_kernel after the cuFFT inverse).
+
+// taps t < leff of the planar (bs, ir_chs, L) rows -> (left, right) pairs in the first half of partition slot t / kB
+// (a mono IR feeds both channels).  grid = (ceil(leff / 256), items)
+__global__ void ir_pack_kernel(const float* __restrict__ ir, float2* __restrict__ Hb, int64_t item0, int J, int64_t L,
+                               int64_t leff, int ir_chs) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t il = blockIdx.y;
+  if (t >= leff) return;
+  const float* rl = ir + ((item0 + il) * ir_chs) * L;
+  const float* rr = ir_chs == 1 ? rl : rl + L;
+  Hb[(il * J + t / kB) * (int64_t)kNbA + t % kB] = make_float2(rl[t], rr[t]);
+}
+
+// unit m = il*J + j: dL/dIR taps [j kB, (j+1) kB) ∩ [0, leff) = mix * first half of IFFT(Epl[m]) (left, right), written
+// straight into the caller's (bs, ir_chs, L) rows; a mono IR receives the sum of both channels
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twiddles, const float* __restrict__ mix,
+                   float* __restrict__ gir, int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  auto fetch = [&](int it, int m) {
+    if (t != 0 || m >= nunits) return;
+    uint64_t* bar = &s.full[it & 1];
+    float* dst = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    const float* src = Epl + (int64_t)m * 2 * kNbA;
+    mbar_arrive_expect_tx(bar, 2u * kNbA * 4u);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
+  };
+  fetch(0, blockIdx.x);
+  fetch(1, blockIdx.x + gridDim.x);
+  int it = 0;
+  for (int m = blockIdx.x; m < nunits; m += gridDim.x, ++it) {
+    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
+    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    const int64_t il = m / J, b = item0 + il;
+    const int j = m - (int)il * J;
+    float xr[16], xi[16];
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
+    const float mx = mix[b];
+    float* row = gir + (b * ir_chs) * L;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int64_t tau = (int64_t)j * kB + t + 512 * q;
+      if (tau < leff) {
+        if (ir_chs == 1) row[tau] = mx * (xr[q] + xi[q]);
+        else { row[tau] = mx * xr[q]; row[L + tau] = mx * xi[q]; }
+      }
+    }
+  }
+}
+
+// dL/dIR taps [t0, L) of the caller's rows: mix * Et (inverse-transformed partitions, pairs in the first half of each
+// slot) below leff, 0 from leff on (those taps cannot reach an output).  t0 = leff writes only the zeros.
+// grid = (ceil((L - t0) / 256), items)
+__global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float* __restrict__ mix, float* __restrict__ gir,
+                                     int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int64_t t0) {
+  const int64_t t = t0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t il = blockIdx.y, b = item0 + il;
+  if (t >= L) return;
+  float2 v = make_float2(0.f, 0.f);
+  float mx = 0.f;
+  if (t < leff) {
+    v = Et[(il * J + t / kB) * (int64_t)kNbA + t % kB];
+    mx = mix[b];
+  }
+  float* row = gir + (b * ir_chs) * L;
+  if (ir_chs == 1) row[t] = mx * (v.x + v.y);
+  else { row[t] = mx * v.x; row[L + t] = mx * v.y; }
+}
+
+// dL/dmix per item: the per-block partials of ifft_dx_kernel / finish_dx_blocks_kernel summed in block order, in fp64
+__global__ void conv_mix_grad_kernel(const float* __restrict__ mix_part, float* __restrict__ gmix, int64_t item0,
+                                     int64_t items, int I) {
+  const int64_t il = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (il >= items) return;
+  double s = 0.0;
+  for (int i = 0; i < I; ++i) s += (double)mix_part[il * I + i];
+  gmix[item0 + il] = (float)s;
 }
 
 // device-resident band spectra H_k: 12 x nb complex (full spectrum of the real taps), scaled by 1/nb;
@@ -1754,6 +1843,7 @@ int configure_fft_kernels() {
     DASP_CUDA_OK(cudaFuncSetAttribute(g_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irtaps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     configured[dev] = true;
   }
   return DASP_OK;
@@ -1940,8 +2030,8 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       DASP_LAUNCH_OK("x_fft_kernel");
       launch_mac<false, true>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
       DASP_LAUNCH_OK("partition_mac_kernel");
-      ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ys), tw, x, params, y,
-                                                                     item0, I, n, (int)in_chs, nblk);
+      ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ys), tw, x,
+                                                                     params + 24, 25, y, item0, I, n, (int)in_chs, nblk);
       DASP_LAUNCH_OK("ifft_mix_kernel");
       continue;
     }
@@ -1956,7 +2046,8 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     launch_mac<false>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
     DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_ys, (cufftComplex*)ws_ys, CUFFT_INVERSE));
-    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, params, y, item0, I, n, (int)in_chs);
+    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, params + 24, 25, y, item0, I, n,
+                                                                          (int)in_chs);
     DASP_LAUNCH_OK("mix_blocks_kernel");
   }
   return DASP_OK;
@@ -2028,8 +2119,9 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
         DASP_LAUNCH_OK("partition_mac_kernel<corr>");
       }
       const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
-      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, x, params,
-                                                                    gx, ws_mixpart, item0, (int)items, I, n, (int)in_chs);
+      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, x,
+                                                                    params + 24, 25, gx, ws_mixpart, item0, (int)items, I,
+                                                                    n, (int)in_chs);
       DASP_LAUNCH_OK("ifft_dx_kernel");
     } else {
       g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, ws_gs, item0, I, n);
@@ -2040,8 +2132,8 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
       launch_mac<true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);
       DASP_LAUNCH_OK("partition_mac_kernel<corr>");
       DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_ds, (cufftComplex*)ws_ds, CUFFT_INVERSE));
-      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ws_ds, params, gx, ws_mixpart, item0,
-                                                                                I, n, (int)in_chs);
+      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ws_ds, params + 24, 25, gx,
+                                                                                ws_mixpart, item0, I, n, (int)in_chs);
       DASP_LAUNCH_OK("finish_dx_blocks_kernel");
     }
     int nparts;
@@ -2077,6 +2169,261 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
     reverb_param_grad_kernel<<<(unsigned)((items * 25 + 127) / 128), 128, 0, st>>>(ws_irpart, ws_mixpart, params, gparams,
                                                                                    item0, items, nparts, I);
     DASP_LAUNCH_OK("reverb_param_grad_kernel");
+  }
+  return DASP_OK;
+}
+
+// ------------------------------------------------------------------ convolution_reverberation
+namespace {
+int g_conv_last_path[2] = {0, 0};                    // test hook: dispatch of the last dasp_conv_fwd / dasp_conv_bwd
+
+struct ConvGeom { int64_t bs, n, L, leff, ib, jb, chunk; };
+int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
+  DASP_REQUIRE(bs >= 0 && n >= 1 && L >= 1, "conv: bad shape bs=%lld n=%lld ir_len=%lld", (long long)bs, (long long)n,
+               (long long)L);
+  g.bs = bs; g.n = n; g.L = L;
+  g.leff = L < n ? L : n;
+  g.ib = (n + kB - 1) / kB;
+  g.jb = (g.leff + kB - 1) / kB;
+  if (chunk <= 0) chunk = 4;
+  g.chunk = chunk < bs ? chunk : (bs > 0 ? bs : 1);
+  return DASP_OK;
+}
+// the cuFFT pipeline's two block transforms (audio windows / dL/dx windows, IR partitions / dL/dIR partitions) for a full
+// chunk and for the remainder
+struct ConvPlans { PlanVal xi, hj; };
+int conv_plans(const ConvGeom& g, ConvPlans& full, ConvPlans& rem, size_t& work) {
+  int rc;
+  work = 0;
+  for (int64_t items : {g.chunk, g.bs % g.chunk}) {
+    if (items == 0) continue;
+    ConvPlans& p = items == g.chunk ? full : rem;
+    if ((rc = get_plan(2, kNbA, items * g.ib, kNbA, kNbA, p.xi)) != DASP_OK) return rc;
+    if ((rc = get_plan(2, kNbA, items * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
+    if (p.xi.work > work) work = p.xi.work;
+    if (p.hj.work > work) work = p.hj.work;
+  }
+  return DASP_OK;
+}
+struct ConvFwdWs { size_t ys, xsp, hsp, cufft, total; };
+struct ConvBwdWs { size_t gs, ds, es, mixpart, cufft, total; };
+void conv_fwd_layout(const ConvGeom& g, size_t cufft_work, ConvFwdWs& w) {
+  size_t o = 0;
+  w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));      // spectra not kept for a backward
+  w.hsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
+  w.cufft = o; o += align256(cufft_work);
+  w.total = o;
+}
+void conv_bwd_layout(const ConvGeom& g, size_t cufft_work, ConvBwdWs& w) {
+  size_t o = 0;
+  w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
+  w.mixpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * g.ib));
+  w.cufft = o; o += align256(cufft_work);
+  w.total = o;
+}
+}  // namespace
+
+int dasp_debug_conv_last_path(int which) { return g_conv_last_path[which ? 1 : 0]; }
+
+int dasp_conv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "conv geometry: null out");
+  ConvGeom g;
+  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  std::lock_guard<std::mutex> lk(g_mu);
+  size_t work = 0;
+  if (bs > 0) {
+    ConvPlans p{}, q{};
+    if ((rc = conv_plans(g, p, q, work)) != DASP_OK) return rc;
+  }
+  ConvFwdWs fw; ConvBwdWs bw;
+  conv_fwd_layout(g, work, fw);
+  conv_bwd_layout(g, work, bw);
+  out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
+  out->xspec_c64 = bs * g.ib * kNbA;
+  out->irspec_c64 = bs * g.jb * kNbA;
+  out->fwd_workspace_bytes = (int64_t)fw.total;
+  out->bwd_workspace_bytes = (int64_t)bw.total;
+  return DASP_OK;
+}
+
+int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, const float* mix,
+                  float* y, void* xspec_save, void* irspec_save, void* workspace, int64_t workspace_bytes, int64_t bs,
+                  int64_t n, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2), "conv: only mono/stereo signals and IRs");
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(x && ir && mix && y && workspace, "conv fwd: null pointer");
+  DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "conv fwd: pass both *_save buffers or neither");
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  ConvPlans pfull{}, prem{};
+  size_t work = 0;
+  if ((rc = conv_plans(g, pfull, prem, work)) != DASP_OK) return rc;
+  ConvFwdWs w;
+  conv_fwd_layout(g, work, w);
+  if ((int64_t)w.total > workspace_bytes) {
+    set_error("conv fwd: workspace needs %lld bytes, got %lld", (long long)w.total, (long long)workspace_bytes);
+    return DASP_ERR_WORKSPACE;
+  }
+  unsigned char* base = (unsigned char*)workspace;
+  float2* ws_ys = (float2*)(base + w.ys);
+  void* ws_cufft = base + w.cufft;
+  const int I = (int)g.ib, J = (int)g.jb;
+  const float* tw = nullptr;
+
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    const ConvPlans& pl = (items == g.chunk) ? pfull : prem;
+    float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
+    float2* hs = irspec_save ? (float2*)irspec_save + item0 * J * (int64_t)kNbA : (float2*)(base + w.hsp);
+    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(x) && aligned16(hs);
+    g_conv_last_path[0] = own_conv ? 1 : 0;
+    // the cuFFT transform of the partitions reads whole slots; x_fft_kernel only the taps ir_pack_kernel writes
+    if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
+    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(ir, hs, item0, J, g.L, g.leff,
+                                                                                          (int)ir_chs);
+    DASP_LAUNCH_OK("ir_pack_kernel");
+    const int nblk = (int)(items * I);
+    if (own_conv) {
+      if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
+      const int nunits = (int)(items * (I + J));
+      const unsigned xh_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
+      x_fft_kernel<<<xh_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, n, g.leff, (int)in_chs, nblk,
+                                                                  nunits);
+      DASP_LAUNCH_OK("x_fft_kernel");
+      launch_mac<false, true>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
+      DASP_LAUNCH_OK("partition_mac_kernel");
+      const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
+      ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ys), tw, x, mix, 1,
+                                                                     y, item0, I, n, (int)in_chs, nblk);
+      DASP_LAUNCH_OK("ifft_mix_kernel");
+      continue;
+    }
+    DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
+    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, ws_cufft));
+    DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
+    x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, n, (int)in_chs);
+    DASP_LAUNCH_OK("x_blocks_kernel");
+    DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
+    DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, ws_cufft));
+    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)xs, (cufftComplex*)xs, CUFFT_FORWARD));
+    launch_mac<false>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
+    DASP_LAUNCH_OK("partition_mac_kernel");
+    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ws_ys, (cufftComplex*)ws_ys, CUFFT_INVERSE));
+    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, mix, 1, y, item0, I, n, (int)in_chs);
+    DASP_LAUNCH_OK("mix_blocks_kernel");
+  }
+  return DASP_OK;
+}
+
+int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, const float* mix,
+                  const void* xspec_save, const void* irspec_save, float* gx, float* gir, float* gmix, void* workspace,
+                  int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2), "conv: only mono/stereo signals and IRs");
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(gy && x && mix && xspec_save && irspec_save && gx && gmix && workspace, "conv bwd: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  ConvPlans pfull{}, prem{};
+  size_t work = 0;
+  if ((rc = conv_plans(g, pfull, prem, work)) != DASP_OK) return rc;
+  ConvBwdWs w;
+  conv_bwd_layout(g, work, w);
+  if ((int64_t)w.total > workspace_bytes) {
+    set_error("conv bwd: workspace needs %lld bytes, got %lld", (long long)w.total, (long long)workspace_bytes);
+    return DASP_ERR_WORKSPACE;
+  }
+  unsigned char* base = (unsigned char*)workspace;
+  float2* ws_gs = (float2*)(base + w.gs);
+  float2* ws_ds = (float2*)(base + w.ds);
+  float2* ws_es = (float2*)(base + w.es);
+  float* ws_mixpart = (float*)(base + w.mixpart);
+  void* ws_cufft = base + w.cufft;
+  const float inv = 1.0f / (float)kNbA;
+  const int I = (int)g.ib, J = (int)g.jb;
+  const int mb = I > J ? I : J;
+
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    const ConvPlans& pl = (items == g.chunk) ? pfull : prem;
+    const float2* xs = (const float2*)xspec_save + item0 * I * (int64_t)kNbA;
+    const float2* hs = (const float2*)irspec_save + item0 * J * (int64_t)kNbA;
+    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(gy);
+    const bool fused_mac = own_conv && gir != nullptr && mb <= 16;
+    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed
+    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_mac ? 2 : 0) | (gir ? 4 : 0);
+    const int nblk = (int)(items * I);
+    const dim3 tail_grid((unsigned)((g.L - g.leff + 255) / 256), (unsigned)items);
+    if (own_conv) {
+      const float* tw = nullptr;
+      if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
+      const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
+      g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, ws_gs, tw, item0, I, n, nblk);
+      DASP_LAUNCH_OK("g_fft_kernel");
+      if (fused_mac) {
+        dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+        if (mb <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(ws_gs, hs, xs, ws_ds, ws_es, I, J, inv);
+        else          partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(ws_gs, hs, xs, ws_ds, ws_es, I, J, inv);
+        DASP_LAUNCH_OK("partition_mac_bwd_kernel");
+      } else {
+        launch_mac<true, true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
+        DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+        if (gir) {
+          launch_mac<true, true>(ws_gs, xs, ws_es, I, I, J, items, inv, st);    // dIR partitions: sum_p conj(X[p]) G[j+p]
+          DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+        }
+      }
+      const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
+      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, x, mix, 1,
+                                                                    gx, ws_mixpart, item0, (int)items, I, n, (int)in_chs);
+      DASP_LAUNCH_OK("ifft_dx_kernel");
+      if (gir) {
+        const int nunits = (int)(items * J);
+        const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
+        ifft_irtaps_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mix,
+                                                                          gir, item0, J, g.L, g.leff, (int)ir_chs, nunits);
+        DASP_LAUNCH_OK("ifft_irtaps_kernel");
+        if (g.L > g.leff) {
+          irtaps_unpack_kernel<<<tail_grid, 256, 0, st>>>(ws_es, mix, gir, item0, J, g.L, g.leff, (int)ir_chs, g.leff);
+          DASP_LAUNCH_OK("irtaps_unpack_kernel");
+        }
+      }
+    } else {
+      g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, ws_gs, item0, I, n);
+      DASP_LAUNCH_OK("g_blocks_kernel");
+      DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
+      DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, ws_cufft));
+      DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ws_gs, (cufftComplex*)ws_gs, CUFFT_FORWARD));
+      launch_mac<true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);
+      DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+      DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ws_ds, (cufftComplex*)ws_ds, CUFFT_INVERSE));
+      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ws_ds, mix, 1, gx, ws_mixpart, item0,
+                                                                                I, n, (int)in_chs);
+      DASP_LAUNCH_OK("finish_dx_blocks_kernel");
+      if (gir) {
+        launch_mac<true>(ws_gs, xs, ws_es, I, I, J, items, inv, st);
+        DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+        DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
+        DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, ws_cufft));
+        DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)ws_es, (cufftComplex*)ws_es, CUFFT_INVERSE));
+        irtaps_unpack_kernel<<<dim3((unsigned)((g.L + 255) / 256), (unsigned)items), 256, 0, st>>>(
+            ws_es, mix, gir, item0, J, g.L, g.leff, (int)ir_chs, 0);
+        DASP_LAUNCH_OK("irtaps_unpack_kernel");
+      }
+    }
+    conv_mix_grad_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(ws_mixpart, gmix, item0, items, I);
+    DASP_LAUNCH_OK("conv_mix_grad_kernel");
   }
   return DASP_OK;
 }

@@ -31,6 +31,7 @@ __all__ = [
     "compressor",
     "expander",
     "noise_shaped_reverberation",
+    "convolution_reverberation",
 ]
 
 
@@ -689,4 +690,98 @@ def noise_shaped_reverberation_packed(x: torch.Tensor, sample_rate: float, param
     noise, seed = _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps)
     y = _ReverbFn.apply(xf, packed, noise, seed, sample_rate, int(num_samples), int(num_bandpass_taps),
                         reverb_chunk_items(xf.device))
+    return y.to(dt)
+
+
+# --------------------------------------------------------------------------------------
+# convolution reverberation (caller-supplied impulse response)
+# --------------------------------------------------------------------------------------
+
+
+class _ConvReverbFn(torch.autograd.Function):
+    """x (bs, 1|2, n), ir (bs, 1|2, L), mix (bs,) -> y (bs, 2, n)."""
+
+    @staticmethod
+    def forward(ctx, x, ir, mix, chunk):
+        lib = _abi.lib()
+        bs, in_chs, n = x.shape
+        _, ir_chs, ir_len = ir.shape
+        dev = x.device
+        y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
+        need_bwd = any(ctx.needs_input_grad[:3])
+        geom = _abi.ConvGeom()
+        with torch.cuda.device(dev):
+            check(lib.dasp_conv_geometry(bs, n, ir_len, chunk, geom), "dasp_conv_geometry")
+            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
+            xspec = irspec = None
+            if need_bwd:
+                xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
+                irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
+            with _timed("conv_fwd", dev):
+                check(lib.dasp_conv_fwd(ptr(x), in_chs, ptr(ir), ir_chs, ir_len, ptr(mix), ptr(y), ptr(xspec),
+                                        ptr(irspec), ptr(ws), ws.numel(), bs, n, chunk, stream_ptr(dev)),
+                      "dasp_conv_fwd")
+        if need_bwd:
+            ctx.save_for_backward(x, xspec, irspec, mix)
+        ctx.cfg = (ir_chs, ir_len, chunk, geom.bwd_workspace_bytes)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _abi.lib()
+        x, xspec, irspec, mix = ctx.saved_tensors
+        ir_chs, ir_len, chunk, bwd_bytes = ctx.cfg
+        bs, in_chs, n = x.shape
+        dev = x.device
+        gy = gy.contiguous()
+        gx = torch.empty_like(x)
+        # a fixed IR (data augmentation with measured rooms) skips every dL/dIR kernel
+        gir = torch.empty(bs, ir_chs, ir_len, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        gmix = torch.empty_like(mix)
+        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev), _timed("conv_bwd", dev):
+            check(lib.dasp_conv_bwd(ptr(gy), ptr(x), in_chs, ir_chs, ir_len, ptr(mix), ptr(xspec), ptr(irspec),
+                                    ptr(gx), ptr(gir), ptr(gmix), ptr(ws), ws.numel(), bs, n, chunk, stream_ptr(dev)),
+                  "dasp_conv_bwd")
+        return gx, gir, gmix, None
+
+
+def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor, mix: torch.Tensor):
+    """Convolution reverb with a caller-supplied impulse response: the apply stage of the reference's
+    ``noise_shaped_reverberation`` (``functional.py:569-575``) with the IR given instead of synthesised::
+
+        x_pad = pad(x, (L-1, 0)); wet = vmap(conv1d(groups=2))(x_pad, flip(IR)); y = (1-mix) x + mix wet
+
+    Args:
+        x: audio ``(bs, 1|2, n)``; mono is used for both channels.
+        sample_rate: unused (kept for the common processor signature).
+        impulse_response: ``(bs, 1|2, L)``, any ``L >= 1``; a mono IR is used for both channels.  One IR shared by the
+            whole batch is passed as ``ir.expand(bs, -1, -1)``, which costs one copy.
+        mix: ``bs`` elements in any shape, or one element that is broadcast over the batch.
+
+    Returns ``(bs, 2, n)`` in x's dtype (computed in fp32), like ``noise_shaped_reverberation``, so the two can replace
+    each other in a chain.  Gradients flow to ``x``, ``impulse_response`` (a mono IR receives the sum of both channel
+    gradients; taps at or beyond ``n`` reach no output and get exactly 0) and ``mix``.  When the IR does not require a
+    gradient, the backward skips all dL/dIR work.  The convolution is the reverb's own: uniformly partitioned
+    overlap-save on 4096-sample partitions with the in-shared-memory 8192-point FFT.
+    """
+    for t, name in ((x, "x"), (impulse_response, "impulse_response")):
+        if not torch.is_tensor(t) or t.dim() != 3:
+            raise ValueError(f"{name} must be a tensor of shape (batch, channels, samples)")
+        if t.shape[1] not in (1, 2):
+            raise ValueError(f"{name}: only mono/stereo is supported, got {t.shape[1]} channels")
+    bs = x.shape[0]
+    if impulse_response.shape[0] != bs:
+        raise ValueError(f"impulse_response has batch {impulse_response.shape[0]}, x has batch {bs}")
+    if impulse_response.shape[2] < 1:
+        raise ValueError("impulse_response needs at least one tap")
+    nmix = mix.numel() if torch.is_tensor(mix) else torch.as_tensor(mix).numel()
+    if nmix not in (1, bs):
+        raise ValueError(f"mix: expected {bs} element(s) (one per batch item) or 1, got {nmix}")
+    xf, dt = _audio(x)
+    irf, _ = _audio(impulse_response, "impulse_response")
+    if irf.device != xf.device:
+        raise DaspError(f"impulse_response is on {irf.device} but x is on {xf.device}")
+    m = _param(mix, bs, xf, "mix", allow_broadcast=True).contiguous()
+    y = _ConvReverbFn.apply(xf, irf, m, reverb_chunk_items(xf.device))
     return y.to(dt)

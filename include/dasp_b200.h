@@ -180,6 +180,38 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
 /* host-only: the 12 x taps fp32 filter bank (scipy.signal.firwin restated; no GPU needed) */
 int dasp_reverb_filterbank(int64_t taps, double sample_rate, float* out);
 
+/* ---- convolution_reverberation: the reverb's apply stage with a caller-supplied impulse response
+ *      (reference functional.py:569-575: y = (1 - mix) x + mix (x * IR), causal, cropped to n) --------------
+ * x is (bs, in_chs, n), ir is (bs, ir_chs, ir_len) with in_chs, ir_chs 1 or 2 (mono is used for both channels),
+ * mix is [bs]; y is always (bs, 2, n).  Any ir_len >= 1; only the first leff = min(ir_len, n) taps reach the output.
+ * The convolution is the reverb's: uniformly partitioned overlap-save on conv_block-sample partitions.
+ * Buffers kept for the backward (pass NULL for both when no backward follows):
+ *   xspec_save  geom.xspec_c64 complex64 (audio block spectra), irspec_save  geom.irspec_c64 complex64 (IR partitions).
+ * Backward: gx is (bs, in_chs, n) (mono receives the sum of both channel gradients), gmix [bs], gir (bs, ir_chs, ir_len)
+ * or NULL, which skips all dL/dIR work; a mono IR receives the sum of both channel gradients and taps >= leff get 0.
+ * workspace: geom.fwd_workspace_bytes / geom.bwd_workspace_bytes bytes of device memory.  A geometry query with
+ * bs = 0 needs no GPU (its workspace sizes then leave out the cuFFT work area). */
+typedef struct dasp_conv_geom {
+  int64_t leff;               /* min(ir_len, n): IR taps that can reach the n output samples */
+  int64_t conv_block;         /* partition / hop length (its FFT length is twice that) */
+  int64_t x_blocks;           /* ceil(n / conv_block) */
+  int64_t ir_partitions;      /* ceil(leff / conv_block) */
+  int64_t chunk_items;        /* items processed per pass */
+  int64_t xspec_c64, irspec_c64;  /* sizes of the buffers kept for the backward */
+  int64_t fwd_workspace_bytes, bwd_workspace_bytes;
+} dasp_conv_geom;
+int dasp_conv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, const float* mix,
+                  float* y, void* xspec_save, void* irspec_save, void* workspace, int64_t workspace_bytes, int64_t bs,
+                  int64_t n, int64_t chunk_items, void* stream);
+int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, const float* mix,
+                  const void* xspec_save, const void* irspec_save, float* gx, float* gir /* may be NULL */, float* gmix,
+                  void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream);
+/* test hook: dispatch of the most recent call.  which = 0: dasp_conv_fwd, 1 = own in-shared-memory FFT, 0 = cuFFT
+   pipeline (dasp_debug_reverb_path(1), n % 4 != 0, rows not 16-byte aligned).  which = 1: dasp_conv_bwd, bit 0 = own
+   FFT, bit 1 = fused correlation kernel, bit 2 = dL/dIR computed */
+int dasp_debug_conv_last_path(int which);
+
 #ifdef __cplusplus
 }
 #endif

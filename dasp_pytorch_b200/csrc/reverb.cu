@@ -27,6 +27,11 @@
 // windows, dL/dIR partitions), ifft_dx_kernel (+ dL/dmix partials), ifft_irgrad_kernel (dL/dIR * env * f reductions for
 // the 24 band parameters; deterministic two-stage sums); the cuFFT variants are g_blocks_kernel, C2C,
 // finish_dx_blocks_kernel, inverse C2C, ir_grad_*_kernel.
+//
+// convolution_reverberation is the audio convolution with the caller's IR (ir_pack_kernel fills the partitions).  The
+// convolution is written once on the host: conv_fwd_chunk / conv_bwd_chunk run a chunk for both ops, on one ConvGeom,
+// one plan set (conv_setup) and one workspace layout per direction; each op adds only its IR fill, its mix stride and
+// its dL/dIR consumer.
 #include <cufft.h>
 #include <curand_kernel.h>
 #include <math.h>
@@ -100,11 +105,30 @@ void octave_filterbank(int taps, double sr, std::vector<float>& out) {
 }
 
 // ------------------------------------------------------------------ geometry
-struct Geom {
-  int64_t bs, n, L, taps, P;
+// the partitioned audio convolution, shared by the reverb and convolution_reverberation
+struct ConvGeom {
+  int64_t bs, n, L;
   int64_t leff;                 // min(L, n): the only IR taps that can reach the output
-  int64_t nb, hop, nbk, chunk;
-  int64_t ib, jb;               // audio convolution: output/input blocks of kB samples, IR partitions of kB taps
+  int64_t ib, jb;               // output/input blocks of kB samples, IR partitions of kB taps
+  int64_t chunk;
+};
+
+int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
+  DASP_REQUIRE(bs >= 0 && n >= 1 && L >= 1, "conv: bad shape bs=%lld n=%lld ir_len=%lld", (long long)bs, (long long)n,
+               (long long)L);
+  g.bs = bs; g.n = n; g.L = L;
+  g.leff = L < n ? L : n;
+  g.ib = (n + kB - 1) / kB;
+  g.jb = (g.leff + kB - 1) / kB;
+  if (chunk <= 0) chunk = 4;
+  g.chunk = chunk < bs ? chunk : (bs > 0 ? bs : 1);
+  return DASP_OK;
+}
+
+// the reverb adds the IR synthesis: band filters of taps = P + 1, overlap-save blocks of nb with hop, or polyphase
+struct Geom : ConvGeom {
+  int64_t taps, P;
+  int64_t nb, hop, nbk;
   int64_t rpp;                  // polyphase factor of the spectral synthesis: n1 = rpp*nb >= leff + P
   int64_t n1() const { return rpp * nb; }
   int64_t n1c() const { return n1() / 2 + 1; }
@@ -117,19 +141,16 @@ int make_geom(int64_t bs, int64_t n, int64_t L, int64_t taps, int64_t chunk, Geo
   DASP_REQUIRE(bs >= 0 && n >= 1 && L >= 2, "reverb: bad shape bs=%lld n=%lld num_samples=%lld", (long long)bs,
                (long long)n, (long long)L);
   DASP_REQUIRE(taps >= 1 && (taps % 2) == 1, "num_bandpass_taps must be odd");
-  g.bs = bs; g.n = n; g.L = L; g.taps = taps; g.P = taps - 1;
+  int rc = make_conv_geom(bs, n, L, chunk, g);
+  if (rc != DASP_OK) return rc;
+  g.taps = taps; g.P = taps - 1;
   const int64_t discard = ((g.P + 3) / 4) * 4;            // >= P, keeps every block 16-byte aligned
   int64_t nb = 8192;
   while (nb < 4 * (discard + 1)) nb *= 2;
   g.nb = nb;
   g.hop = nb - discard;
-  g.leff = L < n ? L : n;
   g.nbk = (g.leff + g.hop - 1) / g.hop;
   g.rpp = (g.leff + g.P + nb - 1) / nb;
-  g.ib = (n + kB - 1) / kB;
-  g.jb = (g.leff + kB - 1) / kB;
-  if (chunk <= 0) chunk = 4;
-  g.chunk = chunk < bs ? chunk : (bs > 0 ? bs : 1);
   return DASP_OK;
 }
 
@@ -1777,47 +1798,89 @@ bool dispatch_fused(int R, const float2* H1, const float* tw, const float* param
   }
 }
 
-struct Plans { PlanVal blk_c2c, pp_c2c, xi_c2c, hj_c2c; size_t work; };
-int get_plans(const Geom& g, int64_t items, Plans& p) {
-  int rc;
-  if ((rc = get_plan(2, g.nb, items * kBands * g.nbk, g.nb, g.nb, p.blk_c2c)) != DASP_OK) return rc;
-  if ((rc = get_plan(2, g.nb, items * kBands * g.rpp, g.nb, g.nb, p.pp_c2c)) != DASP_OK) return rc;
-  if ((rc = get_plan(2, kNbA, items * g.ib, kNbA, kNbA, p.xi_c2c)) != DASP_OK) return rc;
-  if ((rc = get_plan(2, kNbA, items * g.jb, kNbA, kNbA, p.hj_c2c)) != DASP_OK) return rc;
-  p.work = p.blk_c2c.work;
-  if (p.pp_c2c.work > p.work) p.work = p.pp_c2c.work;
-  if (p.xi_c2c.work > p.work) p.work = p.xi_c2c.work;
-  if (p.hj_c2c.work > p.work) p.work = p.hj_c2c.work;
-  return DASP_OK;
-}
-
 inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
-// workspace carve-up shared by the geometry query and the two entry points
-struct FwdWs { size_t ys, xsp, hsp, fchunk, cufft, total; };
-struct BwdWs { size_t gs, ds, es, irpart, mixpart, cufft, total; };
+// workspace carve-up shared by the geometry queries and the entry points; extra: the reverb's own region (the filtered
+// noise of a chunk when f_save is not kept / the per-partition partials of the 24 band-parameter gradients)
+struct FwdWs { size_t ys, xsp, hsp, extra, cufft, total; };
+struct BwdWs { size_t gs, ds, es, extra, mixpart, cufft, total; };
 
-void fwd_layout(const Geom& g, size_t cufft_work, FwdWs& w) {
+void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs& w) {
   size_t o = 0;
   w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   // transient homes for what a forward WITHOUT a backward does not keep (null *_save pointers)
   w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   w.hsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
-  w.fchunk = o; o += align256(sizeof(float2) * (size_t)(g.chunk * kBands * g.pair_c64()));
+  w.extra = o; o += align256(extra_bytes);
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
 }
-void bwd_layout(const Geom& g, size_t cufft_work, BwdWs& w) {
+void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs& w) {
   size_t o = 0;
   w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
-  int64_t nparts = g.nbk > g.nparts_pp() ? g.nbk : g.nparts_pp();
-  if (g.jb > nparts) nparts = g.jb;
-  w.irpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * nparts * kBands * 2));
+  w.extra = o; o += align256(extra_bytes);
   w.mixpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * g.ib));
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
+}
+
+// cuFFT plans for a full chunk and for the remainder (none without a batch), and both workspace layouts around their
+// largest work area.  xi / hj: the block transforms of the convolution's cuFFT pipeline (audio / dL/dx windows, IR /
+// dL/dIR partitions).  With synth (the reverb) also blk / pp, its IR synthesis (overlap-save blocks, polyphase), and
+// the extra regions.
+struct Plans { PlanVal xi, hj, blk, pp; };
+struct Setup { Plans full, rem; FwdWs fwd; BwdWs bwd; };
+int conv_setup(const ConvGeom& g, const Geom* synth, Setup& s) {
+  int rc;
+  size_t work = 0;
+  for (int64_t items : {g.bs > 0 ? g.chunk : 0, g.bs % g.chunk}) {
+    if (items == 0) continue;
+    Plans& p = items == g.chunk ? s.full : s.rem;
+    if ((rc = get_plan(2, kNbA, items * g.ib, kNbA, kNbA, p.xi)) != DASP_OK) return rc;
+    if ((rc = get_plan(2, kNbA, items * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
+    if (p.xi.work > work) work = p.xi.work;
+    if (p.hj.work > work) work = p.hj.work;
+    if (synth) {
+      if ((rc = get_plan(2, synth->nb, items * kBands * synth->nbk, synth->nb, synth->nb, p.blk)) != DASP_OK) return rc;
+      if ((rc = get_plan(2, synth->nb, items * kBands * synth->rpp, synth->nb, synth->nb, p.pp)) != DASP_OK) return rc;
+      if (p.blk.work > work) work = p.blk.work;
+      if (p.pp.work > work) work = p.pp.work;
+    }
+  }
+  size_t fwd_extra = 0, bwd_extra = 0;
+  if (synth) {
+    fwd_extra = sizeof(float2) * (size_t)(g.chunk * kBands * synth->pair_c64());
+    int64_t nparts = synth->nbk > synth->nparts_pp() ? synth->nbk : synth->nparts_pp();
+    if (g.jb > nparts) nparts = g.jb;
+    bwd_extra = sizeof(float) * (size_t)(g.chunk * nparts * kBands * 2);
+  }
+  fwd_layout(g, fwd_extra, work, s.fwd);
+  bwd_layout(g, bwd_extra, work, s.bwd);
+  return DASP_OK;
+}
+int check_workspace(const char* what, size_t need, int64_t have) {
+  if ((int64_t)need > have) {
+    set_error("%s: workspace needs %lld bytes, got %lld", what, (long long)need, (long long)have);
+    return DASP_ERR_WORKSPACE;
+  }
+  return DASP_OK;
+}
+
+// the fields dasp_reverb_geom and dasp_conv_geom share
+template <class Out>
+int put_conv_geometry(const ConvGeom& g, const Geom* synth, Out* out) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  Setup s{};
+  int rc = conv_setup(g, synth, s);
+  if (rc != DASP_OK) return rc;
+  out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
+  out->xspec_c64 = g.bs * g.ib * kNbA;
+  out->irspec_c64 = g.bs * g.jb * kNbA;
+  out->fwd_workspace_bytes = (int64_t)s.fwd.total;
+  out->bwd_workspace_bytes = (int64_t)s.bwd.total;
+  return DASP_OK;
 }
 
 // out = conv / corr of packed block spectra, register-cached when both operands have <= 16 blocks
@@ -1845,6 +1908,130 @@ int configure_fft_kernels() {
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irtaps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     configured[dev] = true;
+  }
+  return DASP_OK;
+}
+
+// ---- the audio convolution of one chunk, forward and backward, for both ops ----
+// The own in-shared-memory FFT runs the block transforms (fused with their neighbours) when the rows allow bulk copies:
+// n % 4 == 0 and 16-byte aligned rows (b may be null).  dasp_debug_reverb_path(1) pins the cuFFT pipeline (the tests
+// compare the two).
+bool own_fft_rows(int64_t n, const void* a, const void* b) {
+  return debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(a) && (b == nullptr || aligned16(b));
+}
+
+// what the backward leaves in the es region for the caller's dL/dIR consumer
+enum class IrGrad {
+  kNone,     // nothing (a fixed impulse response)
+  kPlanar,   // partition spectra, planar, for an own-FFT inverse (own path only)
+  kTime,     // partitions after the inverse cuFFT C2C: (left, right) pairs in the first half of each slot
+};
+// both correlations in one pass over the gradient spectra when the operands fit the register cache
+bool fused_corr(IrGrad e, int I, int J) { return e == IrGrad::kPlanar && (I > J ? I : J) <= 16; }
+
+// y = (1 - mix) x + mix (x * IR), mix of item b at mix[b * mix_stride].  The caller has written IR taps t < leff as
+// (left, right) pairs into the first half of partition slot t / kB of hs, and on the cuFFT pipeline zero-filled the
+// slots first.  xs / hs receive the window / partition spectra.  own (own_fft_rows of x and hs): x_fft_kernel transforms
+// both on the own FFT with the tables tw; otherwise cuFFT C2C does.
+int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, int in_chs, float2* xs,
+                   float2* hs, const float* mix, int mix_stride, float* y, unsigned char* ws, const FwdWs& w,
+                   int64_t item0, int64_t items, cudaStream_t st) {
+  float2* ys = (float2*)(ws + w.ys);
+  const int I = (int)g.ib, J = (int)g.jb;
+  const int nblk = (int)(items * I);
+  if (own) {
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    // one work list: the items*I audio windows, then the items*J IR partitions (transformed in place in hs)
+    const int nunits = (int)(items * (I + J));
+    const unsigned xh_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
+    x_fft_kernel<<<xh_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nblk,
+                                                                nunits);
+    DASP_LAUNCH_OK("x_fft_kernel");
+    launch_mac<false, true>(xs, hs, ys, I, J, I, items, 1.0f / (float)kNbA, st);
+    DASP_LAUNCH_OK("partition_mac_kernel");
+    const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
+    ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
+                                                                   mix_stride, y, item0, I, g.n, in_chs, nblk);
+    DASP_LAUNCH_OK("ifft_mix_kernel");
+    return DASP_OK;
+  }
+  void* cufft = ws + w.cufft;
+  DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
+  DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
+  DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
+  x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, g.n, in_chs);
+  DASP_LAUNCH_OK("x_blocks_kernel");
+  DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
+  DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, cufft));
+  DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)xs, (cufftComplex*)xs, CUFFT_FORWARD));
+  launch_mac<false>(xs, hs, ys, I, J, I, items, 1.0f / (float)kNbA, st);
+  DASP_LAUNCH_OK("partition_mac_kernel");
+  DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ys, (cufftComplex*)ys, CUFFT_INVERSE));
+  mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ys, mix, mix_stride, y, item0, I, g.n, in_chs);
+  DASP_LAUNCH_OK("mix_blocks_kernel");
+  return DASP_OK;
+}
+
+// Backward of conv_fwd_chunk from its saved spectra xs / hs: gx = (1 - mix) g + mix c, c(s) = sum_tau IR(tau) g(s + tau),
+// and per block the dL/dmix partials sum x (c - g) in the mixpart region; then the dL/dIR partitions
+// E[j] = sum_p G[j+p] conj(X[p]) in the es region, in the form e (kPlanar needs own).  own (own_fft_rows of gy): the G
+// transform and ifft_dx_kernel on the own FFT with the tables tw; otherwise the cuFFT pipeline.  Unfused, the dL/dIR
+// correlation runs after the dL/dx inverse (the two correlations read the same inputs and write disjoint regions).
+int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const float* tw, const float* gy,
+                   const float* x, int in_chs, const float2* xs, const float2* hs, const float* mix, int mix_stride,
+                   float* gx, unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) {
+  float2* gs = (float2*)(ws + w.gs);
+  float2* ds = (float2*)(ws + w.ds);
+  float2* es = (float2*)(ws + w.es);
+  float* mixpart = (float*)(ws + w.mixpart);
+  void* cufft = ws + w.cufft;
+  const float inv = 1.0f / (float)kNbA;
+  const int I = (int)g.ib, J = (int)g.jb;
+  const bool fused = fused_corr(e, I, J);
+  if (own) {
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    const int nblk = (int)(items * I);
+    const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
+    g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, I, g.n, nblk);
+    DASP_LAUNCH_OK("g_fft_kernel");
+    if (fused) {
+      dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+      if ((I > J ? I : J) <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(gs, hs, xs, ds, es, I, J, inv);
+      else                       partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(gs, hs, xs, ds, es, I, J, inv);
+      DASP_LAUNCH_OK("partition_mac_bwd_kernel");
+    } else {
+      launch_mac<true, true>(gs, hs, ds, I, J, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
+      DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+    }
+    const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
+    ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gy, x, mix,
+                                                                  mix_stride, gx, mixpart, item0, (int)items, I, g.n,
+                                                                  in_chs);
+    DASP_LAUNCH_OK("ifft_dx_kernel");
+  } else {
+    g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, gs, item0, I, g.n);
+    DASP_LAUNCH_OK("g_blocks_kernel");
+    DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
+    DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, cufft));
+    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)gs, (cufftComplex*)gs, CUFFT_FORWARD));
+    launch_mac<true>(gs, hs, ds, I, J, I, items, inv, st);
+    DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ds, (cufftComplex*)ds, CUFFT_INVERSE));
+    finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ds, mix, mix_stride, gx, mixpart,
+                                                                              item0, I, g.n, in_chs);
+    DASP_LAUNCH_OK("finish_dx_blocks_kernel");
+  }
+  if (e == IrGrad::kPlanar && !fused) {
+    launch_mac<true, true>(gs, xs, es, I, I, J, items, inv, st);        // dIR partitions: sum_p conj(X[p]) G[j+p]
+    DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+  } else if (e == IrGrad::kTime) {
+    launch_mac<true>(gs, xs, es, I, I, J, items, inv, st);
+    DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+    DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
+    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
+    DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)es, (cufftComplex*)es, CUFFT_INVERSE));
   }
   return DASP_OK;
 }
@@ -1879,42 +2066,15 @@ int dasp_reverb_filterbank(int64_t taps, double sample_rate, float* out) {
   return DASP_OK;
 }
 
-namespace {
-int plans_for(const Geom& g, Plans& pfull, Plans& prem, size_t& work) {
-  int rc;
-  if ((rc = get_plans(g, g.chunk, pfull)) != DASP_OK) return rc;
-  work = pfull.work;
-  const int64_t rem = g.bs % g.chunk;
-  if (rem) {
-    if ((rc = get_plans(g, rem, prem)) != DASP_OK) return rc;
-    if (prem.work > work) work = prem.work;
-  }
-  return DASP_OK;
-}
-}  // namespace
-
 int dasp_reverb_geometry(int64_t bs, int64_t n, int64_t num_samples, int64_t taps, int64_t chunk_items,
                          dasp_reverb_geom* out) {
   DASP_REQUIRE(out != nullptr, "reverb geometry: null out");
   Geom g;
   int rc = make_geom(bs, n, num_samples, taps, chunk_items, g);
   if (rc != DASP_OK) return rc;
-  std::lock_guard<std::mutex> lk(g_mu);
-  size_t work = 0;
-  if (bs > 0) {
-    Plans p{}, q{};
-    if ((rc = plans_for(g, p, q, work)) != DASP_OK) return rc;
-  }
-  FwdWs fw; BwdWs bw;
-  fwd_layout(g, work, fw);
-  bwd_layout(g, work, bw);
-  out->nb = g.nb; out->hop = g.hop; out->nbk = g.nbk; out->leff = g.leff; out->rpp = g.rpp;
-  out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
+  if ((rc = put_conv_geometry(g, &g, out)) != DASP_OK) return rc;
+  out->nb = g.nb; out->hop = g.hop; out->nbk = g.nbk; out->rpp = g.rpp;
   out->f_floats = bs * kBands * g.pair_c64() * 2;
-  out->xspec_c64 = bs * g.ib * kNbA;
-  out->irspec_c64 = bs * g.jb * kNbA;
-  out->fwd_workspace_bytes = (int64_t)fw.total;
-  out->bwd_workspace_bytes = (int64_t)bw.total;
   return DASP_OK;
 }
 
@@ -1936,32 +2096,25 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
   const bool spectral = (noise == nullptr) && g.rpp <= kMaxSpectralR;
   if (spectral) { if ((rc = get_filterbank_n1(g, (double)sample_rate, st, &H1)) != DASP_OK) return rc; }
   else          { if ((rc = get_filterbank(g, (double)sample_rate, st, &H)) != DASP_OK) return rc; }
-  Plans pfull{}, prem{};
-  size_t work = 0;
-  if ((rc = plans_for(g, pfull, prem, work)) != DASP_OK) return rc;
-  FwdWs w;
-  fwd_layout(g, work, w);
-  if ((int64_t)w.total > workspace_bytes) {
-    set_error("reverb fwd: workspace needs %lld bytes, got %lld", (long long)w.total, (long long)workspace_bytes);
-    return DASP_ERR_WORKSPACE;
-  }
+  Setup s{};
+  if ((rc = conv_setup(g, &g, s)) != DASP_OK) return rc;
+  if ((rc = check_workspace("reverb fwd", s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
+  const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
-  float2* ws_ys = (float2*)(base + w.ys);
   void* ws_cufft = base + w.cufft;
   const int64_t lp = g.L + g.P;
   const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P, I = (int)g.ib, J = (int)g.jb;
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const Plans& pl = (items == g.chunk) ? pfull : prem;
+    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
     // kept for the backward when the caller passes *_save buffers, transient workspace otherwise
     float2* C = f_save ? reinterpret_cast<float2*>(f_save) + item0 * kBands * g.pair_c64()
-                       : reinterpret_cast<float2*>(base + w.fchunk);
+                       : reinterpret_cast<float2*>(base + w.extra);
     float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? (float2*)irspec_save + item0 * J * (int64_t)kNbA : (float2*)(base + w.hsp);
     const dim3 gblk((unsigned)nbk, kBands, (unsigned)items);
-    // audio convolution: block transforms on the own FFT (fused with their pre/post kernels) when the rows allow bulk copies
-    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(x) && aligned16(hs);
+    const bool own_conv = own_fft_rows(n, x, hs);
 
     // ---- IR synthesis: taps t < leff land as (left, right) pairs in the first half of partition t / kB of hs ----
     // x_fft_kernel reads nothing else of hs; the cuFFT transform of the partitions reads whole slots, so they are
@@ -1995,9 +2148,9 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       // device noise: draw the filtered spectrum directly, one inverse transform (polyphase layout)
       dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st);
       DASP_LAUNCH_OK("spectral_gen_kernel");
-      DASP_CUFFT_OK(cufftSetStream(pl.pp_c2c.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.pp_c2c.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.pp_c2c.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_INVERSE));
+      DASP_CUFFT_OK(cufftSetStream(pl.pp.h, st));
+      DASP_CUFFT_OK(cufftSetWorkArea(pl.pp.h, ws_cufft));
+      DASP_CUFFT_OK(cufftExecC2C(pl.pp.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_INVERSE));
       shape_ir_pp_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(
           C, params + item0 * 25, hs, g.L, g.leff, J, (int)g.rpp, nb);
       DASP_LAUNCH_OK("shape_ir_pp_kernel");
@@ -2006,49 +2159,19 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       if (noise) noise_pairs_layout_kernel<<<gblk, 256, 0, st>>>(noise, C, item0, nbk, nb, hop, lp);
       else       noise_pairs_philox_kernel<<<gblk, 256, 0, st>>>(C, item0, nbk, nb, hop, seed);
       DASP_LAUNCH_OK("reverb noise kernel");
-      DASP_CUFFT_OK(cufftSetStream(pl.blk_c2c.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.blk_c2c.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.blk_c2c.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_FORWARD));
+      DASP_CUFFT_OK(cufftSetStream(pl.blk.h, st));
+      DASP_CUFFT_OK(cufftSetWorkArea(pl.blk.h, ws_cufft));
+      DASP_CUFFT_OK(cufftExecC2C(pl.blk.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_FORWARD));
       cmul_filter_pairs_kernel<<<gblk, 256, 0, st>>>(C, H, nbk, nb);
       DASP_LAUNCH_OK("cmul_filter_pairs_kernel");
-      DASP_CUFFT_OK(cufftExecC2C(pl.blk_c2c.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_INVERSE));
+      DASP_CUFFT_OK(cufftExecC2C(pl.blk.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_INVERSE));
       shape_ir_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, params + item0 * 25, hs, g.L, g.leff,
                                                                                J, nbk, nb, hop, P);
       DASP_LAUNCH_OK("shape_ir_pairs_kernel");
     }
-
-    // ---- audio convolution (partitioned, frequency domain) ----
-    const int nblk = (int)(items * I);
-    const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-    if (own_conv) {
-      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
-      // one work list: the items*I audio windows, then the items*J IR partitions (transformed in place in hs)
-      const int nunits = (int)(items * (I + J));
-      const unsigned xh_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-      x_fft_kernel<<<xh_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, n, g.leff, (int)in_chs, nblk,
-                                                                  nunits);
-      DASP_LAUNCH_OK("x_fft_kernel");
-      launch_mac<false, true>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
-      DASP_LAUNCH_OK("partition_mac_kernel");
-      ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ys), tw, x,
-                                                                     params + 24, 25, y, item0, I, n, (int)in_chs, nblk);
-      DASP_LAUNCH_OK("ifft_mix_kernel");
-      continue;
-    }
-    DASP_CUFFT_OK(cufftSetStream(pl.hj_c2c.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj_c2c.h, ws_cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.hj_c2c.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
-    x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, n, (int)in_chs);
-    DASP_LAUNCH_OK("x_blocks_kernel");
-    DASP_CUFFT_OK(cufftSetStream(pl.xi_c2c.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.xi_c2c.h, ws_cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)xs, (cufftComplex*)xs, CUFFT_FORWARD));
-    launch_mac<false>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
-    DASP_LAUNCH_OK("partition_mac_kernel");
-    DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_ys, (cufftComplex*)ws_ys, CUFFT_INVERSE));
-    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, params + 24, 25, y, item0, I, n,
-                                                                          (int)in_chs);
-    DASP_LAUNCH_OK("mix_blocks_kernel");
+    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, params + 24, 25, y, base, w, item0, items,
+                             st)) != DASP_OK)
+      return rc;
   }
   return DASP_OK;
 }
@@ -2067,81 +2190,33 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
                "reverb bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
-  Plans pfull{}, prem{};
-  size_t work = 0;
-  if ((rc = plans_for(g, pfull, prem, work)) != DASP_OK) return rc;
-  BwdWs w;
-  bwd_layout(g, work, w);
-  if ((int64_t)w.total > workspace_bytes) {
-    set_error("reverb bwd: workspace needs %lld bytes, got %lld", (long long)w.total, (long long)workspace_bytes);
-    return DASP_ERR_WORKSPACE;
-  }
+  Setup s{};
+  if ((rc = conv_setup(g, &g, s)) != DASP_OK) return rc;
+  if ((rc = check_workspace("reverb bwd", s.bwd.total, workspace_bytes)) != DASP_OK) return rc;
+  const BwdWs& w = s.bwd;
   unsigned char* base = (unsigned char*)workspace;
-  float2* ws_gs = (float2*)(base + w.gs);
-  float2* ws_ds = (float2*)(base + w.ds);
-  float2* ws_es = (float2*)(base + w.es);
-  float* ws_irpart = (float*)(base + w.irpart);
-  float* ws_mixpart = (float*)(base + w.mixpart);
-  void* ws_cufft = base + w.cufft;
-  const float inv = 1.0f / (float)kNbA;
+  const float2* ws_es = (const float2*)(base + w.es);
+  float* ws_irpart = (float*)(base + w.extra);
+  const float* ws_mixpart = (const float*)(base + w.mixpart);
   const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P, I = (int)g.ib, J = (int)g.jb;
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const Plans& pl = (items == g.chunk) ? pfull : prem;
+    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
     const float2* C = reinterpret_cast<const float2*>(f_save) + item0 * kBands * g.pair_c64();
     const float2* xs = (const float2*)xspec_save + item0 * I * (int64_t)kNbA;
     const float2* hs = (const float2*)irspec_save + item0 * J * (int64_t)kNbA;
 
-    // block transforms on the own in-shared-memory FFT (fused with their neighbours) when the rows allow bulk copies;
-    // dasp_debug_reverb_path(1) pins the cuFFT pipeline (the two are compared by the tests)
-    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(gy);
+    const bool own_conv = own_fft_rows(n, gy, nullptr);
+    // dL/dIR through the band parameters on the own FFT needs the polyphase f_save at nb = 8192
     const bool own_irgrad = own_conv && polyphase && nb == fft8k::kN && g.L < (int64_t)1 << 31;
     const float* tw = nullptr;
-    if (own_conv) {
-      if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
-    }
-    const int nblk = (int)(items * I);
-    const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-    const int mb = I > J ? I : J;
-    const bool fused_mac = own_irgrad && mb <= 16;
-    if (own_conv) {
-      g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, ws_gs, tw, item0, I, n, nblk);
-      DASP_LAUNCH_OK("g_fft_kernel");
-      if (fused_mac) {
-        dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
-        if (mb <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(ws_gs, hs, xs, ws_ds, ws_es, I, J, inv);
-        else          partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(ws_gs, hs, xs, ws_ds, ws_es, I, J, inv);
-        DASP_LAUNCH_OK("partition_mac_bwd_kernel");
-      } else {
-        launch_mac<true, true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
-        DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-      }
-      const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
-      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, x,
-                                                                    params + 24, 25, gx, ws_mixpart, item0, (int)items, I,
-                                                                    n, (int)in_chs);
-      DASP_LAUNCH_OK("ifft_dx_kernel");
-    } else {
-      g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, ws_gs, item0, I, n);
-      DASP_LAUNCH_OK("g_blocks_kernel");
-      DASP_CUFFT_OK(cufftSetStream(pl.xi_c2c.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.xi_c2c.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_gs, (cufftComplex*)ws_gs, CUFFT_FORWARD));
-      launch_mac<true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);
-      DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-      DASP_CUFFT_OK(cufftExecC2C(pl.xi_c2c.h, (cufftComplex*)ws_ds, (cufftComplex*)ws_ds, CUFFT_INVERSE));
-      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ws_ds, params + 24, 25, gx,
-                                                                                ws_mixpart, item0, I, n, (int)in_chs);
-      DASP_LAUNCH_OK("finish_dx_blocks_kernel");
-    }
+    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    if ((rc = conv_bwd_chunk(g, pl, own_conv, own_irgrad ? IrGrad::kPlanar : IrGrad::kTime, tw, gy, x, (int)in_chs, xs,
+                             hs, params + 24, 25, gx, base, w, item0, items, st)) != DASP_OK)
+      return rc;
     int nparts;
     if (own_irgrad) {
-      if (!fused_mac) {
-        launch_mac<true, true>(ws_gs, xs, ws_es, I, I, J, items, inv, st);      // dIR partitions: sum_p conj(X[p]) G[j+p]
-        DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-      }
       nparts = J;
       const int nunits = (int)(items * J);
       const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
@@ -2150,11 +2225,6 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
                                                                         (int)g.leff, J, (int)g.rpp, nunits);
       DASP_LAUNCH_OK("ifft_irgrad_kernel");
     } else {
-      launch_mac<true>(ws_gs, xs, ws_es, I, I, J, items, inv, st);
-      DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-      DASP_CUFFT_OK(cufftSetStream(pl.hj_c2c.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.hj_c2c.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.hj_c2c.h, (cufftComplex*)ws_es, (cufftComplex*)ws_es, CUFFT_INVERSE));
       if (polyphase) {
         nparts = (int)g.nparts_pp();
         ir_grad_pp_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(ws_es, C, params + item0 * 25, ws_irpart,
@@ -2176,54 +2246,6 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
 // ------------------------------------------------------------------ convolution_reverberation
 namespace {
 int g_conv_last_path[2] = {0, 0};                    // test hook: dispatch of the last dasp_conv_fwd / dasp_conv_bwd
-
-struct ConvGeom { int64_t bs, n, L, leff, ib, jb, chunk; };
-int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
-  DASP_REQUIRE(bs >= 0 && n >= 1 && L >= 1, "conv: bad shape bs=%lld n=%lld ir_len=%lld", (long long)bs, (long long)n,
-               (long long)L);
-  g.bs = bs; g.n = n; g.L = L;
-  g.leff = L < n ? L : n;
-  g.ib = (n + kB - 1) / kB;
-  g.jb = (g.leff + kB - 1) / kB;
-  if (chunk <= 0) chunk = 4;
-  g.chunk = chunk < bs ? chunk : (bs > 0 ? bs : 1);
-  return DASP_OK;
-}
-// the cuFFT pipeline's two block transforms (audio windows / dL/dx windows, IR partitions / dL/dIR partitions) for a full
-// chunk and for the remainder
-struct ConvPlans { PlanVal xi, hj; };
-int conv_plans(const ConvGeom& g, ConvPlans& full, ConvPlans& rem, size_t& work) {
-  int rc;
-  work = 0;
-  for (int64_t items : {g.chunk, g.bs % g.chunk}) {
-    if (items == 0) continue;
-    ConvPlans& p = items == g.chunk ? full : rem;
-    if ((rc = get_plan(2, kNbA, items * g.ib, kNbA, kNbA, p.xi)) != DASP_OK) return rc;
-    if ((rc = get_plan(2, kNbA, items * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
-    if (p.xi.work > work) work = p.xi.work;
-    if (p.hj.work > work) work = p.hj.work;
-  }
-  return DASP_OK;
-}
-struct ConvFwdWs { size_t ys, xsp, hsp, cufft, total; };
-struct ConvBwdWs { size_t gs, ds, es, mixpart, cufft, total; };
-void conv_fwd_layout(const ConvGeom& g, size_t cufft_work, ConvFwdWs& w) {
-  size_t o = 0;
-  w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));      // spectra not kept for a backward
-  w.hsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
-  w.cufft = o; o += align256(cufft_work);
-  w.total = o;
-}
-void conv_bwd_layout(const ConvGeom& g, size_t cufft_work, ConvBwdWs& w) {
-  size_t o = 0;
-  w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
-  w.mixpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * g.ib));
-  w.cufft = o; o += align256(cufft_work);
-  w.total = o;
-}
 }  // namespace
 
 int dasp_debug_conv_last_path(int which) { return g_conv_last_path[which ? 1 : 0]; }
@@ -2233,21 +2255,7 @@ int dasp_conv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_item
   ConvGeom g;
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
-  std::lock_guard<std::mutex> lk(g_mu);
-  size_t work = 0;
-  if (bs > 0) {
-    ConvPlans p{}, q{};
-    if ((rc = conv_plans(g, p, q, work)) != DASP_OK) return rc;
-  }
-  ConvFwdWs fw; ConvBwdWs bw;
-  conv_fwd_layout(g, work, fw);
-  conv_bwd_layout(g, work, bw);
-  out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
-  out->xspec_c64 = bs * g.ib * kNbA;
-  out->irspec_c64 = bs * g.jb * kNbA;
-  out->fwd_workspace_bytes = (int64_t)fw.total;
-  out->bwd_workspace_bytes = (int64_t)bw.total;
-  return DASP_OK;
+  return put_conv_geometry(g, nullptr, out);
 }
 
 int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, const float* mix,
@@ -2262,63 +2270,30 @@ int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_ch
   DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "conv fwd: pass both *_save buffers or neither");
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
-  ConvPlans pfull{}, prem{};
-  size_t work = 0;
-  if ((rc = conv_plans(g, pfull, prem, work)) != DASP_OK) return rc;
-  ConvFwdWs w;
-  conv_fwd_layout(g, work, w);
-  if ((int64_t)w.total > workspace_bytes) {
-    set_error("conv fwd: workspace needs %lld bytes, got %lld", (long long)w.total, (long long)workspace_bytes);
-    return DASP_ERR_WORKSPACE;
-  }
+  Setup s{};
+  if ((rc = conv_setup(g, nullptr, s)) != DASP_OK) return rc;
+  if ((rc = check_workspace("conv fwd", s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
+  const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
-  float2* ws_ys = (float2*)(base + w.ys);
-  void* ws_cufft = base + w.cufft;
   const int I = (int)g.ib, J = (int)g.jb;
   const float* tw = nullptr;
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const ConvPlans& pl = (items == g.chunk) ? pfull : prem;
+    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
     float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? (float2*)irspec_save + item0 * J * (int64_t)kNbA : (float2*)(base + w.hsp);
-    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(x) && aligned16(hs);
+    const bool own_conv = own_fft_rows(n, x, hs);
     g_conv_last_path[0] = own_conv ? 1 : 0;
     // the cuFFT transform of the partitions reads whole slots; x_fft_kernel only the taps ir_pack_kernel writes
     if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
     ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(ir, hs, item0, J, g.L, g.leff,
                                                                                           (int)ir_chs);
     DASP_LAUNCH_OK("ir_pack_kernel");
-    const int nblk = (int)(items * I);
-    if (own_conv) {
-      if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
-      const int nunits = (int)(items * (I + J));
-      const unsigned xh_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-      x_fft_kernel<<<xh_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, n, g.leff, (int)in_chs, nblk,
-                                                                  nunits);
-      DASP_LAUNCH_OK("x_fft_kernel");
-      launch_mac<false, true>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
-      DASP_LAUNCH_OK("partition_mac_kernel");
-      const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-      ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ys), tw, x, mix, 1,
-                                                                     y, item0, I, n, (int)in_chs, nblk);
-      DASP_LAUNCH_OK("ifft_mix_kernel");
-      continue;
-    }
-    DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, ws_cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
-    x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, n, (int)in_chs);
-    DASP_LAUNCH_OK("x_blocks_kernel");
-    DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, ws_cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)xs, (cufftComplex*)xs, CUFFT_FORWARD));
-    launch_mac<false>(xs, hs, ws_ys, I, J, I, items, 1.0f / (float)kNbA, st);
-    DASP_LAUNCH_OK("partition_mac_kernel");
-    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ws_ys, (cufftComplex*)ws_ys, CUFFT_INVERSE));
-    mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ws_ys, mix, 1, y, item0, I, n, (int)in_chs);
-    DASP_LAUNCH_OK("mix_blocks_kernel");
+    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, mix, 1, y, base, w, item0, items, st)) !=
+        DASP_OK)
+      return rc;
   }
   return DASP_OK;
 }
@@ -2334,93 +2309,42 @@ int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_ch
   DASP_REQUIRE(gy && x && mix && xspec_save && irspec_save && gx && gmix && workspace, "conv bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
-  ConvPlans pfull{}, prem{};
-  size_t work = 0;
-  if ((rc = conv_plans(g, pfull, prem, work)) != DASP_OK) return rc;
-  ConvBwdWs w;
-  conv_bwd_layout(g, work, w);
-  if ((int64_t)w.total > workspace_bytes) {
-    set_error("conv bwd: workspace needs %lld bytes, got %lld", (long long)w.total, (long long)workspace_bytes);
-    return DASP_ERR_WORKSPACE;
-  }
+  Setup s{};
+  if ((rc = conv_setup(g, nullptr, s)) != DASP_OK) return rc;
+  if ((rc = check_workspace("conv bwd", s.bwd.total, workspace_bytes)) != DASP_OK) return rc;
+  const BwdWs& w = s.bwd;
   unsigned char* base = (unsigned char*)workspace;
-  float2* ws_gs = (float2*)(base + w.gs);
-  float2* ws_ds = (float2*)(base + w.ds);
-  float2* ws_es = (float2*)(base + w.es);
-  float* ws_mixpart = (float*)(base + w.mixpart);
-  void* ws_cufft = base + w.cufft;
-  const float inv = 1.0f / (float)kNbA;
+  const float2* ws_es = (const float2*)(base + w.es);
+  const float* ws_mixpart = (const float*)(base + w.mixpart);
   const int I = (int)g.ib, J = (int)g.jb;
-  const int mb = I > J ? I : J;
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const ConvPlans& pl = (items == g.chunk) ? pfull : prem;
+    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
     const float2* xs = (const float2*)xspec_save + item0 * I * (int64_t)kNbA;
     const float2* hs = (const float2*)irspec_save + item0 * J * (int64_t)kNbA;
-    const bool own_conv = debug_reverb_path() != 1 && (n % 4 == 0) && aligned16(gy);
-    const bool fused_mac = own_conv && gir != nullptr && mb <= 16;
+    const bool own_conv = own_fft_rows(n, gy, nullptr);
+    const IrGrad e = gir == nullptr ? IrGrad::kNone : (own_conv ? IrGrad::kPlanar : IrGrad::kTime);
     // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed
-    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_mac ? 2 : 0) | (gir ? 4 : 0);
-    const int nblk = (int)(items * I);
-    const dim3 tail_grid((unsigned)((g.L - g.leff + 255) / 256), (unsigned)items);
-    if (own_conv) {
-      const float* tw = nullptr;
-      if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
-      const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-      g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, ws_gs, tw, item0, I, n, nblk);
-      DASP_LAUNCH_OK("g_fft_kernel");
-      if (fused_mac) {
-        dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
-        if (mb <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(ws_gs, hs, xs, ws_ds, ws_es, I, J, inv);
-        else          partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(ws_gs, hs, xs, ws_ds, ws_es, I, J, inv);
-        DASP_LAUNCH_OK("partition_mac_bwd_kernel");
-      } else {
-        launch_mac<true, true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
-        DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-        if (gir) {
-          launch_mac<true, true>(ws_gs, xs, ws_es, I, I, J, items, inv, st);    // dIR partitions: sum_p conj(X[p]) G[j+p]
-          DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-        }
-      }
-      const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
-      ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_ds), tw, gy, x, mix, 1,
-                                                                    gx, ws_mixpart, item0, (int)items, I, n, (int)in_chs);
-      DASP_LAUNCH_OK("ifft_dx_kernel");
-      if (gir) {
-        const int nunits = (int)(items * J);
-        const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-        ifft_irtaps_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mix,
-                                                                          gir, item0, J, g.L, g.leff, (int)ir_chs, nunits);
-        DASP_LAUNCH_OK("ifft_irtaps_kernel");
-        if (g.L > g.leff) {
-          irtaps_unpack_kernel<<<tail_grid, 256, 0, st>>>(ws_es, mix, gir, item0, J, g.L, g.leff, (int)ir_chs, g.leff);
-          DASP_LAUNCH_OK("irtaps_unpack_kernel");
-        }
-      }
-    } else {
-      g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, ws_gs, item0, I, n);
-      DASP_LAUNCH_OK("g_blocks_kernel");
-      DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ws_gs, (cufftComplex*)ws_gs, CUFFT_FORWARD));
-      launch_mac<true>(ws_gs, hs, ws_ds, I, J, I, items, inv, st);
-      DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-      DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ws_ds, (cufftComplex*)ws_ds, CUFFT_INVERSE));
-      finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ws_ds, mix, 1, gx, ws_mixpart, item0,
-                                                                                I, n, (int)in_chs);
-      DASP_LAUNCH_OK("finish_dx_blocks_kernel");
-      if (gir) {
-        launch_mac<true>(ws_gs, xs, ws_es, I, I, J, items, inv, st);
-        DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-        DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
-        DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, ws_cufft));
-        DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)ws_es, (cufftComplex*)ws_es, CUFFT_INVERSE));
-        irtaps_unpack_kernel<<<dim3((unsigned)((g.L + 255) / 256), (unsigned)items), 256, 0, st>>>(
-            ws_es, mix, gir, item0, J, g.L, g.leff, (int)ir_chs, 0);
-        DASP_LAUNCH_OK("irtaps_unpack_kernel");
-      }
+    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_corr(e, I, J) ? 2 : 0) | (gir ? 4 : 0);
+    const float* tw = nullptr;
+    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    if ((rc = conv_bwd_chunk(g, pl, own_conv, e, tw, gy, x, (int)in_chs, xs, hs, mix, 1, gx, base, w, item0, items,
+                             st)) != DASP_OK)
+      return rc;
+    if (e == IrGrad::kPlanar) {
+      const int nunits = (int)(items * J);
+      const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
+      ifft_irtaps_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mix, gir,
+                                                                        item0, J, g.L, g.leff, (int)ir_chs, nunits);
+      DASP_LAUNCH_OK("ifft_irtaps_kernel");
+    }
+    // taps t0 <= t < L: the zeros from leff on after ifft_irtaps_kernel, every tap after the cuFFT inverse
+    const int64_t t0 = e == IrGrad::kPlanar ? g.leff : 0;
+    if (e != IrGrad::kNone && g.L > t0) {
+      irtaps_unpack_kernel<<<dim3((unsigned)((g.L - t0 + 255) / 256), (unsigned)items), 256, 0, st>>>(
+          ws_es, mix, gir, item0, J, g.L, g.leff, (int)ir_chs, t0);
+      DASP_LAUNCH_OK("irtaps_unpack_kernel");
     }
     conv_mix_grad_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(ws_mixpart, gmix, item0, items, I);
     DASP_LAUNCH_OK("conv_mix_grad_kernel");

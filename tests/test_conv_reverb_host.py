@@ -50,6 +50,23 @@ def test_conv_geometry_without_gpu(lib, n, L, leff, J):
     assert g.bwd_workspace_bytes == 2 * _align(8 * I * NFFT) + _align(8 * J * NFFT) + _align(4 * I)
 
 
+# (n, L, taps): L > n, L < n, I = 18 and J = 17, 2047 taps (nb = 16384), a short signal, polyphase factor 19 > 16
+@pytest.mark.parametrize("n,L,taps", [(48000, 96000, 1023), (48000, 30000, 1023), (70000, 66000, 1023),
+                                      (48000, 48000, 2047), (1001, 500, 31), (200000, 150000, 1023)])
+def test_reverb_geometry_workspace_without_gpu(lib, n, L, taps):
+    """the reverb's workspace is the convolution's plus its own region: the filtered noise of a chunk in the forward,
+    the per-partition partials of the 24 band-parameter gradients in the backward"""
+    from dasp_pytorch_b200 import _abi
+    g = _abi.ReverbGeom()
+    assert lib.dasp_reverb_geometry(0, n, L, taps, 7, g) == 0
+    I, J = -(-n // KB), -(-min(L, n) // KB)
+    assert (g.leff, g.x_blocks, g.ir_partitions, g.chunk_items) == (min(L, n), I, J, 1)
+    conv = 2 * _align(8 * I * NFFT) + _align(8 * J * NFFT)
+    pair_c64 = max(g.nbk, g.rpp) * g.nb
+    assert g.fwd_workspace_bytes == conv + _align(8 * 12 * pair_c64)
+    assert g.bwd_workspace_bytes == conv + _align(4 * 24 * max(g.nbk, -(-g.nb // 256), J)) + _align(4 * I)
+
+
 def test_conv_geometry_rejects_bad_shapes(lib):
     from dasp_pytorch_b200 import _abi
     g = _abi.ConvGeom()

@@ -62,7 +62,7 @@ int debug_forced_warps();
 // Test hook (dasp_debug_eq_bwd_stages): 0 = automatic; 1 / 2 pins the number of x / dL/dy stages of the EQ backward
 int debug_eq_bwd_stages();
 // Test hook (dasp_debug_reverb_path): IR synthesis of the device-noise reverb: 0 = automatic, 1 = generator / cuFFT /
-// shaping kernels, 2 = single cluster kernel
+// shaping kernels, 2 = generator -> ifft_shape_kernel for R <= 8 (instead of the default cluster kernel)
 int debug_reverb_path();
 // Test hook (dasp_debug_reverb_flat_filterbank): both IR syntheses use unit-impulse "filters", so the band-filtered
 // noise they keep for the backward IS the white noise they draw -- the periodic sequence w_k of the spectral

@@ -15,7 +15,8 @@
 //   * IR synthesis, device noise (default): spectral_gen_kernel draws the FILTERED noise spectrum directly
 //     (Philox4x32-10 + Box-Muller; see the comment at the kernel); ifft_shape_kernel = own in-shared-memory inverse
 //     FFT (fft8192.cuh) fused with envelope * gain * band mean -> IR written straight into the partition layout of
-//     the convolution.  (Test-hook variants: batched cuFFT + shape_ir_pp_kernel, and one cluster kernel per item.)
+//     the convolution.  For R <= 6 both run as one warp-specialised cluster kernel (ir_synth_cluster_kernel), so the
+//     spectrum never goes to HBM.  (Test-hook variants: batched cuFFT + shape_ir_pp_kernel, and the two kernels.)
 //   * IR synthesis, parity mode (caller's noise tensor): overlap-save blocks -> C2C -> cmul_filter_pairs ->
 //     inverse C2C -> shape_ir_pairs_kernel.
 //   * Audio convolution: uniformly partitioned overlap-save in the frequency domain: x_fft_kernel (window gather +
@@ -1041,134 +1042,206 @@ ifft_irgrad_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
   }
 }
 
-// ---- fused IR synthesis (device-noise mode, nb == 8192, R <= 8) -------------------------------------
-// spectral_gen -> inverse FFT -> shape/accumulate as ONE kernel, so the 4.7 MB-per-item filtered-noise buffer is
-// written at most once (for the backward) instead of being written, transformed in place and read back.
+// ---- warp-specialised cluster IR synthesis (device-noise mode, nb == 8192, R <= 6; the default) --------------
+// spectral_gen_kernel + ifft_shape_kernel as ONE kernel: the 4.7 MB-per-item noise spectrum never leaves the SMs, only
+// the IR taps (and f, when a backward follows) are written.
 //
-// One thread-block CLUSTER of R CTAs per item; CTA c owns polyphase class c, i.e. the IR taps R a + c.
-//   * generation: the 12 * (nb/2 + 1) class pairs of the item are dealt round-robin over the R * 512 threads of
-//     the cluster (so every thread draws the same number of units); a unit's R results go to the R CTAs of the
-//     cluster as remote shared-memory stores (DSMEM) into the band's spectrum buffer G[band & 1] (planar re / im).
-//   * as soon as a band is complete (cluster barrier), every CTA runs the in-shared-memory inverse FFT of its
-//     class (fft8192.cuh) and accumulates  gain_k env_k(t) f_k(t) / 12  for its 16 taps per thread in registers;
-//     f is stored for the backward only when the caller keeps it.
-//   * G is double buffered by band parity: a second (split arrive / wait) cluster barrier hands a buffer back to
-//     the generators once every CTA has finished reading it (after FFT pass 2).
-constexpr int kMaxFusedR = 8;
+// One thread-block CLUSTER of R CTAs per item; CTA c owns polyphase class c, i.e. the IR taps R a + c.  The clusters are
+// persistent (as many as the device co-schedules) and walk the chunk's items.  Every CTA has two roles:
+//   * warps 0-15 (4 warpgroups): the in-shared-memory inverse FFT of fft8192.cuh on the class spectrum of each band,
+//     then exactly the epilogue of ifft_shape_kernel (envelope rho recurrence, accumulation over bands in registers,
+//     IR taps < leff into the partition layout, f into the polyphase f_save layout);
+//   * warps 16-27 (3 warpgroups): spectral_unit<R> for the bands ahead of the one being transformed.  The 12 (nb/2 + 1)
+//     class pairs of an item are dealt round-robin over the R * 384 generator threads of the cluster; a unit's R
+//     results go to the R CTAs as st.async stores into the planar buffer G[band & 1] of that CTA, which complete bytes
+//     on its mbarrier full[band & 1] (armed with expect_tx of 64 KB per band by the FFT side).
+// After FFT pass 2 the FFT side no longer reads G[band & 1]: one thread arrives (remotely) on empty[band & 1] of every
+// CTA of the cluster (arrival count R), and the generators wait on their local empty before writing band + 2 there.
+// No cluster-wide barrier is left in the band loop.  setmaxnreg moves the registers to the FFT warps.
+// Generation is the slower role (H100: 1.6x faster with 256 than with 128 generator threads, 1.15x more with 384), so
+// the generators get every register the FFT side can spare: 512 * 80 + 384 * 56 <= 896 * 72, the pool at launch.  At
+// R = 7, 8 (64 registers per generator) only 128 generators would fit, which is slower than the two-kernel synthesis.
+constexpr int kMaxClusterR = 6;
+constexpr int kSynthGen = 384, kSynthThreads = kFusedThreads + kSynthGen;
+constexpr int kSynthFftRegs = 80, kSynthGenRegs = 56;
+// dasp_debug_reverb_path(2) selects the two-kernel synthesis for R <= 8 (the test matrix pins it there)
+constexpr int kMaxHookR = 8;
+constexpr size_t kSynthSmemBytes =
+    sizeof(float) * (2 * 2 * fft8k::kPlaneG + 2 * fft8k::kPlaneY + fft8k::kTabFloats) + 4 * sizeof(uint64_t);
 
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
 __device__ __forceinline__ unsigned cluster_ctarank() {
   unsigned r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
-// generic pointer to the same shared-memory location in CTA `rank` of the cluster (DSMEM).  Kept 64-bit/generic on
-// purpose: with 32-bit shared::cluster addresses ptxas folded "+ 4 nb" of the mirror index into the store's
-// immediate AFTER widening (base - 4 j1) to 64 bits, which wraps for rank 0 and faults.
-__device__ __forceinline__ float* map_to_cta(float* smem_ptr, unsigned rank) {
-  uint64_t r;
-  asm volatile("mapa.u64 %0, %1, %2;" : "=l"(r) : "l"(reinterpret_cast<uint64_t>(smem_ptr)), "r"(rank));
-  return reinterpret_cast<float*>(r);
+// shared::cluster address of the same shared-memory location in CTA `rank` (32-bit arithmetic only: see st_async)
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
 }
+// 4-byte store into (possibly remote) shared memory that completes 4 bytes of the transaction count of `bar` (same CTA
+// as the destination); the completion has release semantics at cluster scope
+__device__ __forceinline__ void st_async(uint32_t addr, float v, uint32_t bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(addr),
+               "r"(__float_as_uint(v)), "r"(bar)
+               : "memory");
+}
+// relaxed arrive on an mbarrier of any CTA of the cluster; the caller orders its earlier accesses with fence_cluster()
+// (one fence for the R arrives of a band instead of one release each)
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_bar) {
+  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+}
+__device__ __forceinline__ void fence_cluster() { asm volatile("fence.acq_rel.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  uint32_t done;
+  do {
+    asm volatile(
+        "{\n.reg .pred p;\n"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n}\n"
+        : "=r"(done)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+  } while (!done);
+}
+// the 512 FFT threads only (named barrier 1; barrier 0 is __syncthreads)
+__device__ __forceinline__ void fft_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kFusedThreads) : "memory"); }
 
 template <int R>
-__global__ void __launch_bounds__(kFusedThreads, 1)
-ir_synth_fused_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles,
-                      const float* __restrict__ params, float2* __restrict__ Hb, float2* __restrict__ Csave, int64_t item0, int64_t L, int64_t leff, int jb,
-                      const unsigned long long* seed) {
-  constexpr int nb = fft8k::kN, U = nb / 2 + 1, CT = R * kFusedThreads, total = kBands * U;
-  static_assert(CT < U, "at most one band may complete per generation round");
-  extern __shared__ __align__(16) float sm[];
+__global__ void __launch_bounds__(kSynthThreads, 1)
+ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles, const float* __restrict__ params,
+                        float2* __restrict__ Hb, float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
+                        int jb, const unsigned long long* seed) {
+  constexpr int nb = fft8k::kN, U = nb / 2 + 1, NG = kSynthGen, NT = kSynthThreads;
+  constexpr int CT = R * NG, total = kBands * U;
+  constexpr uint32_t kBandBytes = 2u * nb * 4u;    // one class spectrum, planar re / im
+  extern __shared__ __align__(128) float sm[];
   float* G = sm;                                   // [parity][re, im][8192]
   float* Yr = sm + 4 * fft8k::kPlaneG;
   float* Yi = Yr + fft8k::kPlaneY;
   float* tabf = Yi + fft8k::kPlaneY;
-  float* gk = tabf + fft8k::kTabFloats;
-  float* rk = gk + 16;
+  uint64_t* full = reinterpret_cast<uint64_t*>(tabf + fft8k::kTabFloats);
+  uint64_t* empty = full + 2;
   const int t = threadIdx.x;
   const unsigned c = cluster_ctarank();
-  const int64_t il = blockIdx.y;
+  const int my_items = items > (int)blockIdx.y ? (items - 1 - (int)blockIdx.y) / (int)gridDim.y + 1 : 0;
+  const int nbands = my_items * kBands;            // bands this cluster walks: g = item iteration * 12 + band
 
-  for (int e = t; e < fft8k::kTabFloats; e += kFusedThreads) tabf[e] = twiddles[e];
-  if (t < kBands) {
-    gk[t] = params[il * 25 + t] * (1.0f / kBands);
-    rk[t] = -(params[il * 25 + kBands + t] * 10.0f + 1.0f);
+  for (int e = t; e < fft8k::kTabFloats; e += NT) tabf[e] = twiddles[e];
+  if (t == 0) {
+    mbar_init(&full[0], 1);
+    mbar_init(&full[1], 1);
+    mbar_init(&empty[0], R);
+    mbar_init(&empty[1], R);
+    fence_barrier_init();
+    if (nbands > 0) mbar_arrive_expect_tx(&full[0], kBandBytes);
+    if (nbands > 1) mbar_arrive_expect_tx(&full[1], kBandBytes);
   }
-  const fft8k::Tables tb = fft8k::carve_tables(tabf);
-  float* remote[R];                                // G of every CTA of the cluster
-#pragma unroll
-  for (int b = 0; b < R; ++b) remote[b] = map_to_cta(G, (unsigned)b);
-  const PhiloxKeys keys = philox_keys(__ldg(seed));
-  const float step = 1.0f / (float)(L - 1);
-  float accr[16], acci[16];
-#pragma unroll
-  for (int q = 0; q < 16; ++q) { accr[q] = 0.f; acci[q] = 0.f; }
-  // every CTA of the cluster must be resident (and its tables written) before the first remote store
+  __syncthreads();
+  // every CTA of the cluster must be resident with its barriers initialised before the first remote store
   cluster_arrive();
   cluster_wait();
 
-  int processed = 0;
-  bool buffer_handed_back = false;                 // an arrive of the "G is free" barrier is outstanding
-  constexpr int rounds = (total + CT - 1) / CT;
-  for (int r = 0; r < rounds; ++r) {
-    if (buffer_handed_back) { cluster_wait(); buffer_handed_back = false; }
-    const int u = r * CT + (int)c * kFusedThreads + t;
-    if (u < total) {
-      const int k = u / U, j1 = u - k * U;
-      const unsigned long long pair = (unsigned long long)((item0 + il) * kBands + k);
-      const bool self_mirror = (j1 == 0) || (2 * j1 == nb);
-      const int off = (k & 1) * 2 * fft8k::kPlaneG;
-      spectral_unit<R>(j1, nb, H1 + (int64_t)k * (R * nb / 2 + 1), pair, keys, [&](int b, float2 q, float2 qm) {
-        float* base = remote[b] + off;
-        base[j1] = q.x;
-        base[fft8k::kPlaneG + j1] = q.y;
-        if (!self_mirror) {
-          base[nb - j1] = qm.x;
-          base[fft8k::kPlaneG + nb - j1] = qm.y;
+  if (t >= kFusedThreads) {
+    // ---------------- generators
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kSynthGenRegs));
+    const int gt = t - kFusedThreads;
+    const PhiloxKeys keys = philox_keys(__ldg(seed));
+    const uint32_t g_local = smem_u32(G), full_local = smem_u32(full);
+    int waited = 1;                                // bands < 2 need no free buffer
+    for (int i = 0; i < my_items; ++i) {
+      const int64_t il = blockIdx.y + (int64_t)i * gridDim.y;
+      for (int u = (int)c * NG + gt; u < total; u += CT) {
+        const int k = u / U, j1 = u - k * U;
+        const int g = i * kBands + k;
+        if (g > waited) {                          // G[k & 1] of this CTA is free once every CTA finished band g - 2
+          mbar_wait_cluster(&empty[k & 1], (uint32_t)(((g - 2) >> 1) & 1));
+          waited = g;
         }
-      });
+        const unsigned long long pair = (unsigned long long)((item0 + il) * kBands + k);
+        const bool self_mirror = (j1 == 0) || (2 * j1 == nb);
+        const uint32_t off = (uint32_t)(k & 1) * kBandBytes;
+        spectral_unit<R>(j1, nb, H1 + (int64_t)k * (R * nb / 2 + 1), pair, keys, [&](int b, float2 q, float2 qm) {
+          const uint32_t base = mapa_u32(g_local + off, (uint32_t)b);
+          const uint32_t bar = mapa_u32(full_local + 8u * (uint32_t)(k & 1), (uint32_t)b);
+          st_async(base + 4u * j1, q.x, bar);
+          st_async(base + 4u * (fft8k::kPlaneG + j1), q.y, bar);
+          if (!self_mirror) {
+            st_async(base + 4u * (nb - j1), qm.x, bar);
+            st_async(base + 4u * (fft8k::kPlaneG + nb - j1), qm.y, bar);
+          }
+        });
+      }
     }
-    const int done = (r + 1) * CT < total ? (r + 1) * CT : total;
-    if (done / U > processed) {                    // band `processed` is complete in every CTA's G
-      cluster_arrive();
-      cluster_wait();
-      const int kk = processed;
-      float* gr = G + (kk & 1) * 2 * fft8k::kPlaneG;
-      float* gi = gr + fft8k::kPlaneG;
-      fft8k::p1<true>(gr, gi, tb, t);
-      __syncthreads();
-      fft8k::p2<true>(gr, gi, Yr, Yi, tb, t);
-      __syncthreads();
-      cluster_arrive();                            // this CTA no longer reads G[kk & 1]
-      buffer_handed_back = true;
-      fft8k::P3Regs q3;
-      fft8k::p3_load<true>(Yr, Yi, t, q3);
-      __syncthreads();
-      fft8k::p3_store<true>(Yr, Yi, tb, t, q3);
-      __syncthreads();
-      float xr[16], xi[16];
-      fft8k::p4<true>(Yr, Yi, t, xr, xi);
-      const float g = gk[kk], rr = rk[kk];
-      float2* fout = Csave ? Csave + ((il * kBands + kk) * R + c) * (int64_t)nb : nullptr;
+  } else {
+    // ---------------- inverse FFT + shaping (the body of ifft_shape_kernel)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kSynthFftRegs));
+    const fft8k::Tables tb = fft8k::carve_tables(tabf);
+    const float step = 1.0f / (float)(L - 1);
+    for (int i = 0; i < my_items; ++i) {
+      const int64_t il = blockIdx.y + (int64_t)i * gridDim.y;
+      float accr[16], acci[16];
+#pragma unroll
+      for (int q = 0; q < 16; ++q) { accr[q] = 0.f; acci[q] = 0.f; }
+      for (int k = 0; k < kBands; ++k) {
+        const int g = i * kBands + k;
+        // one warp polls the barrier, the others sleep in bar.sync instead of taking issue slots from the generators
+        if (t < 32) mbar_wait_cluster(&full[k & 1], (uint32_t)((g >> 1) & 1));
+        fft_sync();
+        float* gr = G + (k & 1) * 2 * fft8k::kPlaneG;
+        float* gi = gr + fft8k::kPlaneG;
+        fft8k::p1<true>(gr, gi, tb, t);
+        fft_sync();
+        fft8k::p2<true>(gr, gi, Yr, Yi, tb, t);
+        fence_proxy_async_smem();                  // pass-1 stores to G before the generators' next stores there
+        fft_sync();
+        if (t == 0 && g + 2 < nbands) {            // hand G[k & 1] back for band g + 2
+          mbar_arrive_expect_tx(&full[k & 1], kBandBytes);
+          fence_cluster();
+#pragma unroll
+          for (int b = 0; b < R; ++b) {
+            mbar_arrive_remote(mapa_u32(smem_u32(&empty[k & 1]), (uint32_t)b));
+          }
+        }
+        fft8k::P3Regs q3;
+        fft8k::p3_load<true>(Yr, Yi, t, q3);
+        fft_sync();
+        fft8k::p3_store<true>(Yr, Yi, tb, t, q3);
+        fft_sync();
+        float xr[16], xi[16];
+        fft8k::p4<true>(Yr, Yi, t, xr, xi);
+        float e_prev = 0.f;
+        const float g_k = params[il * 25 + k] * (1.0f / kBands), rr = -(params[il * 25 + kBands + k] * 10.0f + 1.0f);
+        float2* fout = Csave ? Csave + ((il * kBands + k) * R + c) * (int64_t)nb : nullptr;
+        // the envelope of ifft_shape_kernel, bit for bit: evaluated at every 4th tap, stepped by rho in between
+        const float rho = __expf(rr * step * (float)(512 * R));
+#pragma unroll
+        for (int q = 0; q < 16; ++q) {
+          const int a = t + 512 * q;
+          float e;
+          if ((q & 3) == 0) e = g_k * __expf(rr * time_axis32(R * a + (int)c, L, step));
+          else e = e_prev * rho;
+          e_prev = e;
+          accr[q] = fmaf(e, xr[q], accr[q]);
+          acci[q] = fmaf(e, xi[q], acci[q]);
+          if (fout) fout[a] = make_float2(xr[q], xi[q]);
+        }
+        // (Y is next written by pass 2 of the following band, behind the barrier after its pass 1)
+      }
+      float2* out = Hb + il * (int64_t)jb * kNbA;
 #pragma unroll
       for (int q = 0; q < 16; ++q) {
-        const int a = t + 512 * q;
-        const float e = g * __expf(rr * time_axis((int64_t)R * a + c, L, step));
-        accr[q] = fmaf(e, xr[q], accr[q]);
-        acci[q] = fmaf(e, xi[q], acci[q]);
-        if (fout) fout[a] = make_float2(xr[q], xi[q]);
+        const int tau = R * (t + 512 * q) + (int)c;
+        if (tau < leff) out[(tau / kB) * kNbA + (tau % kB)] = make_float2(accr[q], acci[q]);
       }
-      ++processed;     // (Y is next written by pass 2 of the following band, behind a cluster barrier)
     }
   }
-  if (buffer_handed_back) cluster_wait();
-  float2* out = Hb + il * (int64_t)jb * kNbA;
-#pragma unroll
-  for (int q = 0; q < 16; ++q) {
-    const int64_t tau = (int64_t)R * (t + 512 * q) + c;
-    if (tau < leff) out[(tau / kB) * kNbA + (tau % kB)] = make_float2(accr[q], acci[q]);
-  }
+  // no CTA may leave while a remote store or arrive could still target it
+  cluster_arrive();
+  cluster_wait();
 }
 
 // part[((item*nparts + blockIdx.x)*12 + k)*2 + {0,1}], nparts = gridDim.x; threads stride over time
@@ -1717,8 +1790,6 @@ bool dispatch_spectral(int R, float2* C, const float2* H1, int64_t item0, int64_
 }
 constexpr int kMaxSpectralR = 16;
 
-// fused synthesis: one cluster of R CTAs per item.  Returns false when the device cannot co-schedule such a
-// cluster (then the three-kernel path is used), true after a launch attempt (check cudaGetLastError).
 // twiddle tables of fft8192.cuh (fp64 on the host, once per device)
 std::map<int, float*> g_fft_tab;
 int get_fft_tables(cudaStream_t st, const float** out) {
@@ -1757,15 +1828,16 @@ int launch_ifft_shape(float2* C, const float* tw, const float* params, float2* h
 }
 int g_last_fused = 0;                                // test hook: IR-synthesis path of the last forward chunk
 std::map<std::pair<int, int>, int> g_fused_ok;      // (device, R) -> clusters that fit, guarded by g_mu
+// cluster synthesis: persistent clusters of R CTAs, as many as the device co-schedules (at most one per item).
+// Returns false when the device cannot co-schedule such a cluster (then generator -> ifft_shape_kernel runs), true after
+// a launch attempt (check cudaGetLastError).
 template <int R>
 bool launch_fused(const float2* H1, const float* tw, const float* params, float2* hs, float2* Csave, int64_t item0, int64_t items,
                   int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st) {
-  auto kern = ir_synth_fused_kernel<R>;
-  const size_t smem = sizeof(float) * kFusedSmemFloats;
+  auto kern = ir_synth_cluster_kernel<R>;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(R, (unsigned)items, 1);
-  cfg.blockDim = dim3(kFusedThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
+  cfg.blockDim = dim3(kSynthThreads, 1, 1);
+  cfg.dynamicSmemBytes = kSynthSmemBytes;
   cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension;
@@ -1777,7 +1849,8 @@ bool launch_fused(const float2* H1, const float* tw, const float* params, float2
   auto it = g_fused_ok.find({dev, R});
   if (it == g_fused_ok.end()) {
     int n = 0;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+    cfg.gridDim = dim3(R, 1, 1);
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSynthSmemBytes) != cudaSuccess ||
         cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) {
       n = 0;
       cudaGetLastError();
@@ -1785,14 +1858,16 @@ bool launch_fused(const float2* H1, const float* tw, const float* params, float2
     it = g_fused_ok.emplace(std::make_pair(dev, R), n).first;
   }
   if (it->second < 1) return false;
-  cudaLaunchKernelEx(&cfg, kern, H1, tw, params, hs, Csave, item0, L, leff, jb, seed);
+  const int64_t clusters = items < it->second ? items : it->second;
+  cfg.gridDim = dim3(R, (unsigned)clusters, 1);
+  cudaLaunchKernelEx(&cfg, kern, H1, tw, params, hs, Csave, item0, (int)items, (int)L, (int)leff, jb, seed);
   return true;
 }
 bool dispatch_fused(int R, const float2* H1, const float* tw, const float* params, float2* hs, float2* Csave, int64_t item0,
                     int64_t items, int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st) {
   switch (R) {
 #define DASP_R(r) case r: return launch_fused<r>(H1, tw, params, hs, Csave, item0, items, L, leff, jb, seed, st);
-    DASP_R(1) DASP_R(2) DASP_R(3) DASP_R(4) DASP_R(5) DASP_R(6) DASP_R(7) DASP_R(8)
+    DASP_R(1) DASP_R(2) DASP_R(3) DASP_R(4) DASP_R(5) DASP_R(6)
 #undef DASP_R
     default: return false;
   }
@@ -2120,27 +2195,26 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     // x_fft_kernel reads nothing else of hs; the cuFFT transform of the partitions reads whole slots, so they are
     // zero-filled first
     if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
-    // device-noise IR synthesis, three variants (same Philox stream, so they agree to transform rounding):
-    //   2 = generator -> ifft_shape_kernel (own in-shared-memory FFT fused with the shaping; default for nb == 8192)
-    //   1 = one thread-block cluster per item (generator + FFT + shaping in one kernel; dasp_debug_reverb_path(2))
-    //   0 = generator -> batched cuFFT -> shape_ir_pp_kernel (dasp_debug_reverb_path(1), and any other nb)
+    // device-noise IR synthesis (every variant draws the same Philox stream; the two own-FFT ones are bit-identical):
+    //   default, nb == 8192: ir_synth_cluster_kernel for R <= 6, generator -> ifft_shape_kernel for 7 <= R <= 16 or
+    //     when the device cannot co-schedule the cluster (last path 2);
+    //   dasp_debug_reverb_path(2), R <= 8: generator -> ifft_shape_kernel (last path 1);
+    //   dasp_debug_reverb_path(1), and any other nb: generator -> batched cuFFT -> shape_ir_pp_kernel (last path 0).
     int synth = 0;
     const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
-    if (own_fft && debug_reverb_path() == 2 && g.rpp <= kMaxFusedR) synth = 1;
-    else if (own_fft && debug_reverb_path() != 1) synth = 2;
+    const bool two_kernel_hook = debug_reverb_path() == 2 && g.rpp <= kMaxHookR;
+    if (own_fft && debug_reverb_path() != 1) synth = two_kernel_hook ? 1 : 2;
     const float* tw = nullptr;
     if ((synth != 0 || own_conv) && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    if (synth == 1) {
-      if (dispatch_fused((int)g.rpp, H1, tw, params + item0 * 25, hs, f_save ? C : nullptr, item0, items, g.L, g.leff, J,
-                         seed, st)) {
-        DASP_LAUNCH_OK("ir_synth_fused_kernel");
-      } else {
-        synth = 2;                                   // the device cannot co-schedule such a cluster
-      }
-    }
     g_last_fused = synth;
-    if (synth == 1) {
-    } else if (synth == 2) {
+    bool clustered = false;
+    if (synth == 2 && g.rpp <= kMaxClusterR) {
+      clustered = dispatch_fused((int)g.rpp, H1, tw, params + item0 * 25, hs, f_save ? C : nullptr, item0, items, g.L,
+                                 g.leff, J, seed, st);
+      if (clustered) DASP_LAUNCH_OK("ir_synth_cluster_kernel");
+    }
+    if (clustered) {
+    } else if (synth != 0) {
       dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, st);
       DASP_LAUNCH_OK("spectral_gen_kernel");
       if ((rc = launch_ifft_shape(C, tw, params + item0 * 25, hs, f_save != nullptr, items, g, J, st)) != DASP_OK) return rc;

@@ -51,11 +51,14 @@ void dasp_debug_force_warps(int warps);
 /* test hook: pin the number of x / dL/dy stages per warp of the EQ backward (1 or 2; 0 = automatic) */
 void dasp_debug_eq_bwd_stages(int stages);
 /* test hook, IR synthesis of the device-noise reverb (all variants draw the same Philox stream and must agree):
-   0 = automatic (generator -> fused in-shared-memory inverse FFT + shaping kernel when the block FFT is 8192 points),
-   1 = generator -> batched cuFFT -> shaping kernel, 2 = one thread-block-cluster kernel per item */
+   0 = automatic (block FFT of 8192 points: one warp-specialised thread-block-cluster kernel for polyphase factors
+   R <= 6, generator -> fused in-shared-memory inverse FFT + shaping kernel otherwise),
+   1 = generator -> batched cuFFT -> shaping kernel,
+   2 = generator -> fused in-shared-memory inverse FFT + shaping kernel for R <= 8 */
 void dasp_debug_reverb_path(int path);
-/* test hook: variant used by the last chunk of the most recent dasp_reverb_fwd: 0 = cuFFT pipeline, 1 = cluster
-   kernel, 2 = generator + fused FFT/shaping kernel */
+/* test hook: variant used by the last chunk of the most recent dasp_reverb_fwd: 0 = cuFFT pipeline, 1 = generator +
+   fused FFT/shaping kernel selected by dasp_debug_reverb_path(2), 2 = the default own-FFT synthesis (cluster kernel
+   or generator + fused FFT/shaping kernel) */
 int dasp_debug_reverb_last_path(void);
 
 /* test hook: 1 = the IR synthesis uses unit-impulse filters, so the f_save buffer of dasp_reverb_fwd returns the white

@@ -44,6 +44,7 @@ def reverb_bytes_per_item(n, in_chs=2):
     return {
         "spectral_gen_kernel": f,                                         # generator spectrum written
         "ifft_shape_kernel": 2 * f + leff * 8,                            # spectrum read, f written, IR taps written
+        "ir_synth_cluster_kernel": f + leff * 8,                          # f written, IR taps written
         "x_fft_kernel": 2 * in_chs * a + J * kB * 8 + (I + J) * c8,       # windows (each sample twice), taps, spectra
         "partition_mac_kernel": (I + J) * c8 + I * c8,                    # X, H read; Y written
         "ifft_mix_kernel": I * c8 + in_chs * a + 2 * a,                   # Y, x read; y written

@@ -244,6 +244,24 @@ __device__ __forceinline__ CurveOut gain_computer(float xdb, const CurveK& k) {
   return o;
 }
 
+// side chain of the generic channel loop: the channel sum accumulated in fp64 and rounded once.  A running fp32 sum
+// of three or more channels loses its relative accuracy where the channels cancel, and dL/dx carries 1/side, which
+// is largest exactly there.  One rounding of the (near-)exact sum is what the stereo path's fp32 a + b gives too, so
+// stereo through this loop stays bit-identical to the ST specialisation.
+template <class Pipe>
+__device__ __forceinline__ void side_chain(float (&xs)[kE], const Pipe& pipe, int st, int C, int off) {
+  double acc[kE];
+#pragma unroll
+  for (int j = 0; j < kE; ++j) acc[j] = 0.0;
+  for (int c = 0; c < C; ++c) {
+    const float* xb = pipe.buf(st, c) + off;
+#pragma unroll
+    for (int j = 0; j < kE; ++j) acc[j] += (double)xb[j];
+  }
+#pragma unroll
+  for (int j = 0; j < kE; ++j) xs[j] = (float)acc[j];
+}
+
 // 20 log10(max(|xs|, eps)); __log2f is the single-instruction MUFU.LG2 (|rel err| < 2^-22 for normal inputs,
 // i.e. < 1e-5 dB here) -- the accurate log2f costs ~15 instructions in a kernel that is issue bound
 __device__ __forceinline__ float level_db(float xs, float eps) { return kDbPerLog2 * __log2f(fmaxf(fabsf(xs), eps)); }
@@ -303,13 +321,7 @@ __global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
 #pragma unroll
         for (int j = 0; j < kE; ++j) { x0[ST ? j : 0] = xa[j]; x1[ST ? j : 0] = xb[j]; xs[j] = xa[j] + xb[j]; }
       } else {
-#pragma unroll
-        for (int j = 0; j < kE; ++j) xs[j] = 0.f;
-        for (int c = 0; c < C; ++c) {
-          const float* xb = pipe.buf(st, c) + off;
-#pragma unroll
-          for (int j = 0; j < kE; ++j) xs[j] += xb[j];
-        }
+        side_chain(xs, pipe, st, C, off);
       }
       float run = 0.f;
 #pragma unroll
@@ -406,13 +418,7 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
         xs[j] = xa[j] + xb[j];
       }
     } else {
-#pragma unroll
-      for (int j = 0; j < kE; ++j) xs[j] = 0.f;
-      for (int c = 0; c < C; ++c) {
-        const float* xb = pipe.buf(st, c) + off;
-#pragma unroll
-        for (int j = 0; j < kE; ++j) xs[j] += xb[j];
-      }
+      side_chain(xs, pipe, st, C, off);
     }
     {
       float run = 0.f;

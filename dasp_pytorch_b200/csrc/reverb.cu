@@ -609,8 +609,15 @@ ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, c
 }
 
 // ---- block transforms of the audio convolution on the same in-shared-memory FFT ---------------------------
-// Persistent CTAs (one per SM) walk the (item, block) list; the input of block m + 2 is bulk-copied into the free
-// half of the double buffer while block m is transformed, so the copy engine, the FFT and the epilogue stores overlap.
+// One CTA per SM at a time; the input of block m + 2 is bulk-copied into the free half of the double buffer while block
+// m is transformed, so the copy engine, the FFT and the epilogue stores overlap.  The forward's two kernels (x_fft_kernel,
+// ifft_mix_kernel) give each CTA a bounded run of kConvRun consecutive units (grid = ceil(units / kConvRun)) rather than
+// a persistent share: while the next chunk's IR synthesis holds most SMs, a CTA that lands on a freed SM gives it back
+// after about 40 us, so the synthesis clusters find whole GPCs again, and the hardware scheduler balances the tail.
+#ifndef DASP_CONV_RUN
+#define DASP_CONV_RUN 8
+#endif
+constexpr int kConvRun = DASP_CONV_RUN;
 struct FftSmem {
   float* G; float* Yr; float* Yi; float* tabf; uint64_t* full;
   __device__ __forceinline__ explicit FftSmem(float* sm) {
@@ -651,7 +658,7 @@ __device__ __forceinline__ void fft8192_in_smem(float* gr, float* gi, const FftS
   fft8k::p4<INV>(s.Yr, s.Yi, t, xr, xi);
 }
 
-// Both forward block transforms of the audio convolution, one persistent work list of nwin + items*J units:
+// Both forward block transforms of the audio convolution, one work list of nwin + items*J units (runs of kConvRun):
 //   unit m < nwin = items*I:  Xb[(il*I + i)*kNbA + f] = FFT of the window (x_left + i x_right)[(i-1) kB + m], m < kNbA
 //                             (zero outside [0, n)): x_blocks_kernel + forward C2C in one kernel.
 //   unit nwin + il*J + j:     IR partition j of item il, in place in Hb: only the first kB (left, right) pairs of the slot
@@ -667,8 +674,10 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __res
   const int t = threadIdx.x;
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int m0 = blockIdx.x * kConvRun;            // this CTA's units [m0, m1)
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
   auto fetch = [&](int it, int m) {                // all threads: zero padding; thread 0: the bulk copies
-    if (m >= nunits) return;
+    if (m >= m1) return;
     if (m >= nwin) {                               // partition: its 32 KB of taps land in the im plane, see below
       if (t == 0) {
         float* im = s.G + (it & 1) * 2 * fft8k::kPlaneG + fft8k::kPlaneG;
@@ -702,11 +711,11 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __res
       }
     }
   };
-  fetch(0, blockIdx.x);
-  fetch(1, blockIdx.x + gridDim.x);
+  fetch(0, m0);
+  fetch(1, m0 + 1);
   __syncthreads();                                 // the zero padding of the first two buffers is in place
   int it = 0;
-  for (int m = blockIdx.x; m < nunits; m += gridDim.x, ++it) {
+  for (int m = m0; m < m1; ++m, ++it) {
     mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
     float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
     float* gi = gr + fft8k::kPlaneG;
@@ -728,7 +737,7 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __res
       __syncthreads();
     }
     float xr[16], xi[16];
-    fft8192_in_smem<false>(gr, gi, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
+    fft8192_in_smem<false>(gr, gi, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
     float2* out = m < nwin ? Xb + (int64_t)m * kNbA : Hb + (int64_t)(m - nwin) * kNbA;
 #pragma unroll
     for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(xr[q], xi[q]);
@@ -746,8 +755,10 @@ ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddle
   const int t = threadIdx.x;
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int m0 = blockIdx.x * kConvRun;            // this CTA's blocks [m0, m1)
+  const int m1 = nblocks - m0 < kConvRun ? nblocks : m0 + kConvRun;
   auto fetch = [&](int it, int m) {
-    if (t != 0 || m >= nblocks) return;
+    if (t != 0 || m >= m1) return;
     uint64_t* bar = &s.full[it & 1];
     float* dst = s.G + (it & 1) * 2 * fft8k::kPlaneG;
     const float* src = Ypl + (int64_t)m * 2 * kNbA;
@@ -755,10 +766,10 @@ ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddle
 #pragma unroll
     for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
   };
-  fetch(0, blockIdx.x);
-  fetch(1, blockIdx.x + gridDim.x);
+  fetch(0, m0);
+  fetch(1, m0 + 1);
   int it = 0;
-  for (int m = blockIdx.x; m < nblocks; m += gridDim.x, ++it) {
+  for (int m = m0; m < m1; ++m, ++it) {
     mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
     float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
     float xr[16], xi[16];
@@ -768,7 +779,7 @@ ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddle
     const float* xl = x + (b * in_chs) * n;
     const float* xrr = in_chs == 1 ? xl : xl + n;
     float a0[8], a1[8];                            // the dry samples of this thread's 8 outputs
-    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); },
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2); },
                           [&] {
 #pragma unroll
                             for (int q = 0; q < 8; ++q) {
@@ -1770,18 +1781,34 @@ int get_filterbank_n1(const Geom& g, double sr, cudaStream_t st, const float2** 
   return DASP_OK;
 }
 
+// Appends a launch priority to cfg (at: its attribute array, with room for one more).  The launch then carries the
+// priority itself, so a captured graph keeps it per kernel node whatever the priority of the stream it is replayed on.
+// prio == nullptr: the stream's priority.
+void add_priority(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* at, const int* prio) {
+  if (!prio) return;
+  at[cfg.numAttrs].id = cudaLaunchAttributePriority;
+  at[cfg.numAttrs].val.priority = *prio;
+  cfg.attrs = at;
+  ++cfg.numAttrs;
+}
+
 template <int R>
 void launch_spectral(float2* C, const float2* H1, int64_t item0, int64_t items, int nb, const unsigned long long* seed,
-                     bool planar, cudaStream_t st) {
+                     bool planar, cudaStream_t st, const int* prio) {
   const int threads = 128;
-  dim3 grid((unsigned)((nb / 2 + 1 + threads - 1) / threads), kBands, (unsigned)items);
-  if (planar) spectral_gen_kernel<R, true><<<grid, threads, 0, st>>>(C, H1, item0, nb, seed);
-  else        spectral_gen_kernel<R, false><<<grid, threads, 0, st>>>(C, H1, item0, nb, seed);
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute at[1];
+  cfg.gridDim = dim3((unsigned)((nb / 2 + 1 + threads - 1) / threads), kBands, (unsigned)items);
+  cfg.blockDim = dim3(threads, 1, 1);
+  cfg.stream = st;
+  add_priority(cfg, at, prio);
+  if (planar) cudaLaunchKernelEx(&cfg, spectral_gen_kernel<R, true>, C, H1, item0, nb, seed);
+  else        cudaLaunchKernelEx(&cfg, spectral_gen_kernel<R, false>, C, H1, item0, nb, seed);
 }
 bool dispatch_spectral(int R, float2* C, const float2* H1, int64_t item0, int64_t items, int nb,
-                       const unsigned long long* seed, bool planar, cudaStream_t st) {
+                       const unsigned long long* seed, bool planar, cudaStream_t st, const int* prio) {
   switch (R) {
-#define DASP_R(r) case r: launch_spectral<r>(C, H1, item0, items, nb, seed, planar, st); return true;
+#define DASP_R(r) case r: launch_spectral<r>(C, H1, item0, items, nb, seed, planar, st, prio); return true;
     DASP_R(1) DASP_R(2) DASP_R(3) DASP_R(4) DASP_R(5) DASP_R(6) DASP_R(7) DASP_R(8) DASP_R(9) DASP_R(10)
     DASP_R(11) DASP_R(12) DASP_R(13) DASP_R(14) DASP_R(15) DASP_R(16)
 #undef DASP_R
@@ -1815,14 +1842,45 @@ int get_fft_tables(cudaStream_t st, const float** out) {
   *out = it->second;
   return DASP_OK;
 }
+// Side streams of the forward's IR synthesis (see dasp_reverb_fwd), created once per device at the greatest stream
+// priority.  fork is recorded on the caller's stream before the first synthesis, done[k % 2] after chunk k's synthesis
+// on side[k % 2].  Reusing the events across chunks and calls is safe: cudaStreamWaitEvent takes the state of the
+// event at the time of the call, and a later record does not change what an earlier wait waits for.
+struct SideStreams { cudaStream_t side[2]; cudaEvent_t fork, done[2]; int prio; };
+std::map<int, SideStreams> g_side;                  // guarded by g_mu
+int get_side_streams(SideStreams** out) {
+  int dev = 0;
+  DASP_CUDA_OK(cudaGetDevice(&dev));
+  auto it = g_side.find(dev);
+  if (it == g_side.end()) {
+    SideStreams s{};
+    int least = 0;
+    DASP_CUDA_OK(cudaDeviceGetStreamPriorityRange(&least, &s.prio));
+    for (int i = 0; i < 2; ++i) {
+      DASP_CUDA_OK(cudaStreamCreateWithPriority(&s.side[i], cudaStreamNonBlocking, s.prio));
+      DASP_CUDA_OK(cudaEventCreateWithFlags(&s.done[i], cudaEventDisableTiming));
+    }
+    DASP_CUDA_OK(cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming));
+    it = g_side.emplace(dev, s).first;
+  }
+  *out = &it->second;
+  return DASP_OK;
+}
+
 int configure_fft_kernels();
 int launch_ifft_shape(float2* C, const float* tw, const float* params, float2* hs, bool save_f, int64_t items,
-                      const Geom& g, int jb, cudaStream_t st) {
+                      const Geom& g, int jb, cudaStream_t st, const int* prio) {
   int rc = configure_fft_kernels();
   if (rc != DASP_OK) return rc;
-  const size_t smem = kFftSmemBytes;
-  ifft_shape_kernel<<<dim3((unsigned)g.rpp, (unsigned)items), kFusedThreads, smem, st>>>(
-      reinterpret_cast<float*>(C), tw, params, hs, save_f ? 1 : 0, (int)g.L, (int)g.leff, jb, (int)g.rpp);
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute at[1];
+  cfg.gridDim = dim3((unsigned)g.rpp, (unsigned)items, 1);
+  cfg.blockDim = dim3(kFusedThreads, 1, 1);
+  cfg.dynamicSmemBytes = kFftSmemBytes;
+  cfg.stream = st;
+  add_priority(cfg, at, prio);
+  cudaLaunchKernelEx(&cfg, ifft_shape_kernel, reinterpret_cast<float*>(C), tw, params, hs, save_f ? 1 : 0, (int)g.L,
+                     (int)g.leff, jb, (int)g.rpp);
   DASP_LAUNCH_OK("ifft_shape_kernel");
   return DASP_OK;
 }
@@ -1833,13 +1891,13 @@ std::map<std::pair<int, int>, int> g_fused_ok;      // (device, R) -> clusters t
 // a launch attempt (check cudaGetLastError).
 template <int R>
 bool launch_fused(const float2* H1, const float* tw, const float* params, float2* hs, float2* Csave, int64_t item0, int64_t items,
-                  int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st) {
+                  int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st, const int* prio) {
   auto kern = ir_synth_cluster_kernel<R>;
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(kSynthThreads, 1, 1);
   cfg.dynamicSmemBytes = kSynthSmemBytes;
   cfg.stream = st;
-  cudaLaunchAttribute at[1];
+  cudaLaunchAttribute at[2];
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = R; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at;
@@ -1860,13 +1918,15 @@ bool launch_fused(const float2* H1, const float* tw, const float* params, float2
   if (it->second < 1) return false;
   const int64_t clusters = items < it->second ? items : it->second;
   cfg.gridDim = dim3(R, (unsigned)clusters, 1);
+  add_priority(cfg, at, prio);
   cudaLaunchKernelEx(&cfg, kern, H1, tw, params, hs, Csave, item0, (int)items, (int)L, (int)leff, jb, seed);
   return true;
 }
 bool dispatch_fused(int R, const float2* H1, const float* tw, const float* params, float2* hs, float2* Csave, int64_t item0,
-                    int64_t items, int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st) {
+                    int64_t items, int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st,
+                    const int* prio) {
   switch (R) {
-#define DASP_R(r) case r: return launch_fused<r>(H1, tw, params, hs, Csave, item0, items, L, leff, jb, seed, st);
+#define DASP_R(r) case r: return launch_fused<r>(H1, tw, params, hs, Csave, item0, items, L, leff, jb, seed, st, prio);
     DASP_R(1) DASP_R(2) DASP_R(3) DASP_R(4) DASP_R(5) DASP_R(6)
 #undef DASP_R
     default: return false;
@@ -2019,14 +2079,12 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
     if (rc != DASP_OK) return rc;
     // one work list: the items*I audio windows, then the items*J IR partitions (transformed in place in hs)
     const int nunits = (int)(items * (I + J));
-    const unsigned xh_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-    x_fft_kernel<<<xh_grid, kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nblk,
+    x_fft_kernel<<<(unsigned)((nunits + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nblk,
                                                                 nunits);
     DASP_LAUNCH_OK("x_fft_kernel");
     launch_mac<false, true>(xs, hs, ys, I, J, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
-    const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-    ifft_mix_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
+    ifft_mix_kernel<<<(unsigned)((nblk + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
                                                                    mix_stride, y, item0, I, g.n, in_chs, nblk);
     DASP_LAUNCH_OK("ifft_mix_kernel");
     return DASP_OK;
@@ -2121,6 +2179,14 @@ void reverb_shutdown() {
   g_fb.clear();
   for (auto& kv : g_fft_tab) cudaFree(kv.second);
   g_fft_tab.clear();
+  for (auto& kv : g_side) {
+    for (int i = 0; i < 2; ++i) {
+      cudaStreamDestroy(kv.second.side[i]);
+      cudaEventDestroy(kv.second.done[i]);
+    }
+    cudaEventDestroy(kv.second.fork);
+  }
+  g_side.clear();
 }
 
 }  // namespace dasp
@@ -2180,9 +2246,37 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
   const int64_t lp = g.L + g.P;
   const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P, I = (int)g.ib, J = (int)g.jb;
 
-  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+  // device-noise IR synthesis (every variant draws the same Philox stream; the two own-FFT ones are bit-identical):
+  //   default, nb == 8192: ir_synth_cluster_kernel for R <= 6, generator -> ifft_shape_kernel for 7 <= R <= 16 or
+  //     when the device cannot co-schedule the cluster (last path 2);
+  //   dasp_debug_reverb_path(2), R <= 8: generator -> ifft_shape_kernel (last path 1);
+  //   dasp_debug_reverb_path(1), and any other nb: generator -> batched cuFFT -> shape_ir_pp_kernel (last path 0).
+  int synth = 0;
+  const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
+  const bool two_kernel_hook = debug_reverb_path() == 2 && g.rpp <= kMaxHookR;
+  if (own_fft && debug_reverb_path() != 1) synth = two_kernel_hook ? 1 : 2;
+  g_last_fused = synth;
+  // Pipeline: chunk k + 1's synthesis runs on a side stream while chunk k's convolution runs on st.  The synthesis holds
+  // only the SMs its clusters fit on (17 clusters of 6 = 102 of 132 on an H100 SXM), the convolution fills the rest.
+  // Chunk k's synthesis goes to side[k % 2] (the next chunk's clusters are queued behind the running ones and take each
+  // slot as it frees), at the greatest priority so that pending clusters are dispatched before convolution CTAs, and
+  // st waits for it before chunk k's convolution; the last of these waits joins every side-stream launch back into st,
+  // so nothing outlives the call, and under stream capture the fork and join are graph edges.  This needs the chunks'
+  // slots disjoint: the synthesis writes only f_save / irspec_save slots (kept when a backward follows; otherwise they
+  // share one workspace slot), and neither side uses the shared cuFFT work area (own-FFT synthesis and convolution).
+  const bool pipelined = synth != 0 && f_save && irspec_save && own_fft_rows(n, x, irspec_save);
+  SideStreams* side = nullptr;
+  if (pipelined) {
+    if ((rc = get_side_streams(&side)) != DASP_OK) return rc;
+    DASP_CUDA_OK(cudaEventRecord(side->fork, st));   // the seed word and the parameters are written on st
+    for (int i = 0; i < 2; ++i) DASP_CUDA_OK(cudaStreamWaitEvent(side->side[i], side->fork, 0));
+  }
+  const int* prio = pipelined ? &side->prio : nullptr;
+
+  for (int64_t item0 = 0, k = 0; item0 < bs; item0 += g.chunk, ++k) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? s.full : s.rem;
+    const cudaStream_t sst = pipelined ? side->side[k & 1] : st;      // the stream of this chunk's synthesis
     // kept for the backward when the caller passes *_save buffers, transient workspace otherwise
     float2* C = f_save ? reinterpret_cast<float2*>(f_save) + item0 * kBands * g.pair_c64()
                        : reinterpret_cast<float2*>(base + w.extra);
@@ -2195,32 +2289,23 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     // x_fft_kernel reads nothing else of hs; the cuFFT transform of the partitions reads whole slots, so they are
     // zero-filled first
     if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
-    // device-noise IR synthesis (every variant draws the same Philox stream; the two own-FFT ones are bit-identical):
-    //   default, nb == 8192: ir_synth_cluster_kernel for R <= 6, generator -> ifft_shape_kernel for 7 <= R <= 16 or
-    //     when the device cannot co-schedule the cluster (last path 2);
-    //   dasp_debug_reverb_path(2), R <= 8: generator -> ifft_shape_kernel (last path 1);
-    //   dasp_debug_reverb_path(1), and any other nb: generator -> batched cuFFT -> shape_ir_pp_kernel (last path 0).
-    int synth = 0;
-    const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
-    const bool two_kernel_hook = debug_reverb_path() == 2 && g.rpp <= kMaxHookR;
-    if (own_fft && debug_reverb_path() != 1) synth = two_kernel_hook ? 1 : 2;
     const float* tw = nullptr;
     if ((synth != 0 || own_conv) && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    g_last_fused = synth;
     bool clustered = false;
     if (synth == 2 && g.rpp <= kMaxClusterR) {
       clustered = dispatch_fused((int)g.rpp, H1, tw, params + item0 * 25, hs, f_save ? C : nullptr, item0, items, g.L,
-                                 g.leff, J, seed, st);
+                                 g.leff, J, seed, sst, prio);
       if (clustered) DASP_LAUNCH_OK("ir_synth_cluster_kernel");
     }
     if (clustered) {
     } else if (synth != 0) {
-      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, st);
+      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, sst, prio);
       DASP_LAUNCH_OK("spectral_gen_kernel");
-      if ((rc = launch_ifft_shape(C, tw, params + item0 * 25, hs, f_save != nullptr, items, g, J, st)) != DASP_OK) return rc;
+      if ((rc = launch_ifft_shape(C, tw, params + item0 * 25, hs, f_save != nullptr, items, g, J, sst, prio)) != DASP_OK)
+        return rc;
     } else if (spectral) {
       // device noise: draw the filtered spectrum directly, one inverse transform (polyphase layout)
-      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st);
+      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st, nullptr);
       DASP_LAUNCH_OK("spectral_gen_kernel");
       DASP_CUFFT_OK(cufftSetStream(pl.pp.h, st));
       DASP_CUFFT_OK(cufftSetWorkArea(pl.pp.h, ws_cufft));
@@ -2242,6 +2327,10 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       shape_ir_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, params + item0 * 25, hs, g.L, g.leff,
                                                                                J, nbk, nb, hop, P);
       DASP_LAUNCH_OK("shape_ir_pairs_kernel");
+    }
+    if (pipelined) {
+      DASP_CUDA_OK(cudaEventRecord(side->done[k & 1], sst));
+      DASP_CUDA_OK(cudaStreamWaitEvent(st, side->done[k & 1], 0));
     }
     if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, params + 24, 25, y, base, w, item0, items,
                              st)) != DASP_OK)

@@ -536,7 +536,10 @@ import os as _os
 # Items per pass of the reverb pipeline (bounds the workspace).  Default: two items per SM of the device, so that the
 # one-CTA-per-SM FFT kernels run in whole waves (ifft_shape_kernel: R CTAs per item -> exactly 2 R waves; the persistent
 # block-transform kernels: the same number of blocks per CTA).  Measured on one H100 SXM (400 W), chain step at batch
-# 1024: 66 items 23.4 ms, 132 items 22.5 ms, 264 items 22.1 ms.  Override for experiments with DASP_REVERB_CHUNK.
+# 1024: 66 items 23.4 ms, 132 items 22.5 ms, 264 items 22.1 ms.  With the forward's convolution of chunk k overlapping
+# the IR synthesis of chunk k + 1 (smaller chunks would shorten the convolution left after the last synthesis), two
+# runs each on an H100 80GB HBM3 at a 400 W limit: 132 items 20.26 / 20.52 ms (reverb_bwd 5.30 / 5.33 ms), 264 items
+# 19.99 / 18.94 ms (reverb_bwd 5.11 / 5.12 ms).  Override for experiments with DASP_REVERB_CHUNK.
 REVERB_CHUNK_ITEMS = int(_os.environ.get("DASP_REVERB_CHUNK", "0"))      # 0 = automatic
 
 

@@ -13,8 +13,13 @@
  *     tensor contract (README.md:38);
  *   - `stream` is a cudaStream_t; all work is enqueued on it, nothing synchronises -- with ONE documented
  *     exception: the first call on a device for a new (taps, sample_rate, geometry) builds library-owned caches
- *     (cuFFT plans, filter-bank spectra, FFT twiddle tables: cudaMalloc + one cudaStreamSynchronize).  Warm the
- *     shapes up once before capturing a CUDA graph; later calls are pure enqueues;
+ *     (cuFFT plans, filter-bank spectra, FFT twiddle tables: cudaMalloc + one cudaStreamSynchronize; for the
+ *     reverb forward also two side streams at the greatest priority and three events).  Warm the shapes up once
+ *     before capturing a CUDA graph -- the first call should not be under capture; later calls are pure enqueues.
+ *     dasp_reverb_fwd with f_save and irspec_save (a backward follows) runs each chunk's IR synthesis on those side
+ *     streams, forked from `stream` by an event recorded on it at the start of the call and joined back into it
+ *     before the call returns (event waits, which stream capture turns into graph edges), so the caller still sees
+ *     one stream;
  *   - return value 0 = ok, negative = error (see DASP_ERR_*); the message is available
  *     from dasp_last_error() (thread-local).  No exception crosses this boundary;
  *   - reentrant from several host threads as long as they use distinct streams.

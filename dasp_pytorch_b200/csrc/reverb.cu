@@ -32,7 +32,8 @@
 // convolution_reverberation is the audio convolution with the caller's IR (ir_pack_kernel fills the partitions).  The
 // convolution is written once on the host: conv_fwd_chunk / conv_bwd_chunk run a chunk for both ops, on one ConvGeom,
 // one plan set (conv_setup) and one workspace layout per direction; each op adds only its IR fill, its mix stride and
-// its dL/dIR consumer.
+// its dL/dIR consumer.  One IR for the whole batch (dasp_conv_shared_*) is the item stride 0 of the IR spectra: they
+// are transformed once, and irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.
 #include <cufft.h>
 #include <curand_kernel.h>
 #include <math.h>
@@ -112,6 +113,7 @@ struct ConvGeom {
   int64_t leff;                 // min(L, n): the only IR taps that can reach the output
   int64_t ib, jb;               // output/input blocks of kB samples, IR partitions of kB taps
   int64_t chunk;
+  bool shared = false;          // one impulse response for the whole batch (convolution_reverberation only)
 };
 
 int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
@@ -1349,7 +1351,8 @@ __device__ __forceinline__ void cfma_conj(float2& acc, float2 p, float2 q) {    
 
 // CORR == false: out[o] = sum_{j<nbm, j<=o} A[o-j] B[j]           (o < nout)      forward
 // CORR == true : out[o] = sum_{j<nbm, o+j<na} A[o+j] conj(B[j])   (o < nout)      both backward products
-// A: [items][na][kNbA], Bm: [items][nbm][kNbA], Out: [items][nout][kNbA]; per channel, packed spectra.
+// A: [items][na][kNbA], Bm: [items][nbm][kNbA] (bstep 1) or [nbm][kNbA] read by every item (bstep 0: the spectra of an
+// IR shared by the batch), Out: [items][nout][kNbA]; per channel, packed spectra.
 // grid = (ceil((kNbA/2+1)/128), items); thread = frequency pair (f, kNbA - f).  MAXB > 0: operands cached
 // in registers (na, nbm <= MAXB); MAXB == 0: generic loop straight from L2.
 // PLANAR: every output block is stored as [re plane kNbA][im plane kNbA] (what ifft_mix_kernel bulk-copies into the
@@ -1357,13 +1360,13 @@ __device__ __forceinline__ void cfma_conj(float2& acc, float2 p, float2 q) {    
 template <int MAXB, bool CORR, bool PLANAR = false>
 __global__ void __launch_bounds__(128) partition_mac_kernel(const float2* __restrict__ A, const float2* __restrict__ Bm,
                                                             float2* __restrict__ Out, int na, int nbm, int nout,
-                                                            float scale) {
+                                                            float scale, int bstep) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f > kNbA / 2) return;
   const int fm = (kNbA - f) & (kNbA - 1);
   const int64_t il = blockIdx.y;
   const float2* a = A + il * (int64_t)na * kNbA;
-  const float2* bq = Bm + il * (int64_t)nbm * kNbA;
+  const float2* bq = Bm + (il * bstep) * (int64_t)nbm * kNbA;
   float2* out = Out + il * (int64_t)nout * kNbA;
   auto emit = [&](int o, float2 sl, float2 sr) {
     sl.x *= scale; sl.y *= scale; sr.x *= scale; sr.y *= scale;
@@ -1420,10 +1423,12 @@ __global__ void __launch_bounds__(128) partition_mac_kernel(const float2* __rest
 //   D[q] = sum_{j<J, q+j<I} G[q+j] conj(H[j])  (q < I)   dL/dx windows
 //   E[j] = sum_{p<I, j+p<I} G[j+p] conj(X[p])  (j < J)   dL/dIR partitions
 // G is read and untangled once; H and X take turns in the same registers.  Planar outputs (own inverse FFT kernels).
+// H's item stride is hstride (J kNbA, or 0 for IR spectra shared by the batch).
 template <int MAXB>
 __global__ void __launch_bounds__(128) partition_mac_bwd_kernel(const float2* __restrict__ G, const float2* __restrict__ H,
-                                                                const float2* __restrict__ X, float2* __restrict__ D,
-                                                                float2* __restrict__ E, int I, int J, float scale) {
+                                                                int64_t hstride, const float2* __restrict__ X,
+                                                                float2* __restrict__ D, float2* __restrict__ E, int I,
+                                                                int J, float scale) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f > kNbA / 2) return;
   const int fm = (kNbA - f) & (kNbA - 1);
@@ -1437,7 +1442,7 @@ __global__ void __launch_bounds__(128) partition_mac_bwd_kernel(const float2* __
   }
 #pragma unroll
   for (int pass = 0; pass < 2; ++pass) {
-    const float2* bq = (pass == 0 ? H + il * (int64_t)J * kNbA : X + il * (int64_t)I * kNbA);
+    const float2* bq = (pass == 0 ? H + il * hstride : X + il * (int64_t)I * kNbA);
     const int nbm = pass == 0 ? J : I, nout = pass == 0 ? I : J;
     float2* out = (pass == 0 ? D + il * (int64_t)I * kNbA : E + il * (int64_t)J * kNbA);
 #pragma unroll
@@ -1621,7 +1626,8 @@ __global__ void ir_pack_kernel(const float* __restrict__ ir, float2* __restrict_
 }
 
 // unit m = il*J + j: dL/dIR taps [j kB, (j+1) kB) ∩ [0, leff) = mix * first half of IFFT(Epl[m]) (left, right), written
-// straight into the caller's (bs, ir_chs, L) rows; a mono IR receives the sum of both channels
+// straight into the caller's (bs, ir_chs, L) rows; a mono IR receives the sum of both channels.  A null mix is a factor
+// of 1 (a shared IR's summed partitions carry their factors already).
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twiddles, const float* __restrict__ mix,
                    float* __restrict__ gir, int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int nunits) {
@@ -1649,7 +1655,7 @@ ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
     const int j = m - (int)il * J;
     float xr[16], xi[16];
     fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
-    const float mx = mix[b];
+    const float mx = mix ? mix[b] : 1.0f;
     float* row = gir + (b * ir_chs) * L;
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
@@ -1663,8 +1669,8 @@ ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
 }
 
 // dL/dIR taps [t0, L) of the caller's rows: mix * Et (inverse-transformed partitions, pairs in the first half of each
-// slot) below leff, 0 from leff on (those taps cannot reach an output).  t0 = leff writes only the zeros.
-// grid = (ceil((L - t0) / 256), items)
+// slot) below leff, 0 from leff on (those taps cannot reach an output).  t0 = leff writes only the zeros.  A null mix is
+// a factor of 1.  grid = (ceil((L - t0) / 256), items)
 __global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float* __restrict__ mix, float* __restrict__ gir,
                                      int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int64_t t0) {
   const int64_t t = t0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1674,11 +1680,43 @@ __global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float*
   float mx = 0.f;
   if (t < leff) {
     v = Et[(il * J + t / kB) * (int64_t)kNbA + t % kB];
-    mx = mix[b];
+    mx = mix ? mix[b] : 1.f;
   }
   float* row = gir + (b * ir_chs) * L;
   if (ir_chs == 1) row[t] = mx * (v.x + v.y);
   else { row[t] = mx * v.x; row[L + t] = mx * v.y; }
+}
+
+// dL/dIR of one impulse response shared by the batch: the sum over items b of mix[b] E_b, taken on the partition spectra
+// E_b of the es region before any inverse transform (the inverse is linear).  Element by element in fp64 and in absolute
+// item order: a product of two floats is exact in fp64, so every element goes through the same sequence of additions
+// however the batch is cut into chunks, and the result is the same bits for every chunk size.  Item 0 writes acc instead
+// of adding to it (the workspace is never cleared); the chunk that holds the last item writes the sum, rounded to fp32,
+// over item 0's slot of Et instead, for the inverse transforms (thread e alone reads and writes element e of every slot).
+// Element-wise, so it serves the planar (own FFT) and the interleaved (cuFFT) spectra alike.
+// grid = ceil(J kNbA / 256), one complex element of the J partitions per thread
+__global__ void irgrad_sum_kernel(float2* Et, const float* __restrict__ mix, double2* __restrict__ acc, int64_t item0,
+                                  int items, int64_t per_item, bool last) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= per_item) return;
+  double2 a = make_double2(0.0, 0.0);
+  int il = 0;
+  if (item0 != 0) {
+    a = acc[e];
+  } else {                                         // item 0: written, not added
+    const float2 v = Et[e];
+    const double m = (double)mix[0];
+    a = make_double2(m * (double)v.x, m * (double)v.y);
+    il = 1;
+  }
+  for (; il < items; ++il) {
+    const float2 v = Et[il * per_item + e];
+    const double m = (double)mix[item0 + il];
+    a.x += m * (double)v.x;
+    a.y += m * (double)v.y;
+  }
+  if (last) Et[e] = make_float2((float)a.x, (float)a.y);
+  else acc[e] = a;
 }
 
 // dL/dmix per item: the per-block partials of ifft_dx_kernel / finish_dx_blocks_kernel summed in block order, in fp64
@@ -1936,16 +1974,17 @@ bool dispatch_fused(int R, const float2* H1, const float* tw, const float* param
 inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // workspace carve-up shared by the geometry queries and the entry points; extra: the reverb's own region (the filtered
-// noise of a chunk when f_save is not kept / the per-partition partials of the 24 band-parameter gradients)
+// noise of a chunk when f_save is not kept / the per-partition partials of the 24 band-parameter gradients); acc: the
+// fp64 sum of a shared IR's dL/dIR partition spectra (0 bytes unless g.shared)
 struct FwdWs { size_t ys, xsp, hsp, extra, cufft, total; };
-struct BwdWs { size_t gs, ds, es, extra, mixpart, cufft, total; };
+struct BwdWs { size_t gs, ds, es, extra, mixpart, acc, cufft, total; };
 
 void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs& w) {
   size_t o = 0;
   w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   // transient homes for what a forward WITHOUT a backward does not keep (null *_save pointers)
   w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.hsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
+  w.hsp = o; o += align256(sizeof(float2) * (size_t)((g.shared ? 1 : g.chunk) * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
@@ -1957,6 +1996,7 @@ void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs&
   w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.mixpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * g.ib));
+  w.acc = o; o += align256(g.shared ? sizeof(double2) * (size_t)(g.jb * kNbA) : 0);
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
 }
@@ -1964,12 +2004,16 @@ void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs&
 // cuFFT plans for a full chunk and for the remainder (none without a batch), and both workspace layouts around their
 // largest work area.  xi / hj: the block transforms of the convolution's cuFFT pipeline (audio / dL/dx windows, IR /
 // dL/dIR partitions).  With synth (the reverb) also blk / pp, its IR synthesis (overlap-save blocks, polyphase), and
-// the extra regions.
+// the extra regions.  With g.shared also ir1: the J partitions of the one IR (forward) and of its summed gradient.
 struct Plans { PlanVal xi, hj, blk, pp; };
-struct Setup { Plans full, rem; FwdWs fwd; BwdWs bwd; };
+struct Setup { Plans full, rem; PlanVal ir1; FwdWs fwd; BwdWs bwd; };
 int conv_setup(const ConvGeom& g, const Geom* synth, Setup& s) {
   int rc;
   size_t work = 0;
+  if (g.shared && g.bs > 0) {
+    if ((rc = get_plan(2, kNbA, g.jb, kNbA, kNbA, s.ir1)) != DASP_OK) return rc;
+    work = s.ir1.work;
+  }
   for (int64_t items : {g.bs > 0 ? g.chunk : 0, g.bs % g.chunk}) {
     if (items == 0) continue;
     Plans& p = items == g.chunk ? s.full : s.rem;
@@ -2012,7 +2056,7 @@ int put_conv_geometry(const ConvGeom& g, const Geom* synth, Out* out) {
   if (rc != DASP_OK) return rc;
   out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
   out->xspec_c64 = g.bs * g.ib * kNbA;
-  out->irspec_c64 = g.bs * g.jb * kNbA;
+  out->irspec_c64 = (g.shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.jb * kNbA;
   out->fwd_workspace_bytes = (int64_t)s.fwd.total;
   out->bwd_workspace_bytes = (int64_t)s.bwd.total;
   return DASP_OK;
@@ -2020,13 +2064,13 @@ int put_conv_geometry(const ConvGeom& g, const Geom* synth, Out* out) {
 
 // out = conv / corr of packed block spectra, register-cached when both operands have <= 16 blocks
 template <bool CORR, bool PLANAR = false>
-void launch_mac(const float2* A, const float2* Bm, float2* Out, int na, int nbm, int nout, int64_t items, float scale,
-                cudaStream_t st) {
+void launch_mac(const float2* A, const float2* Bm, float2* Out, int na, int nbm, int bstep, int nout,
+                int64_t items, float scale, cudaStream_t st) {
   dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
   const int m = na > nbm ? na : nbm;
-  if (m <= 12)      partition_mac_kernel<12, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale);
-  else if (m <= 16) partition_mac_kernel<16, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale);
-  else              partition_mac_kernel<0, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale);
+  if (m <= 12)      partition_mac_kernel<12, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
+  else if (m <= 16) partition_mac_kernel<16, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
+  else              partition_mac_kernel<0, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
 }
 
 // one-off opt-in to the large dynamic shared memory of the FFT kernels (per device, guarded by g_mu)
@@ -2060,17 +2104,38 @@ enum class IrGrad {
   kNone,     // nothing (a fixed impulse response)
   kPlanar,   // partition spectra, planar, for an own-FFT inverse (own path only)
   kTime,     // partitions after the inverse cuFFT C2C: (left, right) pairs in the first half of each slot
+  kSpectra,  // partition spectra as (re, im) pairs, summed over a shared IR's items before the inverse cuFFT
 };
 // both correlations in one pass over the gradient spectra when the operands fit the register cache
 bool fused_corr(IrGrad e, int I, int J) { return e == IrGrad::kPlanar && (I > J ? I : J) <= 16; }
 
+// The partitions of an impulse response shared by the batch, transformed in place in hs once before the first chunk,
+// filled as conv_fwd_chunk expects them; own: x_fft_kernel with no audio windows, otherwise the J-batch cuFFT C2C.
+int conv_shared_ir_spectra(const ConvGeom& g, const PlanVal& ir1, bool own, const float* tw, float2* hs,
+                           unsigned char* ws, const FwdWs& w, cudaStream_t st) {
+  const int J = (int)g.jb;
+  if (own) {
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    x_fft_kernel<<<(unsigned)((J + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
+        nullptr, nullptr, hs, tw, 0, (int)g.ib, J, g.n, g.leff, 1, 0, J);
+    DASP_LAUNCH_OK("x_fft_kernel");
+    return DASP_OK;
+  }
+  DASP_CUFFT_OK(cufftSetStream(ir1.h, st));
+  DASP_CUFFT_OK(cufftSetWorkArea(ir1.h, ws + w.cufft));
+  DASP_CUFFT_OK(cufftExecC2C(ir1.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
+  return DASP_OK;
+}
+
 // y = (1 - mix) x + mix (x * IR), mix of item b at mix[b * mix_stride].  The caller has written IR taps t < leff as
 // (left, right) pairs into the first half of partition slot t / kB of hs, and on the cuFFT pipeline zero-filled the
 // slots first.  xs / hs receive the window / partition spectra.  own (own_fft_rows of x and hs): x_fft_kernel transforms
-// both on the own FFT with the tables tw; otherwise cuFFT C2C does.
+// both on the own FFT with the tables tw; otherwise cuFFT C2C does.  h_stride: item stride of hs in complex elements,
+// J kNbA; 0 for one IR shared by the batch, whose partitions conv_shared_ir_spectra has transformed already.
 int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, int in_chs, float2* xs,
-                   float2* hs, const float* mix, int mix_stride, float* y, unsigned char* ws, const FwdWs& w,
-                   int64_t item0, int64_t items, cudaStream_t st) {
+                   float2* hs, int64_t h_stride, const float* mix, int mix_stride, float* y, unsigned char* ws,
+                   const FwdWs& w, int64_t item0, int64_t items, cudaStream_t st) {
   float2* ys = (float2*)(ws + w.ys);
   const int I = (int)g.ib, J = (int)g.jb;
   const int nblk = (int)(items * I);
@@ -2078,11 +2143,11 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
     int rc = configure_fft_kernels();
     if (rc != DASP_OK) return rc;
     // one work list: the items*I audio windows, then the items*J IR partitions (transformed in place in hs)
-    const int nunits = (int)(items * (I + J));
+    const int nunits = (int)(items * (I + (h_stride != 0 ? J : 0)));
     x_fft_kernel<<<(unsigned)((nunits + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nblk,
                                                                 nunits);
     DASP_LAUNCH_OK("x_fft_kernel");
-    launch_mac<false, true>(xs, hs, ys, I, J, I, items, 1.0f / (float)kNbA, st);
+    launch_mac<false, true>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
     ifft_mix_kernel<<<(unsigned)((nblk + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
                                                                    mix_stride, y, item0, I, g.n, in_chs, nblk);
@@ -2090,15 +2155,17 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
     return DASP_OK;
   }
   void* cufft = ws + w.cufft;
-  DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
-  DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
-  DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
+  if (h_stride != 0) {
+    DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
+    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
+    DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
+  }
   x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, g.n, in_chs);
   DASP_LAUNCH_OK("x_blocks_kernel");
   DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
   DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, cufft));
   DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)xs, (cufftComplex*)xs, CUFFT_FORWARD));
-  launch_mac<false>(xs, hs, ys, I, J, I, items, 1.0f / (float)kNbA, st);
+  launch_mac<false>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
   DASP_LAUNCH_OK("partition_mac_kernel");
   DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ys, (cufftComplex*)ys, CUFFT_INVERSE));
   mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ys, mix, mix_stride, y, item0, I, g.n, in_chs);
@@ -2111,9 +2178,11 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
 // E[j] = sum_p G[j+p] conj(X[p]) in the es region, in the form e (kPlanar needs own).  own (own_fft_rows of gy): the G
 // transform and ifft_dx_kernel on the own FFT with the tables tw; otherwise the cuFFT pipeline.  Unfused, the dL/dIR
 // correlation runs after the dL/dx inverse (the two correlations read the same inputs and write disjoint regions).
+// h_stride: item stride of hs as in conv_fwd_chunk (0: one IR shared by the batch).
 int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const float* tw, const float* gy,
-                   const float* x, int in_chs, const float2* xs, const float2* hs, const float* mix, int mix_stride,
-                   float* gx, unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) {
+                   const float* x, int in_chs, const float2* xs, const float2* hs, int64_t h_stride, const float* mix,
+                   int mix_stride, float* gx, unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items,
+                   cudaStream_t st) {
   float2* gs = (float2*)(ws + w.gs);
   float2* ds = (float2*)(ws + w.ds);
   float2* es = (float2*)(ws + w.es);
@@ -2131,11 +2200,11 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     DASP_LAUNCH_OK("g_fft_kernel");
     if (fused) {
       dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
-      if ((I > J ? I : J) <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(gs, hs, xs, ds, es, I, J, inv);
-      else                       partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(gs, hs, xs, ds, es, I, J, inv);
+      if ((I > J ? I : J) <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
+      else                       partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
       DASP_LAUNCH_OK("partition_mac_bwd_kernel");
     } else {
-      launch_mac<true, true>(gs, hs, ds, I, J, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
+      launch_mac<true, true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
       DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     }
     const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
@@ -2149,7 +2218,7 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
     DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, cufft));
     DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)gs, (cufftComplex*)gs, CUFFT_FORWARD));
-    launch_mac<true>(gs, hs, ds, I, J, I, items, inv, st);
+    launch_mac<true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ds, (cufftComplex*)ds, CUFFT_INVERSE));
     finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ds, mix, mix_stride, gx, mixpart,
@@ -2157,11 +2226,12 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     DASP_LAUNCH_OK("finish_dx_blocks_kernel");
   }
   if (e == IrGrad::kPlanar && !fused) {
-    launch_mac<true, true>(gs, xs, es, I, I, J, items, inv, st);        // dIR partitions: sum_p conj(X[p]) G[j+p]
+    launch_mac<true, true>(gs, xs, es, I, I, 1, J, items, inv, st);        // dIR partitions: sum_p conj(X[p]) G[j+p]
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-  } else if (e == IrGrad::kTime) {
-    launch_mac<true>(gs, xs, es, I, I, J, items, inv, st);
+  } else if (e == IrGrad::kTime || e == IrGrad::kSpectra) {
+    launch_mac<true>(gs, xs, es, I, I, 1, J, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
+    if (e == IrGrad::kSpectra) return DASP_OK;
     DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
     DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
     DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)es, (cufftComplex*)es, CUFFT_INVERSE));
@@ -2332,8 +2402,8 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       DASP_CUDA_OK(cudaEventRecord(side->done[k & 1], sst));
       DASP_CUDA_OK(cudaStreamWaitEvent(st, side->done[k & 1], 0));
     }
-    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, params + 24, 25, y, base, w, item0, items,
-                             st)) != DASP_OK)
+    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, J * (int64_t)kNbA, params + 24, 25, y, base,
+                             w, item0, items, st)) != DASP_OK)
       return rc;
   }
   return DASP_OK;
@@ -2376,7 +2446,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
     const float* tw = nullptr;
     if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
     if ((rc = conv_bwd_chunk(g, pl, own_conv, own_irgrad ? IrGrad::kPlanar : IrGrad::kTime, tw, gy, x, (int)in_chs, xs,
-                             hs, params + 24, 25, gx, base, w, item0, items, st)) != DASP_OK)
+                             hs, J * (int64_t)kNbA, params + 24, 25, gx, base, w, item0, items, st)) != DASP_OK)
       return rc;
     int nparts;
     if (own_irgrad) {
@@ -2408,25 +2478,28 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
 
 // ------------------------------------------------------------------ convolution_reverberation
 namespace {
-int g_conv_last_path[2] = {0, 0};                    // test hook: dispatch of the last dasp_conv_fwd / dasp_conv_bwd
-}  // namespace
+int g_conv_last_path[2] = {0, 0};                    // test hook: dispatch of the last conv forward / backward
 
-int dasp_debug_conv_last_path(int which) { return g_conv_last_path[which ? 1 : 0]; }
-
-int dasp_conv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+// The bodies of dasp_conv_* (one IR per item) and dasp_conv_shared_* (one IR for the whole batch).  Shared, the IR's
+// partitions are filled and transformed once before the first chunk and every item reads the same spectra (item stride
+// 0); the backward sums mix[b] times each item's dL/dIR partition spectra in fp64 (irgrad_sum_kernel) and transforms
+// the sum once after the last chunk.
+int conv_op_geometry(bool shared, int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
   DASP_REQUIRE(out != nullptr, "conv geometry: null out");
   ConvGeom g;
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
+  g.shared = shared;
   return put_conv_geometry(g, nullptr, out);
 }
 
-int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, const float* mix,
-                  float* y, void* xspec_save, void* irspec_save, void* workspace, int64_t workspace_bytes, int64_t bs,
-                  int64_t n, int64_t chunk_items, void* stream) {
+int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,
+                const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
   ConvGeom g;
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
+  g.shared = shared;
   DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2), "conv: only mono/stereo signals and IRs");
   if (bs == 0) return DASP_OK;
   DASP_REQUIRE(x && ir && mix && y && workspace, "conv fwd: null pointer");
@@ -2439,34 +2512,48 @@ int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_ch
   const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
   const int I = (int)g.ib, J = (int)g.jb;
+  const int64_t h_stride = shared ? 0 : J * (int64_t)kNbA;
+  float2* const hs0 = irspec_save ? (float2*)irspec_save : (float2*)(base + w.hsp);
   const float* tw = nullptr;
 
+  // IR taps t < leff of items [item0, item0 + items) into their partition slots; the cuFFT transform of the partitions
+  // reads whole slots, x_fft_kernel only the taps ir_pack_kernel writes
+  auto fill_ir = [&](float2* hs, bool own, int64_t item0, int64_t items) -> int {
+    if (!own) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
+    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(ir, hs, item0, J, g.L,
+                                                                                          g.leff, (int)ir_chs);
+    DASP_LAUNCH_OK("ir_pack_kernel");
+    return DASP_OK;
+  };
+  if (shared) {
+    const bool own = own_fft_rows(n, x, hs0);
+    if ((rc = fill_ir(hs0, own, 0, 1)) != DASP_OK) return rc;
+    if (own && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    if ((rc = conv_shared_ir_spectra(g, s.ir1, own, tw, hs0, base, w, st)) != DASP_OK) return rc;
+  }
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? s.full : s.rem;
     float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
-    float2* hs = irspec_save ? (float2*)irspec_save + item0 * J * (int64_t)kNbA : (float2*)(base + w.hsp);
+    float2* hs = irspec_save ? hs0 + item0 * h_stride : hs0;
     const bool own_conv = own_fft_rows(n, x, hs);
-    g_conv_last_path[0] = own_conv ? 1 : 0;
-    // the cuFFT transform of the partitions reads whole slots; x_fft_kernel only the taps ir_pack_kernel writes
-    if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
-    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(ir, hs, item0, J, g.L, g.leff,
-                                                                                          (int)ir_chs);
-    DASP_LAUNCH_OK("ir_pack_kernel");
+    g_conv_last_path[0] = (own_conv ? 1 : 0) | (shared ? 2 : 0);
+    if (!shared && (rc = fill_ir(hs, own_conv, item0, items)) != DASP_OK) return rc;
     if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, mix, 1, y, base, w, item0, items, st)) !=
-        DASP_OK)
+    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, h_stride, mix, 1, y, base, w, item0, items,
+                             st)) != DASP_OK)
       return rc;
   }
   return DASP_OK;
 }
 
-int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, const float* mix,
-                  const void* xspec_save, const void* irspec_save, float* gx, float* gir, float* gmix, void* workspace,
-                  int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len,
+                const float* mix, const void* xspec_save, const void* irspec_save, float* gx, float* gir, float* gmix,
+                void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
   ConvGeom g;
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
+  g.shared = shared;
   DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2), "conv: only mono/stereo signals and IRs");
   if (bs == 0) return DASP_OK;
   DASP_REQUIRE(gy && x && mix && xspec_save && irspec_save && gx && gmix && workspace, "conv bwd: null pointer");
@@ -2477,42 +2564,108 @@ int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_ch
   if ((rc = check_workspace("conv bwd", s.bwd.total, workspace_bytes)) != DASP_OK) return rc;
   const BwdWs& w = s.bwd;
   unsigned char* base = (unsigned char*)workspace;
-  const float2* ws_es = (const float2*)(base + w.es);
+  float2* ws_es = (float2*)(base + w.es);
   const float* ws_mixpart = (const float*)(base + w.mixpart);
+  double2* ws_acc = (double2*)(base + w.acc);
   const int I = (int)g.ib, J = (int)g.jb;
+  const int64_t h_stride = shared ? 0 : J * (int64_t)kNbA;
+  const float* tw = nullptr;
+  bool own_conv = false;
 
-  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
-    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
-    const float2* xs = (const float2*)xspec_save + item0 * I * (int64_t)kNbA;
-    const float2* hs = (const float2*)irspec_save + item0 * J * (int64_t)kNbA;
-    const bool own_conv = own_fft_rows(n, gy, nullptr);
-    const IrGrad e = gir == nullptr ? IrGrad::kNone : (own_conv ? IrGrad::kPlanar : IrGrad::kTime);
-    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed
-    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_corr(e, I, J) ? 2 : 0) | (gir ? 4 : 0);
-    const float* tw = nullptr;
-    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    if ((rc = conv_bwd_chunk(g, pl, own_conv, e, tw, gy, x, (int)in_chs, xs, hs, mix, 1, gx, base, w, item0, items,
-                             st)) != DASP_OK)
-      return rc;
+  // dL/dIR taps of items [item0, item0 + items) from their partitions in the es region (planar spectra, or time-domain
+  // pairs after the inverse cuFFT), times mix[b] (a null mix: 1)
+  auto ir_taps = [&](IrGrad e, int64_t item0, int64_t items, const float* mx) -> int {
     if (e == IrGrad::kPlanar) {
       const int nunits = (int)(items * J);
       const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-      ifft_irtaps_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mix, gir,
-                                                                        item0, J, g.L, g.leff, (int)ir_chs, nunits);
+      ifft_irtaps_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mx,
+                                                                        gir, item0, J, g.L, g.leff, (int)ir_chs, nunits);
       DASP_LAUNCH_OK("ifft_irtaps_kernel");
     }
     // taps t0 <= t < L: the zeros from leff on after ifft_irtaps_kernel, every tap after the cuFFT inverse
     const int64_t t0 = e == IrGrad::kPlanar ? g.leff : 0;
-    if (e != IrGrad::kNone && g.L > t0) {
+    if (g.L > t0) {
       irtaps_unpack_kernel<<<dim3((unsigned)((g.L - t0 + 255) / 256), (unsigned)items), 256, 0, st>>>(
-          ws_es, mix, gir, item0, J, g.L, g.leff, (int)ir_chs, t0);
+          ws_es, mx, gir, item0, J, g.L, g.leff, (int)ir_chs, t0);
       DASP_LAUNCH_OK("irtaps_unpack_kernel");
+    }
+    return DASP_OK;
+  };
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
+    const float2* xs = (const float2*)xspec_save + item0 * I * (int64_t)kNbA;
+    const float2* hs = (const float2*)irspec_save + item0 * h_stride;
+    own_conv = own_fft_rows(n, gy, nullptr);
+    const IrGrad e = gir == nullptr ? IrGrad::kNone
+                                    : (own_conv ? IrGrad::kPlanar : (shared ? IrGrad::kSpectra : IrGrad::kTime));
+    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed, bit 3: one IR shared by the batch
+    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_corr(e, I, J) ? 2 : 0) | (gir ? 4 : 0) | (shared ? 8 : 0);
+    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    if ((rc = conv_bwd_chunk(g, pl, own_conv, e, tw, gy, x, (int)in_chs, xs, hs, h_stride, mix, 1, gx, base, w, item0,
+                             items, st)) != DASP_OK)
+      return rc;
+    if (e != IrGrad::kNone && shared) {
+      const int64_t per_item = J * (int64_t)kNbA;
+      irgrad_sum_kernel<<<(unsigned)((per_item + 255) / 256), 256, 0, st>>>(ws_es, mix, ws_acc, item0, (int)items,
+                                                                            per_item, item0 + items == bs);
+      DASP_LAUNCH_OK("irgrad_sum_kernel");
+    } else if (e != IrGrad::kNone && (rc = ir_taps(e, item0, items, mix)) != DASP_OK) {
+      return rc;
     }
     conv_mix_grad_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(ws_mixpart, gmix, item0, items, I);
     DASP_LAUNCH_OK("conv_mix_grad_kernel");
   }
+  if (shared && gir) {
+    // the summed partition spectra, rounded to fp32 in item 0's slot of es: J inverse transforms for the one IR
+    if (!own_conv) {
+      DASP_CUFFT_OK(cufftSetStream(s.ir1.h, st));
+      DASP_CUFFT_OK(cufftSetWorkArea(s.ir1.h, base + w.cufft));
+      DASP_CUFFT_OK(cufftExecC2C(s.ir1.h, (cufftComplex*)ws_es, (cufftComplex*)ws_es, CUFFT_INVERSE));
+    }
+    if ((rc = ir_taps(own_conv ? IrGrad::kPlanar : IrGrad::kTime, 0, 1, nullptr)) != DASP_OK) return rc;
+  }
   return DASP_OK;
+}
+}  // namespace
+
+int dasp_debug_conv_last_path(int which) { return g_conv_last_path[which ? 1 : 0]; }
+
+int dasp_conv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+  return conv_op_geometry(false, bs, n, ir_len, chunk_items, out);
+}
+
+int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, const float* mix,
+                  float* y, void* xspec_save, void* irspec_save, void* workspace, int64_t workspace_bytes, int64_t bs,
+                  int64_t n, int64_t chunk_items, void* stream) {
+  return conv_op_fwd(false, x, in_chs, ir, ir_chs, ir_len, mix, y, xspec_save, irspec_save, workspace, workspace_bytes,
+                     bs, n, chunk_items, stream);
+}
+
+int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, const float* mix,
+                  const void* xspec_save, const void* irspec_save, float* gx, float* gir, float* gmix, void* workspace,
+                  int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+  return conv_op_bwd(false, gy, x, in_chs, ir_chs, ir_len, mix, xspec_save, irspec_save, gx, gir, gmix, workspace,
+                     workspace_bytes, bs, n, chunk_items, stream);
+}
+
+int dasp_conv_shared_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+  return conv_op_geometry(true, bs, n, ir_len, chunk_items, out);
+}
+
+int dasp_conv_shared_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,
+                         const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                         int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+  return conv_op_fwd(true, x, in_chs, ir, ir_chs, ir_len, mix, y, xspec_save, irspec_save, workspace, workspace_bytes,
+                     bs, n, chunk_items, stream);
+}
+
+int dasp_conv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len,
+                         const float* mix, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                         float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                         int64_t chunk_items, void* stream) {
+  return conv_op_bwd(true, gy, x, in_chs, ir_chs, ir_len, mix, xspec_save, irspec_save, gx, gir, gmix, workspace,
+                     workspace_bytes, bs, n, chunk_items, stream);
 }
 
 }  // extern "C"

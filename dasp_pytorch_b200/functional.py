@@ -702,50 +702,55 @@ def noise_shaped_reverberation_packed(x: torch.Tensor, sample_rate: float, param
 
 
 class _ConvReverbFn(torch.autograd.Function):
-    """x (bs, 1|2, n), ir (bs, 1|2, L), mix (bs,) -> y (bs, 2, n)."""
+    """x (bs, 1|2, n), ir (bs, 1|2, L), mix (bs,) -> y (bs, 2, n).  An ir of batch 1 with bs > 1 is one IR shared by
+    the batch (the dasp_conv_shared_* entry points): its gradient is the sum over the items, shape (1, 1|2, L)."""
 
     @staticmethod
     def forward(ctx, x, ir, mix, chunk):
         lib = _abi.lib()
         bs, in_chs, n = x.shape
-        _, ir_chs, ir_len = ir.shape
+        ir_bs, ir_chs, ir_len = ir.shape
+        shared = ir_bs == 1 and bs > 1
+        kind = "conv_shared" if shared else "conv"
         dev = x.device
         y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:3])
         geom = _abi.ConvGeom()
         with torch.cuda.device(dev):
-            check(lib.dasp_conv_geometry(bs, n, ir_len, chunk, geom), "dasp_conv_geometry")
+            check(getattr(lib, f"dasp_{kind}_geometry")(bs, n, ir_len, chunk, geom), f"dasp_{kind}_geometry")
             ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
             xspec = irspec = None
             if need_bwd:
                 xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
                 irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
             with _timed("conv_fwd", dev):
-                check(lib.dasp_conv_fwd(ptr(x), in_chs, ptr(ir), ir_chs, ir_len, ptr(mix), ptr(y), ptr(xspec),
-                                        ptr(irspec), ptr(ws), ws.numel(), bs, n, chunk, stream_ptr(dev)),
-                      "dasp_conv_fwd")
+                check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), in_chs, ptr(ir), ir_chs, ir_len, ptr(mix), ptr(y),
+                                                       ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n, chunk,
+                                                       stream_ptr(dev)),
+                      f"dasp_{kind}_fwd")
         if need_bwd:
             ctx.save_for_backward(x, xspec, irspec, mix)
-        ctx.cfg = (ir_chs, ir_len, chunk, geom.bwd_workspace_bytes)
+        ctx.cfg = (kind, ir_bs, ir_chs, ir_len, chunk, geom.bwd_workspace_bytes)
         return y
 
     @staticmethod
     def backward(ctx, gy):
         lib = _abi.lib()
         x, xspec, irspec, mix = ctx.saved_tensors
-        ir_chs, ir_len, chunk, bwd_bytes = ctx.cfg
+        kind, ir_bs, ir_chs, ir_len, chunk, bwd_bytes = ctx.cfg
         bs, in_chs, n = x.shape
         dev = x.device
         gy = gy.contiguous()
         gx = torch.empty_like(x)
         # a fixed IR (data augmentation with measured rooms) skips every dL/dIR kernel
-        gir = torch.empty(bs, ir_chs, ir_len, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        gir = torch.empty(ir_bs, ir_chs, ir_len, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
         gmix = torch.empty_like(mix)
         ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev), _timed("conv_bwd", dev):
-            check(lib.dasp_conv_bwd(ptr(gy), ptr(x), in_chs, ir_chs, ir_len, ptr(mix), ptr(xspec), ptr(irspec),
-                                    ptr(gx), ptr(gir), ptr(gmix), ptr(ws), ws.numel(), bs, n, chunk, stream_ptr(dev)),
-                  "dasp_conv_bwd")
+            check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(x), in_chs, ir_chs, ir_len, ptr(mix), ptr(xspec),
+                                                   ptr(irspec), ptr(gx), ptr(gir), ptr(gmix), ptr(ws), ws.numel(), bs,
+                                                   n, chunk, stream_ptr(dev)),
+                  f"dasp_{kind}_bwd")
         return gx, gir, gmix, None
 
 
@@ -758,15 +763,19 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
     Args:
         x: audio ``(bs, 1|2, n)``; mono is used for both channels.
         sample_rate: unused (kept for the common processor signature).
-        impulse_response: ``(bs, 1|2, L)``, any ``L >= 1``; a mono IR is used for both channels.  One IR shared by the
-            whole batch is passed as ``ir.expand(bs, -1, -1)``, which costs one copy.
+        impulse_response: ``(bs, 1|2, L)``, one IR per item, or ``(1, 1|2, L)``, one IR for the whole batch (a
+            measured room applied to every item, or a single learnt FIR reverb); any ``L >= 1``; a mono IR is used for
+            both channels.
         mix: ``bs`` elements in any shape, or one element that is broadcast over the batch.
 
     Returns ``(bs, 2, n)`` in x's dtype (computed in fp32), like ``noise_shaped_reverberation``, so the two can replace
     each other in a chain.  Gradients flow to ``x``, ``impulse_response`` (a mono IR receives the sum of both channel
-    gradients; taps at or beyond ``n`` reach no output and get exactly 0) and ``mix``.  When the IR does not require a
-    gradient, the backward skips all dL/dIR work.  The convolution is the reverb's own: uniformly partitioned
-    overlap-save on 4096-sample partitions with the in-shared-memory 8192-point FFT.
+    gradients; taps at or beyond ``n`` reach no output and get exactly 0) and ``mix``.  The gradient of a ``(1, 1|2, L)``
+    IR has that shape and is the sum over the items of each item's gradient, accumulated in fp64 in item order, so it
+    does not depend on how the batch is chunked.  A shared IR is transformed once per call rather than once per item,
+    and no per-item copy of it or of its gradient is ever made; ``ir.expand(bs, -1, -1)`` gives the same result at the
+    per-item cost.  When the IR does not require a gradient, the backward skips all dL/dIR work.  The convolution is the
+    reverb's own: uniformly partitioned overlap-save on 4096-sample partitions with the in-shared-memory 8192-point FFT.
     """
     for t, name in ((x, "x"), (impulse_response, "impulse_response")):
         if not torch.is_tensor(t) or t.dim() != 3:
@@ -774,8 +783,8 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
         if t.shape[1] not in (1, 2):
             raise ValueError(f"{name}: only mono/stereo is supported, got {t.shape[1]} channels")
     bs = x.shape[0]
-    if impulse_response.shape[0] != bs:
-        raise ValueError(f"impulse_response has batch {impulse_response.shape[0]}, x has batch {bs}")
+    if impulse_response.shape[0] != bs and not (impulse_response.shape[0] == 1 and bs > 1):
+        raise ValueError(f"impulse_response has batch {impulse_response.shape[0]}, x has batch {bs} (expected {bs} or 1)")
     if impulse_response.shape[2] < 1:
         raise ValueError("impulse_response needs at least one tap")
     nmix = mix.numel() if torch.is_tensor(mix) else torch.as_tensor(mix).numel()

@@ -215,9 +215,23 @@ int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_ch
 int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, const float* mix,
                   const void* xspec_save, const void* irspec_save, float* gx, float* gir /* may be NULL */, float* gmix,
                   void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream);
-/* test hook: dispatch of the most recent call.  which = 0: dasp_conv_fwd, 1 = own in-shared-memory FFT, 0 = cuFFT
-   pipeline (dasp_debug_reverb_path(1), n % 4 != 0, rows not 16-byte aligned).  which = 1: dasp_conv_bwd, bit 0 = own
-   FFT, bit 1 = fused correlation kernel, bit 2 = dL/dIR computed */
+/* One impulse response for the whole batch: the same argument lists, with ir (fwd) and gir (bwd) pointing at ONE
+ * (ir_chs, ir_len) IR that applies to every item.  Its partitions are transformed once per call instead of once per
+ * item, and gir receives the sum over the items of each item's dL/dIR (fp64, in item order: the same bits for every
+ * chunk_items).  The geometry is the same struct: irspec_c64 is one IR's (0 at bs = 0), and the workspace sizes include
+ * the fp64 gradient sum of the backward. */
+int dasp_conv_shared_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_conv_shared_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,
+                         const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                         int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream);
+int dasp_conv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len,
+                         const float* mix, const void* xspec_save, const void* irspec_save, float* gx,
+                         float* gir /* may be NULL */, float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs,
+                         int64_t n, int64_t chunk_items, void* stream);
+/* test hook: dispatch of the most recent call.  which = 0: dasp_conv_fwd / dasp_conv_shared_fwd, bit 0 = own
+   in-shared-memory FFT, clear = cuFFT pipeline (dasp_debug_reverb_path(1), n % 4 != 0, rows not 16-byte aligned),
+   bit 1 = shared IR.  which = 1: dasp_conv_bwd / dasp_conv_shared_bwd, bit 0 = own FFT, bit 1 = fused correlation
+   kernel, bit 2 = dL/dIR computed, bit 3 = shared IR */
 int dasp_debug_conv_last_path(int which);
 
 #ifdef __cplusplus

@@ -34,6 +34,11 @@
 // one plan set (conv_setup) and one workspace layout per direction; each op adds only its IR fill, its mix stride and
 // its dL/dIR consumer.  One IR for the whole batch (dasp_conv_shared_*) is the item stride 0 of the IR spectra: they
 // are transformed once, and irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.
+//
+// Steps that several kernels share are written once: FftSmem (the shared-memory layout of the FFT kernels and their
+// double-buffered bulk-copy input), fft8192_in_smem (the four passes), shape_band / store_ir_taps (the epilogue of both
+// own-FFT IR syntheses, which therefore give the same bits), band_gain / band_rate (the parameter layout), ir_slot (the
+// partition layout of the IR taps) and block_band_sums (the reduction of the 24 band-parameter partials).
 #include <cufft.h>
 #include <curand_kernel.h>
 #include <math.h>
@@ -191,6 +196,14 @@ int get_plan(int type /*0 = R2C, 1 = C2R, 2 = C2C*/, int64_t n, int64_t batch, i
                                     (long long)batch, &pv.work));
   g_plans[key] = pv;
   out = pv;
+  return DASP_OK;
+}
+
+// in-place C2C of a plan on stream st with the work area `work`
+int exec_c2c(const PlanVal& plan, void* work, void* data, int direction, cudaStream_t st) {
+  DASP_CUFFT_OK(cufftSetStream(plan.h, st));
+  DASP_CUFFT_OK(cufftSetWorkArea(plan.h, work));
+  DASP_CUFFT_OK(cufftExecC2C(plan.h, (cufftComplex*)data, (cufftComplex*)data, direction));
   return DASP_OK;
 }
 
@@ -449,6 +462,23 @@ __device__ __forceinline__ float time_axis32(int t, int L, float step) {
   return (t < L / 2) ? step * (float)t : 1.0f - step * (float)(L - 1 - t);
 }
 
+// the 25 parameters of item il: band gains (0..11), band decays (12..23), mix (24).  Band k contributes
+// band_gain exp(band_rate tt) f_k to the IR (the 1/12 of the band mean folded into the gain).
+__device__ __forceinline__ float band_gain(const float* params, int64_t il, int k) {
+  return params[il * 25 + k] * (1.0f / kBands);
+}
+__device__ __forceinline__ float band_rate(const float* params, int64_t il, int k) {
+  return -(params[il * 25 + kBands + k] * 10.0f + 1.0f);
+}
+
+// The partition layout of the audio convolution: IR tap t < leff of item il (and, in the backward, dL/dIR tap t) is the
+// (left, right) pair at element ir_slot(il, J, t), the first half of partition slot t / kB.  The offset inside the
+// item is computed in the tap's own type (int or int64_t), which keeps 32-bit index arithmetic in the FFT kernels.
+template <class Tap>
+__device__ __forceinline__ int64_t ir_slot(int64_t il, int J, Tap t) {
+  return il * J * (int64_t)kNbA + ((t / kB) * kNbA + t % kB);
+}
+
 // IR[c][t] = (1/12) sum_k gain_k exp(-(10 decay_k + 1) tt(t)) f_c[k][t]  for t < leff, written as (left, right)
 // complex pairs into the partition layout of the audio convolution (first half of partition t / kB; every synthesis
 // variant writes these taps and nothing else).
@@ -460,12 +490,11 @@ __global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float*
   const int64_t il = blockIdx.y;
   __shared__ float gk[kBands], rk[kBands];
   if (threadIdx.x < kBands) {
-    gk[threadIdx.x] = params[il * 25 + threadIdx.x] * (1.0f / kBands);
-    rk[threadIdx.x] = -(params[il * 25 + kBands + threadIdx.x] * 10.0f + 1.0f);
+    gk[threadIdx.x] = band_gain(params, il, threadIdx.x);
+    rk[threadIdx.x] = band_rate(params, il, threadIdx.x);
   }
   __syncthreads();
   const float step = 1.0f / (float)(L - 1);
-  float2* out = Hb + il * (int64_t)jb * kNbA;      // partition j holds taps [j kB, (j+1) kB) in its first half
   for (int m = threadIdx.x; m < hop; m += blockDim.x) {
     const int64_t t = (int64_t)b * hop + m;
     if (t >= leff) break;
@@ -479,7 +508,7 @@ __global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float*
       al = fmaf(e, v.x, al);
       ar = fmaf(e, v.y, ar);
     }
-    out[(t / kB) * kNbA + (t % kB)] = make_float2(al, ar);
+    Hb[ir_slot(il, jb, t)] = make_float2(al, ar);
   }
 }
 
@@ -491,8 +520,8 @@ __global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __
   const int64_t il = blockIdx.y;
   __shared__ float gk[kBands], rk[kBands];
   if (threadIdx.x < kBands) {
-    gk[threadIdx.x] = params[il * 25 + threadIdx.x] * (1.0f / kBands);
-    rk[threadIdx.x] = -(params[il * 25 + kBands + threadIdx.x] * 10.0f + 1.0f);
+    gk[threadIdx.x] = band_gain(params, il, threadIdx.x);
+    rk[threadIdx.x] = band_rate(params, il, threadIdx.x);
   }
   __syncthreads();
   if (t >= leff) return;
@@ -509,105 +538,147 @@ __global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __
     al = fmaf(e, v[k].x, al);
     ar = fmaf(e, v[k].y, ar);
   }
-  Hb[il * (int64_t)jb * kNbA + (t / kB) * kNbA + (t % kB)] = make_float2(al, ar);
+  Hb[ir_slot(il, jb, t)] = make_float2(al, ar);
 }
 
-// ---- inverse FFT + envelope / gain / band mean as one kernel (device-noise mode, nb == 8192) -----------
+// ---- the in-shared-memory FFT of fft8192.cuh as the kernels below use it ---------------------------------------
+// One 512-thread CTA per SM; its input is bulk-copied into the planar double buffer G while the other half is transformed.
+constexpr int kFusedThreads = fft8k::kThreads;
+// G [buffer][re, im][8192], Y (re, im planes of the padded layouts), the twiddle tables, and 32 floats of per-kernel
+// scratch (the pad; ifft_shape_kernel keeps the item's band gains and rates there)
+constexpr int kFusedSmemFloats = 2 * 2 * fft8k::kPlaneG + 2 * fft8k::kPlaneY + fft8k::kTabFloats + 32;
+constexpr size_t kFftSmemBytes = sizeof(float) * kFusedSmemFloats + 2 * sizeof(uint64_t);   // + the two mbarriers
+struct FftSmem {
+  float* G; float* Yr; float* Yi; float* tabf; float* pad; uint64_t* full;
+  __device__ __forceinline__ explicit FftSmem(float* sm) {
+    G = sm;
+    Yr = sm + 4 * fft8k::kPlaneG;
+    Yi = Yr + fft8k::kPlaneY;
+    tabf = Yi + fft8k::kPlaneY;
+    pad = tabf + fft8k::kTabFloats;
+    full = reinterpret_cast<uint64_t*>(pad + 32);
+  }
+  __device__ __forceinline__ void init(const float* twiddles, int t) {
+    if (t == 0) {
+      mbar_init(&full[0], 1);
+      mbar_init(&full[1], 1);
+      fence_barrier_init();
+    }
+    for (int e = t; e < fft8k::kTabFloats; e += kFusedThreads) tabf[e] = twiddles[e];
+    __syncthreads();
+  }
+  // the planar buffer of unit `it` of a CTA's work list (units alternate between the two halves)
+  __device__ __forceinline__ float* buf(int it) const { return G + (it & 1) * 2 * fft8k::kPlaneG; }
+  // until the input of unit `it` has landed in buf(it)
+  __device__ __forceinline__ void wait(int it) const { mbar_wait(&full[it & 1], (uint32_t)((it >> 1) & 1)); }
+  // thread 0 only: bulk-copy the 64 KB planar block src (re plane, im plane) into buf(it)
+  __device__ __forceinline__ void load_planar(int it, const float* src) const {
+    uint64_t* bar = &full[it & 1];
+    float* dst = buf(it);
+    mbar_arrive_expect_tx(bar, 2u * kNbA * 4u);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
+  }
+};
+// the 512 FFT threads only (named barrier 1; barrier 0 is __syncthreads): the FFT warps of ir_synth_cluster_kernel
+__device__ __forceinline__ void fft_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kFusedThreads) : "memory"); }
+// the four passes on buffer (gr, gi); `refill()` runs as soon as nobody reads the buffer any more, `early()` two
+// passes before the results exist (the place to issue global loads the epilogue needs, so that their latency is
+// covered by passes 3 and 4 -- with one lock-stepped CTA per SM nothing else would hide it).  FFT_WARPS: the barriers
+// are fft_sync() instead of __syncthreads().
+template <bool INV, bool FFT_WARPS = false, class Refill, class Early>
+__device__ __forceinline__ void fft8192_in_smem(float* gr, float* gi, const FftSmem& s, const fft8k::Tables& tb, int t,
+                                                Refill&& refill, Early&& early, float (&xr)[16], float (&xi)[16]) {
+  auto sync = [] { if constexpr (FFT_WARPS) fft_sync(); else __syncthreads(); };
+  fft8k::p1<INV>(gr, gi, tb, t);
+  sync();
+  fft8k::p2<INV>(gr, gi, s.Yr, s.Yi, tb, t);
+  fence_proxy_async_smem();                        // pass-1 stores to G (generic proxy) before the refill's async writes
+  sync();
+  refill();
+  fft8k::P3Regs q3;
+  fft8k::p3_load<INV>(s.Yr, s.Yi, t, q3);
+  sync();
+  early();
+  fft8k::p3_store<INV>(s.Yr, s.Yi, tb, t, q3);
+  sync();
+  fft8k::p4<INV>(s.Yr, s.Yi, t, xr, xi);
+}
+
+// ---- inverse FFT + envelope / gain / band mean (device-noise mode, nb == 8192) ----------------------------------
+// One band of the IR synthesis after its inverse transform (x = the pass-4 outputs of FFT thread t, i.e. the filtered
+// noise f of band k at the taps tau_q = R (t + 512 q) + c of polyphase class c): acc += gain_k env_k(tau) f(tau), and f
+// is stored as (left, right) pairs at fout[t + 512 q] unless fout is null.  The envelope g_k exp(rr tt(tau)) is
+// evaluated at every 4th tap; the three taps in between follow by the constant ratio exp(rr step 512 R) (tt is linear in
+// tau up to fp32 rounding of the linspace, so this stays within ~1e-6 of the per-tap evaluation).
+__device__ __forceinline__ void shape_band(const float (&xr)[16], const float (&xi)[16], float g_k, float rr, int R, int c,
+                                           int L, float step, int t, float2* fout, float (&accr)[16], float (&acci)[16]) {
+  float e_prev = 0.f;
+  const float rho = __expf(rr * step * (float)(512 * R));
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    const int a = t + 512 * q;
+    float e;
+    if ((q & 3) == 0) e = g_k * __expf(rr * time_axis32(R * a + c, L, step));
+    else e = e_prev * rho;
+    e_prev = e;
+    accr[q] = fmaf(e, xr[q], accr[q]);
+    acci[q] = fmaf(e, xi[q], acci[q]);
+    if (fout) fout[a] = make_float2(xr[q], xi[q]);
+  }
+}
+// the accumulated IR taps tau_q = R (t + 512 q) + c below leff of item il into the partition layout
+__device__ __forceinline__ void store_ir_taps(float2* Hb, int64_t il, int jb, int R, int c, int leff, int t,
+                                              const float (&accr)[16], const float (&acci)[16]) {
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    const int tau = R * (t + 512 * q) + c;
+    if (tau < leff) Hb[ir_slot(il, jb, tau)] = make_float2(accr[q], acci[q]);
+  }
+}
+
 // Replaces the batched cuFFT C2C + shape_ir_pp_kernel pair: the generator's spectrum is read ONCE (bulk copies
 // straight into the planar shared-memory layout of fft8192.cuh, double buffered across the 12 bands), transformed
 // in shared memory, and each thread accumulates  gain_k env_k(t) f_k(t) / 12  for its 16 taps in registers.  The
 // filtered noise f is written back (over the consumed spectrum block, as (left, right) pairs) only when the
 // backward needs it.  grid = (R, items): CTA (c, item) owns polyphase class c, i.e. the IR taps R a + c.
-constexpr int kFusedThreads = fft8k::kThreads;
-constexpr int kFusedSmemFloats = 2 * 2 * fft8k::kPlaneG + 2 * fft8k::kPlaneY + fft8k::kTabFloats + 32;
-constexpr size_t kFftSmemBytes = sizeof(float) * kFusedSmemFloats + 2 * sizeof(uint64_t);   // + the two mbarriers
-
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params,
                   float2* __restrict__ Hb, int save_f, int L, int leff, int jb, int R) {
   constexpr int nb = fft8k::kN;
   extern __shared__ __align__(128) float sm[];
-  float* G = sm;                                   // [buffer][re, im][8192]
-  float* Yr = sm + 4 * fft8k::kPlaneG;
-  float* Yi = Yr + fft8k::kPlaneY;
-  float* tabf = Yi + fft8k::kPlaneY;
-  float* gk = tabf + fft8k::kTabFloats;
-  float* rk = gk + 16;
-  uint64_t* full = reinterpret_cast<uint64_t*>(rk + 16);
+  FftSmem s(sm);
+  float* gk = s.pad;
+  float* rk = s.pad + 16;
   const int t = threadIdx.x, c = blockIdx.x;
   const int64_t il = blockIdx.y;
   float* blk = Cpl + ((il * kBands) * R + c) * (int64_t)(2 * nb);      // band k at blk + k * R * 2 nb
   const int64_t band_stride = (int64_t)R * 2 * nb;
 
-  if (t == 0) {
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
-    fence_barrier_init();
-  }
-  for (int e = t; e < fft8k::kTabFloats; e += kFusedThreads) tabf[e] = twiddles[e];
   if (t < kBands) {
-    gk[t] = params[il * 25 + t] * (1.0f / kBands);
-    rk[t] = -(params[il * 25 + kBands + t] * 10.0f + 1.0f);
+    gk[t] = band_gain(params, il, t);
+    rk[t] = band_rate(params, il, t);
   }
-  __syncthreads();
-  auto fetch = [&](int k) {                        // thread 0: 64 KB spectrum block of band k -> G[k & 1]
-    uint64_t* bar = &full[k & 1];
-    float* dst = G + (k & 1) * 2 * fft8k::kPlaneG;
-    const float* src = blk + k * band_stride;
-    mbar_arrive_expect_tx(bar, 2u * nb * 4u);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) tma_load_1d(dst + i * 4096, src + i * 4096, 16384u, bar);
-  };
-  if (t == 0) { fetch(0); fetch(1); }
-  const fft8k::Tables tb = fft8k::carve_tables(tabf);
+  s.init(twiddles, t);
+  if (t == 0) { s.load_planar(0, blk); s.load_planar(1, blk + band_stride); }
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
   const float step = 1.0f / (float)(L - 1);
   float accr[16], acci[16];
 #pragma unroll
   for (int q = 0; q < 16; ++q) { accr[q] = 0.f; acci[q] = 0.f; }
 
   for (int k = 0; k < kBands; ++k) {
-    mbar_wait(&full[k & 1], (uint32_t)((k >> 1) & 1));
-    float* gr = G + (k & 1) * 2 * fft8k::kPlaneG;
-    float* gi = gr + fft8k::kPlaneG;
-    fft8k::p1<true>(gr, gi, tb, t);
-    __syncthreads();
-    fft8k::p2<true>(gr, gi, Yr, Yi, tb, t);
-    fence_proxy_async_smem();                      // pass-1 stores to G (generic proxy) before the bulk refill
-    __syncthreads();
-    if (t == 0 && k + 2 < kBands) fetch(k + 2);
-    fft8k::P3Regs q3;
-    fft8k::p3_load<true>(Yr, Yi, t, q3);
-    __syncthreads();
-    fft8k::p3_store<true>(Yr, Yi, tb, t, q3);
-    __syncthreads();
+    s.wait(k);
+    float* gr = s.buf(k);
     float xr[16], xi[16];
-    fft8k::p4<true>(Yr, Yi, t, xr, xi);
-    float e_prev = 0.f;
-    const float g = gk[k], rr = rk[k];
-    float2* fout = reinterpret_cast<float2*>(blk + k * band_stride);
-    // envelope gain_k exp(rr tt(tau)) at the thread's taps tau_q = R (t + 512 q) + c: evaluated at every 4th tap,
-    // the three taps in between follow by the constant ratio exp(rr step 512 R) (tt is linear in tau up to fp32
-    // rounding of the linspace, so this stays within ~1e-6 of the per-tap evaluation)
-    const float rho = __expf(rr * step * (float)(512 * R));
-#pragma unroll
-    for (int q = 0; q < 16; ++q) {
-      const int a = t + 512 * q;
-      float e;
-      if ((q & 3) == 0) e = g * __expf(rr * time_axis32(R * a + c, L, step));
-      else e = e_prev * rho;
-      e_prev = e;
-      accr[q] = fmaf(e, xr[q], accr[q]);
-      acci[q] = fmaf(e, xi[q], acci[q]);
-      if (save_f) fout[a] = make_float2(xr[q], xi[q]);
-    }
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t,
+                          [&] { if (t == 0 && k + 2 < kBands) s.load_planar(k + 2, blk + (k + 2) * band_stride); },
+                          [] {}, xr, xi);
+    shape_band(xr, xi, gk[k], rk[k], R, c, L, step, t,
+               save_f ? reinterpret_cast<float2*>(blk + k * band_stride) : nullptr, accr, acci);
     // (Y is next written by pass 2 of the following band, behind the barrier after its pass 1)
   }
-  float2* out = Hb + il * (int64_t)jb * kNbA;
-#pragma unroll
-  for (int q = 0; q < 16; ++q) {
-    const int tau = R * (t + 512 * q) + c;
-    if (tau < leff) out[(tau / kB) * kNbA + (tau % kB)] = make_float2(accr[q], acci[q]);
-  }
+  store_ir_taps(Hb, il, jb, R, c, leff, t, accr, acci);
 }
 
 // ---- block transforms of the audio convolution on the same in-shared-memory FFT ---------------------------
@@ -620,45 +691,6 @@ ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, c
 #define DASP_CONV_RUN 8
 #endif
 constexpr int kConvRun = DASP_CONV_RUN;
-struct FftSmem {
-  float* G; float* Yr; float* Yi; float* tabf; uint64_t* full;
-  __device__ __forceinline__ explicit FftSmem(float* sm) {
-    G = sm;
-    Yr = sm + 4 * fft8k::kPlaneG;
-    Yi = Yr + fft8k::kPlaneY;
-    tabf = Yi + fft8k::kPlaneY;
-    full = reinterpret_cast<uint64_t*>(tabf + fft8k::kTabFloats + 32);
-  }
-  __device__ __forceinline__ void init(const float* twiddles, int t) {
-    if (t == 0) {
-      mbar_init(&full[0], 1);
-      mbar_init(&full[1], 1);
-      fence_barrier_init();
-    }
-    for (int e = t; e < fft8k::kTabFloats; e += kFusedThreads) tabf[e] = twiddles[e];
-    __syncthreads();
-  }
-};
-// the four passes on buffer (gr, gi); `refill()` runs as soon as nobody reads the buffer any more, `early()` two
-// passes before the results exist (the place to issue global loads the epilogue needs, so that their latency is
-// covered by passes 3 and 4 -- with one lock-stepped CTA per SM nothing else would hide it)
-template <bool INV, class Refill, class Early>
-__device__ __forceinline__ void fft8192_in_smem(float* gr, float* gi, const FftSmem& s, const fft8k::Tables& tb, int t,
-                                                Refill&& refill, Early&& early, float (&xr)[16], float (&xi)[16]) {
-  fft8k::p1<INV>(gr, gi, tb, t);
-  __syncthreads();
-  fft8k::p2<INV>(gr, gi, s.Yr, s.Yi, tb, t);
-  fence_proxy_async_smem();                        // pass-1 stores to G (generic proxy) before the bulk refill
-  __syncthreads();
-  refill();
-  fft8k::P3Regs q3;
-  fft8k::p3_load<INV>(s.Yr, s.Yi, t, q3);
-  __syncthreads();
-  early();
-  fft8k::p3_store<INV>(s.Yr, s.Yi, tb, t, q3);
-  __syncthreads();
-  fft8k::p4<INV>(s.Yr, s.Yi, t, xr, xi);
-}
 
 // Both forward block transforms of the audio convolution, one work list of nwin + items*J units (runs of kConvRun):
 //   unit m < nwin = items*I:  Xb[(il*I + i)*kNbA + f] = FFT of the window (x_left + i x_right)[(i-1) kB + m], m < kNbA
@@ -678,7 +710,10 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __res
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
   const int m0 = blockIdx.x * kConvRun;            // this CTA's units [m0, m1)
   const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
-  auto fetch = [&](int it, int m) {                // all threads: zero padding; thread 0: the bulk copies
+  // all threads: zero padding; thread 0: the bulk copies.  The buffer is addressed as below rather than by s.buf(it):
+  // with s.buf(it), nvcc 12.9 schedules the whole kernel differently (same arithmetic); this form keeps the code the
+  // timings in DESIGN.md were taken with.
+  auto fetch = [&](int it, int m) {
     if (m >= m1) return;
     if (m >= nwin) {                               // partition: its 32 KB of taps land in the im plane, see below
       if (t == 0) {
@@ -718,8 +753,8 @@ x_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xb, float2* __res
   __syncthreads();                                 // the zero padding of the first two buffers is in place
   int it = 0;
   for (int m = m0; m < m1; ++m, ++it) {
-    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
-    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    s.wait(it);
+    float* gr = s.buf(it);
     float* gi = gr + fft8k::kPlaneG;
     if (m >= nwin) {                               // deinterleave the partition's (left, right) pairs into the planes
       const int64_t lim = leff - (int64_t)((m - nwin) % J) * kB;      // taps e < lim exist (lim > 0)
@@ -760,20 +795,14 @@ ifft_mix_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddle
   const int m0 = blockIdx.x * kConvRun;            // this CTA's blocks [m0, m1)
   const int m1 = nblocks - m0 < kConvRun ? nblocks : m0 + kConvRun;
   auto fetch = [&](int it, int m) {
-    if (t != 0 || m >= m1) return;
-    uint64_t* bar = &s.full[it & 1];
-    float* dst = s.G + (it & 1) * 2 * fft8k::kPlaneG;
-    const float* src = Ypl + (int64_t)m * 2 * kNbA;
-    mbar_arrive_expect_tx(bar, 2u * kNbA * 4u);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
+    if (t == 0 && m < m1) s.load_planar(it, Ypl + (int64_t)m * 2 * kNbA);
   };
   fetch(0, m0);
   fetch(1, m0 + 1);
   int it = 0;
   for (int m = m0; m < m1; ++m, ++it) {
-    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
-    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    s.wait(it);
+    float* gr = s.buf(it);
     float xr[16], xi[16];
     const int64_t il = m / I, b = item0 + il;
     const int i = m - (int)il * I;
@@ -830,7 +859,7 @@ g_fft_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, const float*
     if (m >= nblocks) return;
     const int64_t il = m / I;
     const int i = m - (int)il * I;
-    float* re = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    float* re = s.buf(it);
     float* im = re + fft8k::kPlaneG;
     const int64_t s0 = (int64_t)i * kB;            // first sample of the block (lands at offset kB of the window)
     const int64_t rem = n - s0;
@@ -850,8 +879,8 @@ g_fft_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, const float*
   __syncthreads();
   int it = 0;
   for (int m = blockIdx.x; m < nblocks; m += gridDim.x, ++it) {
-    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
-    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    s.wait(it);
+    float* gr = s.buf(it);
     float xr_[16], xi_[16];
     fft8192_in_smem<false>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr_, xi_);
     float2* out = Gb + (int64_t)m * kNbA;
@@ -880,19 +909,14 @@ ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles
     if (t != 0 || it >= total) return;
     const int64_t il = blockIdx.x + (int64_t)(it / I) * gridDim.x;
     const int i = it % I;
-    uint64_t* bar = &s.full[it & 1];
-    float* dst = s.G + (it & 1) * 2 * fft8k::kPlaneG;
-    const float* src = Dpl + (il * I + i) * (int64_t)(2 * kNbA);
-    mbar_arrive_expect_tx(bar, 2u * kNbA * 4u);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
+    s.load_planar(it, Dpl + (il * I + i) * (int64_t)(2 * kNbA));
   };
   fetch(0);
   fetch(1);
   float pr[8], pi[8];                                // second half of the previous window of this item
   for (int it = 0; it < total; ++it) {
-    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
-    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    s.wait(it);
+    float* gr = s.buf(it);
     const int64_t il = blockIdx.x + (int64_t)(it / I) * gridDim.x, b = item0 + il;
     const int i = it % I;
     const float mix = mix_p[b * mix_stride];
@@ -962,6 +986,26 @@ ifft_dx_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles
   }
 }
 
+// The partials of the 24 band-parameter gradients of a block: part[2k] = the sum of s0[k] and part[2k + 1] = the sum of
+// s1[k] over the block's threads (t = threadIdx.x), warp by warp and then over the nwarps warps in order from warp 0
+// (the order fixes the bits of the parameter gradients).  red: [nwarps][24] floats of shared memory, which the caller
+// rewrites only behind a later barrier.
+__device__ __forceinline__ void block_band_sums(const float (&s0)[kBands], const float (&s1)[kBands],
+                                                float (*red)[2 * kBands], int nwarps, int t, float* part) {
+  const int lane = t & 31, warp = t >> 5;
+#pragma unroll
+  for (int k = 0; k < kBands; ++k) {
+    const float x0 = warp_sum(s0[k]), x1 = warp_sum(s1[k]);
+    if (lane == 0) { red[warp][2 * k] = x0; red[warp][2 * k + 1] = x1; }
+  }
+  __syncthreads();
+  if (t < 2 * kBands) {
+    float acc = 0.f;
+    for (int w = 0; w < nwarps; ++w) acc += red[w][t];
+    part[t] = acc;
+  }
+}
+
 // unit (il, j): dIR taps [j kB, (j+1) kB) = first half of IFFT(Epl[il][j]) (left, right);
 // part[((il*J + j)*12 + k)*2 + {0,1}] = sum_t (dIR_l f_l + dIR_r f_r) env_k(t) {1, tt(t)}  over the partition's taps,
 // f in the polyphase layout C[((il*12 + k)*R + c)*nb + a] = f[R a + c].
@@ -979,13 +1023,7 @@ ifft_irgrad_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
   auto fetch = [&](int it, int m) {
-    if (t != 0 || m >= nunits) return;
-    uint64_t* bar = &s.full[it & 1];
-    float* dst = s.G + (it & 1) * 2 * fft8k::kPlaneG;
-    const float* src = Epl + (int64_t)m * 2 * kNbA;
-    mbar_arrive_expect_tx(bar, 2u * kNbA * 4u);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
+    if (t == 0 && m < nunits) s.load_planar(it, Epl + (int64_t)m * 2 * kNbA);
   };
   fetch(0, blockIdx.x);
   fetch(1, blockIdx.x + gridDim.x);
@@ -993,15 +1031,15 @@ ifft_irgrad_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
   float2* D = reinterpret_cast<float2*>(s.Yr);        // the partition's taps, after pass 4 has consumed Y
   int it = 0;
   for (int m = blockIdx.x; m < nunits; m += gridDim.x, ++it) {
-    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
-    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    s.wait(it);
+    float* gr = s.buf(it);
     const int64_t il = m / J;
     const int j = m - (int)il * J;
     const int lo = j * kB, hi = (lo + kB < leff) ? lo + kB : leff;      // taps [lo, hi)
     float xr[16], xi[16];
     fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
     __syncthreads();                                  // every thread is done reading Y (pass 4) and the previous unit's D
-    if (t < kBands) rk[t] = -(params[il * 25 + kBands + t] * 10.0f + 1.0f);
+    if (t < kBands) rk[t] = band_rate(params, il, t);
     if (t == 0) {
       int off = 0;
       for (int c = 0; c < R; ++c) {
@@ -1038,19 +1076,7 @@ ifft_irgrad_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
         s1[k] = fmaf(w, tt, s1[k]);
       }
     }
-    const int lane = t & 31, warp = t >> 5;
-#pragma unroll
-    for (int k = 0; k < kBands; ++k) {
-      const float x0 = warp_sum(s0[k]), x1 = warp_sum(s1[k]);
-      if (lane == 0) { red[warp][2 * k] = x0; red[warp][2 * k + 1] = x1; }
-    }
-    __syncthreads();
-    if (t < 2 * kBands) {
-      float acc = 0.f;
-#pragma unroll
-      for (int w = 0; w < kFusedThreads / 32; ++w) acc += red[w][t];
-      part[((int64_t)m * kBands) * 2 + t] = acc;
-    }
+    block_band_sums(s0, s1, red, kFusedThreads / 32, t, part + ((int64_t)m * kBands) * 2);
     // red / rk / cls_* / D are rewritten only after the __syncthreads that follows the next transform
   }
 }
@@ -1061,9 +1087,9 @@ ifft_irgrad_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
 //
 // One thread-block CLUSTER of R CTAs per item; CTA c owns polyphase class c, i.e. the IR taps R a + c.  The clusters are
 // persistent (as many as the device co-schedules) and walk the chunk's items.  Every CTA has two roles:
-//   * warps 0-15 (4 warpgroups): the in-shared-memory inverse FFT of fft8192.cuh on the class spectrum of each band,
-//     then exactly the epilogue of ifft_shape_kernel (envelope rho recurrence, accumulation over bands in registers,
-//     IR taps < leff into the partition layout, f into the polyphase f_save layout);
+//   * warps 0-15 (4 warpgroups): the band loop of ifft_shape_kernel on the same device functions (fft8192_in_smem on
+//     the class spectrum of each band, shape_band, store_ir_taps; f into the polyphase f_save layout), so the two give
+//     the same bits;
 //   * warps 16-27 (3 warpgroups): spectral_unit<R> for the bands ahead of the one being transformed.  The 12 (nb/2 + 1)
 //     class pairs of an item are dealt round-robin over the R * 384 generator threads of the cluster; a unit's R
 //     results go to the R CTAs as st.async stores into the planar buffer G[band & 1] of that CTA, which complete bytes
@@ -1120,9 +1146,6 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
         : "memory");
   } while (!done);
 }
-// the 512 FFT threads only (named barrier 1; barrier 0 is __syncthreads)
-__device__ __forceinline__ void fft_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kFusedThreads) : "memory"); }
-
 template <int R>
 __global__ void __launch_bounds__(kSynthThreads, 1)
 ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles, const float* __restrict__ params,
@@ -1132,18 +1155,16 @@ ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__
   constexpr int CT = R * NG, total = kBands * U;
   constexpr uint32_t kBandBytes = 2u * nb * 4u;    // one class spectrum, planar re / im
   extern __shared__ __align__(128) float sm[];
-  float* G = sm;                                   // [parity][re, im][8192]
-  float* Yr = sm + 4 * fft8k::kPlaneG;
-  float* Yi = Yr + fft8k::kPlaneY;
-  float* tabf = Yi + fft8k::kPlaneY;
-  uint64_t* full = reinterpret_cast<uint64_t*>(tabf + fft8k::kTabFloats);
+  const FftSmem s(sm);                             // G, Y and the tables; s.full is not used:
+  // full[2] and empty[2] follow the tables directly (no pad, kSynthSmemBytes)
+  uint64_t* full = reinterpret_cast<uint64_t*>(s.tabf + fft8k::kTabFloats);
   uint64_t* empty = full + 2;
   const int t = threadIdx.x;
   const unsigned c = cluster_ctarank();
   const int my_items = items > (int)blockIdx.y ? (items - 1 - (int)blockIdx.y) / (int)gridDim.y + 1 : 0;
   const int nbands = my_items * kBands;            // bands this cluster walks: g = item iteration * 12 + band
 
-  for (int e = t; e < fft8k::kTabFloats; e += NT) tabf[e] = twiddles[e];
+  for (int e = t; e < fft8k::kTabFloats; e += NT) s.tabf[e] = twiddles[e];
   if (t == 0) {
     mbar_init(&full[0], 1);
     mbar_init(&full[1], 1);
@@ -1163,7 +1184,7 @@ ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kSynthGenRegs));
     const int gt = t - kFusedThreads;
     const PhiloxKeys keys = philox_keys(__ldg(seed));
-    const uint32_t g_local = smem_u32(G), full_local = smem_u32(full);
+    const uint32_t g_local = smem_u32(s.G), full_local = smem_u32(full);
     int waited = 1;                                // bands < 2 need no free buffer
     for (int i = 0; i < my_items; ++i) {
       const int64_t il = blockIdx.y + (int64_t)i * gridDim.y;
@@ -1190,9 +1211,9 @@ ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__
       }
     }
   } else {
-    // ---------------- inverse FFT + shaping (the body of ifft_shape_kernel)
+    // ---------------- inverse FFT + shaping (the band loop of ifft_shape_kernel)
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kSynthFftRegs));
-    const fft8k::Tables tb = fft8k::carve_tables(tabf);
+    const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
     const float step = 1.0f / (float)(L - 1);
     for (int i = 0; i < my_items; ++i) {
       const int64_t il = blockIdx.y + (int64_t)i * gridDim.y;
@@ -1204,52 +1225,25 @@ ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__
         // one warp polls the barrier, the others sleep in bar.sync instead of taking issue slots from the generators
         if (t < 32) mbar_wait_cluster(&full[k & 1], (uint32_t)((g >> 1) & 1));
         fft_sync();
-        float* gr = G + (k & 1) * 2 * fft8k::kPlaneG;
-        float* gi = gr + fft8k::kPlaneG;
-        fft8k::p1<true>(gr, gi, tb, t);
-        fft_sync();
-        fft8k::p2<true>(gr, gi, Yr, Yi, tb, t);
-        fence_proxy_async_smem();                  // pass-1 stores to G before the generators' next stores there
-        fft_sync();
-        if (t == 0 && g + 2 < nbands) {            // hand G[k & 1] back for band g + 2
-          mbar_arrive_expect_tx(&full[k & 1], kBandBytes);
-          fence_cluster();
-#pragma unroll
-          for (int b = 0; b < R; ++b) {
-            mbar_arrive_remote(mapa_u32(smem_u32(&empty[k & 1]), (uint32_t)b));
-          }
-        }
-        fft8k::P3Regs q3;
-        fft8k::p3_load<true>(Yr, Yi, t, q3);
-        fft_sync();
-        fft8k::p3_store<true>(Yr, Yi, tb, t, q3);
-        fft_sync();
+        float* gr = s.buf(k);
         float xr[16], xi[16];
-        fft8k::p4<true>(Yr, Yi, t, xr, xi);
-        float e_prev = 0.f;
-        const float g_k = params[il * 25 + k] * (1.0f / kBands), rr = -(params[il * 25 + kBands + k] * 10.0f + 1.0f);
-        float2* fout = Csave ? Csave + ((il * kBands + k) * R + c) * (int64_t)nb : nullptr;
-        // the envelope of ifft_shape_kernel, bit for bit: evaluated at every 4th tap, stepped by rho in between
-        const float rho = __expf(rr * step * (float)(512 * R));
+        fft8192_in_smem<true, true>(gr, gr + fft8k::kPlaneG, s, tb, t,
+                                    [&] {
+                                      if (t == 0 && g + 2 < nbands) {      // hand G[k & 1] back for band g + 2
+                                        mbar_arrive_expect_tx(&full[k & 1], kBandBytes);
+                                        fence_cluster();
 #pragma unroll
-        for (int q = 0; q < 16; ++q) {
-          const int a = t + 512 * q;
-          float e;
-          if ((q & 3) == 0) e = g_k * __expf(rr * time_axis32(R * a + (int)c, L, step));
-          else e = e_prev * rho;
-          e_prev = e;
-          accr[q] = fmaf(e, xr[q], accr[q]);
-          acci[q] = fmaf(e, xi[q], acci[q]);
-          if (fout) fout[a] = make_float2(xr[q], xi[q]);
-        }
+                                        for (int b = 0; b < R; ++b) {
+                                          mbar_arrive_remote(mapa_u32(smem_u32(&empty[k & 1]), (uint32_t)b));
+                                        }
+                                      }
+                                    },
+                                    [] {}, xr, xi);
+        shape_band(xr, xi, band_gain(params, il, k), band_rate(params, il, k), R, (int)c, L, step, t,
+                   Csave ? Csave + ((il * kBands + k) * R + c) * (int64_t)nb : nullptr, accr, acci);
         // (Y is next written by pass 2 of the following band, behind the barrier after its pass 1)
       }
-      float2* out = Hb + il * (int64_t)jb * kNbA;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) {
-        const int tau = R * (t + 512 * q) + (int)c;
-        if (tau < leff) out[(tau / kB) * kNbA + (tau % kB)] = make_float2(accr[q], acci[q]);
-      }
+      store_ir_taps(Hb, il, jb, R, (int)c, leff, t, accr, acci);
     }
   }
   // no CTA may leave while a remote store or arrive could still target it
@@ -1264,10 +1258,9 @@ __global__ void ir_grad_pp_kernel(const float2* __restrict__ Et, const float2* _
   const int64_t il = blockIdx.y;
   __shared__ float rk[kBands];
   __shared__ float red[8][2 * kBands];
-  if (threadIdx.x < kBands) rk[threadIdx.x] = -(params[il * 25 + kBands + threadIdx.x] * 10.0f + 1.0f);
+  if (threadIdx.x < kBands) rk[threadIdx.x] = band_rate(params, il, threadIdx.x);
   __syncthreads();
   const float step = 1.0f / (float)(L - 1);
-  const float2* de = Et + il * (int64_t)jb * kNbA;       // dL/dIR (left, right) in the first half of partition t/kB
   const float2* cb = C + (il * kBands) * (int64_t)R * nb;
   float s0[kBands], s1[kBands];
 #pragma unroll
@@ -1279,8 +1272,8 @@ __global__ void ir_grad_pp_kernel(const float2* __restrict__ Et, const float2* _
     const bool has2 = t2 < leff;
     const int a = t / R, ph = t - a * R;
     const int a2 = has2 ? t2 / R : a, ph2 = has2 ? t2 - a2 * R : ph;
-    const float2 gd = de[(t / kB) * kNbA + (t % kB)];
-    const float2 gd2 = has2 ? de[(t2 / kB) * kNbA + (t2 % kB)] : make_float2(0.f, 0.f);
+    const float2 gd = Et[ir_slot(il, jb, t)];
+    const float2 gd2 = has2 ? Et[ir_slot(il, jb, t2)] : make_float2(0.f, 0.f);
     const float2* c0 = cb + (int64_t)ph * nb + a;
     const float2* c1 = cb + (int64_t)ph2 * nb + a2;
     float2 v[kBands], v2[kBands];
@@ -1295,18 +1288,8 @@ __global__ void ir_grad_pp_kernel(const float2* __restrict__ Et, const float2* _
       s1[k] = fmaf(w, tt, fmaf(w2, tt2, s1[k]));
     }
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kBands; ++k) {
-    const float x0 = warp_sum(s0[k]), x1 = warp_sum(s1[k]);
-    if (lane == 0) { red[warp][2 * k] = x0; red[warp][2 * k + 1] = x1; }
-  }
-  __syncthreads();
-  if (threadIdx.x < 2 * kBands) {
-    float acc = 0.f;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) acc += red[w][threadIdx.x];
-    part[((il * gridDim.x + blockIdx.x) * kBands) * 2 + threadIdx.x] = acc;
-  }
+  block_band_sums(s0, s1, red, (int)(blockDim.x >> 5), threadIdx.x,
+                  part + ((il * gridDim.x + blockIdx.x) * kBands) * 2);
 }
 
 // ---- audio convolution: uniformly partitioned overlap-save in the frequency domain -----------------
@@ -1547,10 +1530,9 @@ __global__ void ir_grad_pairs_kernel(const float2* __restrict__ Et, const float2
   const int64_t il = blockIdx.y;
   __shared__ float rk[kBands];
   __shared__ float red[8][2 * kBands];
-  if (threadIdx.x < kBands) rk[threadIdx.x] = -(params[il * 25 + kBands + threadIdx.x] * 10.0f + 1.0f);
+  if (threadIdx.x < kBands) rk[threadIdx.x] = band_rate(params, il, threadIdx.x);
   __syncthreads();
   const float step = 1.0f / (float)(L - 1);
-  const float2* de = Et + il * (int64_t)jb * kNbA;
   float s0[kBands], s1[kBands];
 #pragma unroll
   for (int k = 0; k < kBands; ++k) { s0[k] = 0.f; s1[k] = 0.f; }
@@ -1558,7 +1540,7 @@ __global__ void ir_grad_pairs_kernel(const float2* __restrict__ Et, const float2
     const int64_t t = (int64_t)b * hop + m;
     if (t >= leff) break;
     const float tt = time_axis(t, L, step);
-    const float2 gd = de[(t / kB) * kNbA + (t % kB)];
+    const float2 gd = Et[ir_slot(il, jb, t)];
     const float gl = gd.x, gr = gd.y;
     const float2* c = C + ((il * kBands) * nbk + b) * (int64_t)nb + m + P;
 #pragma unroll
@@ -1569,18 +1551,7 @@ __global__ void ir_grad_pairs_kernel(const float2* __restrict__ Et, const float2
       s1[k] = fmaf(w, tt, s1[k]);
     }
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kBands; ++k) {
-    const float a = warp_sum(s0[k]), c1 = warp_sum(s1[k]);
-    if (lane == 0) { red[warp][2 * k] = a; red[warp][2 * k + 1] = c1; }
-  }
-  __syncthreads();
-  if (threadIdx.x < 2 * kBands) {
-    float a = 0.f;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) a += red[w][threadIdx.x];
-    part[((il * nbk + b) * kBands) * 2 + threadIdx.x] = a;
-  }
+  block_band_sums(s0, s1, red, (int)(blockDim.x >> 5), threadIdx.x, part + ((il * nbk + b) * kBands) * 2);
 }
 
 // one thread per (item, param): gains (0..11), decays (12..23), mix (24).  The dL/dIR partials come from gradient
@@ -1622,7 +1593,7 @@ __global__ void ir_pack_kernel(const float* __restrict__ ir, float2* __restrict_
   if (t >= leff) return;
   const float* rl = ir + ((item0 + il) * ir_chs) * L;
   const float* rr = ir_chs == 1 ? rl : rl + L;
-  Hb[(il * J + t / kB) * (int64_t)kNbA + t % kB] = make_float2(rl[t], rr[t]);
+  Hb[ir_slot(il, J, t)] = make_float2(rl[t], rr[t]);
 }
 
 // unit m = il*J + j: dL/dIR taps [j kB, (j+1) kB) ∩ [0, leff) = mix * first half of IFFT(Epl[m]) (left, right), written
@@ -1637,20 +1608,14 @@ ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
   s.init(twiddles, t);
   const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
   auto fetch = [&](int it, int m) {
-    if (t != 0 || m >= nunits) return;
-    uint64_t* bar = &s.full[it & 1];
-    float* dst = s.G + (it & 1) * 2 * fft8k::kPlaneG;
-    const float* src = Epl + (int64_t)m * 2 * kNbA;
-    mbar_arrive_expect_tx(bar, 2u * kNbA * 4u);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) tma_load_1d(dst + q * 4096, src + q * 4096, 16384u, bar);
+    if (t == 0 && m < nunits) s.load_planar(it, Epl + (int64_t)m * 2 * kNbA);
   };
   fetch(0, blockIdx.x);
   fetch(1, blockIdx.x + gridDim.x);
   int it = 0;
   for (int m = blockIdx.x; m < nunits; m += gridDim.x, ++it) {
-    mbar_wait(&s.full[it & 1], (uint32_t)((it >> 1) & 1));
-    float* gr = s.G + (it & 1) * 2 * fft8k::kPlaneG;
+    s.wait(it);
+    float* gr = s.buf(it);
     const int64_t il = m / J, b = item0 + il;
     const int j = m - (int)il * J;
     float xr[16], xi[16];
@@ -1679,7 +1644,7 @@ __global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float*
   float2 v = make_float2(0.f, 0.f);
   float mx = 0.f;
   if (t < leff) {
-    v = Et[(il * J + t / kB) * (int64_t)kNbA + t % kB];
+    v = Et[ir_slot(il, J, t)];
     mx = mix ? mix[b] : 1.f;
   }
   float* row = gir + (b * ir_chs) * L;
@@ -1757,9 +1722,7 @@ int get_filterbank(const Geom& g, double sr, cudaStream_t st, const float2** out
   int rc = get_plan(2, g.nb, kBands, g.nb, g.nb, pv);
   if (rc != DASP_OK) return rc;
   DASP_CUDA_OK(cudaMalloc(&d_work, pv.work > 0 ? pv.work : 16));
-  DASP_CUFFT_OK(cufftSetStream(pv.h, st));
-  DASP_CUFFT_OK(cufftSetWorkArea(pv.h, d_work));
-  DASP_CUFFT_OK(cufftExecC2C(pv.h, d_buf, d_buf, CUFFT_FORWARD));
+  if ((rc = exec_c2c(pv, d_work, d_buf, CUFFT_FORWARD, st)) != DASP_OK) return rc;
   DASP_CUDA_OK(cudaStreamSynchronize(st));   // one-off (cache fill): host vector and temp buffers die here
   cudaFree(d_work);
   g_fb[key] = d_buf;
@@ -2073,6 +2036,9 @@ void launch_mac(const float2* A, const float2* Bm, float2* Out, int na, int nbm,
   else              partition_mac_kernel<0, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
 }
 
+// grid of a persistent FFT kernel: one CTA per SM, at most one per unit of work
+unsigned persistent_grid(int64_t units) { return (unsigned)(units < sm_count() ? units : sm_count()); }
+
 // one-off opt-in to the large dynamic shared memory of the FFT kernels (per device, guarded by g_mu)
 int configure_fft_kernels() {
   static std::map<int, bool> configured;
@@ -2122,10 +2088,7 @@ int conv_shared_ir_spectra(const ConvGeom& g, const PlanVal& ir1, bool own, cons
     DASP_LAUNCH_OK("x_fft_kernel");
     return DASP_OK;
   }
-  DASP_CUFFT_OK(cufftSetStream(ir1.h, st));
-  DASP_CUFFT_OK(cufftSetWorkArea(ir1.h, ws + w.cufft));
-  DASP_CUFFT_OK(cufftExecC2C(ir1.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
-  return DASP_OK;
+  return exec_c2c(ir1, ws + w.cufft, hs, CUFFT_FORWARD, st);
 }
 
 // y = (1 - mix) x + mix (x * IR), mix of item b at mix[b * mix_stride].  The caller has written IR taps t < leff as
@@ -2155,19 +2118,14 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
     return DASP_OK;
   }
   void* cufft = ws + w.cufft;
-  if (h_stride != 0) {
-    DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)hs, (cufftComplex*)hs, CUFFT_FORWARD));
-  }
+  int rc;
+  if (h_stride != 0 && (rc = exec_c2c(pl.hj, cufft, hs, CUFFT_FORWARD, st)) != DASP_OK) return rc;
   x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, g.n, in_chs);
   DASP_LAUNCH_OK("x_blocks_kernel");
-  DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
-  DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, cufft));
-  DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)xs, (cufftComplex*)xs, CUFFT_FORWARD));
+  if ((rc = exec_c2c(pl.xi, cufft, xs, CUFFT_FORWARD, st)) != DASP_OK) return rc;
   launch_mac<false>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
   DASP_LAUNCH_OK("partition_mac_kernel");
-  DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ys, (cufftComplex*)ys, CUFFT_INVERSE));
+  if ((rc = exec_c2c(pl.xi, cufft, ys, CUFFT_INVERSE, st)) != DASP_OK) return rc;
   mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ys, mix, mix_stride, y, item0, I, g.n, in_chs);
   DASP_LAUNCH_OK("mix_blocks_kernel");
   return DASP_OK;
@@ -2191,12 +2149,11 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
   const float inv = 1.0f / (float)kNbA;
   const int I = (int)g.ib, J = (int)g.jb;
   const bool fused = fused_corr(e, I, J);
+  int rc;
   if (own) {
-    int rc = configure_fft_kernels();
-    if (rc != DASP_OK) return rc;
+    if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
     const int nblk = (int)(items * I);
-    const unsigned fft_grid = (unsigned)(nblk < sm_count() ? nblk : sm_count());
-    g_fft_kernel<<<fft_grid, kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, I, g.n, nblk);
+    g_fft_kernel<<<persistent_grid(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, I, g.n, nblk);
     DASP_LAUNCH_OK("g_fft_kernel");
     if (fused) {
       dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
@@ -2207,20 +2164,17 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
       launch_mac<true, true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
       DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     }
-    const unsigned dx_grid = (unsigned)(items < sm_count() ? items : sm_count());
-    ifft_dx_kernel<<<dx_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gy, x, mix,
+    ifft_dx_kernel<<<persistent_grid(items), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gy, x, mix,
                                                                   mix_stride, gx, mixpart, item0, (int)items, I, g.n,
                                                                   in_chs);
     DASP_LAUNCH_OK("ifft_dx_kernel");
   } else {
     g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, gs, item0, I, g.n);
     DASP_LAUNCH_OK("g_blocks_kernel");
-    DASP_CUFFT_OK(cufftSetStream(pl.xi.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.xi.h, cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)gs, (cufftComplex*)gs, CUFFT_FORWARD));
+    if ((rc = exec_c2c(pl.xi, cufft, gs, CUFFT_FORWARD, st)) != DASP_OK) return rc;
     launch_mac<true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
-    DASP_CUFFT_OK(cufftExecC2C(pl.xi.h, (cufftComplex*)ds, (cufftComplex*)ds, CUFFT_INVERSE));
+    if ((rc = exec_c2c(pl.xi, cufft, ds, CUFFT_INVERSE, st)) != DASP_OK) return rc;
     finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ds, mix, mix_stride, gx, mixpart,
                                                                               item0, I, g.n, in_chs);
     DASP_LAUNCH_OK("finish_dx_blocks_kernel");
@@ -2232,9 +2186,7 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     launch_mac<true>(gs, xs, es, I, I, 1, J, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     if (e == IrGrad::kSpectra) return DASP_OK;
-    DASP_CUFFT_OK(cufftSetStream(pl.hj.h, st));
-    DASP_CUFFT_OK(cufftSetWorkArea(pl.hj.h, cufft));
-    DASP_CUFFT_OK(cufftExecC2C(pl.hj.h, (cufftComplex*)es, (cufftComplex*)es, CUFFT_INVERSE));
+    return exec_c2c(pl.hj, cufft, es, CUFFT_INVERSE, st);
   }
   return DASP_OK;
 }
@@ -2377,9 +2329,7 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       // device noise: draw the filtered spectrum directly, one inverse transform (polyphase layout)
       dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st, nullptr);
       DASP_LAUNCH_OK("spectral_gen_kernel");
-      DASP_CUFFT_OK(cufftSetStream(pl.pp.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.pp.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.pp.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_INVERSE));
+      if ((rc = exec_c2c(pl.pp, ws_cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
       shape_ir_pp_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(
           C, params + item0 * 25, hs, g.L, g.leff, J, (int)g.rpp, nb);
       DASP_LAUNCH_OK("shape_ir_pp_kernel");
@@ -2388,12 +2338,10 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
       if (noise) noise_pairs_layout_kernel<<<gblk, 256, 0, st>>>(noise, C, item0, nbk, nb, hop, lp);
       else       noise_pairs_philox_kernel<<<gblk, 256, 0, st>>>(C, item0, nbk, nb, hop, seed);
       DASP_LAUNCH_OK("reverb noise kernel");
-      DASP_CUFFT_OK(cufftSetStream(pl.blk.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(pl.blk.h, ws_cufft));
-      DASP_CUFFT_OK(cufftExecC2C(pl.blk.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_FORWARD));
+      if ((rc = exec_c2c(pl.blk, ws_cufft, C, CUFFT_FORWARD, st)) != DASP_OK) return rc;
       cmul_filter_pairs_kernel<<<gblk, 256, 0, st>>>(C, H, nbk, nb);
       DASP_LAUNCH_OK("cmul_filter_pairs_kernel");
-      DASP_CUFFT_OK(cufftExecC2C(pl.blk.h, (cufftComplex*)C, (cufftComplex*)C, CUFFT_INVERSE));
+      if ((rc = exec_c2c(pl.blk, ws_cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
       shape_ir_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, params + item0 * 25, hs, g.L, g.leff,
                                                                                J, nbk, nb, hop, P);
       DASP_LAUNCH_OK("shape_ir_pairs_kernel");
@@ -2452,8 +2400,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
     if (own_irgrad) {
       nparts = J;
       const int nunits = (int)(items * J);
-      const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-      ifft_irgrad_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, C,
+      ifft_irgrad_kernel<<<persistent_grid(nunits), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, C,
                                                                         params + item0 * 25, ws_irpart, (int)g.L,
                                                                         (int)g.leff, J, (int)g.rpp, nunits);
       DASP_LAUNCH_OK("ifft_irgrad_kernel");
@@ -2577,8 +2524,7 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
   auto ir_taps = [&](IrGrad e, int64_t item0, int64_t items, const float* mx) -> int {
     if (e == IrGrad::kPlanar) {
       const int nunits = (int)(items * J);
-      const unsigned ig_grid = (unsigned)(nunits < sm_count() ? nunits : sm_count());
-      ifft_irtaps_kernel<<<ig_grid, kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mx,
+      ifft_irtaps_kernel<<<persistent_grid(nunits), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mx,
                                                                         gir, item0, J, g.L, g.leff, (int)ir_chs, nunits);
       DASP_LAUNCH_OK("ifft_irtaps_kernel");
     }
@@ -2618,11 +2564,7 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
   }
   if (shared && gir) {
     // the summed partition spectra, rounded to fp32 in item 0's slot of es: J inverse transforms for the one IR
-    if (!own_conv) {
-      DASP_CUFFT_OK(cufftSetStream(s.ir1.h, st));
-      DASP_CUFFT_OK(cufftSetWorkArea(s.ir1.h, base + w.cufft));
-      DASP_CUFFT_OK(cufftExecC2C(s.ir1.h, (cufftComplex*)ws_es, (cufftComplex*)ws_es, CUFFT_INVERSE));
-    }
+    if (!own_conv && (rc = exec_c2c(s.ir1, base + w.cufft, ws_es, CUFFT_INVERSE, st)) != DASP_OK) return rc;
     if ((rc = ir_taps(own_conv ? IrGrad::kPlanar : IrGrad::kTime, 0, 1, nullptr)) != DASP_OK) return rc;
   }
   return DASP_OK;

@@ -81,6 +81,8 @@ _SIGNATURES = {
     "dasp_conv_shared_geometry": (c_int, [I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
     "dasp_conv_shared_fwd": (c_int, [P, I64, P, I64, I64, P, P, P, P, P, I64, I64, I64, I64, P]),
     "dasp_conv_shared_bwd": (c_int, [P, P, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, P]),
+    "dasp_conv_ts_geometry": (c_int, [I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
+    "dasp_conv_shared_ts_geometry": (c_int, [I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
     "dasp_debug_conv_last_path": (c_int, [c_int]),
     "dasp_dynamics_tile_len": (I64, [I64, I64]),
     "dasp_dynamics_fwd": (c_int, [c_int, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),

@@ -33,7 +33,9 @@
 // convolution is written once on the host: conv_fwd_chunk / conv_bwd_chunk run a chunk for both ops, on one ConvGeom,
 // one plan set (conv_setup) and one workspace layout per direction; each op adds only its IR fill, its mix stride and
 // its dL/dIR consumer.  One IR for the whole batch (dasp_conv_shared_*) is the item stride 0 of the IR spectra: they
-// are transformed once, and irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.
+// are transformed once, and irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.  A
+// true-stereo IR (ir_chs 4) is two partition sets per IR (ConvGeom::sets), multiplied by the TS variants of the MAC
+// kernels.
 //
 // Steps that several kernels share are written once: FftSmem (the shared-memory layout of the FFT kernels and their
 // double-buffered bulk-copy input), fft8192_in_smem (the four passes), shape_band / store_ir_taps (the epilogue of both
@@ -119,6 +121,7 @@ struct ConvGeom {
   int64_t ib, jb;               // output/input blocks of kB samples, IR partitions of kB taps
   int64_t chunk;
   bool shared = false;          // one impulse response for the whole batch (convolution_reverberation only)
+  int sets = 1;                 // partition sets per IR: 2 for a true-stereo IR (convolution_reverberation only)
 };
 
 int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
@@ -1340,17 +1343,26 @@ __device__ __forceinline__ void cfma_conj(float2& acc, float2 p, float2 q) {    
 // in registers (na, nbm <= MAXB); MAXB == 0: generic loop straight from L2.
 // PLANAR: every output block is stored as [re plane kNbA][im plane kNbA] (what ifft_mix_kernel bulk-copies into the
 // shared-memory layout of fft8192.cuh) instead of (re, im) pairs (what cuFFT reads).
-template <int MAXB, bool CORR, bool PLANAR = false>
+// TS: a true-stereo IR, stored as two partition sets per IR, set A = h_LL + i h_LR then set B = h_RL + i h_RR:
+//   TS == 1, forward: out[o] = sum_j XL[o-j] SA[j] + XR[o-j] SB[j], A untangled into (XL, XR), the sets SA = Bm[j] and
+//            SB = Bm[nbm + j] used as stored (A = H_LL + i H_LR, so this is the packed wet spectrum WL + i WR)
+//   TS == 1, CORR: DL[o] = sum_j GL[o+j] conj(H_LL[j]) + GR[o+j] conj(H_LR[j]), DR[o] likewise with H_RL, H_RR (both
+//            operands untangled), stored packed as DL + i DR: the dL/dx windows
+//   TS == 2, CORR: out[o] = sum_j A[o+j] conj(BL[j]), out[nout + o] = sum_j A[o+j] conj(BR[j]), A used as stored, B
+//            untangled: the dL/dIR partitions of set A (from XL) and set B (from XR)
+// Bm (TS == 1) and Out (TS == 2) then hold 2 nbm / 2 nout blocks per item.
+template <int MAXB, bool CORR, bool PLANAR = false, int TS = 0>
 __global__ void __launch_bounds__(128) partition_mac_kernel(const float2* __restrict__ A, const float2* __restrict__ Bm,
                                                             float2* __restrict__ Out, int na, int nbm, int nout,
                                                             float scale, int bstep) {
+  static_assert(TS == 0 || TS == 1 || (TS == 2 && CORR), "TS == 2 is the dL/dIR correlation");
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f > kNbA / 2) return;
   const int fm = (kNbA - f) & (kNbA - 1);
   const int64_t il = blockIdx.y;
   const float2* a = A + il * (int64_t)na * kNbA;
-  const float2* bq = Bm + (il * bstep) * (int64_t)nbm * kNbA;
-  float2* out = Out + il * (int64_t)nout * kNbA;
+  const float2* bq = Bm + (il * bstep) * (int64_t)(TS == 1 ? 2 : 1) * nbm * kNbA;
+  float2* out = Out + il * (int64_t)(TS == 2 ? 2 : 1) * nout * kNbA;
   auto emit = [&](int o, float2 sl, float2 sr) {
     sl.x *= scale; sl.y *= scale; sr.x *= scale; sr.y *= scale;
     if (PLANAR) {
@@ -1362,7 +1374,79 @@ __global__ void __launch_bounds__(128) partition_mac_kernel(const float2* __rest
       if (fm != f) out[(int64_t)o * kNbA + fm] = make_float2(sl.x + sr.y, sr.x - sl.y);   // conj(L) + i conj(R)
     }
   };
-  if constexpr (MAXB > 0) {
+  if constexpr (TS != 0) {
+    // a0, a1: block i of A (untangled, or for TS == 2 as stored at f and fm); b0..b3: partition j of Bm (TS == 1
+    // forward: set A at f, fm, set B at f, fm; TS == 1 CORR: H_LL, H_LR, H_RL, H_RR; TS == 2: BL, BR)
+    auto load_a = [&](int i, float2& a0, float2& a1) {
+      if (TS == 1) untangle(a[(int64_t)i * kNbA + f], a[(int64_t)i * kNbA + fm], a0, a1);
+      else { a0 = a[(int64_t)i * kNbA + f]; a1 = a[(int64_t)i * kNbA + fm]; }
+    };
+    auto load_b = [&](int j, float2& b0, float2& b1, float2& b2, float2& b3) {
+      const float2* sa = bq + (int64_t)j * kNbA;
+      const float2* sb = sa + (int64_t)nbm * kNbA;
+      if (TS == 2) { untangle(sa[f], sa[fm], b0, b1); b2 = b3 = make_float2(0.f, 0.f); }
+      else if (CORR) { untangle(sa[f], sa[fm], b0, b1); untangle(sb[f], sb[fm], b2, b3); }
+      else { b0 = sa[f]; b1 = sa[fm]; b2 = sb[f]; b3 = sb[fm]; }
+    };
+    // one product term: block ia of A with partition j of Bm into the accumulators (p, q) of output pair (f, fm) or
+    // (TS == 1 CORR) (DL, DR), and for TS == 2 (r, s) of set B's output
+    auto term = [&](float2 a0, float2 a1, float2 b0, float2 b1, float2 b2, float2 b3, float2& p, float2& q, float2& r,
+                    float2& s) {
+      if (TS == 2) { cfma_conj(p, a0, b0); cfma(q, a1, b0); cfma_conj(r, a0, b1); cfma(s, a1, b1); }
+      else if (CORR) { cfma_conj(p, a0, b0); cfma_conj(p, a1, b1); cfma_conj(q, a0, b2); cfma_conj(q, a1, b3); }
+      else { cfma(p, a0, b0); cfma(p, a1, b2); cfma_conj(q, b1, a0); cfma_conj(q, b3, a1); }   // conj(XL(f)) = XL(fm)
+    };
+    auto store = [&](int o, float2 p, float2 q) {
+      p.x *= scale; p.y *= scale; q.x *= scale; q.y *= scale;
+      if (PLANAR) {
+        float* pl = reinterpret_cast<float*>(out + (int64_t)o * kNbA);
+        pl[f] = p.x; pl[kNbA + f] = p.y;
+        if (fm != f) { pl[fm] = q.x; pl[kNbA + fm] = q.y; }
+      } else {
+        out[(int64_t)o * kNbA + f] = p;
+        if (fm != f) out[(int64_t)o * kNbA + fm] = q;
+      }
+    };
+    auto finish = [&](int o, float2 p, float2 q, float2 r, float2 s) {
+      if (TS == 2) { store(o, p, q); store(nout + o, r, s); }
+      else if (CORR) emit(o, p, q);
+      else store(o, p, q);
+    };
+    if constexpr (MAXB > 0) {
+      float2 a0[MAXB], a1[MAXB], b0[MAXB], b1[MAXB], b2[MAXB], b3[MAXB];
+#pragma unroll
+      for (int i = 0; i < MAXB; ++i) {
+        a0[i] = a1[i] = b0[i] = b1[i] = b2[i] = b3[i] = make_float2(0.f, 0.f);   // operands beyond na / nbm are zero
+        if (i < na) load_a(i, a0[i], a1[i]);
+        if (i < nbm) load_b(i, b0[i], b1[i], b2[i], b3[i]);
+      }
+#pragma unroll
+      for (int o = 0; o < MAXB; ++o) {
+        if (o < nout) {
+          float2 p = make_float2(0.f, 0.f), q = p, r = p, s = p;
+#pragma unroll
+          for (int j = 0; j < MAXB; ++j) {
+            const int ia = CORR ? o + j : o - j;                     // compile-time after unrolling
+            if (ia >= 0 && ia < MAXB) term(a0[ia], a1[ia], b0[j], b1[j], b2[j], b3[j], p, q, r, s);
+          }
+          finish(o, p, q, r, s);
+        }
+      }
+    } else {
+      for (int o = 0; o < nout; ++o) {
+        float2 p = make_float2(0.f, 0.f), q = p, r = p, s = p;
+        for (int j = 0; j < nbm; ++j) {
+          const int ia = CORR ? o + j : o - j;
+          if (ia < 0 || ia >= na) continue;
+          float2 a0, a1, b0, b1, b2, b3;
+          load_a(ia, a0, a1);
+          load_b(j, b0, b1, b2, b3);
+          term(a0, a1, b0, b1, b2, b3, p, q, r, s);
+        }
+        finish(o, p, q, r, s);
+      }
+    }
+  } else if constexpr (MAXB > 0) {
     float2 al[MAXB], ar[MAXB], bl[MAXB], br[MAXB];
 #pragma unroll
     for (int i = 0; i < MAXB; ++i) {
@@ -1407,7 +1491,10 @@ __global__ void __launch_bounds__(128) partition_mac_kernel(const float2* __rest
 //   E[j] = sum_{p<I, j+p<I} G[j+p] conj(X[p])  (j < J)   dL/dIR partitions
 // G is read and untangled once; H and X take turns in the same registers.  Planar outputs (own inverse FFT kernels).
 // H's item stride is hstride (J kNbA, or 0 for IR spectra shared by the batch).
-template <int MAXB>
+// TS: a true-stereo IR (two partition sets, see partition_mac_kernel; hstride 2 J kNbA or 0): the products of
+// partition_mac_kernel<TS 1, CORR> into D and of <TS 2> into the 2 J partitions per item of E, the latter from G
+// repacked out of its untangled halves.
+template <int MAXB, bool TS = false>
 __global__ void __launch_bounds__(128) partition_mac_bwd_kernel(const float2* __restrict__ G, const float2* __restrict__ H,
                                                                 int64_t hstride, const float2* __restrict__ X,
                                                                 float2* __restrict__ D, float2* __restrict__ E, int I,
@@ -1423,28 +1510,83 @@ __global__ void __launch_bounds__(128) partition_mac_bwd_kernel(const float2* __
     al[i] = ar[i] = make_float2(0.f, 0.f);
     if (i < I) untangle(g[(int64_t)i * kNbA + f], g[(int64_t)i * kNbA + fm], al[i], ar[i]);
   }
+  if constexpr (TS) {
+    auto store = [&](float2* blk, float2 p, float2 q) {
+      float* pl = reinterpret_cast<float*>(blk);
+      pl[f] = p.x * scale; pl[kNbA + f] = p.y * scale;
+      if (fm != f) { pl[fm] = q.x * scale; pl[kNbA + fm] = q.y * scale; }
+    };
+    float2 cl[MAXB], cr[MAXB];                     // bl, br, cl, cr: H_LL, H_LR, H_RL, H_RR, then XL, XR
+    const float2* h = H + il * hstride;
 #pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    const float2* bq = (pass == 0 ? H + il * hstride : X + il * (int64_t)I * kNbA);
-    const int nbm = pass == 0 ? J : I, nout = pass == 0 ? I : J;
-    float2* out = (pass == 0 ? D + il * (int64_t)I * kNbA : E + il * (int64_t)J * kNbA);
-#pragma unroll
-    for (int i = 0; i < MAXB; ++i) {
-      bl[i] = br[i] = make_float2(0.f, 0.f);
-      if (i < nbm) untangle(bq[(int64_t)i * kNbA + f], bq[(int64_t)i * kNbA + fm], bl[i], br[i]);
+    for (int j = 0; j < MAXB; ++j) {
+      bl[j] = br[j] = cl[j] = cr[j] = make_float2(0.f, 0.f);
+      if (j < J) {
+        untangle(h[(int64_t)j * kNbA + f], h[(int64_t)j * kNbA + fm], bl[j], br[j]);
+        untangle(h[(int64_t)(J + j) * kNbA + f], h[(int64_t)(J + j) * kNbA + fm], cl[j], cr[j]);
+      }
     }
 #pragma unroll
     for (int o = 0; o < MAXB; ++o) {
-      if (o < nout) {
-        float2 sl = make_float2(0.f, 0.f), sr = make_float2(0.f, 0.f);
+      if (o < I) {
+        float2 dl = make_float2(0.f, 0.f), dr = dl;
 #pragma unroll
         for (int j = 0; j < MAXB; ++j) {
-          if (o + j < MAXB) { cfma_conj(sl, al[o + j], bl[j]); cfma_conj(sr, ar[o + j], br[j]); }   // operands beyond I / nbm are zero
+          if (o + j < MAXB) {
+            cfma_conj(dl, al[o + j], bl[j]); cfma_conj(dl, ar[o + j], br[j]);
+            cfma_conj(dr, al[o + j], cl[j]); cfma_conj(dr, ar[o + j], cr[j]);
+          }
         }
-        sl.x *= scale; sl.y *= scale; sr.x *= scale; sr.y *= scale;
-        float* pl = reinterpret_cast<float*>(out + (int64_t)o * kNbA);
-        pl[f] = sl.x - sr.y; pl[kNbA + f] = sl.y + sr.x;
-        if (fm != f) { pl[fm] = sl.x + sr.y; pl[kNbA + fm] = sr.x - sl.y; }
+        store(D + (il * I + o) * (int64_t)kNbA, make_float2(dl.x - dr.y, dl.y + dr.x), make_float2(dl.x + dr.y, dr.x - dl.y));
+      }
+    }
+    const float2* xq = X + il * (int64_t)I * kNbA;
+#pragma unroll
+    for (int i = 0; i < MAXB; ++i) {
+      bl[i] = br[i] = make_float2(0.f, 0.f);
+      if (i < I) untangle(xq[(int64_t)i * kNbA + f], xq[(int64_t)i * kNbA + fm], bl[i], br[i]);
+      cl[i] = make_float2(al[i].x - ar[i].y, al[i].y + ar[i].x);          // G at f and fm, repacked
+      cr[i] = make_float2(al[i].x + ar[i].y, ar[i].x - al[i].y);
+    }
+#pragma unroll
+    for (int o = 0; o < MAXB; ++o) {
+      if (o < J) {
+        float2 pa = make_float2(0.f, 0.f), qa = pa, pb = pa, qb = pa;
+#pragma unroll
+        for (int p = 0; p < MAXB; ++p) {
+          if (o + p < MAXB) {
+            cfma_conj(pa, cl[o + p], bl[p]); cfma(qa, cr[o + p], bl[p]);
+            cfma_conj(pb, cl[o + p], br[p]); cfma(qb, cr[o + p], br[p]);
+          }
+        }
+        store(E + (il * 2 * J + o) * (int64_t)kNbA, pa, qa);
+        store(E + (il * 2 * J + J + o) * (int64_t)kNbA, pb, qb);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int pass = 0; pass < 2; ++pass) {
+      const float2* bq = (pass == 0 ? H + il * hstride : X + il * (int64_t)I * kNbA);
+      const int nbm = pass == 0 ? J : I, nout = pass == 0 ? I : J;
+      float2* out = (pass == 0 ? D + il * (int64_t)I * kNbA : E + il * (int64_t)J * kNbA);
+#pragma unroll
+      for (int i = 0; i < MAXB; ++i) {
+        bl[i] = br[i] = make_float2(0.f, 0.f);
+        if (i < nbm) untangle(bq[(int64_t)i * kNbA + f], bq[(int64_t)i * kNbA + fm], bl[i], br[i]);
+      }
+#pragma unroll
+      for (int o = 0; o < MAXB; ++o) {
+        if (o < nout) {
+          float2 sl = make_float2(0.f, 0.f), sr = make_float2(0.f, 0.f);
+#pragma unroll
+          for (int j = 0; j < MAXB; ++j) {
+            if (o + j < MAXB) { cfma_conj(sl, al[o + j], bl[j]); cfma_conj(sr, ar[o + j], br[j]); }   // operands beyond I / nbm are zero
+          }
+          sl.x *= scale; sl.y *= scale; sr.x *= scale; sr.y *= scale;
+          float* pl = reinterpret_cast<float*>(out + (int64_t)o * kNbA);
+          pl[f] = sl.x - sr.y; pl[kNbA + f] = sl.y + sr.x;
+          if (fm != f) { pl[fm] = sl.x + sr.y; pl[kNbA + fm] = sr.x - sl.y; }
+        }
       }
     }
   }
@@ -1585,23 +1727,28 @@ __global__ void reverb_param_grad_kernel(const float* __restrict__ ir_part, cons
 // the caller's rows by ifft_irtaps_kernel (or irtaps_unpack_kernel after the cuFFT inverse).
 
 // taps t < leff of the planar (bs, ir_chs, L) rows -> (left, right) pairs in the first half of partition slot t / kB
-// (a mono IR feeds both channels).  grid = (ceil(leff / 256), items)
+// (a mono IR feeds both channels).  A true-stereo IR (ir_chs 4, rows L->L, L->R, R->L, R->R) fills two partition sets
+// per item: set s = gridDim.z index packs rows 2s and 2s + 1 into the slots of (il * 2 + s).
+// grid = (ceil(leff / 256), items, 1 or 2 sets)
 __global__ void ir_pack_kernel(const float* __restrict__ ir, float2* __restrict__ Hb, int64_t item0, int J, int64_t L,
                                int64_t leff, int ir_chs) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t il = blockIdx.y;
+  const int s = blockIdx.z;
   if (t >= leff) return;
-  const float* rl = ir + ((item0 + il) * ir_chs) * L;
+  const float* rl = ir + ((item0 + il) * ir_chs + 2 * s) * L;
   const float* rr = ir_chs == 1 ? rl : rl + L;
-  Hb[ir_slot(il, J, t)] = make_float2(rl[t], rr[t]);
+  Hb[ir_slot(il * gridDim.z + s, J, t)] = make_float2(rl[t], rr[t]);
 }
 
-// unit m = il*J + j: dL/dIR taps [j kB, (j+1) kB) ∩ [0, leff) = mix * first half of IFFT(Epl[m]) (left, right), written
-// straight into the caller's (bs, ir_chs, L) rows; a mono IR receives the sum of both channels.  A null mix is a factor
-// of 1 (a shared IR's summed partitions carry their factors already).
+// unit m = (il*sets + s)*J + j: dL/dIR taps [j kB, (j+1) kB) ∩ [0, leff) = mix * first half of IFFT(Epl[m]) (left,
+// right), written straight into rows 2s, 2s + 1 of the caller's (bs, ir_chs, L) rows; a mono IR receives the sum of both
+// channels.  sets = 2 only for a true-stereo IR.  A null mix is a factor of 1 (a shared IR's summed partitions carry
+// their factors already).
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twiddles, const float* __restrict__ mix,
-                   float* __restrict__ gir, int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int nunits) {
+                   float* __restrict__ gir, int64_t item0, int J, int sets, int64_t L, int64_t leff, int ir_chs,
+                   int nunits) {
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
   const int t = threadIdx.x;
@@ -1616,12 +1763,13 @@ ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
   for (int m = blockIdx.x; m < nunits; m += gridDim.x, ++it) {
     s.wait(it);
     float* gr = s.buf(it);
-    const int64_t il = m / J, b = item0 + il;
-    const int j = m - (int)il * J;
+    const int q = m / J;                           // partition set il * sets + set
+    const int64_t il = q / sets, b = item0 + il;
+    const int j = m - q * J, set = q - (int)il * sets;
     float xr[16], xi[16];
     fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2 * gridDim.x); }, [] {}, xr, xi);
     const float mx = mix ? mix[b] : 1.0f;
-    float* row = gir + (b * ir_chs) * L;
+    float* row = gir + (b * ir_chs + 2 * set) * L;
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
       const int64_t tau = (int64_t)j * kB + t + 512 * q;
@@ -1635,19 +1783,21 @@ ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
 
 // dL/dIR taps [t0, L) of the caller's rows: mix * Et (inverse-transformed partitions, pairs in the first half of each
 // slot) below leff, 0 from leff on (those taps cannot reach an output).  t0 = leff writes only the zeros.  A null mix is
-// a factor of 1.  grid = (ceil((L - t0) / 256), items)
+// a factor of 1.  Partition set s (gridDim.z = 2 for a true-stereo IR) goes to rows 2s, 2s + 1.
+// grid = (ceil((L - t0) / 256), items, 1 or 2 sets)
 __global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float* __restrict__ mix, float* __restrict__ gir,
                                      int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int64_t t0) {
   const int64_t t = t0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t il = blockIdx.y, b = item0 + il;
+  const int s = blockIdx.z;
   if (t >= L) return;
   float2 v = make_float2(0.f, 0.f);
   float mx = 0.f;
   if (t < leff) {
-    v = Et[ir_slot(il, J, t)];
+    v = Et[ir_slot(il * gridDim.z + s, J, t)];
     mx = mix ? mix[b] : 1.f;
   }
-  float* row = gir + (b * ir_chs) * L;
+  float* row = gir + (b * ir_chs + 2 * s) * L;
   if (ir_chs == 1) row[t] = mx * (v.x + v.y);
   else { row[t] = mx * v.x; row[L + t] = mx * v.y; }
 }
@@ -1659,7 +1809,7 @@ __global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float*
 // of adding to it (the workspace is never cleared); the chunk that holds the last item writes the sum, rounded to fp32,
 // over item 0's slot of Et instead, for the inverse transforms (thread e alone reads and writes element e of every slot).
 // Element-wise, so it serves the planar (own FFT) and the interleaved (cuFFT) spectra alike.
-// grid = ceil(J kNbA / 256), one complex element of the J partitions per thread
+// grid = ceil(sets J kNbA / 256), one complex element of the sets * J partitions per thread
 __global__ void irgrad_sum_kernel(float2* Et, const float* __restrict__ mix, double2* __restrict__ acc, int64_t item0,
                                   int items, int64_t per_item, bool last) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1947,7 +2097,7 @@ void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs&
   w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   // transient homes for what a forward WITHOUT a backward does not keep (null *_save pointers)
   w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.hsp = o; o += align256(sizeof(float2) * (size_t)((g.shared ? 1 : g.chunk) * g.jb * kNbA));
+  w.hsp = o; o += align256(sizeof(float2) * (size_t)((g.shared ? 1 : g.chunk) * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
@@ -1956,10 +2106,10 @@ void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs&
   size_t o = 0;
   w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
+  w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.mixpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * g.ib));
-  w.acc = o; o += align256(g.shared ? sizeof(double2) * (size_t)(g.jb * kNbA) : 0);
+  w.acc = o; o += align256(g.shared ? sizeof(double2) * (size_t)(g.sets * g.jb * kNbA) : 0);
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
 }
@@ -1968,20 +2118,21 @@ void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs&
 // largest work area.  xi / hj: the block transforms of the convolution's cuFFT pipeline (audio / dL/dx windows, IR /
 // dL/dIR partitions).  With synth (the reverb) also blk / pp, its IR synthesis (overlap-save blocks, polyphase), and
 // the extra regions.  With g.shared also ir1: the J partitions of the one IR (forward) and of its summed gradient.
+// Every IR plan transforms g.sets partition sets of J partitions per IR.
 struct Plans { PlanVal xi, hj, blk, pp; };
 struct Setup { Plans full, rem; PlanVal ir1; FwdWs fwd; BwdWs bwd; };
 int conv_setup(const ConvGeom& g, const Geom* synth, Setup& s) {
   int rc;
   size_t work = 0;
   if (g.shared && g.bs > 0) {
-    if ((rc = get_plan(2, kNbA, g.jb, kNbA, kNbA, s.ir1)) != DASP_OK) return rc;
+    if ((rc = get_plan(2, kNbA, g.sets * g.jb, kNbA, kNbA, s.ir1)) != DASP_OK) return rc;
     work = s.ir1.work;
   }
   for (int64_t items : {g.bs > 0 ? g.chunk : 0, g.bs % g.chunk}) {
     if (items == 0) continue;
     Plans& p = items == g.chunk ? s.full : s.rem;
     if ((rc = get_plan(2, kNbA, items * g.ib, kNbA, kNbA, p.xi)) != DASP_OK) return rc;
-    if ((rc = get_plan(2, kNbA, items * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
+    if ((rc = get_plan(2, kNbA, items * g.sets * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
     if (p.xi.work > work) work = p.xi.work;
     if (p.hj.work > work) work = p.hj.work;
     if (synth) {
@@ -2019,21 +2170,21 @@ int put_conv_geometry(const ConvGeom& g, const Geom* synth, Out* out) {
   if (rc != DASP_OK) return rc;
   out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
   out->xspec_c64 = g.bs * g.ib * kNbA;
-  out->irspec_c64 = (g.shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.jb * kNbA;
+  out->irspec_c64 = (g.shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.sets * g.jb * kNbA;
   out->fwd_workspace_bytes = (int64_t)s.fwd.total;
   out->bwd_workspace_bytes = (int64_t)s.bwd.total;
   return DASP_OK;
 }
 
 // out = conv / corr of packed block spectra, register-cached when both operands have <= 16 blocks
-template <bool CORR, bool PLANAR = false>
+template <bool CORR, bool PLANAR = false, int TS = 0>
 void launch_mac(const float2* A, const float2* Bm, float2* Out, int na, int nbm, int bstep, int nout,
                 int64_t items, float scale, cudaStream_t st) {
   dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
   const int m = na > nbm ? na : nbm;
-  if (m <= 12)      partition_mac_kernel<12, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
-  else if (m <= 16) partition_mac_kernel<16, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
-  else              partition_mac_kernel<0, CORR, PLANAR><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
+  if (m <= 12)      partition_mac_kernel<12, CORR, PLANAR, TS><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
+  else if (m <= 16) partition_mac_kernel<16, CORR, PLANAR, TS><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
+  else              partition_mac_kernel<0, CORR, PLANAR, TS><<<grid, 128, 0, st>>>(A, Bm, Out, na, nbm, nout, scale, bstep);
 }
 
 // grid of a persistent FFT kernel: one CTA per SM, at most one per unit of work
@@ -2072,19 +2223,23 @@ enum class IrGrad {
   kTime,     // partitions after the inverse cuFFT C2C: (left, right) pairs in the first half of each slot
   kSpectra,  // partition spectra as (re, im) pairs, summed over a shared IR's items before the inverse cuFFT
 };
-// both correlations in one pass over the gradient spectra when the operands fit the register cache
-bool fused_corr(IrGrad e, int I, int J) { return e == IrGrad::kPlanar && (I > J ? I : J) <= 16; }
+// both correlations in one pass over the gradient spectra when the operands fit the register cache (a true-stereo IR,
+// sets == 2, caches twice the IR operands: kTsFusedMaxB)
+constexpr int kTsFusedMaxB = 16;
+bool fused_corr(IrGrad e, int I, int J, int sets) {
+  return e == IrGrad::kPlanar && (I > J ? I : J) <= (sets == 2 ? kTsFusedMaxB : 16);
+}
 
 // The partitions of an impulse response shared by the batch, transformed in place in hs once before the first chunk,
 // filled as conv_fwd_chunk expects them; own: x_fft_kernel with no audio windows, otherwise the J-batch cuFFT C2C.
 int conv_shared_ir_spectra(const ConvGeom& g, const PlanVal& ir1, bool own, const float* tw, float2* hs,
                            unsigned char* ws, const FwdWs& w, cudaStream_t st) {
-  const int J = (int)g.jb;
+  const int J = (int)g.jb, nparts = g.sets * J;
   if (own) {
     int rc = configure_fft_kernels();
     if (rc != DASP_OK) return rc;
-    x_fft_kernel<<<(unsigned)((J + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
-        nullptr, nullptr, hs, tw, 0, (int)g.ib, J, g.n, g.leff, 1, 0, J);
+    x_fft_kernel<<<(unsigned)((nparts + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
+        nullptr, nullptr, hs, tw, 0, (int)g.ib, J, g.n, g.leff, 1, 0, nparts);
     DASP_LAUNCH_OK("x_fft_kernel");
     return DASP_OK;
   }
@@ -2095,7 +2250,8 @@ int conv_shared_ir_spectra(const ConvGeom& g, const PlanVal& ir1, bool own, cons
 // (left, right) pairs into the first half of partition slot t / kB of hs, and on the cuFFT pipeline zero-filled the
 // slots first.  xs / hs receive the window / partition spectra.  own (own_fft_rows of x and hs): x_fft_kernel transforms
 // both on the own FFT with the tables tw; otherwise cuFFT C2C does.  h_stride: item stride of hs in complex elements,
-// J kNbA; 0 for one IR shared by the batch, whose partitions conv_shared_ir_spectra has transformed already.
+// g.sets J kNbA; 0 for one IR shared by the batch, whose partitions conv_shared_ir_spectra has transformed already.
+// g.sets == 2 (a true-stereo IR): hs holds set A then set B per IR, and the product is partition_mac_kernel<TS 1>.
 int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, int in_chs, float2* xs,
                    float2* hs, int64_t h_stride, const float* mix, int mix_stride, float* y, unsigned char* ws,
                    const FwdWs& w, int64_t item0, int64_t items, cudaStream_t st) {
@@ -2105,12 +2261,14 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
   if (own) {
     int rc = configure_fft_kernels();
     if (rc != DASP_OK) return rc;
-    // one work list: the items*I audio windows, then the items*J IR partitions (transformed in place in hs)
-    const int nunits = (int)(items * (I + (h_stride != 0 ? J : 0)));
+    // one work list: the items*I audio windows, then the items*sets*J IR partitions (transformed in place in hs; the
+    // zero padding of a partition depends on its index within its set, slot mod J)
+    const int nunits = (int)(items * (I + (h_stride != 0 ? g.sets * J : 0)));
     x_fft_kernel<<<(unsigned)((nunits + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nblk,
                                                                 nunits);
     DASP_LAUNCH_OK("x_fft_kernel");
-    launch_mac<false, true>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
+    if (g.sets == 2) launch_mac<false, true, 1>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
+    else             launch_mac<false, true>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
     ifft_mix_kernel<<<(unsigned)((nblk + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
                                                                    mix_stride, y, item0, I, g.n, in_chs, nblk);
@@ -2123,7 +2281,8 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
   x_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, xs, item0, I, g.n, in_chs);
   DASP_LAUNCH_OK("x_blocks_kernel");
   if ((rc = exec_c2c(pl.xi, cufft, xs, CUFFT_FORWARD, st)) != DASP_OK) return rc;
-  launch_mac<false>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
+  if (g.sets == 2) launch_mac<false, false, 1>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
+  else             launch_mac<false>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
   DASP_LAUNCH_OK("partition_mac_kernel");
   if ((rc = exec_c2c(pl.xi, cufft, ys, CUFFT_INVERSE, st)) != DASP_OK) return rc;
   mix_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(x, ys, mix, mix_stride, y, item0, I, g.n, in_chs);
@@ -2136,7 +2295,8 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
 // E[j] = sum_p G[j+p] conj(X[p]) in the es region, in the form e (kPlanar needs own).  own (own_fft_rows of gy): the G
 // transform and ifft_dx_kernel on the own FFT with the tables tw; otherwise the cuFFT pipeline.  Unfused, the dL/dIR
 // correlation runs after the dL/dx inverse (the two correlations read the same inputs and write disjoint regions).
-// h_stride: item stride of hs as in conv_fwd_chunk (0: one IR shared by the batch).
+// h_stride: item stride of hs as in conv_fwd_chunk (0: one IR shared by the batch).  g.sets == 2 (a true-stereo IR): the
+// products of partition_mac_kernel<TS 1 / TS 2>, and es receives 2 J partitions per item, set A then set B.
 int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const float* tw, const float* gy,
                    const float* x, int in_chs, const float2* xs, const float2* hs, int64_t h_stride, const float* mix,
                    int mix_stride, float* gx, unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items,
@@ -2148,7 +2308,8 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
   void* cufft = ws + w.cufft;
   const float inv = 1.0f / (float)kNbA;
   const int I = (int)g.ib, J = (int)g.jb;
-  const bool fused = fused_corr(e, I, J);
+  const bool fused = fused_corr(e, I, J, g.sets);
+  const bool ts = g.sets == 2;
   int rc;
   if (own) {
     if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
@@ -2157,11 +2318,16 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     DASP_LAUNCH_OK("g_fft_kernel");
     if (fused) {
       dim3 mgrid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
-      if ((I > J ? I : J) <= 12) partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
-      else                       partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
+      const bool m12 = (I > J ? I : J) <= 12;
+      if (ts && m12)  partition_mac_bwd_kernel<12, true><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
+      else if (ts)    partition_mac_bwd_kernel<kTsFusedMaxB, true><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
+      else if (m12)   partition_mac_bwd_kernel<12><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
+      else            partition_mac_bwd_kernel<16><<<mgrid, 128, 0, st>>>(gs, hs, h_stride, xs, ds, es, I, J, inv);
       DASP_LAUNCH_OK("partition_mac_bwd_kernel");
     } else {
-      launch_mac<true, true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);      // dx windows: sum_j conj(H[j]) G[q+j]
+      // dx windows: sum_j conj(H[j]) G[q+j]
+      if (ts) launch_mac<true, true, 1>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
+      else    launch_mac<true, true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
       DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     }
     ifft_dx_kernel<<<persistent_grid(items), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gy, x, mix,
@@ -2172,7 +2338,8 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     g_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, gs, item0, I, g.n);
     DASP_LAUNCH_OK("g_blocks_kernel");
     if ((rc = exec_c2c(pl.xi, cufft, gs, CUFFT_FORWARD, st)) != DASP_OK) return rc;
-    launch_mac<true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
+    if (ts) launch_mac<true, false, 1>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
+    else    launch_mac<true>(gs, hs, ds, I, J, h_stride != 0, I, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     if ((rc = exec_c2c(pl.xi, cufft, ds, CUFFT_INVERSE, st)) != DASP_OK) return rc;
     finish_dx_blocks_kernel<<<dim3((unsigned)I, (unsigned)items), 256, 0, st>>>(gy, x, ds, mix, mix_stride, gx, mixpart,
@@ -2180,10 +2347,13 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
     DASP_LAUNCH_OK("finish_dx_blocks_kernel");
   }
   if (e == IrGrad::kPlanar && !fused) {
-    launch_mac<true, true>(gs, xs, es, I, I, 1, J, items, inv, st);        // dIR partitions: sum_p conj(X[p]) G[j+p]
+    // dIR partitions: sum_p conj(X[p]) G[j+p]
+    if (ts) launch_mac<true, true, 2>(gs, xs, es, I, I, 1, J, items, inv, st);
+    else    launch_mac<true, true>(gs, xs, es, I, I, 1, J, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
   } else if (e == IrGrad::kTime || e == IrGrad::kSpectra) {
-    launch_mac<true>(gs, xs, es, I, I, 1, J, items, inv, st);
+    if (ts) launch_mac<true, false, 2>(gs, xs, es, I, I, 1, J, items, inv, st);
+    else    launch_mac<true>(gs, xs, es, I, I, 1, J, items, inv, st);
     DASP_LAUNCH_OK("partition_mac_kernel<corr>");
     if (e == IrGrad::kSpectra) return DASP_OK;
     return exec_c2c(pl.hj, cufft, es, CUFFT_INVERSE, st);
@@ -2430,15 +2600,19 @@ int g_conv_last_path[2] = {0, 0};                    // test hook: dispatch of t
 // The bodies of dasp_conv_* (one IR per item) and dasp_conv_shared_* (one IR for the whole batch).  Shared, the IR's
 // partitions are filled and transformed once before the first chunk and every item reads the same spectra (item stride
 // 0); the backward sums mix[b] times each item's dL/dIR partition spectra in fp64 (irgrad_sum_kernel) and transforms
-// the sum once after the last chunk.
-int conv_op_geometry(bool shared, int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+// the sum once after the last chunk.  A true-stereo IR (ir_chs 4) is two partition sets per IR (g.sets = 2), carried
+// through the same routines.
+int conv_op_geometry(bool shared, int sets, int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items,
+                     dasp_conv_geom* out) {
   DASP_REQUIRE(out != nullptr, "conv geometry: null out");
   ConvGeom g;
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
   g.shared = shared;
+  g.sets = sets;
   return put_conv_geometry(g, nullptr, out);
 }
+int ir_sets(int64_t ir_chs) { return ir_chs == 4 ? 2 : 1; }
 
 int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,
                 const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
@@ -2447,7 +2621,9 @@ int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, in
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
   g.shared = shared;
-  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2), "conv: only mono/stereo signals and IRs");
+  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2 || ir_chs == 4),
+               "conv: only mono/stereo signals and mono/stereo/true-stereo IRs");
+  g.sets = ir_sets(ir_chs);
   if (bs == 0) return DASP_OK;
   DASP_REQUIRE(x && ir && mix && y && workspace, "conv fwd: null pointer");
   DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "conv fwd: pass both *_save buffers or neither");
@@ -2458,17 +2634,17 @@ int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, in
   if ((rc = check_workspace("conv fwd", s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
   const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
-  const int I = (int)g.ib, J = (int)g.jb;
-  const int64_t h_stride = shared ? 0 : J * (int64_t)kNbA;
+  const int I = (int)g.ib, J = (int)g.jb, S = g.sets;
+  const int64_t h_stride = shared ? 0 : S * J * (int64_t)kNbA;
   float2* const hs0 = irspec_save ? (float2*)irspec_save : (float2*)(base + w.hsp);
   const float* tw = nullptr;
 
   // IR taps t < leff of items [item0, item0 + items) into their partition slots; the cuFFT transform of the partitions
   // reads whole slots, x_fft_kernel only the taps ir_pack_kernel writes
   auto fill_ir = [&](float2* hs, bool own, int64_t item0, int64_t items) -> int {
-    if (!own) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
-    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(ir, hs, item0, J, g.L,
-                                                                                          g.leff, (int)ir_chs);
+    if (!own) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * S * J * kNbA, st));
+    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, (unsigned)S), 256, 0, st>>>(
+        ir, hs, item0, J, g.L, g.leff, (int)ir_chs);
     DASP_LAUNCH_OK("ir_pack_kernel");
     return DASP_OK;
   };
@@ -2484,7 +2660,7 @@ int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, in
     float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? hs0 + item0 * h_stride : hs0;
     const bool own_conv = own_fft_rows(n, x, hs);
-    g_conv_last_path[0] = (own_conv ? 1 : 0) | (shared ? 2 : 0);
+    g_conv_last_path[0] = (own_conv ? 1 : 0) | (shared ? 2 : 0) | (S == 2 ? 4 : 0);
     if (!shared && (rc = fill_ir(hs, own_conv, item0, items)) != DASP_OK) return rc;
     if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
     if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, h_stride, mix, 1, y, base, w, item0, items,
@@ -2501,7 +2677,9 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
   int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
   if (rc != DASP_OK) return rc;
   g.shared = shared;
-  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2), "conv: only mono/stereo signals and IRs");
+  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2 || ir_chs == 4),
+               "conv: only mono/stereo signals and mono/stereo/true-stereo IRs");
+  g.sets = ir_sets(ir_chs);
   if (bs == 0) return DASP_OK;
   DASP_REQUIRE(gy && x && mix && xspec_save && irspec_save && gx && gmix && workspace, "conv bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -2514,8 +2692,8 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
   float2* ws_es = (float2*)(base + w.es);
   const float* ws_mixpart = (const float*)(base + w.mixpart);
   double2* ws_acc = (double2*)(base + w.acc);
-  const int I = (int)g.ib, J = (int)g.jb;
-  const int64_t h_stride = shared ? 0 : J * (int64_t)kNbA;
+  const int I = (int)g.ib, J = (int)g.jb, S = g.sets;
+  const int64_t h_stride = shared ? 0 : S * J * (int64_t)kNbA;
   const float* tw = nullptr;
   bool own_conv = false;
 
@@ -2523,15 +2701,15 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
   // pairs after the inverse cuFFT), times mix[b] (a null mix: 1)
   auto ir_taps = [&](IrGrad e, int64_t item0, int64_t items, const float* mx) -> int {
     if (e == IrGrad::kPlanar) {
-      const int nunits = (int)(items * J);
+      const int nunits = (int)(items * S * J);
       ifft_irtaps_kernel<<<persistent_grid(nunits), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mx,
-                                                                        gir, item0, J, g.L, g.leff, (int)ir_chs, nunits);
+                                                                        gir, item0, J, S, g.L, g.leff, (int)ir_chs, nunits);
       DASP_LAUNCH_OK("ifft_irtaps_kernel");
     }
     // taps t0 <= t < L: the zeros from leff on after ifft_irtaps_kernel, every tap after the cuFFT inverse
     const int64_t t0 = e == IrGrad::kPlanar ? g.leff : 0;
     if (g.L > t0) {
-      irtaps_unpack_kernel<<<dim3((unsigned)((g.L - t0 + 255) / 256), (unsigned)items), 256, 0, st>>>(
+      irtaps_unpack_kernel<<<dim3((unsigned)((g.L - t0 + 255) / 256), (unsigned)items, (unsigned)S), 256, 0, st>>>(
           ws_es, mx, gir, item0, J, g.L, g.leff, (int)ir_chs, t0);
       DASP_LAUNCH_OK("irtaps_unpack_kernel");
     }
@@ -2545,14 +2723,16 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
     own_conv = own_fft_rows(n, gy, nullptr);
     const IrGrad e = gir == nullptr ? IrGrad::kNone
                                     : (own_conv ? IrGrad::kPlanar : (shared ? IrGrad::kSpectra : IrGrad::kTime));
-    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed, bit 3: one IR shared by the batch
-    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_corr(e, I, J) ? 2 : 0) | (gir ? 4 : 0) | (shared ? 8 : 0);
+    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed, bit 3: one IR shared by the batch, bit 4: a
+    // true-stereo IR
+    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_corr(e, I, J, S) ? 2 : 0) | (gir ? 4 : 0) | (shared ? 8 : 0) |
+                          (S == 2 ? 16 : 0);
     if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
     if ((rc = conv_bwd_chunk(g, pl, own_conv, e, tw, gy, x, (int)in_chs, xs, hs, h_stride, mix, 1, gx, base, w, item0,
                              items, st)) != DASP_OK)
       return rc;
     if (e != IrGrad::kNone && shared) {
-      const int64_t per_item = J * (int64_t)kNbA;
+      const int64_t per_item = S * J * (int64_t)kNbA;
       irgrad_sum_kernel<<<(unsigned)((per_item + 255) / 256), 256, 0, st>>>(ws_es, mix, ws_acc, item0, (int)items,
                                                                             per_item, item0 + items == bs);
       DASP_LAUNCH_OK("irgrad_sum_kernel");
@@ -2563,7 +2743,7 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
     DASP_LAUNCH_OK("conv_mix_grad_kernel");
   }
   if (shared && gir) {
-    // the summed partition spectra, rounded to fp32 in item 0's slot of es: J inverse transforms for the one IR
+    // the summed partition spectra, rounded to fp32 in item 0's slots of es: S J inverse transforms for the one IR
     if (!own_conv && (rc = exec_c2c(s.ir1, base + w.cufft, ws_es, CUFFT_INVERSE, st)) != DASP_OK) return rc;
     if ((rc = ir_taps(own_conv ? IrGrad::kPlanar : IrGrad::kTime, 0, 1, nullptr)) != DASP_OK) return rc;
   }
@@ -2574,7 +2754,11 @@ int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, in
 int dasp_debug_conv_last_path(int which) { return g_conv_last_path[which ? 1 : 0]; }
 
 int dasp_conv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
-  return conv_op_geometry(false, bs, n, ir_len, chunk_items, out);
+  return conv_op_geometry(false, 1, bs, n, ir_len, chunk_items, out);
+}
+
+int dasp_conv_ts_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+  return conv_op_geometry(false, 2, bs, n, ir_len, chunk_items, out);
 }
 
 int dasp_conv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, const float* mix,
@@ -2592,7 +2776,11 @@ int dasp_conv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_ch
 }
 
 int dasp_conv_shared_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
-  return conv_op_geometry(true, bs, n, ir_len, chunk_items, out);
+  return conv_op_geometry(true, 1, bs, n, ir_len, chunk_items, out);
+}
+
+int dasp_conv_shared_ts_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out) {
+  return conv_op_geometry(true, 2, bs, n, ir_len, chunk_items, out);
 }
 
 int dasp_conv_shared_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,

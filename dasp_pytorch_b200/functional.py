@@ -702,8 +702,9 @@ def noise_shaped_reverberation_packed(x: torch.Tensor, sample_rate: float, param
 
 
 class _ConvReverbFn(torch.autograd.Function):
-    """x (bs, 1|2, n), ir (bs, 1|2, L), mix (bs,) -> y (bs, 2, n).  An ir of batch 1 with bs > 1 is one IR shared by
-    the batch (the dasp_conv_shared_* entry points): its gradient is the sum over the items, shape (1, 1|2, L)."""
+    """x (bs, 1|2, n), ir (bs, 1|2|4, L), mix (bs,) -> y (bs, 2, n).  An ir of batch 1 with bs > 1 is one IR shared by
+    the batch (the dasp_conv_shared_* entry points): its gradient is the sum over the items, shape (1, 1|2|4, L).  A
+    4-channel (true-stereo) IR is sized by the *_ts_geometry queries and runs through the same entry points."""
 
     @staticmethod
     def forward(ctx, x, ir, mix, chunk):
@@ -712,12 +713,13 @@ class _ConvReverbFn(torch.autograd.Function):
         ir_bs, ir_chs, ir_len = ir.shape
         shared = ir_bs == 1 and bs > 1
         kind = "conv_shared" if shared else "conv"
+        geom_fn = f"dasp_{kind}{'_ts' if ir_chs == 4 else ''}_geometry"
         dev = x.device
         y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:3])
         geom = _abi.ConvGeom()
         with torch.cuda.device(dev):
-            check(getattr(lib, f"dasp_{kind}_geometry")(bs, n, ir_len, chunk, geom), f"dasp_{kind}_geometry")
+            check(getattr(lib, geom_fn)(bs, n, ir_len, chunk, geom), geom_fn)
             ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
             xspec = irspec = None
             if need_bwd:
@@ -763,9 +765,14 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
     Args:
         x: audio ``(bs, 1|2, n)``; mono is used for both channels.
         sample_rate: unused (kept for the common processor signature).
-        impulse_response: ``(bs, 1|2, L)``, one IR per item, or ``(1, 1|2, L)``, one IR for the whole batch (a
+        impulse_response: ``(bs, 1|2|4, L)``, one IR per item, or ``(1, 1|2|4, L)``, one IR for the whole batch (a
             measured room applied to every item, or a single learnt FIR reverb); any ``L >= 1``; a mono IR is used for
-            both channels.
+            both channels.  Four channels are a true-stereo IR in input-major order: channel ``2 i + o`` is the path
+            from input channel ``i`` to output channel ``o``, i.e. L->L, L->R, R->L, R->R, so that::
+
+                wet_L = x_L * h0 + x_R * h2,   wet_R = x_L * h1 + x_R * h3,   y = (1 - mix) x + mix wet
+
+            (``*`` the causal convolution cropped to ``n``; a mono ``x`` feeds both inputs, ``wet_L = x * (h0 + h2)``).
         mix: ``bs`` elements in any shape, or one element that is broadcast over the batch.
 
     Returns ``(bs, 2, n)`` in x's dtype (computed in fp32), like ``noise_shaped_reverberation``, so the two can replace
@@ -774,14 +781,17 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
     IR has that shape and is the sum over the items of each item's gradient, accumulated in fp64 in item order, so it
     does not depend on how the batch is chunked.  A shared IR is transformed once per call rather than once per item,
     and no per-item copy of it or of its gradient is ever made; ``ir.expand(bs, -1, -1)`` gives the same result at the
-    per-item cost.  When the IR does not require a gradient, the backward skips all dL/dIR work.  The convolution is the
+    per-item cost.  A true-stereo IR takes one window transform and one inverse transform per block, like a stereo one,
+    where two stereo calls with ``(h0, h1)`` and ``(h2, h3)`` would take two of each; its gradient reaches all four
+    channels.  When the IR does not require a gradient, the backward skips all dL/dIR work.  The convolution is the
     reverb's own: uniformly partitioned overlap-save on 4096-sample partitions with the in-shared-memory 8192-point FFT.
     """
-    for t, name in ((x, "x"), (impulse_response, "impulse_response")):
+    for t, name, chans, what in ((x, "x", (1, 2), "mono/stereo"),
+                                 (impulse_response, "impulse_response", (1, 2, 4), "mono/stereo/true-stereo (4)")):
         if not torch.is_tensor(t) or t.dim() != 3:
             raise ValueError(f"{name} must be a tensor of shape (batch, channels, samples)")
-        if t.shape[1] not in (1, 2):
-            raise ValueError(f"{name}: only mono/stereo is supported, got {t.shape[1]} channels")
+        if t.shape[1] not in chans:
+            raise ValueError(f"{name}: only {what} is supported, got {t.shape[1]} channels")
     bs = x.shape[0]
     if impulse_response.shape[0] != bs and not (impulse_response.shape[0] == 1 and bs > 1):
         raise ValueError(f"impulse_response has batch {impulse_response.shape[0]}, x has batch {bs} (expected {bs} or 1)")

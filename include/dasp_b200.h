@@ -190,8 +190,8 @@ int dasp_reverb_filterbank(int64_t taps, double sample_rate, float* out);
 
 /* ---- convolution_reverberation: the reverb's apply stage with a caller-supplied impulse response
  *      (reference functional.py:569-575: y = (1 - mix) x + mix (x * IR), causal, cropped to n) --------------
- * x is (bs, in_chs, n), ir is (bs, ir_chs, ir_len) with in_chs, ir_chs 1 or 2 (mono is used for both channels),
- * mix is [bs]; y is always (bs, 2, n).  Any ir_len >= 1; only the first leff = min(ir_len, n) taps reach the output.
+ * x is (bs, in_chs, n), ir is (bs, ir_chs, ir_len) with in_chs 1 or 2 and ir_chs 1, 2 or 4 (mono is used for both
+ * channels; 4 is a true-stereo IR, see below), mix is [bs]; y is always (bs, 2, n).  Any ir_len >= 1; only the first leff = min(ir_len, n) taps reach the output.
  * The convolution is the reverb's: uniformly partitioned overlap-save on conv_block-sample partitions.
  * Buffers kept for the backward (pass NULL for both when no backward follows):
  *   xspec_save  geom.xspec_c64 complex64 (audio block spectra), irspec_save  geom.irspec_c64 complex64 (IR partitions).
@@ -228,10 +228,19 @@ int dasp_conv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_
                          const float* mix, const void* xspec_save, const void* irspec_save, float* gx,
                          float* gir /* may be NULL */, float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs,
                          int64_t n, int64_t chunk_items, void* stream);
+/* True-stereo IR: ir_chs = 4 in all four dasp_conv[_shared]_fwd / _bwd calls above.  Rows are input-major, row 2 i + o
+ * is the path from input channel i to output channel o (L->L, L->R, R->L, R->R):
+ *   wet_L = x_L * h0 + x_R * h2,  wet_R = x_L * h1 + x_R * h3,  y = (1 - mix) x + mix wet.
+ * gir is (bs, 4, ir_len) (shared: (4, ir_len)).  Its buffers are larger than a mono/stereo IR's (irspec_save, the IR
+ * partition regions of both workspaces and the shared backward's fp64 sum hold two partition sets per IR), so size them
+ * with these two queries; ir_partitions is still ceil(leff / conv_block), the partitions of one set, and irspec_c64 is
+ * 2 * ir_partitions * 2 * conv_block per IR. */
+int dasp_conv_ts_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_conv_shared_ts_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, dasp_conv_geom* out);
 /* test hook: dispatch of the most recent call.  which = 0: dasp_conv_fwd / dasp_conv_shared_fwd, bit 0 = own
    in-shared-memory FFT, clear = cuFFT pipeline (dasp_debug_reverb_path(1), n % 4 != 0, rows not 16-byte aligned),
-   bit 1 = shared IR.  which = 1: dasp_conv_bwd / dasp_conv_shared_bwd, bit 0 = own FFT, bit 1 = fused correlation
-   kernel, bit 2 = dL/dIR computed, bit 3 = shared IR */
+   bit 1 = shared IR, bit 2 = true-stereo IR.  which = 1: dasp_conv_bwd / dasp_conv_shared_bwd, bit 0 = own FFT,
+   bit 1 = fused correlation kernel, bit 2 = dL/dIR computed, bit 3 = shared IR, bit 4 = true-stereo IR */
 int dasp_debug_conv_last_path(int which);
 
 #ifdef __cplusplus

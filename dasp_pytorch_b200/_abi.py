@@ -87,6 +87,11 @@ _SIGNATURES = {
     "dasp_dynamics_tile_len": (I64, [I64, I64]),
     "dasp_dynamics_fwd": (c_int, [c_int, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),
     "dasp_dynamics_bwd": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),
+    "dasp_dynamics_sidechain_tile_len": (I64, [I64, I64, I64]),
+    "dasp_dynamics_sidechain_fwd": (c_int, [c_int, P, P, I64, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float,
+                                            I64, P]),
+    "dasp_dynamics_sidechain_bwd": (c_int, [c_int, P, P, P, I64, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, c_float,
+                                            c_float, I64, P]),
 }
 
 

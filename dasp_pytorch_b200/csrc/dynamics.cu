@@ -247,14 +247,15 @@ __device__ __forceinline__ CurveOut gain_computer(float xdb, const CurveK& k) {
 // side chain of the generic channel loop: the channel sum accumulated in fp64 and rounded once.  A running fp32 sum
 // of three or more channels loses its relative accuracy where the channels cancel, and dL/dx carries 1/side, which
 // is largest exactly there.  One rounding of the (near-)exact sum is what the stereo path's fp32 a + b gives too, so
-// stereo through this loop stays bit-identical to the ST specialisation.
+// stereo through this loop stays bit-identical to the ST specialisation.  The C summed buffers start at buffer b0 of
+// the stage (the side-chain kernels sum the key buffers that follow the audio's).
 template <class Pipe>
-__device__ __forceinline__ void side_chain(float (&xs)[kE], const Pipe& pipe, int st, int C, int off) {
+__device__ __forceinline__ void side_chain(float (&xs)[kE], const Pipe& pipe, int st, int C, int off, int b0 = 0) {
   double acc[kE];
 #pragma unroll
   for (int j = 0; j < kE; ++j) acc[j] = 0.0;
   for (int c = 0; c < C; ++c) {
-    const float* xb = pipe.buf(st, c) + off;
+    const float* xb = pipe.buf(st, b0 + c) + off;
 #pragma unroll
     for (int j = 0; j < kE; ++j) acc[j] += (double)xb[j];
   }
@@ -367,6 +368,38 @@ __global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
 }
 
 // =============================================================================== backward
+// block reduction of the five per-thread sums, chain rule to the user parameters, written to gparams[item][0..5]
+template <int W>
+__device__ __forceinline__ void param_grads(float (&red)[5][W], float acc_m, float acc_a, float acc_t, float acc_r,
+                                            float acc_w, float alpha, float attack, float sample_rate, float* gparams,
+                                            int item, int lane, int warp) {
+  acc_m = warp_sum(acc_m); acc_a = warp_sum(acc_a); acc_t = warp_sum(acc_t);
+  acc_r = warp_sum(acc_r); acc_w = warp_sum(acc_w);
+  if (lane == 0) {
+    red[0][warp] = acc_m; red[1][warp] = acc_a; red[2][warp] = acc_t; red[3][warp] = acc_r; red[4][warp] = acc_w;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float sm_[5];
+#pragma unroll
+    for (int q = 0; q < 5; ++q) {
+      float a = 0.f;
+#pragma unroll
+      for (int w = 0; w < W; ++w) a += red[q][w];
+      sm_[q] = a;
+    }
+    // d alpha / d attack_ms = alpha * ln9 * 1e3 / (sr * attack_ms^2)
+    const double dalpha = (double)alpha * 2.1972245773362196 * 1e3 / ((double)sample_rate * (double)attack * (double)attack);
+    float* gp = gparams + (int64_t)item * 6;
+    gp[0] = sm_[2];
+    gp[1] = sm_[3];
+    gp[2] = (float)((double)sm_[1] * dalpha);
+    gp[3] = 0.f;                       // release_ms is unused by the reference (functional.py:343-344)
+    gp[4] = sm_[4];
+    gp[5] = sm_[0];
+  }
+}
+
 template <Curve CV, int W, bool LA, bool ST = false>
 __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1)) dynamics_bwd_kernel(DynParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -515,33 +548,8 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
     pipe.release(i, g, rows);
   }
   pipe.drain();
-
-  // ---- block reduction of the five sums, chain rule to the user parameters ----
-  acc_m = warp_sum(acc_m); acc_a = warp_sum(acc_a); acc_t = warp_sum(acc_t);
-  acc_r = warp_sum(acc_r); acc_w = warp_sum(acc_w);
-  if (lane == 0) {
-    red[0][warp] = acc_m; red[1][warp] = acc_a; red[2][warp] = acc_t; red[3][warp] = acc_r; red[4][warp] = acc_w;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float sm_[5];
-#pragma unroll
-    for (int q = 0; q < 5; ++q) {
-      float a = 0.f;
-#pragma unroll
-      for (int w = 0; w < W; ++w) a += red[q][w];
-      sm_[q] = a;
-    }
-    // d alpha / d attack_ms = alpha * ln9 * 1e3 / (sr * attack_ms^2)
-    const double dalpha = (double)tb.alpha * 2.1972245773362196 * 1e3 / ((double)p.sample_rate * (double)attack * (double)attack);
-    float* gp = p.gparams + (int64_t)item * 6;
-    gp[0] = sm_[2];
-    gp[1] = sm_[3];
-    gp[2] = (float)((double)sm_[1] * dalpha);
-    gp[3] = 0.f;                       // release_ms is unused by the reference (functional.py:343-344)
-    gp[4] = sm_[4];
-    gp[5] = sm_[0];
-  }
+  param_grads<W>(red, acc_m, acc_a, acc_t, acc_r, acc_w, tb.alpha, attack, p.sample_rate,
+                 p.gparams, item, lane, warp);
 }
 
 // lookahead > 0 only: gx[b,c,m] += gy[b,c,m+la] * G[b,m+la]
@@ -555,11 +563,251 @@ __global__ void dynamics_lookahead_fixup_kernel(const float* __restrict__ gy, co
   if (m + la < n) gx[idx] += gy[idx + la] * G[item * n + m + la];
 }
 
+// =============================================================================== external side chain
+// The detector listens to a key (bs, K, N) instead of x: side = the sum of the K key channels (side_chain over the
+// key buffers, fp64, rounded once), G from it exactly as above, y = x[n - la] * G[n].  The key is never delayed.
+// Backward: x gets gy G only (no detector term), and every key channel gets the same dL/dside.
+struct ScParams {
+  DynParams d;
+  const float* key;      // (bs, K, N)
+  float* gkey;           // (bs, K, N) backward out, or null: no dL/dkey, the key rows are only read
+  int key_chs;
+};
+struct ScFwdRows {        // buffers [0,C) = x (in) -> y (out), [C,C+K) = key (read only)
+  const float* x0; float* y0; const float* k0; int64_t n; int chs;
+  __device__ __forceinline__ const float* src(int b) const {
+    return b < chs ? x0 + (int64_t)b * n : k0 + (int64_t)(b - chs) * n;
+  }
+  __device__ __forceinline__ float* dst(int b) const { return b < chs ? y0 + (int64_t)b * n : nullptr; }
+};
+struct ScBwdRows {        // [0,C) = x (read only), [C,2C) = gy (in) -> gx (out), [2C,2C+K) = key (in) -> dL/dkey (out)
+  const float* x0; const float* g0; float* gx0; const float* k0; float* gk0; int64_t n; int chs;
+  __device__ __forceinline__ const float* src(int b) const {
+    if (b < chs) return x0 + (int64_t)b * n;
+    if (b < 2 * chs) return g0 + (int64_t)(b - chs) * n;
+    return k0 + (int64_t)(b - 2 * chs) * n;
+  }
+  __device__ __forceinline__ float* dst(int b) const {
+    if (b < chs) return nullptr;
+    if (b < 2 * chs) return gx0 + (int64_t)(b - chs) * n;
+    return gk0 ? gk0 + (int64_t)(b - 2 * chs) * n : nullptr;
+  }
+};
+
+template <Curve CV, int W, bool LA>
+__global__ void __launch_bounds__(W * 32) dynamics_sc_fwd_kernel(ScParams sp) {
+  const DynParams& p = sp.d;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  Smem<W> sm(smem_raw);
+  const int item = blockIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int C = p.chs, K = sp.key_chs;
+  const int tile_len = W * 32 * kE;
+
+  const float M = p.makeup_db[item];
+  const CurveK ck = make_curve(CV, p.threshold_db[item], p.ratio[item], p.knee_db[item]);
+  PoleTables tb;
+  make_tables(tb, p.attack_ms[item], p.sample_rate, lane);
+
+  TileGeom g{p.n, tile_len, p.ntiles, false};
+  ScFwdRows rows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, sp.key + (int64_t)item * K * p.n, p.n, C};
+  TilePipe<kStages> pipe;
+  pipe.init(sm.bars, sm.stages, C + K, tile_len, p.bulk != 0);
+  pipe.prologue(g, rows);
+
+  float c_tile = 0.f;
+  const int off = threadIdx.x * kE;
+  for (int i = 0; i < p.ntiles; ++i) {
+    pipe.acquire(i, g, rows);
+    const int st = i % kStages;
+    const int64_t n0 = (int64_t)i * tile_len + off;
+    if (p.ckpt && threadIdx.x == 0) p.ckpt[(int64_t)item * p.ntiles + i] = c_tile;
+
+    float s[kE];
+    {
+      float xs[kE];
+      side_chain(xs, pipe, st, K, off, C);
+      float run = 0.f;
+#pragma unroll
+      for (int j = 0; j < kE; ++j) {
+        float gc = 0.f;
+        if (n0 + j < p.n) gc = gain_computer<CV, false>(level_db(xs[j], p.eps), ck).gc;
+        run = fmaf(tb.alpha, run, tb.beta * gc);
+        s[j] = run;
+      }
+    }
+    const float c_in = scan_forward<W>(s[kE - 1], c_tile, tb, sm.agg + (i & 1) * W, lane, warp);
+
+    float G[kE];
+#pragma unroll
+    for (int j = 0; j < kE; ++j) G[j] = exp2f((fmaf(tb.apow[j], c_in, s[j]) + M) * kLog2Of10Over20);
+    if (!LA) {
+      for (int c = 0; c < C; ++c) {
+        float* xb = pipe.buf(st, c) + off;
+#pragma unroll
+        for (int j = 0; j < kE; ++j) xb[j] *= G[j];
+      }
+    } else {
+      // y[n] = x[n - la] * G[n]: delayed input straight from global/L2
+      for (int c = 0; c < C; ++c) {
+        float* xb = pipe.buf(st, c) + off;
+        const float* xr = rows.x0 + (int64_t)c * p.n;
+#pragma unroll
+        for (int j = 0; j < kE; ++j) {
+          const int64_t m = n0 + j - p.lookahead;
+          xb[j] = (m >= 0 && n0 + j < p.n) ? __ldg(xr + m) * G[j] : 0.f;
+        }
+      }
+    }
+    pipe.release(i, g, rows);
+  }
+  pipe.drain();
+}
+
+template <Curve CV, int W, bool LA>
+__global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1))
+    dynamics_sc_bwd_kernel(ScParams sp) {
+  const DynParams p = sp.d;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  Smem<W> sm(smem_raw);
+  __shared__ float red[5][W];
+  const int item = blockIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int C = p.chs, K = sp.key_chs;
+  const int tile_len = W * 32 * kE;
+  const int la = p.lookahead;
+
+  const float M = p.makeup_db[item];
+  const CurveK ck = make_curve(CV, p.threshold_db[item], p.ratio[item], p.knee_db[item]);
+  const float attack = p.attack_ms[item];
+  PoleTables tb;
+  make_tables(tb, attack, p.sample_rate, lane);
+  PoleTables tr;
+  make_tables(tr, attack, p.sample_rate, 31 - lane);
+  const float rlane_pow = tr.lane_pow;
+
+  TileGeom g{p.n, tile_len, p.ntiles, true};
+  const int64_t base = (int64_t)item * C * p.n, kbase = (int64_t)item * K * p.n;
+  ScBwdRows rows{p.x + base, p.gy + base, p.y + base, sp.key + kbase, sp.gkey ? sp.gkey + kbase : nullptr, p.n, C};
+  TilePipe<kStages> pipe;
+  pipe.init(sm.bars, sm.stages, 2 * C + K, tile_len, p.bulk != 0);
+  pipe.prologue(g, rows);
+
+  float w_tile = 0.f;
+  float acc_m = 0.f, acc_a = 0.f, acc_t = 0.f, acc_r = 0.f, acc_w = 0.f;
+  const int off = threadIdx.x * kE;
+  for (int i = 0; i < p.ntiles; ++i) {
+    pipe.acquire(i, g, rows);
+    const int st = i % kStages;
+    const int tile = g.tile_of(i);
+    const int64_t n0 = (int64_t)tile * tile_len + off;
+
+    // ---- recompute the forward quantities of this tile from its checkpoint ----
+    float xs[kE], s[kE], gcv[kE], dxdbv[kE], drv[kE], dwv[kE];
+    side_chain(xs, pipe, st, K, off, 2 * C);
+    {
+      float run = 0.f;
+#pragma unroll
+      for (int j = 0; j < kE; ++j) {
+        CurveOut o; o.gc = 0.f; o.d_xdb = 0.f; o.d_t = 0.f; o.d_r = 0.f; o.d_w = 0.f;
+        if (n0 + j < p.n) o = gain_computer<CV, true>(level_db(xs[j], p.eps), ck);
+        gcv[j] = o.gc; dxdbv[j] = o.d_xdb; drv[j] = o.d_r; dwv[j] = o.d_w;
+        run = fmaf(tb.alpha, run, tb.beta * o.gc);
+        s[j] = run;
+      }
+    }
+    float c_tile = p.ckpt[(int64_t)item * p.ntiles + tile];
+    const float c_in = scan_forward<W>(s[kE - 1], c_tile, tb, sm.agg + (i & 1) * 2 * W, lane, warp);
+#pragma unroll
+    for (int j = 0; j < kE; ++j) s[j] = fmaf(tb.apow[j], c_in, s[j]);
+
+    // ---- dL/ds = ln10/20 G sum_c gy_c x_c (x delayed under LA) and the zero-state local adjoint pass ----
+    float G[kE], wv[kE];
+    {
+      float dG[kE];
+#pragma unroll
+      for (int j = 0; j < kE; ++j) dG[j] = 0.f;
+      for (int c = 0; c < C; ++c) {
+        const float* xb = pipe.buf(st, c) + off;
+        const float* gb = pipe.buf(st, C + c) + off;
+        if (!LA) {
+#pragma unroll
+          for (int j = 0; j < kE; ++j) dG[j] = fmaf(gb[j], xb[j], dG[j]);
+        } else {
+          const float* xr = rows.x0 + (int64_t)c * p.n;
+#pragma unroll
+          for (int j = 0; j < kE; ++j) {
+            const int64_t m = n0 + j - la;
+            if (m >= 0 && n0 + j < p.n) dG[j] = fmaf(gb[j], xr[m], dG[j]);
+          }
+        }
+      }
+      float run = 0.f;
+#pragma unroll
+      for (int j = kE - 1; j >= 0; --j) {
+        const bool valid = (n0 + j < p.n);
+        G[j] = exp2f((s[j] + M) * kLog2Of10Over20);
+        const float ds = valid ? dG[j] * G[j] * kLn10Over20 : 0.f;
+        acc_m += ds;
+        run = fmaf(tb.alpha, run, ds);
+        wv[j] = run;
+      }
+    }
+    const float w_in = scan_reverse<W>(wv[0], w_tile, tb, rlane_pow, sm.agg + (i & 1) * 2 * W + W, lane, warp);
+
+    // ---- parameter-gradient integrands and dL/dside ----
+    float dxs[kE];
+#pragma unroll
+    for (int j = 0; j < kE; ++j) {
+      const float w = fmaf(tb.apow[kE - 1 - j], w_in, wv[j]);
+      const bool valid = (n0 + j < p.n);
+      const float s_prev = (j == 0) ? c_in : s[j - 1];
+      float dx = 0.f;
+      if (valid) {
+        acc_a = fmaf(w, s_prev - gcv[j], acc_a);
+        const float dgc = tb.beta * w;
+        acc_t = fmaf(dgc, -dxdbv[j], acc_t);
+        acc_r = fmaf(dgc, drv[j], acc_r);
+        acc_w = fmaf(dgc, dwv[j], acc_w);
+        if (fabsf(xs[j]) >= p.eps) dx = __fdividef(dgc * dxdbv[j] * kDbGradScale, xs[j]);
+      }
+      dxs[j] = dx;
+    }
+    // dL/dx = gy G; under LA the direct term gy[m+la] G[m+la] is added to zeros by dynamics_lookahead_fixup_kernel
+    if (LA) {
+      float* gs = p.g_scratch + (int64_t)item * p.n;
+#pragma unroll
+      for (int j = 0; j < kE; ++j)
+        if (n0 + j < p.n) gs[n0 + j] = G[j];
+    }
+    for (int c = 0; c < C; ++c) {
+      float* gb = pipe.buf(st, C + c) + off;
+#pragma unroll
+      for (int j = 0; j < kE; ++j) gb[j] = LA ? 0.f : gb[j] * G[j];
+    }
+    if (sp.gkey) {
+      for (int k = 0; k < K; ++k) {
+        float* kb = pipe.buf(st, 2 * C + k) + off;
+#pragma unroll
+        for (int j = 0; j < kE; ++j) kb[j] = dxs[j];
+      }
+    }
+    pipe.release(i, g, rows);
+  }
+  pipe.drain();
+  param_grads<W>(red, acc_m, acc_a, acc_t, acc_r, acc_w, tb.alpha, attack, p.sample_rate,
+                 p.gparams, item, lane, warp);
+}
+
 // ---- host side -----------------------------------------------------------------------------
 // shared memory a CTA of w warps may ask for: 96 KB (two or more CTAs per SM) up to 8 warps, 200 KB for the one-CTA-per-SM
 // geometry W = 16
 constexpr size_t kSmemLimit = 96 * 1024, kSmemLimit16 = 200 * 1024;
-int pick_warps(int64_t bs, int chs, int nbuf_per_ch) {
+// buffers per stage the largest (one-warp) tiles leave room for in the opt-in: 76 with the default E and stages.
+// The side-chain backward holds 2C + K of them (x, dL/dy -> dL/dx, key -> dL/dkey).
+constexpr int kMaxBufs = (int)((kSmemLimit16 - kSmemHeader) / ((size_t)kStages * 32 * kE * 4));
+// nbuf: tile buffers per stage of the backward (2 per channel; 2C + K with a side-chain key)
+int pick_warps(int64_t bs, int nbuf) {
   // enough warps to fill the chip, limited by shared memory (S stages * nbuf * tile bytes)
   const int64_t want = 16ll * sm_count();
   int w = 1;
@@ -569,7 +817,7 @@ int pick_warps(int64_t bs, int chs, int nbuf_per_ch) {
   if (w == 8 && bs <= sm_count()) w = 16;
   { const int f = debug_forced_warps(); if (f == 1 || f == 2 || f == 4 || f == 8 || f == 16) w = f; }
   auto fits = [&](int ww) {
-    return (size_t)kStages * nbuf_per_ch * chs * (ww * 32 * kE) * 4 + kSmemHeader <= (ww == 16 ? kSmemLimit16 : kSmemLimit);
+    return (size_t)kStages * nbuf * (ww * 32 * kE) * 4 + kSmemHeader <= (ww == 16 ? kSmemLimit16 : kSmemLimit);
   };
   while (w > 1 && !fits(w)) w /= 2;
   return w;
@@ -636,6 +884,35 @@ int dispatch(bool bwd, int w, const DynParams& p, int64_t bs, cudaStream_t st) {
   }
 }
 
+template <Curve CV, int W, bool LA>
+int launch_sc(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
+  const int C = sp.d.chs, K = sp.key_chs;
+  if (bwd) {
+    { int rc = ensure_smem_optin<dynamics_sc_bwd_kernel<CV, W, LA>>(); if (rc != DASP_OK) return rc; }
+    dynamics_sc_bwd_kernel<CV, W, LA><<<(unsigned)bs, W * 32, smem_bytes(W, 2 * C + K), st>>>(sp);
+    DASP_LAUNCH_OK("dynamics_sc_bwd_kernel");
+  } else {
+    { int rc = ensure_smem_optin<dynamics_sc_fwd_kernel<CV, W, LA>>(); if (rc != DASP_OK) return rc; }
+    dynamics_sc_fwd_kernel<CV, W, LA><<<(unsigned)bs, W * 32, smem_bytes(W, C + K), st>>>(sp);
+    DASP_LAUNCH_OK("dynamics_sc_fwd_kernel");
+  }
+  return DASP_OK;
+}
+template <Curve CV, int W>
+int launch_sc_w(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
+  return sp.d.lookahead > 0 ? launch_sc<CV, W, true>(bwd, sp, bs, st) : launch_sc<CV, W, false>(bwd, sp, bs, st);
+}
+template <Curve CV>
+int dispatch_sc(bool bwd, int w, const ScParams& sp, int64_t bs, cudaStream_t st) {
+  switch (w) {
+    case 1: return launch_sc_w<CV, 1>(bwd, sp, bs, st);
+    case 2: return launch_sc_w<CV, 2>(bwd, sp, bs, st);
+    case 4: return launch_sc_w<CV, 4>(bwd, sp, bs, st);
+    case 16: return launch_sc_w<CV, 16>(bwd, sp, bs, st);
+    default: return launch_sc_w<CV, 8>(bwd, sp, bs, st);
+  }
+}
+
 int check_common(const float* x, const float* params5[5], int64_t bs, int64_t chs, int64_t n, int64_t lookahead) {
   if (bs > 0 && n > 0) {
     DASP_REQUIRE(x != nullptr, "dynamics: null x");
@@ -649,6 +926,30 @@ int check_common(const float* x, const float* params5[5], int64_t bs, int64_t ch
   return DASP_OK;
 }
 
+// key checks of the side-chain entry points, after check_common; no CUDA call
+int check_key(const float* key, int64_t key_chs, int64_t bs, int64_t chs, int64_t n) {
+  DASP_REQUIRE(key_chs >= 1 && key_chs <= kMaxChs, "dynamics side chain: 1 to %d key channels are supported, got %lld",
+               kMaxChs, (long long)key_chs);
+  DASP_REQUIRE(2 * chs + key_chs <= kMaxBufs,
+               "dynamics side chain: 2 * chs + key_chs = %lld exceeds %d (the backward's tile buffers per stage)",
+               (long long)(2 * chs + key_chs), kMaxBufs);
+  if (bs > 0 && n > 0) DASP_REQUIRE(key != nullptr, "dynamics side chain: null key");
+  return DASP_OK;
+}
+
+// the fields both side-chain directions share, for tiles of w warps
+ScParams sc_params(int w, const float* x, const float* key, int64_t key_chs, const float* ps[5], int64_t chs,
+                   int64_t n, float sample_rate, float eps, int64_t lookahead) {
+  const int tile_len = w * 32 * kE;
+  ScParams sp{};
+  DynParams& p = sp.d;
+  p.x = x; p.threshold_db = ps[0]; p.ratio = ps[1]; p.attack_ms = ps[2]; p.knee_db = ps[3]; p.makeup_db = ps[4];
+  p.n = n; p.chs = (int)chs; p.ntiles = (int)((n + tile_len - 1) / tile_len); p.lookahead = (int)lookahead;
+  p.sample_rate = sample_rate; p.eps = eps;
+  sp.key = key; sp.key_chs = (int)key_chs;
+  return sp;
+}
+
 }  // namespace
 }  // namespace dasp
 
@@ -660,7 +961,7 @@ extern "C" {
 int64_t dasp_dynamics_tile_len(int64_t bs, int64_t chs) {
   if (chs < 1 || chs > kMaxChs) return 0;
   // the backward holds 2 buffers per channel: pick the geometry that fits both directions
-  return (int64_t)pick_warps(bs, (int)chs, 2) * 32 * kE;
+  return (int64_t)pick_warps(bs, 2 * (int)chs) * 32 * kE;
 }
 
 int dasp_dynamics_fwd(int kind, const float* x, const float* threshold_db, const float* ratio,
@@ -673,7 +974,7 @@ int dasp_dynamics_fwd(int kind, const float* x, const float* threshold_db, const
   DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
   if (bs == 0 || n == 0) return DASP_OK;
   DASP_REQUIRE(y != nullptr, "dynamics fwd: null y");
-  const int w = pick_warps(bs, (int)chs, 2);
+  const int w = pick_warps(bs, 2 * (int)chs);
   const int tile_len = w * 32 * kE;
   DynParams p{};
   p.x = x; p.y = y; p.threshold_db = threshold_db; p.ratio = ratio; p.attack_ms = attack_ms;
@@ -699,7 +1000,7 @@ int dasp_dynamics_bwd(int kind, const float* gy, const float* x, const float* th
   if (n == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 6 * bs, st)); return DASP_OK; }
   DASP_REQUIRE(gy && gx && ckpt, "dynamics bwd: null pointer");
   DASP_REQUIRE(lookahead == 0 || g_scratch != nullptr, "dynamics bwd: lookahead > 0 needs g_scratch (bs*n floats)");
-  const int w = pick_warps(bs, (int)chs, 2);
+  const int w = pick_warps(bs, 2 * (int)chs);
   const int tile_len = w * 32 * kE;
   DynParams p{};
   p.x = x; p.gy = gy; p.y = gx; p.threshold_db = threshold_db; p.ratio = ratio; p.attack_ms = attack_ms;
@@ -711,6 +1012,68 @@ int dasp_dynamics_bwd(int kind, const float* gy, const float* x, const float* th
   rc = kind == 0 ? dispatch<Curve::Compress>(true, w, p, bs, st) : dispatch<Curve::Expand>(true, w, p, bs, st);
   if (rc != DASP_OK) return rc;
   if (lookahead > 0) {
+    const int64_t total = bs * chs * n;
+    dynamics_lookahead_fixup_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gy, g_scratch, gx, n, (int)chs,
+                                                                                     (int)lookahead, total);
+    DASP_LAUNCH_OK("dynamics_lookahead_fixup_kernel");
+  }
+  return DASP_OK;
+}
+
+// ---- external side chain (key) ----
+int64_t dasp_dynamics_sidechain_tile_len(int64_t bs, int64_t chs, int64_t key_chs) {
+  if (chs < 1 || chs > kMaxChs || key_chs < 1 || key_chs > kMaxChs || 2 * chs + key_chs > kMaxBufs) return 0;
+  return (int64_t)pick_warps(bs, (int)(2 * chs + key_chs)) * 32 * kE;
+}
+
+int dasp_dynamics_sidechain_fwd(int kind, const float* x, const float* key, int64_t key_chs, const float* threshold_db,
+                                const float* ratio, const float* attack_ms, const float* knee_db,
+                                const float* makeup_db, float* y, float* ckpt, int64_t bs, int64_t chs, int64_t n,
+                                float sample_rate, float eps, int64_t lookahead, void* stream) {
+  const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
+  int rc = check_common(x, ps, bs, chs, n, lookahead);
+  if (rc != DASP_OK) return rc;
+  rc = check_key(key, key_chs, bs, chs, n);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
+  if (bs == 0 || n == 0) return DASP_OK;
+  DASP_REQUIRE(y != nullptr, "dynamics side chain fwd: null y");
+  const int w = pick_warps(bs, (int)(2 * chs + key_chs));
+  ScParams sp = sc_params(w, x, key, key_chs, ps, chs, n, sample_rate, eps, lookahead);
+  sp.d.y = y; sp.d.ckpt = ckpt;
+  sp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(y) && aligned16(key);
+  return kind == 0 ? dispatch_sc<Curve::Compress>(false, w, sp, bs, (cudaStream_t)stream)
+                   : dispatch_sc<Curve::Expand>(false, w, sp, bs, (cudaStream_t)stream);
+}
+
+int dasp_dynamics_sidechain_bwd(int kind, const float* gy, const float* x, const float* key, int64_t key_chs,
+                                const float* threshold_db, const float* ratio, const float* attack_ms,
+                                const float* knee_db, const float* makeup_db, const float* ckpt, float* gx,
+                                float* gkey, float* gparams, float* g_scratch, int64_t bs, int64_t chs, int64_t n,
+                                float sample_rate, float eps, int64_t lookahead, void* stream) {
+  const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
+  int rc = check_common(x, ps, bs, chs, n, lookahead);
+  if (rc != DASP_OK) return rc;
+  rc = check_key(key, key_chs, bs, chs, n);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
+  if (bs == 0) return DASP_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  DASP_REQUIRE(gparams != nullptr, "dynamics side chain bwd: null gparams");
+  if (n == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 6 * bs, st)); return DASP_OK; }
+  DASP_REQUIRE(gy && gx && ckpt, "dynamics side chain bwd: null pointer");
+  DASP_REQUIRE(lookahead == 0 || g_scratch != nullptr,
+               "dynamics side chain bwd: lookahead > 0 needs g_scratch (bs*n floats)");
+  const int w = pick_warps(bs, (int)(2 * chs + key_chs));
+  ScParams sp = sc_params(w, x, key, key_chs, ps, chs, n, sample_rate, eps, lookahead);
+  sp.d.gy = gy; sp.d.y = gx; sp.d.ckpt = const_cast<float*>(ckpt); sp.d.gparams = gparams; sp.d.g_scratch = g_scratch;
+  sp.gkey = gkey;
+  sp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(gy) && aligned16(gx) && aligned16(key) &&
+              (gkey == nullptr || aligned16(gkey));
+  rc = kind == 0 ? dispatch_sc<Curve::Compress>(true, w, sp, bs, st) : dispatch_sc<Curve::Expand>(true, w, sp, bs, st);
+  if (rc != DASP_OK) return rc;
+  if (lookahead > 0) {
+    // the kernel wrote gx = 0; add the direct term gy[m+la] G[m+la]
     const int64_t total = bs * chs * n;
     dynamics_lookahead_fixup_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gy, g_scratch, gx, n, (int)chs,
                                                                                      (int)lookahead, total);

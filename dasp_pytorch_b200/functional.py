@@ -30,6 +30,8 @@ __all__ = [
     "parametric_eq",
     "compressor",
     "expander",
+    "sidechain_compressor",
+    "sidechain_expander",
     "noise_shaped_reverberation",
     "convolution_reverberation",
 ]
@@ -333,8 +335,80 @@ class _DynamicsFn(torch.autograd.Function):
         return gx, gp[:, 0], gp[:, 1], gp[:, 2], gp[:, 4], gp[:, 5], None, None, None, None
 
 
+SIDECHAIN_MAX_CHANNELS = 32
+# the backward streams x, dL/dy and the key through shared memory: 2 * channels + key channels tiles per stage
+SIDECHAIN_MAX_BUFFERS = 76
+
+
+class _DynamicsSidechainFn(torch.autograd.Function):
+    """The dynamics processor with the detector on a key (bs, K, n): kind 0 = compressor, 1 = expander."""
+
+    @staticmethod
+    def forward(ctx, x, key, threshold, ratio, attack, knee, makeup, kind, sample_rate, eps, lookahead):
+        lib = _abi.lib()
+        bs, chs, n = x.shape
+        kc = key.shape[1]
+        y = torch.empty_like(x)
+        need_bwd = any(ctx.needs_input_grad[:7])
+        ckpt = None
+        with torch.cuda.device(x.device):
+            if need_bwd:
+                tile = lib.dasp_dynamics_sidechain_tile_len(bs, chs, kc)
+                if tile <= 0:
+                    raise DaspError(f"dynamics: unsupported channel counts {chs} (x) and {kc} (sidechain)")
+                ckpt = torch.empty(bs * max(1, -(-n // tile)), dtype=torch.float32, device=x.device)
+            with _timed("comp_sc_fwd", x.device):
+                check(lib.dasp_dynamics_sidechain_fwd(kind, ptr(x), ptr(key), kc, ptr(threshold), ptr(ratio),
+                                                      ptr(attack), ptr(knee), ptr(makeup), ptr(y), ptr(ckpt), bs, chs,
+                                                      n, float(sample_rate), float(eps), int(lookahead),
+                                                      stream_ptr(x.device)), "dasp_dynamics_sidechain_fwd")
+        if need_bwd:
+            ctx.save_for_backward(x, key, threshold, ratio, attack, knee, makeup, ckpt)
+        ctx.cfg = (kind, float(sample_rate), float(eps), int(lookahead))
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _abi.lib()
+        x, key, threshold, ratio, attack, knee, makeup, ckpt = ctx.saved_tensors
+        kind, sample_rate, eps, lookahead = ctx.cfg
+        bs, chs, n = x.shape
+        gy = gy.contiguous()
+        gx = torch.empty_like(x)
+        # a fixed key (e.g. a voice-over ducking music) writes no key gradient
+        gkey = torch.empty_like(key) if ctx.needs_input_grad[1] else None
+        gp = torch.empty(bs, 6, dtype=torch.float32, device=x.device)
+        scratch = torch.empty(bs * n, dtype=torch.float32, device=x.device) if lookahead > 0 else None
+        with torch.cuda.device(x.device), _timed("comp_sc_bwd", x.device):
+            check(lib.dasp_dynamics_sidechain_bwd(kind, ptr(gy), ptr(x), ptr(key), key.shape[1], ptr(threshold),
+                                                  ptr(ratio), ptr(attack), ptr(knee), ptr(makeup), ptr(ckpt), ptr(gx),
+                                                  ptr(gkey), ptr(gp), ptr(scratch), bs, chs, n, sample_rate, eps,
+                                                  lookahead, stream_ptr(x.device)), "dasp_dynamics_sidechain_bwd")
+        return gx, gkey, gp[:, 0], gp[:, 1], gp[:, 2], gp[:, 4], gp[:, 5], None, None, None, None
+
+
+def _sidechain(sidechain, x):
+    """validate the key against x (before any conversion or launch) -> (fp32 contiguous key, its dtype)"""
+    if not torch.is_tensor(sidechain) or sidechain.dim() != 3:
+        raise ValueError("sidechain must be a tensor of shape (batch, key_channels, samples)")
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, channels, samples)")
+    bs, chs, n = x.shape
+    kb, kc, kn = sidechain.shape
+    if kb != bs or kn != n:
+        raise ValueError(f"sidechain has shape {tuple(sidechain.shape)}: its batch and length must equal x's {(bs, n)}")
+    if not 1 <= kc <= SIDECHAIN_MAX_CHANNELS:
+        raise ValueError(f"sidechain: 1 to {SIDECHAIN_MAX_CHANNELS} key channels are supported, got {kc}")
+    if 2 * chs + kc > SIDECHAIN_MAX_BUFFERS:
+        raise ValueError(f"sidechain: 2 * {chs} channels + {kc} key channels exceeds {SIDECHAIN_MAX_BUFFERS}")
+    if sidechain.device != x.device:
+        raise DaspError(f"sidechain is on {sidechain.device} but x is on {x.device}")
+    return _audio(sidechain, "sidechain")
+
+
 def _dynamics(kind, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-              lookahead_samples):
+              lookahead_samples, sidechain=None):
+    key = _sidechain(sidechain, x)[0] if sidechain is not None else None
     xf, dt = _audio(x)
     bs = xf.shape[0]
     ps = [
@@ -350,17 +424,26 @@ def _dynamics(kind, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, 
     # release_ms is validated for shape only: the reference accepts and ignores it
     # (functional.py:333,343-344), so it receives no gradient here either.
     _param(release_ms, bs, xf, "release_ms", allow_broadcast=True)
-    y = _DynamicsFn.apply(xf, *ps, kind, sample_rate, eps, int(lookahead_samples))
+    if key is not None:
+        y = _DynamicsSidechainFn.apply(xf, key, *ps, kind, sample_rate, eps, int(lookahead_samples))
+    else:
+        y = _DynamicsFn.apply(xf, *ps, kind, sample_rate, eps, int(lookahead_samples))
     return y.to(dt)
 
 
 def dynamics_packed(kind: int, x: torch.Tensor, sample_rate: float, params: torch.Tensor, eps: float = 1e-8,
-                    lookahead_samples: int = 0):
+                    lookahead_samples: int = 0, *, sidechain: Optional[torch.Tensor] = None):
     """compressor (kind 0) / expander (kind 1) with the six parameters stacked as ``(bs, 6)`` in signature order
-    (threshold, ratio, attack, release, knee, makeup).  One transpose instead of six column copies."""
+    (threshold, ratio, attack, release, knee, makeup).  One transpose instead of six column copies.  ``sidechain``:
+    ``None`` for ``compressor`` / ``expander``, a key tensor for ``sidechain_compressor`` / ``sidechain_expander``."""
+    key = _sidechain(sidechain, x)[0] if sidechain is not None else None
     xf, dt = _audio(x)
     pt = _packed(params, xf.shape[0], 6, xf, "params").t().contiguous()        # (6, bs): rows are contiguous
-    y = _DynamicsFn.apply(xf, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, int(lookahead_samples))
+    if key is not None:
+        y = _DynamicsSidechainFn.apply(xf, key, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps,
+                                       int(lookahead_samples))
+    else:
+        y = _DynamicsFn.apply(xf, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, int(lookahead_samples))
     return y.to(dt)
 
 
@@ -415,6 +498,61 @@ def expander(
     """
     return _dynamics(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
                      lookahead_samples)
+
+
+def sidechain_compressor(
+    x: torch.Tensor,
+    sample_rate: float,
+    threshold_db: torch.Tensor,
+    ratio: torch.Tensor,
+    attack_ms: torch.Tensor,
+    release_ms: torch.Tensor,
+    knee_db: torch.Tensor,
+    makeup_gain_db: torch.Tensor,
+    eps: float = 1e-8,
+    lookahead_samples: int = 0,
+    *,
+    sidechain: torch.Tensor,
+):
+    """``compressor`` whose detector listens to an external side chain, the *key* (no reference counterpart: the
+    reference always detects on ``x.sum(dim=1)``).  ``compressor`` keeps the reference's signature; this function has
+    the same parameters plus the keyword-only ``sidechain``.
+
+    ``sidechain`` is a tensor ``(bs, K, n)`` with ``1 <= K <= 32`` and ``2 * channels + K <= 76``, with x's batch and
+    length and any channel count of its own.  The detector reads ``side = sidechain.sum(dim=1)`` (accumulated in fp64,
+    rounded once to fp32) instead of x; level, static curve, attack smoother and makeup are the compressor's, and the
+    gain is applied to every channel of x: ``y[b, c, t] = x[b, c, t - lookahead_samples] * G[b, t]``.  The look-ahead
+    delays the audio path only, not the key.  Uses: ducking (music keyed by a voice-over), a de-esser keyed by
+    ``parametric_eq(x, ...)`` with a presence boost (gradients reach the EQ parameters).
+
+    Gradients: x receives ``dL/dy * G`` (shifted by the look-ahead, no detector term); every key channel receives the
+    same ``dL/dside``, which carries ``1/side`` and is 0 where ``|side| < eps``; the parameters as in ``compressor``
+    (``release_ms`` gets none).  The key may be in any floating dtype (computed in fp32, its gradient returned in its
+    dtype); a key that does not require a gradient gets none written.  ``sidechain=x`` gives the same ``y`` as
+    ``compressor``; x's gradient is then the sum of both paths.
+    """
+    return _dynamics(0, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
+                     lookahead_samples, sidechain)
+
+
+def sidechain_expander(
+    x: torch.Tensor,
+    sample_rate: float,
+    threshold_db: torch.Tensor,
+    ratio: torch.Tensor,
+    attack_ms: torch.Tensor,
+    release_ms: torch.Tensor,
+    knee_db: torch.Tensor,
+    makeup_gain_db: torch.Tensor,
+    eps: float = 1e-8,
+    lookahead_samples: int = 0,
+    *,
+    sidechain: torch.Tensor,
+):
+    """``expander`` whose detector listens to the key ``sidechain``, exactly as ``sidechain_compressor`` does for
+    the compressor: gating one track from another."""
+    return _dynamics(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
+                     lookahead_samples, sidechain)
 
 
 # --------------------------------------------------------------------------------------

@@ -33,6 +33,8 @@ from dasp_pytorch_b200.functional import (
     gain,
     noise_shaped_reverberation,
     parametric_eq,
+    sidechain_compressor,
+    sidechain_expander,
 )
 
 
@@ -110,6 +112,11 @@ class Processor:
         tensor, which then goes to the kernels as is -- instead of the reference's per-parameter slicing,
         2 host syncs and ~3 tiny kernels per parameter (modules.py:56-91).  Same errors, same results.
         """
+        return self._process_normalized(x, param_tensor)
+
+    def _process_normalized(self, x: torch.Tensor, param_tensor: torch.Tensor, by_name=None, **fn_kw):
+        """process_normalized; ``fn_kw`` (keyword arguments beyond the parameters) goes to either path's call, and
+        ``by_name`` (default ``process_fn``) is the function the by-name path calls"""
         if self._packed_path is not None and self.process_fn is self._packed_path[1] and param_tensor.is_cuda:
             if param_tensor.dim() != 2 or param_tensor.shape[1] != len(self.param_ranges):
                 raise ValueError(
@@ -123,10 +130,10 @@ class Processor:
                 if int(flag.item()) != 0:
                     flag.zero_()
                     self.denormalize_param_dict(self.extract_param_dict(param_tensor))      # raises with the name
-            return self._packed_path[0](x, self.sample_rate, phys)
+            return self._packed_path[0](x, self.sample_rate, phys, **fn_kw)
         param_dict = self.extract_param_dict(param_tensor)
         denorm = self.denormalize_param_dict(param_dict, _checked=self._range_check(param_tensor))
-        return self.process_fn(x, self.sample_rate, **denorm)
+        return (by_name or self.process_fn)(x, self.sample_rate, **denorm, **fn_kw)
 
     def _affine(self, device):
         key = (str(device), tuple(self.param_ranges.values()))
@@ -245,12 +252,26 @@ class _Dynamics(Processor):
             "makeup_gain_db": (min_makeup_gain_db, max_makeup_gain_db),
         }
 
+    # the side-chain counterpart of the package's process_fn (functional.sidechain_compressor / _expander)
+    _sidechain_fn = None
+
+    def process_normalized(self, x: torch.Tensor, param_tensor: torch.Tensor, sidechain=None):
+        """``Processor.process_normalized`` with an optional key: ``sidechain`` (bs, K, n) drives the detector
+        instead of x (see ``functional.sidechain_compressor``); ``None`` runs the plain processor.  With a key, the
+        by-name path calls the side-chain function while ``process_fn`` is still this package's, otherwise
+        ``process_fn(x, sample_rate, **params, sidechain=sidechain)``."""
+        if sidechain is None:
+            return self._process_normalized(x, param_tensor)
+        by_name = self._sidechain_fn if self.process_fn is self._packed_path[1] else None
+        return self._process_normalized(x, param_tensor, by_name, sidechain=sidechain)
+
 
 class Compressor(_Dynamics):
     def __init__(self, sample_rate: int, **kw):
         super().__init__(sample_rate, **kw)
         self.process_fn = compressor
-        self._packed_path = (lambda x, sr, p: _F.dynamics_packed(0, x, sr, p), compressor)
+        self._sidechain_fn = sidechain_compressor
+        self._packed_path = (lambda x, sr, p, **kw: _F.dynamics_packed(0, x, sr, p, **kw), compressor)
 
 
 class Expander(_Dynamics):
@@ -259,7 +280,8 @@ class Expander(_Dynamics):
     def __init__(self, sample_rate: int, max_ratio: float = 4.0, **kw):
         super().__init__(sample_rate, max_ratio=max_ratio, **kw)
         self.process_fn = expander
-        self._packed_path = (lambda x, sr, p: _F.dynamics_packed(1, x, sr, p), expander)
+        self._sidechain_fn = sidechain_expander
+        self._packed_path = (lambda x, sr, p, **kw: _F.dynamics_packed(1, x, sr, p, **kw), expander)
 
 
 class NoiseShapedReverb(Processor):

@@ -130,6 +130,26 @@ int dasp_dynamics_bwd(int kind, const float* gy, const float* x, const float* th
                       const float* makeup_db, const float* ckpt, float* gx, float* gparams,
                       float* g_scratch, int64_t bs, int64_t chs, int64_t n, float sample_rate, float eps,
                       int64_t lookahead, void* stream);
+/* External side chain: the gain is computed from a key (bs, key_chs, n) instead of from x (ducking, de-essing with an
+ * EQ'd copy of x, gating one track from another).  side = the sum of the key_chs key channels (fp64, rounded once),
+ * then the same level, static curve, attack smoother and makeup; y[b,c,t] = x[b,c,t-lookahead] * G[b,t] (the key is
+ * not delayed).  1 <= key_chs <= 32 and 2 * chs + key_chs <= 76: the backward streams x, dL/dy -> dL/dx and
+ * key -> dL/dkey through three shared-memory stages, which hold 76 tiles of the smallest (224-sample) geometry in
+ * 200 KB.  Other combinations return -1 before any CUDA call, and the tile-length query returns 0 for them.
+ * ckpt holds bs * ceil(n / dasp_dynamics_sidechain_tile_len(bs, chs, key_chs)) floats.  Backward: gx = gy * G with no
+ * detector term (shifted by the look-ahead); gkey (bs, key_chs, n) receives dL/dside, so all its key_chs rows of an
+ * item are equal; gkey may be NULL, which writes no key gradient.  gparams and g_scratch as above. */
+int64_t dasp_dynamics_sidechain_tile_len(int64_t bs, int64_t chs, int64_t key_chs);
+int dasp_dynamics_sidechain_fwd(int kind, const float* x, const float* key, int64_t key_chs,
+                                const float* threshold_db, const float* ratio, const float* attack_ms,
+                                const float* knee_db, const float* makeup_db, float* y, float* ckpt, int64_t bs,
+                                int64_t chs, int64_t n, float sample_rate, float eps, int64_t lookahead, void* stream);
+int dasp_dynamics_sidechain_bwd(int kind, const float* gy, const float* x, const float* key, int64_t key_chs,
+                                const float* threshold_db, const float* ratio, const float* attack_ms,
+                                const float* knee_db, const float* makeup_db, const float* ckpt, float* gx,
+                                float* gkey /* may be NULL */, float* gparams, float* g_scratch, int64_t bs,
+                                int64_t chs, int64_t n, float sample_rate, float eps, int64_t lookahead,
+                                void* stream);
 
 /* ---- parametric_eq: six cascaded biquads   (reference functional.py:118-272 with
  *      signal.biquad signal.py:242-306 and signal.sosfilt_via_fsm signal.py:136-166) ------

@@ -50,6 +50,8 @@ _SIGNATURES = {
     "dasp_shutdown": (None, []),
     "dasp_debug_force_warps": (None, [c_int]),
     "dasp_debug_eq_bwd_stages": (None, [c_int]),
+    "dasp_debug_eq_fwd_stages": (None, [c_int]),
+    "dasp_debug_eq_pair_tables": (None, [c_int]),
     "dasp_debug_reverb_path": (None, [c_int]),
     "dasp_debug_reverb_last_path": (c_int, []),
     "dasp_debug_reverb_flat_filterbank": (None, [c_int]),

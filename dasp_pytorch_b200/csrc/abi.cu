@@ -37,6 +37,10 @@ int debug_reverb_path() { return g_reverb_path; }
 
 static int g_eq_bwd_stages = 0;
 int debug_eq_bwd_stages() { return g_eq_bwd_stages; }
+static int g_eq_fwd_stages = 0;
+int debug_eq_fwd_stages() { return g_eq_fwd_stages; }
+static int g_eq_pair_tables = 0;
+int debug_eq_pair_tables() { return g_eq_pair_tables; }
 static int g_flat_fb = 0;
 int debug_flat_filterbank() { return g_flat_fb; }
 
@@ -81,6 +85,8 @@ int dasp_denormalize(const float* p01, const float* lo, const float* span, float
 }
 
 void dasp_debug_eq_bwd_stages(int stages) { dasp::g_eq_bwd_stages = (stages == 1 || stages == 2) ? stages : 0; }
+void dasp_debug_eq_fwd_stages(int stages) { dasp::g_eq_fwd_stages = (stages == 1 || stages == 2) ? stages : 0; }
+void dasp_debug_eq_pair_tables(int on) { dasp::g_eq_pair_tables = on ? 1 : 0; }
 
 void dasp_debug_reverb_flat_filterbank(int on) { dasp::g_flat_fb = on ? 1 : 0; }
 

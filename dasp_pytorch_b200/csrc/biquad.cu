@@ -812,14 +812,21 @@ int env_int(const char* name) {
   return v ? atoi(v) : 0;
 }
 int tune_fwd_w() { static const int v = env_int("DASP_EQ_FWD_W"); return v; }
-int tune_fwd_s() { static const int v = env_int("DASP_EQ_FWD_S"); return v; }
+int tune_fwd_s() {
+  static const int v = env_int("DASP_EQ_FWD_S");
+  return debug_eq_fwd_stages() ? debug_eq_fwd_stages() : v;
+}
 int tune_bwd_w() { static const int v = env_int("DASP_EQ_BWD_W"); return v; }
 int tune_bwd_s() {
   static const int v = env_int("DASP_EQ_BWD_S");
   return debug_eq_bwd_stages() ? debug_eq_bwd_stages() : v;
 }
-// force the general (pair-coefficient) tables even when every pair lies inside one item: test hook via the env
-int tune_force_pair_tables() { static const int v = env_int("DASP_EQ_PAIR_TABLES"); return v; }
+// force the general (pair-coefficient) tables even when every pair lies inside one item: test hook
+// (dasp_debug_eq_pair_tables) or the env
+int tune_force_pair_tables() {
+  static const int v = env_int("DASP_EQ_PAIR_TABLES");
+  return debug_eq_pair_tables() ? debug_eq_pair_tables() : v;
+}
 
 // Warps per row pair (W in {1, 2, 3, 4, 8}, forward also 16; 0 / other = automatic).  The automatic choice: forward W=4
 // with two load stages at large batches; small batches want W=8 to fill the SMs at all.  The backward holds 255

@@ -61,6 +61,11 @@ int sm_count();  // cached cudaDevAttrMultiProcessorCount of the current device
 int debug_forced_warps();
 // Test hook (dasp_debug_eq_bwd_stages): 0 = automatic; 1 / 2 pins the number of x / dL/dy stages of the EQ backward
 int debug_eq_bwd_stages();
+// Test hook (dasp_debug_eq_fwd_stages): 0 = automatic; 1 / 2 pins the number of load stages of the EQ forward
+int debug_eq_fwd_stages();
+// Test hook (dasp_debug_eq_pair_tables): 0 = automatic; 1 = the EQ kernels use (row A, row B) pair coefficient tables
+// even when both rows of every pair belong to one item
+int debug_eq_pair_tables();
 // Test hook (dasp_debug_reverb_path): IR synthesis of the device-noise reverb: 0 = automatic, 1 = generator / cuFFT /
 // shaping kernels, 2 = generator -> ifft_shape_kernel for R <= 8 (instead of the default cluster kernel)
 int debug_reverb_path();

@@ -55,6 +55,11 @@ void dasp_shutdown(void);
 void dasp_debug_force_warps(int warps);
 /* test hook: pin the number of x / dL/dy stages per warp of the EQ backward (1 or 2; 0 = automatic) */
 void dasp_debug_eq_bwd_stages(int stages);
+/* test hook: pin the number of load stages per warp of the EQ forward (1 or 2; 0 = automatic) */
+void dasp_debug_eq_fwd_stages(int stages);
+/* test hook: 1 = the EQ kernels use (row A, row B) pair coefficient tables even when both rows of every pair belong
+ * to one item (even channel counts); 0 = automatic (pair tables only where a pair straddles two items) */
+void dasp_debug_eq_pair_tables(int on);
 /* test hook, IR synthesis of the device-noise reverb (all variants draw the same Philox stream and must agree):
    0 = automatic (block FFT of 8192 points: one warp-specialised thread-block-cluster kernel for polyphase factors
    R <= 6, generator -> fused in-shared-memory inverse FFT + shaping kernel otherwise),

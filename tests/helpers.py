@@ -42,6 +42,28 @@ def peak_err(a, b):
     return (a - b).reshape(bs, -1).abs().amax(1) / b.reshape(bs, -1).abs().amax(1).clamp_min(1e-30)
 
 
+def eq_kernel_instantiations(lib_path):
+    """{(direction, table type, W, S)} of the eq_fwd_kernel / eq_bwd_kernel entry points in the library, read from
+    its symbol table with cuobjdump; None where cuobjdump is not installed"""
+    import os
+    import re
+    import shutil
+    import subprocess
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(cuobjdump):
+        return None
+    out = subprocess.run([cuobjdump, "-symbols", lib_path], capture_output=True, text=True).stdout
+    pat = re.compile(r"STO_ENTRY\s+\S*eq_(fwd|bwd)_kernelI(f|6float2)Li(\d+)ELi(\d+)E")
+    return {(m[1], "float" if m[2] == "f" else "float2", int(m[3]), int(m[4])) for m in pat.finditer(out)}
+
+
+# the EQ kernels dispatch_fwd / dispatch_bwd (biquad.cu) can launch: the backward has no W = 16, and its (8, 2) does
+# not fit in shared memory (eight warps x eight units of 2 x 480 floats), so a request for it falls through to (8, 1)
+EQ_INSTANTIATIONS = ({("fwd", c, w, s) for c in ("float", "float2") for w in (1, 2, 3, 4, 8, 16) for s in (1, 2)}
+                     | {("bwd", c, w, s) for c in ("float", "float2") for w in (1, 2, 3, 4) for s in (1, 2)}
+                     | {("bwd", c, 8, 1) for c in ("float", "float2")})
+
+
 def param_grad_err(got, ref):
     """per-item |got-ref| / max_over_params|ref| for lists of (bs,) gradients (SURVEY.md 8c)."""
     keep = [i for i, r in enumerate(ref) if r is not None]

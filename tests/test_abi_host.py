@@ -44,6 +44,17 @@ def test_sm90a_sass_and_tma(lib):
     assert "UBLKCP" in sass and "SYNCS" in sass               # cp.async.bulk + mbarrier in the scan kernels
 
 
+def test_eq_kernel_instantiations(lib):
+    """the library holds exactly the EQ kernels the dispatch can launch (tests/test_gpu_eq_variants.py pins and
+    profiles each of them)"""
+    from dasp_pytorch_b200 import _abi
+    from helpers import EQ_INSTANTIATIONS, eq_kernel_instantiations
+    got = eq_kernel_instantiations(_abi.LIB_PATH)
+    if got is None:
+        pytest.skip("cuobjdump not available")
+    assert got == EQ_INSTANTIATIONS, (sorted(got - EQ_INSTANTIATIONS), sorted(EQ_INSTANTIATIONS - got))
+
+
 @pytest.mark.parametrize("taps,sr", [(1023, 44100.0), (255, 44100.0), (1023, 48000.0), (511, 96000.0)])
 def test_filterbank_matches_scipy(lib, taps, sr):
     import oracle

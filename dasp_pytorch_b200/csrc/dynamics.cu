@@ -18,6 +18,13 @@
 // it recomputes the forward quantities from that checkpoint, then runs the adjoint recurrence
 // w[n] = ds[n] + a w[n+1] with the mirrored scan (shfl_down), accumulates the five parameter
 // gradients in registers across tiles (deterministic), and writes dL/dx in place.
+//
+// External side chain: the detector listens to a key (bs, K, N) instead of x.  The plain kernels
+// (dynamics_fwd_kernel / dynamics_bwd_kernel) and the keyed ones (dynamics_sc_fwd_kernel /
+// dynamics_sc_bwd_kernel) are instantiations of one forward and one backward body, templated on KEY.
+// They differ in three places only: which stage buffers the detector sums (x from buffer 0, or the
+// key from buffer C, 2C in the backward); what the backward writes to the dL/dx buffers (plain:
+// gy G + the detector term; keyed: gy G); and where dL/dside goes (into x's rows, or into the key's).
 #include <math.h>
 #include <stdlib.h>
 
@@ -77,6 +84,57 @@ struct BwdRows {          // backward: buffers [0,C) = x (read only), [C,2C) = g
   }
   __device__ __forceinline__ float* dst(int b) const { return b < chs ? nullptr : gx0 + (int64_t)(b - chs) * n; }
 };
+
+// the keyed kernels' arguments: side = the sum of the K key channels, y = x[n - la] * G[n]; the key is never delayed
+struct ScParams {
+  DynParams d;
+  const float* key;      // (bs, K, N)
+  float* gkey;           // (bs, K, N) backward out, or null: no dL/dkey, the key rows are only read
+  int key_chs;
+};
+struct ScFwdRows {        // buffers [0,C) = x (in) -> y (out), [C,C+K) = key (read only)
+  const float* x0; float* y0; const float* k0; int64_t n; int chs;
+  __device__ __forceinline__ const float* src(int b) const {
+    return b < chs ? x0 + (int64_t)b * n : k0 + (int64_t)(b - chs) * n;
+  }
+  __device__ __forceinline__ float* dst(int b) const { return b < chs ? y0 + (int64_t)b * n : nullptr; }
+};
+struct ScBwdRows {        // [0,C) = x (read only), [C,2C) = gy (in) -> gx (out), [2C,2C+K) = key (in) -> dL/dkey (out)
+  const float* x0; const float* g0; float* gx0; const float* k0; float* gk0; int64_t n; int chs;
+  __device__ __forceinline__ const float* src(int b) const {
+    if (b < chs) return x0 + (int64_t)b * n;
+    if (b < 2 * chs) return g0 + (int64_t)(b - chs) * n;
+    return k0 + (int64_t)(b - 2 * chs) * n;
+  }
+  __device__ __forceinline__ float* dst(int b) const {
+    if (b < chs) return nullptr;
+    if (b < 2 * chs) return gx0 + (int64_t)(b - chs) * n;
+    return gk0 ? gk0 + (int64_t)(b - 2 * chs) * n : nullptr;
+  }
+};
+
+// the stage-buffer rows of one item, without (ChannelRows / BwdRows) or with a key (ScFwdRows / ScBwdRows)
+template <bool KEY>
+__device__ __forceinline__ auto fwd_rows(const DynParams& p, const float* key, int K, int item) {
+  const int C = p.chs;
+  if constexpr (KEY) {
+    return ScFwdRows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, key + (int64_t)item * K * p.n, p.n,
+                     C};
+  } else {
+    return ChannelRows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, p.n};
+  }
+}
+template <bool KEY>
+__device__ __forceinline__ auto bwd_rows(const DynParams& p, const float* key, float* gkey, int K, int item) {
+  const int C = p.chs;
+  const int64_t base = (int64_t)item * C * p.n;
+  if constexpr (KEY) {
+    const int64_t kbase = (int64_t)item * K * p.n;
+    return ScBwdRows{p.x + base, p.gy + base, p.y + base, key + kbase, gkey ? gkey + kbase : nullptr, p.n, C};
+  } else {
+    return BwdRows{p.x + base, p.gy + base, p.y + base, p.n, C};
+  }
+}
 
 // ---- per-item constants of the smoother ---------------------------------------------------
 struct PoleTables {
@@ -283,8 +341,9 @@ constexpr size_t kSmemHeader = 512;
 // LA: lookahead_samples > 0 (rare; kept out of the common instantiation).  ST: stereo specialisation (C == 2, no
 // look-ahead): the two channel values of a sample stay in registers between the side-chain sum and the gain application
 // instead of being read from shared memory twice (round 2: the scan kernels are bound by the shared-memory pipe).
-template <Curve CV, int W, bool LA, bool ST = false>
-__global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
+// KEY: the detector sums the K key buffers that follow x's C (K = 0 without a key); ST is for the plain path only.
+template <Curve CV, int W, bool LA, bool ST, bool KEY>
+__device__ __forceinline__ void dynamics_fwd(const DynParams p, const float* key, int K) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem<W> sm(smem_raw);
   const int item = blockIdx.x;
@@ -298,9 +357,9 @@ __global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
   make_tables(tb, p.attack_ms[item], p.sample_rate, lane);
 
   TileGeom g{p.n, tile_len, p.ntiles, false};
-  ChannelRows rows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, p.n};
+  auto rows = fwd_rows<KEY>(p, key, K, item);
   TilePipe<kStages> pipe;
-  pipe.init(sm.bars, sm.stages, C, tile_len, p.bulk != 0);
+  pipe.init(sm.bars, sm.stages, KEY ? C + K : C, tile_len, p.bulk != 0);
   pipe.prologue(g, rows);
 
   float c_tile = 0.f;                      // smoother state entering the current tile
@@ -322,7 +381,7 @@ __global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
 #pragma unroll
         for (int j = 0; j < kE; ++j) { x0[ST ? j : 0] = xa[j]; x1[ST ? j : 0] = xb[j]; xs[j] = xa[j] + xb[j]; }
       } else {
-        side_chain(xs, pipe, st, C, off);
+        side_chain(xs, pipe, st, KEY ? K : C, off, KEY ? C : 0);     // the key, or x
       }
       float run = 0.f;
 #pragma unroll
@@ -351,20 +410,31 @@ __global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
         for (int j = 0; j < kE; ++j) xb[j] *= G[j];
       }
     } else {
-      // y[n] = x[n - la] * G[n]  (functional.py:383-385): delayed input straight from global/L2
+      // y[n] = x[n - la] * G[n]  (functional.py:383-385): delayed input straight from global/L2 (the keyed kernels
+      // through the read-only path: with a plain load the compressor's keyed W = 4 look-ahead forward spills)
       for (int c = 0; c < C; ++c) {
         float* xb = pipe.buf(st, c) + off;
         const float* xr = rows.src(c);
 #pragma unroll
         for (int j = 0; j < kE; ++j) {
           const int64_t m = n0 + j - p.lookahead;
-          xb[j] = (m >= 0 && n0 + j < p.n) ? xr[m] * G[j] : 0.f;
+          xb[j] = (m >= 0 && n0 + j < p.n) ? (KEY ? __ldg(xr + m) : xr[m]) * G[j] : 0.f;
         }
       }
     }
     pipe.release(i, g, rows);
   }
   pipe.drain();
+}
+
+template <Curve CV, int W, bool LA, bool ST = false>
+__global__ void __launch_bounds__(W * 32) dynamics_fwd_kernel(DynParams p) {
+  dynamics_fwd<CV, W, LA, ST, false>(p, nullptr, 0);
+}
+
+template <Curve CV, int W, bool LA>
+__global__ void __launch_bounds__(W * 32) dynamics_sc_fwd_kernel(ScParams sp) {
+  dynamics_fwd<CV, W, LA, false, true>(sp.d, sp.key, sp.key_chs);
 }
 
 // =============================================================================== backward
@@ -400,8 +470,9 @@ __device__ __forceinline__ void param_grads(float (&red)[5][W], float acc_m, flo
   }
 }
 
-template <Curve CV, int W, bool LA, bool ST = false>
-__global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1)) dynamics_bwd_kernel(DynParams p) {
+// KEY: the detector sums the K key buffers that follow x's C and dL/dy's C; gkey (may be null) receives dL/dside
+template <Curve CV, int W, bool LA, bool ST, bool KEY>
+__device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key, float* gkey, int K) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem<W> sm(smem_raw);
   __shared__ float red[5][W];
@@ -422,10 +493,9 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
   const float rlane_pow = tr.lane_pow;
 
   TileGeom g{p.n, tile_len, p.ntiles, true};
-  const int64_t base = (int64_t)item * C * p.n;
-  BwdRows rows{p.x + base, p.gy + base, p.y + base, p.n, C};
+  auto rows = bwd_rows<KEY>(p, key, gkey, K, item);
   TilePipe<kStages> pipe;
-  pipe.init(sm.bars, sm.stages, 2 * C, tile_len, p.bulk != 0);
+  pipe.init(sm.bars, sm.stages, KEY ? 2 * C + K : 2 * C, tile_len, p.bulk != 0);
   pipe.prologue(g, rows);
 
   float w_tile = 0.f;                                 // adjoint state w[first sample of the next tile]
@@ -451,7 +521,7 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
         xs[j] = xa[j] + xb[j];
       }
     } else {
-      side_chain(xs, pipe, st, C, off);
+      side_chain(xs, pipe, st, KEY ? K : C, off, KEY ? 2 * C : 0);     // the key, or x
     }
     {
       float run = 0.f;
@@ -503,7 +573,7 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
     }
     const float w_in = scan_reverse<W>(wv[0], w_tile, tb, rlane_pow, sm.agg + (i & 1) * 2 * W + W, lane, warp);
 
-    // ---- parameter-gradient integrands and dL/dx ----
+    // ---- parameter-gradient integrands and dL/dside ----
     float dxs[kE];
 #pragma unroll
     for (int j = 0; j < kE; ++j) {
@@ -522,6 +592,7 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
       }
       dxs[j] = dx;
     }
+    // dL/dx = gy G, plus dL/dside on the plain path (x is the detector's input there)
     if (ST) {
       float* ga = pipe.buf(st, 2) + off;
       float* gb = pipe.buf(st, 3) + off;
@@ -531,7 +602,7 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
       for (int c = 0; c < C; ++c) {
         float* gb = pipe.buf(st, C + c) + off;
 #pragma unroll
-        for (int j = 0; j < kE; ++j) gb[j] = fmaf(gb[j], G[j], dxs[j]);
+        for (int j = 0; j < kE; ++j) gb[j] = KEY ? gb[j] * G[j] : fmaf(gb[j], G[j], dxs[j]);
       }
     } else {
       // direct term gy[m+la]*G[m+la] is added by dynamics_lookahead_fixup_kernel from g_scratch
@@ -542,250 +613,11 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
       for (int c = 0; c < C; ++c) {
         float* gb = pipe.buf(st, C + c) + off;
 #pragma unroll
-        for (int j = 0; j < kE; ++j) gb[j] = dxs[j];
+        for (int j = 0; j < kE; ++j) gb[j] = KEY ? 0.f : dxs[j];
       }
     }
-    pipe.release(i, g, rows);
-  }
-  pipe.drain();
-  param_grads<W>(red, acc_m, acc_a, acc_t, acc_r, acc_w, tb.alpha, attack, p.sample_rate,
-                 p.gparams, item, lane, warp);
-}
-
-// lookahead > 0 only: gx[b,c,m] += gy[b,c,m+la] * G[b,m+la]
-__global__ void dynamics_lookahead_fixup_kernel(const float* __restrict__ gy, const float* __restrict__ G,
-                                                float* __restrict__ gx, int64_t n, int chs, int la, int64_t total) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int64_t m = idx % n;
-  const int64_t row = idx / n;
-  const int64_t item = row / chs;
-  if (m + la < n) gx[idx] += gy[idx + la] * G[item * n + m + la];
-}
-
-// =============================================================================== external side chain
-// The detector listens to a key (bs, K, N) instead of x: side = the sum of the K key channels (side_chain over the
-// key buffers, fp64, rounded once), G from it exactly as above, y = x[n - la] * G[n].  The key is never delayed.
-// Backward: x gets gy G only (no detector term), and every key channel gets the same dL/dside.
-struct ScParams {
-  DynParams d;
-  const float* key;      // (bs, K, N)
-  float* gkey;           // (bs, K, N) backward out, or null: no dL/dkey, the key rows are only read
-  int key_chs;
-};
-struct ScFwdRows {        // buffers [0,C) = x (in) -> y (out), [C,C+K) = key (read only)
-  const float* x0; float* y0; const float* k0; int64_t n; int chs;
-  __device__ __forceinline__ const float* src(int b) const {
-    return b < chs ? x0 + (int64_t)b * n : k0 + (int64_t)(b - chs) * n;
-  }
-  __device__ __forceinline__ float* dst(int b) const { return b < chs ? y0 + (int64_t)b * n : nullptr; }
-};
-struct ScBwdRows {        // [0,C) = x (read only), [C,2C) = gy (in) -> gx (out), [2C,2C+K) = key (in) -> dL/dkey (out)
-  const float* x0; const float* g0; float* gx0; const float* k0; float* gk0; int64_t n; int chs;
-  __device__ __forceinline__ const float* src(int b) const {
-    if (b < chs) return x0 + (int64_t)b * n;
-    if (b < 2 * chs) return g0 + (int64_t)(b - chs) * n;
-    return k0 + (int64_t)(b - 2 * chs) * n;
-  }
-  __device__ __forceinline__ float* dst(int b) const {
-    if (b < chs) return nullptr;
-    if (b < 2 * chs) return gx0 + (int64_t)(b - chs) * n;
-    return gk0 ? gk0 + (int64_t)(b - 2 * chs) * n : nullptr;
-  }
-};
-
-template <Curve CV, int W, bool LA>
-__global__ void __launch_bounds__(W * 32) dynamics_sc_fwd_kernel(ScParams sp) {
-  const DynParams& p = sp.d;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  Smem<W> sm(smem_raw);
-  const int item = blockIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int C = p.chs, K = sp.key_chs;
-  const int tile_len = W * 32 * kE;
-
-  const float M = p.makeup_db[item];
-  const CurveK ck = make_curve(CV, p.threshold_db[item], p.ratio[item], p.knee_db[item]);
-  PoleTables tb;
-  make_tables(tb, p.attack_ms[item], p.sample_rate, lane);
-
-  TileGeom g{p.n, tile_len, p.ntiles, false};
-  ScFwdRows rows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, sp.key + (int64_t)item * K * p.n, p.n, C};
-  TilePipe<kStages> pipe;
-  pipe.init(sm.bars, sm.stages, C + K, tile_len, p.bulk != 0);
-  pipe.prologue(g, rows);
-
-  float c_tile = 0.f;
-  const int off = threadIdx.x * kE;
-  for (int i = 0; i < p.ntiles; ++i) {
-    pipe.acquire(i, g, rows);
-    const int st = i % kStages;
-    const int64_t n0 = (int64_t)i * tile_len + off;
-    if (p.ckpt && threadIdx.x == 0) p.ckpt[(int64_t)item * p.ntiles + i] = c_tile;
-
-    float s[kE];
-    {
-      float xs[kE];
-      side_chain(xs, pipe, st, K, off, C);
-      float run = 0.f;
-#pragma unroll
-      for (int j = 0; j < kE; ++j) {
-        float gc = 0.f;
-        if (n0 + j < p.n) gc = gain_computer<CV, false>(level_db(xs[j], p.eps), ck).gc;
-        run = fmaf(tb.alpha, run, tb.beta * gc);
-        s[j] = run;
-      }
-    }
-    const float c_in = scan_forward<W>(s[kE - 1], c_tile, tb, sm.agg + (i & 1) * W, lane, warp);
-
-    float G[kE];
-#pragma unroll
-    for (int j = 0; j < kE; ++j) G[j] = exp2f((fmaf(tb.apow[j], c_in, s[j]) + M) * kLog2Of10Over20);
-    if (!LA) {
-      for (int c = 0; c < C; ++c) {
-        float* xb = pipe.buf(st, c) + off;
-#pragma unroll
-        for (int j = 0; j < kE; ++j) xb[j] *= G[j];
-      }
-    } else {
-      // y[n] = x[n - la] * G[n]: delayed input straight from global/L2
-      for (int c = 0; c < C; ++c) {
-        float* xb = pipe.buf(st, c) + off;
-        const float* xr = rows.x0 + (int64_t)c * p.n;
-#pragma unroll
-        for (int j = 0; j < kE; ++j) {
-          const int64_t m = n0 + j - p.lookahead;
-          xb[j] = (m >= 0 && n0 + j < p.n) ? __ldg(xr + m) * G[j] : 0.f;
-        }
-      }
-    }
-    pipe.release(i, g, rows);
-  }
-  pipe.drain();
-}
-
-template <Curve CV, int W, bool LA>
-__global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1))
-    dynamics_sc_bwd_kernel(ScParams sp) {
-  const DynParams p = sp.d;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  Smem<W> sm(smem_raw);
-  __shared__ float red[5][W];
-  const int item = blockIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int C = p.chs, K = sp.key_chs;
-  const int tile_len = W * 32 * kE;
-  const int la = p.lookahead;
-
-  const float M = p.makeup_db[item];
-  const CurveK ck = make_curve(CV, p.threshold_db[item], p.ratio[item], p.knee_db[item]);
-  const float attack = p.attack_ms[item];
-  PoleTables tb;
-  make_tables(tb, attack, p.sample_rate, lane);
-  PoleTables tr;
-  make_tables(tr, attack, p.sample_rate, 31 - lane);
-  const float rlane_pow = tr.lane_pow;
-
-  TileGeom g{p.n, tile_len, p.ntiles, true};
-  const int64_t base = (int64_t)item * C * p.n, kbase = (int64_t)item * K * p.n;
-  ScBwdRows rows{p.x + base, p.gy + base, p.y + base, sp.key + kbase, sp.gkey ? sp.gkey + kbase : nullptr, p.n, C};
-  TilePipe<kStages> pipe;
-  pipe.init(sm.bars, sm.stages, 2 * C + K, tile_len, p.bulk != 0);
-  pipe.prologue(g, rows);
-
-  float w_tile = 0.f;
-  float acc_m = 0.f, acc_a = 0.f, acc_t = 0.f, acc_r = 0.f, acc_w = 0.f;
-  const int off = threadIdx.x * kE;
-  for (int i = 0; i < p.ntiles; ++i) {
-    pipe.acquire(i, g, rows);
-    const int st = i % kStages;
-    const int tile = g.tile_of(i);
-    const int64_t n0 = (int64_t)tile * tile_len + off;
-
-    // ---- recompute the forward quantities of this tile from its checkpoint ----
-    float xs[kE], s[kE], gcv[kE], dxdbv[kE], drv[kE], dwv[kE];
-    side_chain(xs, pipe, st, K, off, 2 * C);
-    {
-      float run = 0.f;
-#pragma unroll
-      for (int j = 0; j < kE; ++j) {
-        CurveOut o; o.gc = 0.f; o.d_xdb = 0.f; o.d_t = 0.f; o.d_r = 0.f; o.d_w = 0.f;
-        if (n0 + j < p.n) o = gain_computer<CV, true>(level_db(xs[j], p.eps), ck);
-        gcv[j] = o.gc; dxdbv[j] = o.d_xdb; drv[j] = o.d_r; dwv[j] = o.d_w;
-        run = fmaf(tb.alpha, run, tb.beta * o.gc);
-        s[j] = run;
-      }
-    }
-    float c_tile = p.ckpt[(int64_t)item * p.ntiles + tile];
-    const float c_in = scan_forward<W>(s[kE - 1], c_tile, tb, sm.agg + (i & 1) * 2 * W, lane, warp);
-#pragma unroll
-    for (int j = 0; j < kE; ++j) s[j] = fmaf(tb.apow[j], c_in, s[j]);
-
-    // ---- dL/ds = ln10/20 G sum_c gy_c x_c (x delayed under LA) and the zero-state local adjoint pass ----
-    float G[kE], wv[kE];
-    {
-      float dG[kE];
-#pragma unroll
-      for (int j = 0; j < kE; ++j) dG[j] = 0.f;
-      for (int c = 0; c < C; ++c) {
-        const float* xb = pipe.buf(st, c) + off;
-        const float* gb = pipe.buf(st, C + c) + off;
-        if (!LA) {
-#pragma unroll
-          for (int j = 0; j < kE; ++j) dG[j] = fmaf(gb[j], xb[j], dG[j]);
-        } else {
-          const float* xr = rows.x0 + (int64_t)c * p.n;
-#pragma unroll
-          for (int j = 0; j < kE; ++j) {
-            const int64_t m = n0 + j - la;
-            if (m >= 0 && n0 + j < p.n) dG[j] = fmaf(gb[j], xr[m], dG[j]);
-          }
-        }
-      }
-      float run = 0.f;
-#pragma unroll
-      for (int j = kE - 1; j >= 0; --j) {
-        const bool valid = (n0 + j < p.n);
-        G[j] = exp2f((s[j] + M) * kLog2Of10Over20);
-        const float ds = valid ? dG[j] * G[j] * kLn10Over20 : 0.f;
-        acc_m += ds;
-        run = fmaf(tb.alpha, run, ds);
-        wv[j] = run;
-      }
-    }
-    const float w_in = scan_reverse<W>(wv[0], w_tile, tb, rlane_pow, sm.agg + (i & 1) * 2 * W + W, lane, warp);
-
-    // ---- parameter-gradient integrands and dL/dside ----
-    float dxs[kE];
-#pragma unroll
-    for (int j = 0; j < kE; ++j) {
-      const float w = fmaf(tb.apow[kE - 1 - j], w_in, wv[j]);
-      const bool valid = (n0 + j < p.n);
-      const float s_prev = (j == 0) ? c_in : s[j - 1];
-      float dx = 0.f;
-      if (valid) {
-        acc_a = fmaf(w, s_prev - gcv[j], acc_a);
-        const float dgc = tb.beta * w;
-        acc_t = fmaf(dgc, -dxdbv[j], acc_t);
-        acc_r = fmaf(dgc, drv[j], acc_r);
-        acc_w = fmaf(dgc, dwv[j], acc_w);
-        if (fabsf(xs[j]) >= p.eps) dx = __fdividef(dgc * dxdbv[j] * kDbGradScale, xs[j]);
-      }
-      dxs[j] = dx;
-    }
-    // dL/dx = gy G; under LA the direct term gy[m+la] G[m+la] is added to zeros by dynamics_lookahead_fixup_kernel
-    if (LA) {
-      float* gs = p.g_scratch + (int64_t)item * p.n;
-#pragma unroll
-      for (int j = 0; j < kE; ++j)
-        if (n0 + j < p.n) gs[n0 + j] = G[j];
-    }
-    for (int c = 0; c < C; ++c) {
-      float* gb = pipe.buf(st, C + c) + off;
-#pragma unroll
-      for (int j = 0; j < kE; ++j) gb[j] = LA ? 0.f : gb[j] * G[j];
-    }
-    if (sp.gkey) {
+    // with a key, dL/dside goes to every key channel instead (if a key gradient is wanted)
+    if (KEY && gkey) {
       for (int k = 0; k < K; ++k) {
         float* kb = pipe.buf(st, 2 * C + k) + off;
 #pragma unroll
@@ -797,6 +629,28 @@ __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W
   pipe.drain();
   param_grads<W>(red, acc_m, acc_a, acc_t, acc_r, acc_w, tb.alpha, attack, p.sample_rate,
                  p.gparams, item, lane, warp);
+}
+
+template <Curve CV, int W, bool LA, bool ST = false>
+__global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1)) dynamics_bwd_kernel(DynParams p) {
+  dynamics_bwd<CV, W, LA, ST, false>(p, nullptr, nullptr, 0);
+}
+
+template <Curve CV, int W, bool LA>
+__global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1))
+    dynamics_sc_bwd_kernel(ScParams sp) {
+  dynamics_bwd<CV, W, LA, false, true>(sp.d, sp.key, sp.gkey, sp.key_chs);
+}
+
+// lookahead > 0 only: gx[b,c,m] += gy[b,c,m+la] * G[b,m+la]
+__global__ void dynamics_lookahead_fixup_kernel(const float* __restrict__ gy, const float* __restrict__ G,
+                                                float* __restrict__ gx, int64_t n, int chs, int la, int64_t total) {
+  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int64_t m = idx % n;
+  const int64_t row = idx / n;
+  const int64_t item = row / chs;
+  if (m + la < n) gx[idx] += gy[idx + la] * G[item * n + m + la];
 }
 
 // ---- host side -----------------------------------------------------------------------------
@@ -844,72 +698,39 @@ int ensure_smem_optin() {
 }
 size_t smem_bytes(int w, int nbuf) { return kSmemHeader + (size_t)kStages * nbuf * (w * 32 * kE) * 4; }
 
+// one launch of Kernel (a plain kernel takes DynParams, a keyed one ScParams) with nbuf tile buffers per stage
+template <auto Kernel, class Args>
+int launch(const char* name, const Args& args, int w, int nbuf, int64_t bs, cudaStream_t st) {
+  { int rc = ensure_smem_optin<Kernel>(); if (rc != DASP_OK) return rc; }
+  Kernel<<<(unsigned)bs, w * 32, smem_bytes(w, nbuf), st>>>(args);
+  DASP_LAUNCH_OK(name);
+  return DASP_OK;
+}
+// the keyed kernels when sp.key_chs > 0 (ST is plain-only), the plain ones otherwise
 template <Curve CV, int W, bool LA, bool ST>
-int launch_fwd_la(const DynParams& p, int64_t bs, cudaStream_t st) {
-  const size_t smem = smem_bytes(W, p.chs);
-  { int rc = ensure_smem_optin<dynamics_fwd_kernel<CV, W, LA, ST>>(); if (rc != DASP_OK) return rc; }
-  dynamics_fwd_kernel<CV, W, LA, ST><<<(unsigned)bs, W * 32, smem, st>>>(p);
-  DASP_LAUNCH_OK("dynamics_fwd_kernel");
-  return DASP_OK;
-}
-template <Curve CV, int W, bool LA, bool ST>
-int launch_bwd_la(const DynParams& p, int64_t bs, cudaStream_t st) {
-  const size_t smem = smem_bytes(W, 2 * p.chs);
-  { int rc = ensure_smem_optin<dynamics_bwd_kernel<CV, W, LA, ST>>(); if (rc != DASP_OK) return rc; }
-  dynamics_bwd_kernel<CV, W, LA, ST><<<(unsigned)bs, W * 32, smem, st>>>(p);
-  DASP_LAUNCH_OK("dynamics_bwd_kernel");
-  return DASP_OK;
-}
-template <Curve CV, int W>
-int launch_fwd_w(const DynParams& p, int64_t bs, cudaStream_t st) {
-  if (p.lookahead > 0) return launch_fwd_la<CV, W, true, false>(p, bs, st);
-  return (p.chs == 2 && !debug_generic_channels()) ? launch_fwd_la<CV, W, false, true>(p, bs, st)
-                                                   : launch_fwd_la<CV, W, false, false>(p, bs, st);
-}
-template <Curve CV, int W>
-int launch_bwd_w(const DynParams& p, int64_t bs, cudaStream_t st) {
-  if (p.lookahead > 0) return launch_bwd_la<CV, W, true, false>(p, bs, st);
-  return (p.chs == 2 && !debug_generic_channels()) ? launch_bwd_la<CV, W, false, true>(p, bs, st)
-                                                   : launch_bwd_la<CV, W, false, false>(p, bs, st);
-}
-
-template <Curve CV>
-int dispatch(bool bwd, int w, const DynParams& p, int64_t bs, cudaStream_t st) {
-  switch (w) {
-    case 1: return bwd ? launch_bwd_w<CV, 1>(p, bs, st) : launch_fwd_w<CV, 1>(p, bs, st);
-    case 2: return bwd ? launch_bwd_w<CV, 2>(p, bs, st) : launch_fwd_w<CV, 2>(p, bs, st);
-    case 4: return bwd ? launch_bwd_w<CV, 4>(p, bs, st) : launch_fwd_w<CV, 4>(p, bs, st);
-    case 16: return bwd ? launch_bwd_w<CV, 16>(p, bs, st) : launch_fwd_w<CV, 16>(p, bs, st);
-    default: return bwd ? launch_bwd_w<CV, 8>(p, bs, st) : launch_fwd_w<CV, 8>(p, bs, st);
+int launch_variant(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
+  const int nbuf = (bwd ? 2 : 1) * sp.d.chs + sp.key_chs;     // x (and dL/dy), then the key
+  if (sp.key_chs > 0) {
+    return bwd ? launch<dynamics_sc_bwd_kernel<CV, W, LA>>("dynamics_sc_bwd_kernel", sp, W, nbuf, bs, st)
+               : launch<dynamics_sc_fwd_kernel<CV, W, LA>>("dynamics_sc_fwd_kernel", sp, W, nbuf, bs, st);
   }
-}
-
-template <Curve CV, int W, bool LA>
-int launch_sc(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
-  const int C = sp.d.chs, K = sp.key_chs;
-  if (bwd) {
-    { int rc = ensure_smem_optin<dynamics_sc_bwd_kernel<CV, W, LA>>(); if (rc != DASP_OK) return rc; }
-    dynamics_sc_bwd_kernel<CV, W, LA><<<(unsigned)bs, W * 32, smem_bytes(W, 2 * C + K), st>>>(sp);
-    DASP_LAUNCH_OK("dynamics_sc_bwd_kernel");
-  } else {
-    { int rc = ensure_smem_optin<dynamics_sc_fwd_kernel<CV, W, LA>>(); if (rc != DASP_OK) return rc; }
-    dynamics_sc_fwd_kernel<CV, W, LA><<<(unsigned)bs, W * 32, smem_bytes(W, C + K), st>>>(sp);
-    DASP_LAUNCH_OK("dynamics_sc_fwd_kernel");
-  }
-  return DASP_OK;
+  return bwd ? launch<dynamics_bwd_kernel<CV, W, LA, ST>>("dynamics_bwd_kernel", sp.d, W, nbuf, bs, st)
+             : launch<dynamics_fwd_kernel<CV, W, LA, ST>>("dynamics_fwd_kernel", sp.d, W, nbuf, bs, st);
 }
 template <Curve CV, int W>
-int launch_sc_w(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
-  return sp.d.lookahead > 0 ? launch_sc<CV, W, true>(bwd, sp, bs, st) : launch_sc<CV, W, false>(bwd, sp, bs, st);
+int launch_w(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
+  if (sp.d.lookahead > 0) return launch_variant<CV, W, true, false>(bwd, sp, bs, st);
+  const bool stereo = sp.key_chs == 0 && sp.d.chs == 2 && !debug_generic_channels();
+  return stereo ? launch_variant<CV, W, false, true>(bwd, sp, bs, st) : launch_variant<CV, W, false, false>(bwd, sp, bs, st);
 }
 template <Curve CV>
-int dispatch_sc(bool bwd, int w, const ScParams& sp, int64_t bs, cudaStream_t st) {
+int dispatch(bool bwd, int w, const ScParams& sp, int64_t bs, cudaStream_t st) {
   switch (w) {
-    case 1: return launch_sc_w<CV, 1>(bwd, sp, bs, st);
-    case 2: return launch_sc_w<CV, 2>(bwd, sp, bs, st);
-    case 4: return launch_sc_w<CV, 4>(bwd, sp, bs, st);
-    case 16: return launch_sc_w<CV, 16>(bwd, sp, bs, st);
-    default: return launch_sc_w<CV, 8>(bwd, sp, bs, st);
+    case 1: return launch_w<CV, 1>(bwd, sp, bs, st);
+    case 2: return launch_w<CV, 2>(bwd, sp, bs, st);
+    case 4: return launch_w<CV, 4>(bwd, sp, bs, st);
+    case 16: return launch_w<CV, 16>(bwd, sp, bs, st);
+    default: return launch_w<CV, 8>(bwd, sp, bs, st);
   }
 }
 
@@ -937,9 +758,13 @@ int check_key(const float* key, int64_t key_chs, int64_t bs, int64_t chs, int64_
   return DASP_OK;
 }
 
-// the fields both side-chain directions share, for tiles of w warps
-ScParams sc_params(int w, const float* x, const float* key, int64_t key_chs, const float* ps[5], int64_t chs,
-                   int64_t n, float sample_rate, float eps, int64_t lookahead) {
+// warps per item for both directions: the backward holds 2 buffers per channel plus one per key channel (key_chs = 0
+// without a key), so that is the geometry that has to fit
+int dyn_warps(int64_t bs, int64_t chs, int64_t key_chs) { return pick_warps(bs, (int)(2 * chs + key_chs)); }
+
+// the fields both directions share, for tiles of w warps; key = nullptr, key_chs = 0 on the plain path
+ScParams dyn_params(int w, const float* x, const float* key, int64_t key_chs, const float* ps[5], int64_t chs,
+                    int64_t n, float sample_rate, float eps, int64_t lookahead) {
   const int tile_len = w * 32 * kE;
   ScParams sp{};
   DynParams& p = sp.d;
@@ -948,6 +773,47 @@ ScParams sc_params(int w, const float* x, const float* key, int64_t key_chs, con
   p.sample_rate = sample_rate; p.eps = eps;
   sp.key = key; sp.key_chs = (int)key_chs;
   return sp;
+}
+
+// the forward and backward of both paths, after the entry points' argument checks
+int dyn_fwd(int kind, const float* x, const float* key, int64_t key_chs, const float* ps[5], float* y, float* ckpt,
+            int64_t bs, int64_t chs, int64_t n, float sample_rate, float eps, int64_t lookahead, cudaStream_t st) {
+  const char* what = key_chs ? "dynamics side chain" : "dynamics";
+  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
+  if (bs == 0 || n == 0) return DASP_OK;
+  DASP_REQUIRE(y != nullptr, "%s fwd: null y", what);
+  const int w = dyn_warps(bs, chs, key_chs);
+  ScParams sp = dyn_params(w, x, key, key_chs, ps, chs, n, sample_rate, eps, lookahead);
+  sp.d.y = y; sp.d.ckpt = ckpt;
+  sp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(y) && aligned16(key);      // a null pointer counts as aligned
+  return kind == 0 ? dispatch<Curve::Compress>(false, w, sp, bs, st) : dispatch<Curve::Expand>(false, w, sp, bs, st);
+}
+
+int dyn_bwd(int kind, const float* gy, const float* x, const float* key, int64_t key_chs, const float* ps[5],
+            const float* ckpt, float* gx, float* gkey, float* gparams, float* g_scratch, int64_t bs, int64_t chs,
+            int64_t n, float sample_rate, float eps, int64_t lookahead, cudaStream_t st) {
+  const char* what = key_chs ? "dynamics side chain" : "dynamics";
+  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(gparams != nullptr, "%s bwd: null gparams", what);
+  if (n == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 6 * bs, st)); return DASP_OK; }
+  DASP_REQUIRE(gy && gx && ckpt, "%s bwd: null pointer", what);
+  DASP_REQUIRE(lookahead == 0 || g_scratch != nullptr, "%s bwd: lookahead > 0 needs g_scratch (bs*n floats)", what);
+  const int w = dyn_warps(bs, chs, key_chs);
+  ScParams sp = dyn_params(w, x, key, key_chs, ps, chs, n, sample_rate, eps, lookahead);
+  sp.d.gy = gy; sp.d.y = gx; sp.d.ckpt = const_cast<float*>(ckpt); sp.d.gparams = gparams; sp.d.g_scratch = g_scratch;
+  sp.gkey = gkey;
+  sp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(gy) && aligned16(gx) && aligned16(key) && aligned16(gkey);
+  int rc = kind == 0 ? dispatch<Curve::Compress>(true, w, sp, bs, st) : dispatch<Curve::Expand>(true, w, sp, bs, st);
+  if (rc != DASP_OK) return rc;
+  if (lookahead > 0) {
+    // the kernel left dL/dx without the direct term gy[m+la] G[m+la]; add it
+    const int64_t total = bs * chs * n;
+    dynamics_lookahead_fixup_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gy, g_scratch, gx, n, (int)chs,
+                                                                                     (int)lookahead, total);
+    DASP_LAUNCH_OK("dynamics_lookahead_fixup_kernel");
+  }
+  return DASP_OK;
 }
 
 }  // namespace
@@ -960,8 +826,7 @@ extern "C" {
 // samples per tile the forward/backward pair will use for this problem shape (checkpoint pitch)
 int64_t dasp_dynamics_tile_len(int64_t bs, int64_t chs) {
   if (chs < 1 || chs > kMaxChs) return 0;
-  // the backward holds 2 buffers per channel: pick the geometry that fits both directions
-  return (int64_t)pick_warps(bs, 2 * (int)chs) * 32 * kE;
+  return (int64_t)dyn_warps(bs, chs, 0) * 32 * kE;
 }
 
 int dasp_dynamics_fwd(int kind, const float* x, const float* threshold_db, const float* ratio,
@@ -971,19 +836,7 @@ int dasp_dynamics_fwd(int kind, const float* x, const float* threshold_db, const
   const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
   int rc = check_common(x, ps, bs, chs, n, lookahead);
   if (rc != DASP_OK) return rc;
-  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
-  if (bs == 0 || n == 0) return DASP_OK;
-  DASP_REQUIRE(y != nullptr, "dynamics fwd: null y");
-  const int w = pick_warps(bs, 2 * (int)chs);
-  const int tile_len = w * 32 * kE;
-  DynParams p{};
-  p.x = x; p.y = y; p.threshold_db = threshold_db; p.ratio = ratio; p.attack_ms = attack_ms;
-  p.knee_db = knee_db; p.makeup_db = makeup_db; p.ckpt = ckpt; p.n = n; p.chs = (int)chs;
-  p.ntiles = (int)((n + tile_len - 1) / tile_len); p.lookahead = (int)lookahead;
-  p.sample_rate = sample_rate; p.eps = eps;
-  p.bulk = (n % 4 == 0) && aligned16(x) && aligned16(y);
-  return kind == 0 ? dispatch<Curve::Compress>(false, w, p, bs, (cudaStream_t)stream)
-                   : dispatch<Curve::Expand>(false, w, p, bs, (cudaStream_t)stream);
+  return dyn_fwd(kind, x, nullptr, 0, ps, y, ckpt, bs, chs, n, sample_rate, eps, lookahead, (cudaStream_t)stream);
 }
 
 int dasp_dynamics_bwd(int kind, const float* gy, const float* x, const float* threshold_db, const float* ratio,
@@ -993,37 +846,14 @@ int dasp_dynamics_bwd(int kind, const float* gy, const float* x, const float* th
   const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
   int rc = check_common(x, ps, bs, chs, n, lookahead);
   if (rc != DASP_OK) return rc;
-  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
-  if (bs == 0) return DASP_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  DASP_REQUIRE(gparams != nullptr, "dynamics bwd: null gparams");
-  if (n == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 6 * bs, st)); return DASP_OK; }
-  DASP_REQUIRE(gy && gx && ckpt, "dynamics bwd: null pointer");
-  DASP_REQUIRE(lookahead == 0 || g_scratch != nullptr, "dynamics bwd: lookahead > 0 needs g_scratch (bs*n floats)");
-  const int w = pick_warps(bs, 2 * (int)chs);
-  const int tile_len = w * 32 * kE;
-  DynParams p{};
-  p.x = x; p.gy = gy; p.y = gx; p.threshold_db = threshold_db; p.ratio = ratio; p.attack_ms = attack_ms;
-  p.knee_db = knee_db; p.makeup_db = makeup_db; p.ckpt = const_cast<float*>(ckpt); p.gparams = gparams;
-  p.g_scratch = g_scratch; p.n = n; p.chs = (int)chs;
-  p.ntiles = (int)((n + tile_len - 1) / tile_len); p.lookahead = (int)lookahead;
-  p.sample_rate = sample_rate; p.eps = eps;
-  p.bulk = (n % 4 == 0) && aligned16(x) && aligned16(gy) && aligned16(gx);
-  rc = kind == 0 ? dispatch<Curve::Compress>(true, w, p, bs, st) : dispatch<Curve::Expand>(true, w, p, bs, st);
-  if (rc != DASP_OK) return rc;
-  if (lookahead > 0) {
-    const int64_t total = bs * chs * n;
-    dynamics_lookahead_fixup_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gy, g_scratch, gx, n, (int)chs,
-                                                                                     (int)lookahead, total);
-    DASP_LAUNCH_OK("dynamics_lookahead_fixup_kernel");
-  }
-  return DASP_OK;
+  return dyn_bwd(kind, gy, x, nullptr, 0, ps, ckpt, gx, nullptr, gparams, g_scratch, bs, chs, n, sample_rate, eps,
+                 lookahead, (cudaStream_t)stream);
 }
 
 // ---- external side chain (key) ----
 int64_t dasp_dynamics_sidechain_tile_len(int64_t bs, int64_t chs, int64_t key_chs) {
   if (chs < 1 || chs > kMaxChs || key_chs < 1 || key_chs > kMaxChs || 2 * chs + key_chs > kMaxBufs) return 0;
-  return (int64_t)pick_warps(bs, (int)(2 * chs + key_chs)) * 32 * kE;
+  return (int64_t)dyn_warps(bs, chs, key_chs) * 32 * kE;
 }
 
 int dasp_dynamics_sidechain_fwd(int kind, const float* x, const float* key, int64_t key_chs, const float* threshold_db,
@@ -1032,18 +862,9 @@ int dasp_dynamics_sidechain_fwd(int kind, const float* x, const float* key, int6
                                 float sample_rate, float eps, int64_t lookahead, void* stream) {
   const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
   int rc = check_common(x, ps, bs, chs, n, lookahead);
+  if (rc == DASP_OK) rc = check_key(key, key_chs, bs, chs, n);
   if (rc != DASP_OK) return rc;
-  rc = check_key(key, key_chs, bs, chs, n);
-  if (rc != DASP_OK) return rc;
-  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
-  if (bs == 0 || n == 0) return DASP_OK;
-  DASP_REQUIRE(y != nullptr, "dynamics side chain fwd: null y");
-  const int w = pick_warps(bs, (int)(2 * chs + key_chs));
-  ScParams sp = sc_params(w, x, key, key_chs, ps, chs, n, sample_rate, eps, lookahead);
-  sp.d.y = y; sp.d.ckpt = ckpt;
-  sp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(y) && aligned16(key);
-  return kind == 0 ? dispatch_sc<Curve::Compress>(false, w, sp, bs, (cudaStream_t)stream)
-                   : dispatch_sc<Curve::Expand>(false, w, sp, bs, (cudaStream_t)stream);
+  return dyn_fwd(kind, x, key, key_chs, ps, y, ckpt, bs, chs, n, sample_rate, eps, lookahead, (cudaStream_t)stream);
 }
 
 int dasp_dynamics_sidechain_bwd(int kind, const float* gy, const float* x, const float* key, int64_t key_chs,
@@ -1053,33 +874,10 @@ int dasp_dynamics_sidechain_bwd(int kind, const float* gy, const float* x, const
                                 float sample_rate, float eps, int64_t lookahead, void* stream) {
   const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
   int rc = check_common(x, ps, bs, chs, n, lookahead);
+  if (rc == DASP_OK) rc = check_key(key, key_chs, bs, chs, n);
   if (rc != DASP_OK) return rc;
-  rc = check_key(key, key_chs, bs, chs, n);
-  if (rc != DASP_OK) return rc;
-  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics: kind must be 0 (compressor) or 1 (expander)");
-  if (bs == 0) return DASP_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  DASP_REQUIRE(gparams != nullptr, "dynamics side chain bwd: null gparams");
-  if (n == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 6 * bs, st)); return DASP_OK; }
-  DASP_REQUIRE(gy && gx && ckpt, "dynamics side chain bwd: null pointer");
-  DASP_REQUIRE(lookahead == 0 || g_scratch != nullptr,
-               "dynamics side chain bwd: lookahead > 0 needs g_scratch (bs*n floats)");
-  const int w = pick_warps(bs, (int)(2 * chs + key_chs));
-  ScParams sp = sc_params(w, x, key, key_chs, ps, chs, n, sample_rate, eps, lookahead);
-  sp.d.gy = gy; sp.d.y = gx; sp.d.ckpt = const_cast<float*>(ckpt); sp.d.gparams = gparams; sp.d.g_scratch = g_scratch;
-  sp.gkey = gkey;
-  sp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(gy) && aligned16(gx) && aligned16(key) &&
-              (gkey == nullptr || aligned16(gkey));
-  rc = kind == 0 ? dispatch_sc<Curve::Compress>(true, w, sp, bs, st) : dispatch_sc<Curve::Expand>(true, w, sp, bs, st);
-  if (rc != DASP_OK) return rc;
-  if (lookahead > 0) {
-    // the kernel wrote gx = 0; add the direct term gy[m+la] G[m+la]
-    const int64_t total = bs * chs * n;
-    dynamics_lookahead_fixup_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gy, g_scratch, gx, n, (int)chs,
-                                                                                     (int)lookahead, total);
-    DASP_LAUNCH_OK("dynamics_lookahead_fixup_kernel");
-  }
-  return DASP_OK;
+  return dyn_bwd(kind, gy, x, key, key_chs, ps, ckpt, gx, gkey, gparams, g_scratch, bs, chs, n, sample_rate, eps,
+                 lookahead, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -293,75 +293,43 @@ def stereo_bus(x: torch.Tensor, sample_rate: int, send_db: torch.Tensor):
 # --------------------------------------------------------------------------------------
 
 
-class _DynamicsFn(torch.autograd.Function):
-    """Feed-forward dynamics processor: kind 0 = compressor, 1 = expander."""
-
-    @staticmethod
-    def forward(ctx, x, threshold, ratio, attack, knee, makeup, kind, sample_rate, eps, lookahead):
-        lib = _abi.lib()
-        bs, chs, n = x.shape
-        y = torch.empty_like(x)
-        need_bwd = any(ctx.needs_input_grad[:6])
-        ckpt = None
-        with torch.cuda.device(x.device):
-            if need_bwd:
-                tile = lib.dasp_dynamics_tile_len(bs, chs)     # depends on the device's SM count
-                if tile <= 0:
-                    raise DaspError(f"dynamics: unsupported channel count {chs}")
-                ckpt = torch.empty(bs * max(1, -(-n // tile)), dtype=torch.float32, device=x.device)
-            with _timed("comp_fwd", x.device):
-                check(lib.dasp_dynamics_fwd(kind, ptr(x), ptr(threshold), ptr(ratio), ptr(attack), ptr(knee),
-                                            ptr(makeup), ptr(y), ptr(ckpt), bs, chs, n, float(sample_rate),
-                                            float(eps), int(lookahead), stream_ptr(x.device)), "dasp_dynamics_fwd")
-        if need_bwd:
-            ctx.save_for_backward(x, threshold, ratio, attack, knee, makeup, ckpt)
-        ctx.cfg = (kind, float(sample_rate), float(eps), int(lookahead))
-        return y
-
-    @staticmethod
-    def backward(ctx, gy):
-        lib = _abi.lib()
-        x, threshold, ratio, attack, knee, makeup, ckpt = ctx.saved_tensors
-        kind, sample_rate, eps, lookahead = ctx.cfg
-        bs, chs, n = x.shape
-        gy = gy.contiguous()
-        gx = torch.empty_like(x)
-        gp = torch.empty(bs, 6, dtype=torch.float32, device=x.device)
-        scratch = torch.empty(bs * n, dtype=torch.float32, device=x.device) if lookahead > 0 else None
-        with torch.cuda.device(x.device), _timed("comp_bwd", x.device):
-            check(lib.dasp_dynamics_bwd(kind, ptr(gy), ptr(x), ptr(threshold), ptr(ratio), ptr(attack), ptr(knee),
-                                        ptr(makeup), ptr(ckpt), ptr(gx), ptr(gp), ptr(scratch), bs, chs, n,
-                                        sample_rate, eps, lookahead, stream_ptr(x.device)), "dasp_dynamics_bwd")
-        return gx, gp[:, 0], gp[:, 1], gp[:, 2], gp[:, 4], gp[:, 5], None, None, None, None
-
-
 SIDECHAIN_MAX_CHANNELS = 32
 # the backward streams x, dL/dy and the key through shared memory: 2 * channels + key channels tiles per stage
 SIDECHAIN_MAX_BUFFERS = 76
 
 
-class _DynamicsSidechainFn(torch.autograd.Function):
-    """The dynamics processor with the detector on a key (bs, K, n): kind 0 = compressor, 1 = expander."""
+class _DynamicsFn(torch.autograd.Function):
+    """Feed-forward dynamics processor: kind 0 = compressor, 1 = expander.  The detector listens to x, or to
+    ``key`` (bs, K, n) when one is given."""
 
     @staticmethod
     def forward(ctx, x, key, threshold, ratio, attack, knee, makeup, kind, sample_rate, eps, lookahead):
         lib = _abi.lib()
         bs, chs, n = x.shape
-        kc = key.shape[1]
         y = torch.empty_like(x)
         need_bwd = any(ctx.needs_input_grad[:7])
         ckpt = None
         with torch.cuda.device(x.device):
             if need_bwd:
-                tile = lib.dasp_dynamics_sidechain_tile_len(bs, chs, kc)
+                # depends on the device's SM count
+                if key is None:
+                    tile = lib.dasp_dynamics_tile_len(bs, chs)
+                    what = f"channel count {chs}"
+                else:
+                    tile = lib.dasp_dynamics_sidechain_tile_len(bs, chs, key.shape[1])
+                    what = f"channel counts {chs} (x) and {key.shape[1]} (sidechain)"
                 if tile <= 0:
-                    raise DaspError(f"dynamics: unsupported channel counts {chs} (x) and {kc} (sidechain)")
+                    raise DaspError(f"dynamics: unsupported {what}")
                 ckpt = torch.empty(bs * max(1, -(-n // tile)), dtype=torch.float32, device=x.device)
-            with _timed("comp_sc_fwd", x.device):
-                check(lib.dasp_dynamics_sidechain_fwd(kind, ptr(x), ptr(key), kc, ptr(threshold), ptr(ratio),
-                                                      ptr(attack), ptr(knee), ptr(makeup), ptr(y), ptr(ckpt), bs, chs,
-                                                      n, float(sample_rate), float(eps), int(lookahead),
-                                                      stream_ptr(x.device)), "dasp_dynamics_sidechain_fwd")
+            args = (ptr(threshold), ptr(ratio), ptr(attack), ptr(knee), ptr(makeup), ptr(y), ptr(ckpt), bs, chs, n,
+                    float(sample_rate), float(eps), int(lookahead), stream_ptr(x.device))
+            if key is None:
+                with _timed("comp_fwd", x.device):
+                    check(lib.dasp_dynamics_fwd(kind, ptr(x), *args), "dasp_dynamics_fwd")
+            else:
+                with _timed("comp_sc_fwd", x.device):
+                    check(lib.dasp_dynamics_sidechain_fwd(kind, ptr(x), ptr(key), key.shape[1], *args),
+                          "dasp_dynamics_sidechain_fwd")
         if need_bwd:
             ctx.save_for_backward(x, key, threshold, ratio, attack, knee, makeup, ckpt)
         ctx.cfg = (kind, float(sample_rate), float(eps), int(lookahead))
@@ -379,11 +347,16 @@ class _DynamicsSidechainFn(torch.autograd.Function):
         gkey = torch.empty_like(key) if ctx.needs_input_grad[1] else None
         gp = torch.empty(bs, 6, dtype=torch.float32, device=x.device)
         scratch = torch.empty(bs * n, dtype=torch.float32, device=x.device) if lookahead > 0 else None
-        with torch.cuda.device(x.device), _timed("comp_sc_bwd", x.device):
-            check(lib.dasp_dynamics_sidechain_bwd(kind, ptr(gy), ptr(x), ptr(key), key.shape[1], ptr(threshold),
-                                                  ptr(ratio), ptr(attack), ptr(knee), ptr(makeup), ptr(ckpt), ptr(gx),
-                                                  ptr(gkey), ptr(gp), ptr(scratch), bs, chs, n, sample_rate, eps,
-                                                  lookahead, stream_ptr(x.device)), "dasp_dynamics_sidechain_bwd")
+        with torch.cuda.device(x.device):
+            params = (ptr(threshold), ptr(ratio), ptr(attack), ptr(knee), ptr(makeup), ptr(ckpt), ptr(gx))
+            tail = (ptr(gp), ptr(scratch), bs, chs, n, sample_rate, eps, lookahead, stream_ptr(x.device))
+            if key is None:
+                with _timed("comp_bwd", x.device):
+                    check(lib.dasp_dynamics_bwd(kind, ptr(gy), ptr(x), *params, *tail), "dasp_dynamics_bwd")
+            else:
+                with _timed("comp_sc_bwd", x.device):
+                    check(lib.dasp_dynamics_sidechain_bwd(kind, ptr(gy), ptr(x), ptr(key), key.shape[1], *params,
+                                                          ptr(gkey), *tail), "dasp_dynamics_sidechain_bwd")
         return gx, gkey, gp[:, 0], gp[:, 1], gp[:, 2], gp[:, 4], gp[:, 5], None, None, None, None
 
 
@@ -424,10 +397,7 @@ def _dynamics(kind, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, 
     # release_ms is validated for shape only: the reference accepts and ignores it
     # (functional.py:333,343-344), so it receives no gradient here either.
     _param(release_ms, bs, xf, "release_ms", allow_broadcast=True)
-    if key is not None:
-        y = _DynamicsSidechainFn.apply(xf, key, *ps, kind, sample_rate, eps, int(lookahead_samples))
-    else:
-        y = _DynamicsFn.apply(xf, *ps, kind, sample_rate, eps, int(lookahead_samples))
+    y = _DynamicsFn.apply(xf, key, *ps, kind, sample_rate, eps, int(lookahead_samples))
     return y.to(dt)
 
 
@@ -439,11 +409,7 @@ def dynamics_packed(kind: int, x: torch.Tensor, sample_rate: float, params: torc
     key = _sidechain(sidechain, x)[0] if sidechain is not None else None
     xf, dt = _audio(x)
     pt = _packed(params, xf.shape[0], 6, xf, "params").t().contiguous()        # (6, bs): rows are contiguous
-    if key is not None:
-        y = _DynamicsSidechainFn.apply(xf, key, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps,
-                                       int(lookahead_samples))
-    else:
-        y = _DynamicsFn.apply(xf, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, int(lookahead_samples))
+    y = _DynamicsFn.apply(xf, key, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, int(lookahead_samples))
     return y.to(dt)
 
 

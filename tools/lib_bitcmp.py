@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Run seeded forward + backward calls of the reverbs through two builds of the library and compare every result byte
-for byte.
+"""Run seeded forward + backward calls of the reverbs and of the compressor / expander through two builds of the library
+and compare every result byte for byte.
 
     python tools/lib_bitcmp.py LIB_A LIB_B --out DIR
 
@@ -9,8 +9,11 @@ what its calls computed to DIR/a/<case>.npy and DIR/b/<case>.npy; then the files
 paths bench.py does not: the cuFFT pipeline and the two-kernel IR synthesis (dasp_debug_reverb_path 1 and 2), R = 9
 (two-kernel synthesis by default) and R = 17 (time-domain overlap-save), parity mode with a noise tensor, 2047 taps
 (nb = 16384: cuFFT polyphase synthesis), n % 4 != 0 (cuFFT convolution), mono input, and convolution_reverberation with
-per-item and shared impulse responses.  Refactors that must keep the bits use it; it needs a CUDA device.  Exit code 1
-on any difference.
+per-item and shared impulse responses.  The dynamics cases run both curves at every warps-per-item W the library can be
+pinned to (dasp_debug_force_warps), at lengths where that W fits: without a key mono (the generic channel loop), stereo
+(the stereo kernels), stereo through the generic loop (DASP_DYN_GENERIC=1) and a look-ahead; with a key a mono key, a
+stereo key, a look-ahead and a key that needs no gradient.  Refactors that must keep the bits use it; it needs a CUDA
+device.  Exit code 1 on any difference.
 """
 from __future__ import annotations
 
@@ -40,6 +43,21 @@ CASES = {
     "conv_item_n_odd": ("conv", 3, 2, 48001, 30000, 2, False, False),
     "conv_shared": ("conv", 4, 2, 48000, 30000, 2, True, False),
     "conv_shared_n_odd": ("conv", 4, 1, 48003, 20000, 1, True, False),
+}
+
+# dynamics: name: (x channels, key channels (0: no key), look-ahead, DASP_DYN_GENERIC, key gradient); each runs for
+# curve x W {1, 2, 4, 8, 16}.  2C + K <= 4 keeps every forced W; the look-ahead cases take an n % 4 != 0 (cooperative
+# copies instead of TMA)
+DYN_E = 7
+DYN_CASES = {
+    "mono": (1, 0, False, False, False),
+    "stereo": (2, 0, False, False, False),
+    "stereo_generic": (2, 0, False, True, False),
+    "lookahead": (2, 0, True, False, False),
+    "key_mono": (1, 1, False, False, True),
+    "key_stereo": (1, 2, False, False, True),
+    "key_lookahead": (1, 1, True, False, True),
+    "key_fixed": (1, 1, False, False, False),
 }
 
 
@@ -88,6 +106,64 @@ def run_cases(out_dir):
             a = v.detach().cpu().numpy() if torch.is_tensor(v) else v
             np.save(os.path.join(out_dir, f"{name}.{k}.npy"), a)
         print(f"{name}: done", flush=True)
+    run_dynamics_cases(out_dir)
+
+
+def run_dynamics_cases(out_dir):
+    """the dynamics cases: y, dL/dx, dL/dkey and the five parameter gradients of each"""
+    import torch
+
+    import dasp_pytorch_b200 as D
+    from dasp_pytorch_b200 import _abi
+
+    lib = _abi.lib()
+    dev = torch.device("cuda:0")
+    ci = 0
+    for curve in ("comp", "exp"):
+        for w in (1, 2, 4, 8, 16):
+            for case, (chs, kc, la, generic, key_grad) in DYN_CASES.items():
+                name = f"dyn_{curve}_W{w}_{case}"
+                ci += 1
+                g = torch.Generator().manual_seed(5000 + ci)
+                bs, T = 3, w * 32 * DYN_E
+                n = 2 * T + (37 if la else 36)
+                x = ((torch.rand(bs, chs, n, generator=g) * 2 - 1) * 0.5).to(dev).requires_grad_(True)
+                gy = torch.randn(bs, chs, n, generator=g).to(dev)
+                key = None
+                if kc:
+                    key = ((torch.rand(bs, kc, n, generator=g) * 2 - 1) * 0.5).to(dev).requires_grad_(key_grad)
+                u = [torch.rand(bs, generator=g) for _ in range(6)]
+                ratio = 1.5 + 4 * u[1] if curve == "comp" else 1.2 + 1.3 * u[1]
+                ps = [(-35 + 25 * u[0]), ratio, 1 + 20 * u[2], 50 + 100 * u[3], 1 + 10 * u[4], -3 + 6 * u[5]]
+                ps = [p.to(dev).requires_grad_(True) for p in ps]
+                lookahead = T + T // 2 + 5 if la else 0
+                if generic:
+                    os.environ["DASP_DYN_GENERIC"] = "1"
+                lib.dasp_debug_force_warps(w)
+                try:
+                    tile = (lib.dasp_dynamics_sidechain_tile_len(bs, chs, kc) if kc
+                            else lib.dasp_dynamics_tile_len(bs, chs))
+                    assert tile == T, (name, tile, T)
+                    if kc:
+                        fn = D.functional.sidechain_compressor if curve == "comp" else D.functional.sidechain_expander
+                        y = fn(x, SR, *ps, lookahead_samples=lookahead, sidechain=key)
+                    else:
+                        fn = D.functional.compressor if curve == "comp" else D.functional.expander
+                        y = fn(x, SR, *ps, lookahead_samples=lookahead)
+                    y.backward(gy)
+                    torch.cuda.synchronize(dev)
+                finally:
+                    lib.dasp_debug_force_warps(0)
+                    os.environ.pop("DASP_DYN_GENERIC", None)
+                res = {"y": y, "x_grad": x.grad}
+                if key_grad:
+                    res["key_grad"] = key.grad
+                for pn, i in (("threshold", 0), ("ratio", 1), ("attack", 2), ("knee", 4), ("makeup", 5)):
+                    res[f"{pn}_grad"] = ps[i].grad
+                assert ps[3].grad is None                          # release_ms receives no gradient
+                for k, v in res.items():
+                    np.save(os.path.join(out_dir, f"{name}.{k}.npy"), v.detach().cpu().numpy())
+    print(f"dynamics: {ci} cases done", flush=True)
 
 
 def main():

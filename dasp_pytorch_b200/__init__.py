@@ -4,7 +4,8 @@ Drop-in surface: the same names the reference package exports (``dasp_pytorch/__
 path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_shaped_reverberation`` and the
 ``Processor`` classes, ``stereo_bus``, ``stereo_panner``, ``stereo_widener`` -- plus ``expander`` (stubbed upstream)
 ``convolution_reverberation`` (the reverb's convolution with a caller-supplied impulse response) and
-``sidechain_compressor`` / ``sidechain_expander`` (the detector on an external key signal).
+``sidechain_compressor`` / ``sidechain_expander`` (the detector on an external key signal) and
+``noise_shaped_impulse_response`` (the reverb's impulse response on its own, with gradients to its band parameters).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
@@ -13,6 +14,8 @@ from dasp_pytorch_b200.functional import (  # noqa: F401
     distortion,
     expander,
     gain,
+    noise_shaped_impulse_response,
+    noise_shaped_impulse_response_packed,
     noise_shaped_reverberation,
     parametric_eq,
     sidechain_compressor,

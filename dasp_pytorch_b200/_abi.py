@@ -77,6 +77,9 @@ _SIGNATURES = {
     "dasp_reverb_fwd": (c_int, [P, I64, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, c_float, P]),
     "dasp_reverb_bwd": (c_int, [P, P, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_reverb_filterbank": (c_int, [I64, c_double, ctypes.POINTER(c_float)]),
+    "dasp_nsir_geometry": (c_int, [I64, I64, I64, I64, ctypes.POINTER(ReverbGeom)]),
+    "dasp_nsir_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, c_float, P]),
+    "dasp_nsir_bwd": (c_int, [P, P, P, P, P, I64, I64, I64, I64, I64, I64, P]),
     "dasp_conv_geometry": (c_int, [I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
     "dasp_conv_fwd": (c_int, [P, I64, P, I64, I64, P, P, P, P, P, I64, I64, I64, I64, P]),
     "dasp_conv_bwd": (c_int, [P, P, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, P]),

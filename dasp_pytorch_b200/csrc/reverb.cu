@@ -37,6 +37,11 @@
 // true-stereo IR (ir_chs 4) is two partition sets per IR (ConvGeom::sets), multiplied by the TS variants of the MAC
 // kernels.
 //
+// noise_shaped_impulse_response (dasp_nsir_*) is the IR synthesis without the convolution: every synthesis variant takes
+// its output sink as a template parameter (PartitionSink: the convolution's partition slots; PlanarSink: the caller's
+// (bs, 2, L) rows), with the geometry of the reverb at n = L.  Its backward packs the planar dL/dIR with ir_pack_kernel
+// and runs the reverb's band contraction (ir_grad_pp_kernel / ir_grad_pairs_kernel, reverb_param_grad_kernel).
+//
 // Steps that several kernels share are written once: FftSmem (the shared-memory layout of the FFT kernels and their
 // double-buffered bulk-copy input), fft8192_in_smem (the four passes), shape_band / store_ir_taps (the epilogue of both
 // own-FFT IR syntheses, which therefore give the same bits), band_gain / band_rate (the parameter layout), ir_slot (the
@@ -48,6 +53,7 @@
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -482,13 +488,35 @@ __device__ __forceinline__ int64_t ir_slot(int64_t il, int J, Tap t) {
   return il * J * (int64_t)kNbA + ((t / kB) * kNbA + t % kB);
 }
 
-// IR[c][t] = (1/12) sum_k gain_k exp(-(10 decay_k + 1) tt(t)) f_c[k][t]  for t < leff, written as (left, right)
-// complex pairs into the partition layout of the audio convolution (first half of partition t / kB; every synthesis
-// variant writes these taps and nothing else).
+// Output sinks of the IR synthesis: where tap t (left, right) of chunk item il goes.  The reverb writes the partition
+// layout of its audio convolution; noise_shaped_impulse_response writes planar (items, 2, L) rows (ir points at the
+// chunk's first item).  Every synthesis variant takes the sink as a template parameter, so both ops run the same
+// generator and epilogue arithmetic.
+struct PartitionSink {
+  float2* Hb; int jb;
+  template <class Tap>
+  __device__ __forceinline__ void operator()(int64_t il, Tap t, float l, float r) const {
+    Hb[ir_slot(il, jb, t)] = make_float2(l, r);
+  }
+};
+struct PlanarSink {
+  float* ir; int64_t L;
+  template <class Tap>
+  __device__ __forceinline__ void operator()(int64_t il, Tap t, float l, float r) const {
+    float* row = ir + il * 2 * L;
+    row[t] = l;
+    row[L + t] = r;
+  }
+};
+
+// IR[c][t] = (1/12) sum_k gain_k exp(-(10 decay_k + 1) tt(t)) f_c[k][t]  for t < leff, handed to the sink (the reverb:
+// (left, right) complex pairs in the first half of partition t / kB; every synthesis variant writes these taps and
+// nothing else).
 // grid = (nbk, items): CTA (b, item) produces samples [b*hop, (b+1)*hop).
-__global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params /* chunk x 25 */,
-                                      float2* __restrict__ Hb, int64_t L, int64_t leff, int jb, int nbk, int nb,
-                                      int hop, int P) {
+template <class Sink>
+__device__ __forceinline__ void shape_ir_pairs(const float2* __restrict__ C, const float* __restrict__ params,
+                                               const Sink& out, int64_t L, int64_t leff, int nbk, int nb, int hop,
+                                               int P) {
   const int b = blockIdx.x;
   const int64_t il = blockIdx.y;
   __shared__ float gk[kBands], rk[kBands];
@@ -511,14 +539,24 @@ __global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float*
       al = fmaf(e, v.x, al);
       ar = fmaf(e, v.y, ar);
     }
-    Hb[ir_slot(il, jb, t)] = make_float2(al, ar);
+    out(il, t, al, ar);
   }
+}
+__global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params /* chunk x 25 */,
+                                      float2* __restrict__ Hb, int64_t L, int64_t leff, int jb, int nbk, int nb,
+                                      int hop, int P) {
+  shape_ir_pairs(C, params, PartitionSink{Hb, jb}, L, leff, nbk, nb, hop, P);
+}
+__global__ void nsir_shape_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params,
+                                        PlanarSink out, int64_t L, int64_t leff, int nbk, int nb, int hop, int P) {
+  shape_ir_pairs(C, params, out, L, leff, nbk, nb, hop, P);
 }
 
 // polyphase layout variant, threads in TIME order (coalesced IR stores; the 12 band loads of a thread are
 // issued together).  grid = (ceil(leff / 256), items)
-__global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __restrict__ params, float2* __restrict__ Hb,
-                                   int64_t L, int64_t leff, int jb, int R, int nb) {
+template <class Sink>
+__device__ __forceinline__ void shape_ir_pp(const float2* __restrict__ C, const float* __restrict__ params,
+                                            const Sink& out, int64_t L, int64_t leff, int R, int nb) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t il = blockIdx.y;
   __shared__ float gk[kBands], rk[kBands];
@@ -541,7 +579,15 @@ __global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __
     al = fmaf(e, v[k].x, al);
     ar = fmaf(e, v[k].y, ar);
   }
-  Hb[ir_slot(il, jb, t)] = make_float2(al, ar);
+  out(il, t, al, ar);
+}
+__global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __restrict__ params, float2* __restrict__ Hb,
+                                   int64_t L, int64_t leff, int jb, int R, int nb) {
+  shape_ir_pp(C, params, PartitionSink{Hb, jb}, L, leff, R, nb);
+}
+__global__ void nsir_shape_pp_kernel(const float2* __restrict__ C, const float* __restrict__ params, PlanarSink out,
+                                     int64_t L, int64_t leff, int R, int nb) {
+  shape_ir_pp(C, params, out, L, leff, R, nb);
 }
 
 // ---- the in-shared-memory FFT of fft8192.cuh as the kernels below use it ---------------------------------------
@@ -630,13 +676,16 @@ __device__ __forceinline__ void shape_band(const float (&xr)[16], const float (&
     if (fout) fout[a] = make_float2(xr[q], xi[q]);
   }
 }
-// the accumulated IR taps tau_q = R (t + 512 q) + c below leff of item il into the partition layout
-__device__ __forceinline__ void store_ir_taps(float2* Hb, int64_t il, int jb, int R, int c, int leff, int t,
+// the accumulated IR taps tau_q = R (t + 512 q) + c below leff of item il to the sink.  A planar sink stores them R
+// floats apart; the R CTAs of an item (one per class c) fill the rest of every 32-byte sector in the same kernel, so the
+// partial sectors can meet in L2 instead of costing a packed copy and an unpack pass (DESIGN.md 4.4).
+template <class Sink>
+__device__ __forceinline__ void store_ir_taps(const Sink& out, int64_t il, int R, int c, int leff, int t,
                                               const float (&accr)[16], const float (&acci)[16]) {
 #pragma unroll
   for (int q = 0; q < 16; ++q) {
     const int tau = R * (t + 512 * q) + c;
-    if (tau < leff) Hb[ir_slot(il, jb, tau)] = make_float2(accr[q], acci[q]);
+    if (tau < leff) out(il, tau, accr[q], acci[q]);
   }
 }
 
@@ -645,9 +694,10 @@ __device__ __forceinline__ void store_ir_taps(float2* Hb, int64_t il, int jb, in
 // in shared memory, and each thread accumulates  gain_k env_k(t) f_k(t) / 12  for its 16 taps in registers.  The
 // filtered noise f is written back (over the consumed spectrum block, as (left, right) pairs) only when the
 // backward needs it.  grid = (R, items): CTA (c, item) owns polyphase class c, i.e. the IR taps R a + c.
-__global__ void __launch_bounds__(kFusedThreads, 1)
-ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params,
-                  float2* __restrict__ Hb, int save_f, int L, int leff, int jb, int R) {
+template <class Sink>
+__device__ __forceinline__ void ifft_shape(float* __restrict__ Cpl, const float* __restrict__ twiddles,
+                                           const float* __restrict__ params, const Sink& out, int save_f, int L,
+                                           int leff, int R) {
   constexpr int nb = fft8k::kN;
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
@@ -681,7 +731,17 @@ ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, c
                save_f ? reinterpret_cast<float2*>(blk + k * band_stride) : nullptr, accr, acci);
     // (Y is next written by pass 2 of the following band, behind the barrier after its pass 1)
   }
-  store_ir_taps(Hb, il, jb, R, c, leff, t, accr, acci);
+  store_ir_taps(out, il, R, c, leff, t, accr, acci);
+}
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params,
+                  float2* __restrict__ Hb, int save_f, int L, int leff, int jb, int R) {
+  ifft_shape(Cpl, twiddles, params, PartitionSink{Hb, jb}, save_f, L, leff, R);
+}
+__global__ void __launch_bounds__(kFusedThreads, 1)
+nsir_ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params,
+                       PlanarSink out, int save_f, int L, int leff, int R) {
+  ifft_shape(Cpl, twiddles, params, out, save_f, L, leff, R);
 }
 
 // ---- block transforms of the audio convolution on the same in-shared-memory FFT ---------------------------
@@ -1149,11 +1209,11 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
         : "memory");
   } while (!done);
 }
-template <int R>
-__global__ void __launch_bounds__(kSynthThreads, 1)
-ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles, const float* __restrict__ params,
-                        float2* __restrict__ Hb, float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
-                        int jb, const unsigned long long* seed) {
+template <int R, class Sink>
+__device__ __forceinline__ void ir_synth_cluster(const float2* __restrict__ H1, const float* __restrict__ twiddles,
+                                                 const float* __restrict__ params, const Sink& out,
+                                                 float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
+                                                 const unsigned long long* seed) {
   constexpr int nb = fft8k::kN, U = nb / 2 + 1, NG = kSynthGen, NT = kSynthThreads;
   constexpr int CT = R * NG, total = kBands * U;
   constexpr uint32_t kBandBytes = 2u * nb * 4u;    // one class spectrum, planar re / im
@@ -1246,12 +1306,26 @@ ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__
                    Csave ? Csave + ((il * kBands + k) * R + c) * (int64_t)nb : nullptr, accr, acci);
         // (Y is next written by pass 2 of the following band, behind the barrier after its pass 1)
       }
-      store_ir_taps(Hb, il, jb, R, (int)c, leff, t, accr, acci);
+      store_ir_taps(out, il, R, (int)c, leff, t, accr, acci);
     }
   }
   // no CTA may leave while a remote store or arrive could still target it
   cluster_arrive();
   cluster_wait();
+}
+template <int R>
+__global__ void __launch_bounds__(kSynthThreads, 1)
+ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles, const float* __restrict__ params,
+                        float2* __restrict__ Hb, float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
+                        int jb, const unsigned long long* seed) {
+  ir_synth_cluster<R>(H1, twiddles, params, PartitionSink{Hb, jb}, Csave, item0, items, L, leff, seed);
+}
+template <int R>
+__global__ void __launch_bounds__(kSynthThreads, 1)
+nsir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles,
+                          const float* __restrict__ params, PlanarSink out, float2* __restrict__ Csave, int64_t item0,
+                          int items, int L, int leff, const unsigned long long* seed) {
+  ir_synth_cluster<R>(H1, twiddles, params, out, Csave, item0, items, L, leff, seed);
 }
 
 // part[((item*nparts + blockIdx.x)*12 + k)*2 + {0,1}], nparts = gridDim.x; threads stride over time
@@ -1720,6 +1794,16 @@ __global__ void reverb_param_grad_kernel(const float* __restrict__ ir_part, cons
   gparams[(item0 + bl) * 25 + q] = (float)s;
 }
 
+// noise_shaped_impulse_response: its [items][24] parameter rows as the reverb's [items][25] rows with a mix of 1, so
+// band_gain / band_rate and reverb_param_grad_kernel read them unchanged (the factor 1 keeps every gradient's bits)
+__global__ void nsir_params_kernel(const float* __restrict__ p24, float* __restrict__ p25, int64_t items) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= items * 25) return;
+  const int64_t row = i / 25;
+  const int q = (int)(i - row * 25);
+  p25[i] = q < 24 ? p24[row * 24 + q] : 1.0f;
+}
+
 // ---- convolution_reverberation: the audio convolution above with an impulse response supplied by the caller ----------
 // Forward: ir_pack_kernel puts the caller's taps where the IR synthesis puts its own; x_fft_kernel, partition_mac_kernel
 // and ifft_mix_kernel (or the cuFFT pipeline) then run unchanged.  Backward: g_fft_kernel, the correlations and
@@ -2019,8 +2103,10 @@ int get_side_streams(SideStreams** out) {
 }
 
 int configure_fft_kernels();
-int launch_ifft_shape(float2* C, const float* tw, const float* params, float2* hs, bool save_f, int64_t items,
-                      const Geom& g, int jb, cudaStream_t st, const int* prio) {
+// generator output -> ifft_shape_kernel (or its planar-sink twin) for the items of a chunk
+template <class Sink>
+int launch_ifft_shape(float2* C, const float* tw, const float* params, const Sink& out, bool save_f, int64_t items,
+                      const Geom& g, cudaStream_t st, const int* prio) {
   int rc = configure_fft_kernels();
   if (rc != DASP_OK) return rc;
   cudaLaunchConfig_t cfg = {};
@@ -2030,20 +2116,30 @@ int launch_ifft_shape(float2* C, const float* tw, const float* params, float2* h
   cfg.dynamicSmemBytes = kFftSmemBytes;
   cfg.stream = st;
   add_priority(cfg, at, prio);
-  cudaLaunchKernelEx(&cfg, ifft_shape_kernel, reinterpret_cast<float*>(C), tw, params, hs, save_f ? 1 : 0, (int)g.L,
-                     (int)g.leff, jb, (int)g.rpp);
+  if constexpr (std::is_same<Sink, PartitionSink>::value) {
+    cudaLaunchKernelEx(&cfg, ifft_shape_kernel, reinterpret_cast<float*>(C), tw, params, out.Hb, save_f ? 1 : 0,
+                       (int)g.L, (int)g.leff, out.jb, (int)g.rpp);
+  } else {
+    cudaLaunchKernelEx(&cfg, nsir_ifft_shape_kernel, reinterpret_cast<float*>(C), tw, params, out, save_f ? 1 : 0,
+                       (int)g.L, (int)g.leff, (int)g.rpp);
+  }
   DASP_LAUNCH_OK("ifft_shape_kernel");
   return DASP_OK;
 }
 int g_last_fused = 0;                                // test hook: IR-synthesis path of the last forward chunk
-std::map<std::pair<int, int>, int> g_fused_ok;      // (device, R) -> clusters that fit, guarded by g_mu
+std::map<std::pair<int, const void*>, int> g_fused_ok;   // (device, kernel) -> clusters that fit, guarded by g_mu
 // cluster synthesis: persistent clusters of R CTAs, as many as the device co-schedules (at most one per item).
 // Returns false when the device cannot co-schedule such a cluster (then generator -> ifft_shape_kernel runs), true after
 // a launch attempt (check cudaGetLastError).
-template <int R>
-bool launch_fused(const float2* H1, const float* tw, const float* params, float2* hs, float2* Csave, int64_t item0, int64_t items,
-                  int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st, const int* prio) {
-  auto kern = ir_synth_cluster_kernel<R>;
+template <int R, class Sink>
+bool launch_fused(const float2* H1, const float* tw, const float* params, const Sink& out, float2* Csave, int64_t item0,
+                  int64_t items, int64_t L, int64_t leff, const unsigned long long* seed, cudaStream_t st,
+                  const int* prio) {
+  constexpr bool part = std::is_same<Sink, PartitionSink>::value;
+  auto kern = [] {
+    if constexpr (part) return ir_synth_cluster_kernel<R>;
+    else return nsir_synth_cluster_kernel<R>;
+  }();
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(kSynthThreads, 1, 1);
   cfg.dynamicSmemBytes = kSynthSmemBytes;
@@ -2055,7 +2151,7 @@ bool launch_fused(const float2* H1, const float* tw, const float* params, float2
   cfg.numAttrs = 1;
   int dev = 0;
   cudaGetDevice(&dev);
-  auto it = g_fused_ok.find({dev, R});
+  auto it = g_fused_ok.find({dev, (const void*)kern});
   if (it == g_fused_ok.end()) {
     int n = 0;
     cfg.gridDim = dim3(R, 1, 1);
@@ -2064,20 +2160,22 @@ bool launch_fused(const float2* H1, const float* tw, const float* params, float2
       n = 0;
       cudaGetLastError();
     }
-    it = g_fused_ok.emplace(std::make_pair(dev, R), n).first;
+    it = g_fused_ok.emplace(std::make_pair(dev, (const void*)kern), n).first;
   }
   if (it->second < 1) return false;
   const int64_t clusters = items < it->second ? items : it->second;
   cfg.gridDim = dim3(R, (unsigned)clusters, 1);
   add_priority(cfg, at, prio);
-  cudaLaunchKernelEx(&cfg, kern, H1, tw, params, hs, Csave, item0, (int)items, (int)L, (int)leff, jb, seed);
+  if constexpr (part) cudaLaunchKernelEx(&cfg, kern, H1, tw, params, out.Hb, Csave, item0, (int)items, (int)L, (int)leff, out.jb, seed);
+  else                cudaLaunchKernelEx(&cfg, kern, H1, tw, params, out, Csave, item0, (int)items, (int)L, (int)leff, seed);
   return true;
 }
-bool dispatch_fused(int R, const float2* H1, const float* tw, const float* params, float2* hs, float2* Csave, int64_t item0,
-                    int64_t items, int64_t L, int64_t leff, int jb, const unsigned long long* seed, cudaStream_t st,
-                    const int* prio) {
+template <class Sink>
+bool dispatch_fused(int R, const float2* H1, const float* tw, const float* params, const Sink& out, float2* Csave,
+                    int64_t item0, int64_t items, int64_t L, int64_t leff, const unsigned long long* seed,
+                    cudaStream_t st, const int* prio) {
   switch (R) {
-#define DASP_R(r) case r: return launch_fused<r>(H1, tw, params, hs, Csave, item0, items, L, leff, jb, seed, st, prio);
+#define DASP_R(r) case r: return launch_fused<r>(H1, tw, params, out, Csave, item0, items, L, leff, seed, st, prio);
     DASP_R(1) DASP_R(2) DASP_R(3) DASP_R(4) DASP_R(5) DASP_R(6)
 #undef DASP_R
     default: return false;
@@ -2197,6 +2295,8 @@ int configure_fft_kernels() {
   DASP_CUDA_OK(cudaGetDevice(&dev));
   if (!configured[dev]) {
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_shape_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(nsir_ifft_shape_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(x_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_mix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(g_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
@@ -2485,15 +2585,16 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     if ((synth != 0 || own_conv) && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
     bool clustered = false;
     if (synth == 2 && g.rpp <= kMaxClusterR) {
-      clustered = dispatch_fused((int)g.rpp, H1, tw, params + item0 * 25, hs, f_save ? C : nullptr, item0, items, g.L,
-                                 g.leff, J, seed, sst, prio);
+      clustered = dispatch_fused((int)g.rpp, H1, tw, params + item0 * 25, PartitionSink{hs, J}, f_save ? C : nullptr,
+                                 item0, items, g.L, g.leff, seed, sst, prio);
       if (clustered) DASP_LAUNCH_OK("ir_synth_cluster_kernel");
     }
     if (clustered) {
     } else if (synth != 0) {
       dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, sst, prio);
       DASP_LAUNCH_OK("spectral_gen_kernel");
-      if ((rc = launch_ifft_shape(C, tw, params + item0 * 25, hs, f_save != nullptr, items, g, J, sst, prio)) != DASP_OK)
+      if ((rc = launch_ifft_shape(C, tw, params + item0 * 25, PartitionSink{hs, J}, f_save != nullptr, items, g, sst,
+                                  prio)) != DASP_OK)
         return rc;
     } else if (spectral) {
       // device noise: draw the filtered spectrum directly, one inverse transform (polyphase layout)
@@ -2796,6 +2897,191 @@ int dasp_conv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_
                          int64_t chunk_items, void* stream) {
   return conv_op_bwd(true, gy, x, in_chs, ir_chs, ir_len, mix, xspec_save, irspec_save, gx, gir, gmix, workspace,
                      workspace_bytes, bs, n, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ noise_shaped_impulse_response
+// The reverb's IR synthesis with the planar sink: the geometry of the reverb at n = L (leff = L, every tap), the same
+// synthesis variants, chunk loop and Philox keys, no convolution.  L = 1 runs the kernels with a time axis of length 2,
+// whose tap 0 is 0 like torch.linspace(0, 1, 1); everything that addresses memory (the noise rows, the IR rows) uses
+// the true L.  Backward: dL/dIR is time-domain and planar, so ir_pack_kernel puts it where the reverb's inverse
+// transform leaves its dL/dIR, and the reverb's band contraction (ir_grad_pp_kernel / ir_grad_pairs_kernel) and
+// two-stage sums (reverb_param_grad_kernel) run unchanged on the 25-wide rows of nsir_params_kernel.
+namespace {
+int make_nsir_geom(int64_t bs, int64_t L, int64_t taps, int64_t chunk, Geom& g) {
+  DASP_REQUIRE(L >= 1, "impulse response: bad num_samples=%lld", (long long)L);
+  return make_geom(bs, L, L < 2 ? 2 : L, taps, chunk, g);
+}
+
+// workspace: fwd = 25-wide parameter rows, the filtered noise of a chunk when f_save is not kept, the cuFFT work area;
+// bwd = the parameter rows, their 25-wide gradients, dL/dIR in the partition layout, the band-gradient partials
+struct NsirWs { size_t p25, f, cufft, fwd_total, g25, et, part, bwd_total; Plans full, rem; };
+int64_t nsir_nparts(const Geom& g) { return g.nbk > g.nparts_pp() ? g.nbk : g.nparts_pp(); }
+int nsir_setup(const Geom& g, NsirWs& w) {
+  int rc;
+  size_t work = 0;
+  for (int64_t items : {g.bs > 0 ? g.chunk : 0, g.bs % g.chunk}) {
+    if (items == 0) continue;
+    Plans& p = items == g.chunk ? w.full : w.rem;
+    if ((rc = get_plan(2, g.nb, items * kBands * g.nbk, g.nb, g.nb, p.blk)) != DASP_OK) return rc;
+    if ((rc = get_plan(2, g.nb, items * kBands * g.rpp, g.nb, g.nb, p.pp)) != DASP_OK) return rc;
+    if (p.blk.work > work) work = p.blk.work;
+    if (p.pp.work > work) work = p.pp.work;
+  }
+  size_t o = 0;
+  w.p25 = o;  o += align256(sizeof(float) * (size_t)(g.chunk * 25));
+  w.f = o;    o += align256(sizeof(float2) * (size_t)(g.chunk * kBands * g.pair_c64()));
+  w.cufft = o; o += align256(work);
+  w.fwd_total = o;
+  o = w.p25 + align256(sizeof(float) * (size_t)(g.chunk * 25));
+  w.g25 = o;  o += align256(sizeof(float) * (size_t)(g.chunk * 25));
+  w.et = o;   o += align256(sizeof(float2) * (size_t)(g.chunk * g.jb * kNbA));
+  w.part = o; o += align256(sizeof(float) * (size_t)(g.chunk * nsir_nparts(g) * kBands * 2));
+  w.bwd_total = o;
+  return DASP_OK;
+}
+}  // namespace
+
+int dasp_nsir_geometry(int64_t bs, int64_t num_samples, int64_t taps, int64_t chunk_items, dasp_reverb_geom* out) {
+  DASP_REQUIRE(out != nullptr, "impulse response geometry: null out");
+  Geom g;
+  int rc = make_nsir_geom(bs, num_samples, taps, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  std::lock_guard<std::mutex> lk(g_mu);
+  NsirWs w{};
+  if ((rc = nsir_setup(g, w)) != DASP_OK) return rc;
+  out->nb = g.nb; out->hop = g.hop; out->nbk = g.nbk; out->leff = g.leff; out->rpp = g.rpp;
+  out->conv_block = kB; out->x_blocks = 0; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
+  out->f_floats = bs * kBands * g.pair_c64() * 2;
+  out->xspec_c64 = 0; out->irspec_c64 = 0;
+  out->fwd_workspace_bytes = (int64_t)w.fwd_total;
+  out->bwd_workspace_bytes = (int64_t)w.bwd_total;
+  return DASP_OK;
+}
+
+int dasp_nsir_fwd(const float* params, const float* noise, const uint64_t* seed_dev, float* ir_out, float* f_save,
+                  void* workspace, int64_t workspace_bytes, int64_t bs, int64_t num_samples, int64_t taps,
+                  int64_t chunk_items, float sample_rate, void* stream) {
+  Geom g;
+  int rc = make_nsir_geom(bs, num_samples, taps, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(params && ir_out && workspace, "impulse response fwd: null pointer");
+  DASP_REQUIRE(noise != nullptr || seed_dev != nullptr,
+               "impulse response fwd: device-noise mode needs seed_dev (a device pointer)");
+  const unsigned long long* seed = reinterpret_cast<const unsigned long long*>(seed_dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  const float2 *H = nullptr, *H1 = nullptr;
+  const bool spectral = (noise == nullptr) && g.rpp <= kMaxSpectralR;
+  if (spectral) { if ((rc = get_filterbank_n1(g, (double)sample_rate, st, &H1)) != DASP_OK) return rc; }
+  else          { if ((rc = get_filterbank(g, (double)sample_rate, st, &H)) != DASP_OK) return rc; }
+  NsirWs w{};
+  if ((rc = nsir_setup(g, w)) != DASP_OK) return rc;
+  if ((rc = check_workspace("impulse response fwd", w.fwd_total, workspace_bytes)) != DASP_OK) return rc;
+  unsigned char* base = (unsigned char*)workspace;
+  float* p25 = (float*)(base + w.p25);
+  const int64_t lp = num_samples + g.P;
+  const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P;
+
+  // the reverb's choice of synthesis variant (dasp_reverb_fwd), with the same test hooks and last-path values
+  int synth = 0;
+  const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
+  const bool two_kernel_hook = debug_reverb_path() == 2 && g.rpp <= kMaxHookR;
+  if (own_fft && debug_reverb_path() != 1) synth = two_kernel_hook ? 1 : 2;
+  g_last_fused = synth;
+  const float* tw = nullptr;
+  if (synth != 0 && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    const Plans& pl = (items == g.chunk) ? w.full : w.rem;
+    float2* C = f_save ? reinterpret_cast<float2*>(f_save) + item0 * kBands * g.pair_c64()
+                       : reinterpret_cast<float2*>(base + w.f);
+    const PlanarSink out{ir_out + item0 * 2 * num_samples, num_samples};
+    const dim3 gblk((unsigned)nbk, kBands, (unsigned)items);
+    nsir_params_kernel<<<(unsigned)((items * 25 + 255) / 256), 256, 0, st>>>(params + item0 * 24, p25, items);
+    DASP_LAUNCH_OK("nsir_params_kernel");
+
+    bool clustered = false;
+    if (synth == 2 && g.rpp <= kMaxClusterR) {
+      clustered = dispatch_fused((int)g.rpp, H1, tw, p25, out, f_save ? C : nullptr, item0, items, g.L, g.leff, seed,
+                                 st, nullptr);
+      if (clustered) DASP_LAUNCH_OK("nsir_synth_cluster_kernel");
+    }
+    if (clustered) {
+    } else if (synth != 0) {
+      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, st, nullptr);
+      DASP_LAUNCH_OK("spectral_gen_kernel");
+      if ((rc = launch_ifft_shape(C, tw, p25, out, f_save != nullptr, items, g, st, nullptr)) != DASP_OK) return rc;
+    } else if (spectral) {
+      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st, nullptr);
+      DASP_LAUNCH_OK("spectral_gen_kernel");
+      if ((rc = exec_c2c(pl.pp, base + w.cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
+      nsir_shape_pp_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(
+          C, p25, out, g.L, g.leff, (int)g.rpp, nb);
+      DASP_LAUNCH_OK("nsir_shape_pp_kernel");
+    } else {
+      if (noise) noise_pairs_layout_kernel<<<gblk, 256, 0, st>>>(noise, C, item0, nbk, nb, hop, lp);
+      else       noise_pairs_philox_kernel<<<gblk, 256, 0, st>>>(C, item0, nbk, nb, hop, seed);
+      DASP_LAUNCH_OK("reverb noise kernel");
+      if ((rc = exec_c2c(pl.blk, base + w.cufft, C, CUFFT_FORWARD, st)) != DASP_OK) return rc;
+      cmul_filter_pairs_kernel<<<gblk, 256, 0, st>>>(C, H, nbk, nb);
+      DASP_LAUNCH_OK("cmul_filter_pairs_kernel");
+      if ((rc = exec_c2c(pl.blk, base + w.cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
+      nsir_shape_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, p25, out, g.L, g.leff, nbk, nb,
+                                                                                   hop, P);
+      DASP_LAUNCH_OK("nsir_shape_pairs_kernel");
+    }
+  }
+  return DASP_OK;
+}
+
+int dasp_nsir_bwd(const float* gir, const float* params, const float* f_save, float* gparams, void* workspace,
+                  int64_t workspace_bytes, int64_t bs, int64_t num_samples, int64_t taps, int64_t chunk_items,
+                  int64_t device_noise, void* stream) {
+  Geom g;
+  int rc = make_nsir_geom(bs, num_samples, taps, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(gir && params && f_save && gparams && workspace, "impulse response bwd: null pointer");
+  const bool polyphase = device_noise != 0 && g.rpp <= kMaxSpectralR;   // layout the forward left in f_save
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  NsirWs w{};
+  if ((rc = nsir_setup(g, w)) != DASP_OK) return rc;
+  if ((rc = check_workspace("impulse response bwd", w.bwd_total, workspace_bytes)) != DASP_OK) return rc;
+  unsigned char* base = (unsigned char*)workspace;
+  float* p25 = (float*)(base + w.p25);
+  float* g25 = (float*)(base + w.g25);
+  float2* et = (float2*)(base + w.et);
+  float* part = (float*)(base + w.part);
+  const int J = (int)g.jb;
+  const int nparts = (int)(polyphase ? g.nparts_pp() : g.nbk);
+
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    const float2* C = reinterpret_cast<const float2*>(f_save) + item0 * kBands * g.pair_c64();
+    nsir_params_kernel<<<(unsigned)((items * 25 + 255) / 256), 256, 0, st>>>(params + item0 * 24, p25, items);
+    DASP_LAUNCH_OK("nsir_params_kernel");
+    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, 1), 256, 0, st>>>(gir, et, item0, J,
+                                                                                              num_samples, g.leff, 2);
+    DASP_LAUNCH_OK("ir_pack_kernel");
+    if (polyphase) {
+      ir_grad_pp_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(et, C, p25, part, g.L, g.leff, J,
+                                                                                 (int)g.rpp, (int)g.nb);
+    } else {
+      ir_grad_pairs_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(
+          et, C, p25, part, g.L, g.leff, J, (int)g.nbk, (int)g.nb, (int)g.hop, (int)g.P);
+    }
+    DASP_LAUNCH_OK("ir_grad kernel");
+    // mix_blocks 0: the mix column of g25 is 0 and is not copied out
+    reverb_param_grad_kernel<<<(unsigned)((items * 25 + 127) / 128), 128, 0, st>>>(part, nullptr, p25, g25, 0, items,
+                                                                                   nparts, 0);
+    DASP_LAUNCH_OK("reverb_param_grad_kernel");
+    DASP_CUDA_OK(cudaMemcpy2DAsync(gparams + item0 * 24, 24 * sizeof(float), g25, 25 * sizeof(float),
+                                   24 * sizeof(float), (size_t)items, cudaMemcpyDeviceToDevice, st));
+  }
+  return DASP_OK;
 }
 
 }  // extern "C"

@@ -34,6 +34,8 @@ __all__ = [
     "sidechain_expander",
     "noise_shaped_reverberation",
     "convolution_reverberation",
+    "noise_shaped_impulse_response",
+    "noise_shaped_impulse_response_packed",
 ]
 
 
@@ -798,6 +800,184 @@ def noise_shaped_reverberation_packed(x: torch.Tensor, sample_rate: float, param
     y = _ReverbFn.apply(xf, packed, noise, seed, sample_rate, int(num_samples), int(num_bandpass_taps),
                         reverb_chunk_items(xf.device))
     return y.to(dt)
+
+
+# --------------------------------------------------------------------------------------
+# the reverb's impulse response on its own
+# --------------------------------------------------------------------------------------
+
+
+class _NsirFn(torch.autograd.Function):
+    """params (bs, 24) -> IR (bs, 2, num_samples)."""
+
+    @staticmethod
+    def forward(ctx, params, noise, seed, sample_rate, num_samples, taps, chunk):
+        lib = _abi.lib()
+        bs = params.shape[0]
+        dev = params.device
+        ir = torch.empty(bs, 2, num_samples, dtype=torch.float32, device=dev)
+        need_bwd = ctx.needs_input_grad[0]
+        geom = _abi.ReverbGeom()
+        with torch.cuda.device(dev):
+            check(lib.dasp_nsir_geometry(bs, num_samples, taps, chunk, geom), "dasp_nsir_geometry")
+            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
+            fsave = torch.empty(geom.f_floats, dtype=torch.float32, device=dev) if need_bwd else None
+            with _timed("nsir_fwd", dev):
+                check(lib.dasp_nsir_fwd(ptr(params), ptr(noise), ptr(seed), ptr(ir), ptr(fsave), ptr(ws), ws.numel(),
+                                        bs, num_samples, taps, chunk, float(sample_rate), stream_ptr(dev)),
+                      "dasp_nsir_fwd")
+        if need_bwd:
+            ctx.save_for_backward(params, fsave)
+        ctx.cfg = (num_samples, taps, chunk, geom.bwd_workspace_bytes, 1 if noise is None else 0)
+        return ir
+
+    @staticmethod
+    def backward(ctx, gir):
+        lib = _abi.lib()
+        params, fsave = ctx.saved_tensors
+        num_samples, taps, chunk, bwd_bytes, device_noise = ctx.cfg
+        bs = params.shape[0]
+        dev = params.device
+        gir = gir.to(torch.float32).contiguous()
+        gp = torch.empty_like(params)
+        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev), _timed("nsir_bwd", dev):
+            check(lib.dasp_nsir_bwd(ptr(gir), ptr(params), ptr(fsave), ptr(gp), ptr(ws), ws.numel(), bs, num_samples,
+                                    taps, chunk, device_noise, stream_ptr(dev)), "dasp_nsir_bwd")
+        return gp, None, None, None, None, None, None
+
+
+def _nsir_checks(sample_rate, num_samples, num_bandpass_taps):
+    if int(num_bandpass_taps) != num_bandpass_taps or num_bandpass_taps < 1 or num_bandpass_taps % 2 != 1:
+        raise ValueError(f"num_bandpass_taps must be a positive odd integer, got {num_bandpass_taps}")
+    if int(num_samples) != num_samples or num_samples < 1:
+        raise ValueError(f"num_samples must be a positive integer, got {num_samples}")
+    if not float(sample_rate) / 2.0 > 18000.0:
+        raise ValueError(f"sample_rate {sample_rate} too low: the filter bank's 18 kHz high-pass needs sample_rate > 36000")
+
+
+def _nsir_device(tensors):
+    devs = {t.device for t in tensors if torch.is_tensor(t)}
+    if len(devs) > 1:
+        raise DaspError(f"noise_shaped_impulse_response: parameters on several devices {sorted(map(str, devs))}")
+    dev = next(iter(devs)) if devs else torch.device("cpu")
+    if dev.type != "cuda":
+        raise DaspError(f"noise_shaped_impulse_response: parameters are on {dev}: dasp_pytorch_b200 only runs on CUDA "
+                        "(H100) tensors and has no CPU path")
+    return dev
+
+
+def _nsir_dtype(tensors):
+    dts = [t.dtype for t in tensors if torch.is_tensor(t) and t.is_floating_point()]
+    out = dts[0] if dts else torch.float32
+    for d in dts[1:]:
+        out = torch.promote_types(out, d)
+    return out
+
+
+def _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, dt):
+    bs = packed.shape[0]
+    noise, seed = _noise_or_seed(noise, packed, bs, num_samples, num_bandpass_taps)
+    ir = _NsirFn.apply(packed, noise, seed, sample_rate, int(num_samples), int(num_bandpass_taps),
+                       reverb_chunk_items(packed.device))
+    return ir.to(dt)
+
+
+def _nsir_noise_shape(noise, bs, num_samples, num_bandpass_taps):
+    if noise is not None:
+        expect = (bs * 2, 12, num_samples + num_bandpass_taps - 1)
+        if tuple(noise.shape) != expect:
+            raise ValueError(f"noise must have shape {expect}, got {tuple(noise.shape)}")
+
+
+def noise_shaped_impulse_response(
+    sample_rate: float,
+    band0_gain: torch.Tensor,
+    band1_gain: torch.Tensor,
+    band2_gain: torch.Tensor,
+    band3_gain: torch.Tensor,
+    band4_gain: torch.Tensor,
+    band5_gain: torch.Tensor,
+    band6_gain: torch.Tensor,
+    band7_gain: torch.Tensor,
+    band8_gain: torch.Tensor,
+    band9_gain: torch.Tensor,
+    band10_gain: torch.Tensor,
+    band11_gain: torch.Tensor,
+    band0_decay: torch.Tensor,
+    band1_decay: torch.Tensor,
+    band2_decay: torch.Tensor,
+    band3_decay: torch.Tensor,
+    band4_decay: torch.Tensor,
+    band5_decay: torch.Tensor,
+    band6_decay: torch.Tensor,
+    band7_decay: torch.Tensor,
+    band8_decay: torch.Tensor,
+    band9_decay: torch.Tensor,
+    band10_decay: torch.Tensor,
+    band11_decay: torch.Tensor,
+    num_samples: int = 65536,
+    num_bandpass_taps: int = 1023,
+    *,
+    noise: Optional[torch.Tensor] = None,
+):
+    """The stereo impulse response ``noise_shaped_reverberation`` synthesises (reference ``functional.py:547-567``),
+    returned instead of applied::
+
+        IR[b, c, t] = (1/12) sum_k gain_k exp(-(10 decay_k + 1) t / (L - 1)) f[b, c, k, t],   t < L = num_samples
+
+    with f the band-filtered noise of band k (the reverb's filter bank; ``t / (L - 1)`` is ``torch.linspace(0, 1, L)``,
+    0 when ``L == 1``).  Every tap is synthesised: no audio length bounds the IR here.
+
+    Args:
+        sample_rate: must exceed 36 kHz (the filter bank's 18 kHz high-pass).
+        band*_gain, band*_decay: the first 24 parameters of ``noise_shaped_reverberation`` (no ``mix``).  Each holds
+            ``bs`` elements in any shape or one element that is broadcast; bs is the largest element count.  The
+            parameters' device must be CUDA.
+        num_samples, num_bandpass_taps: as in ``noise_shaped_reverberation`` (taps odd).
+        noise: the ``(bs*2, 12, num_samples + num_bandpass_taps - 1)`` tensor the reference draws; by default the
+            noise is drawn on the device exactly as ``noise_shaped_reverberation`` draws it (Philox keyed by one word of
+            torch's CUDA generator: ``torch.manual_seed`` reproduces, a captured graph draws fresh noise per replay).
+
+    Returns ``(bs, 2, num_samples)``, computed in fp32, in the parameters' promoted floating dtype (fp32 when none is
+    floating).  Gradients flow to all 24 parameters.  With the same seed and ``n >= num_samples``,
+    ``convolution_reverberation(x, sr, noise_shaped_impulse_response(...), mix)`` gives the bits of
+    ``noise_shaped_reverberation(x, ..., mix)``.  When a parameter requires a gradient the forward keeps the
+    band-filtered noise of every item for the backward (``f_floats`` of ``dasp_nsir_geometry``: 11 MB per item at
+    ``L = 96000`` with 1023 taps, so about 11.3 GB for 1024 items); the backward does not regenerate it.
+    """
+    _nsir_checks(sample_rate, num_samples, num_bandpass_taps)
+    plist = (
+        band0_gain, band1_gain, band2_gain, band3_gain, band4_gain, band5_gain,
+        band6_gain, band7_gain, band8_gain, band9_gain, band10_gain, band11_gain,
+        band0_decay, band1_decay, band2_decay, band3_decay, band4_decay, band5_decay,
+        band6_decay, band7_decay, band8_decay, band9_decay, band10_decay, band11_decay,
+    )
+    counts = [p.numel() if torch.is_tensor(p) else torch.as_tensor(p).numel() for p in plist]
+    bs = max(counts)
+    for i, c in enumerate(counts):
+        if c not in (1, bs):
+            raise ValueError(f"noise_shaped_impulse_response parameter {i}: expected {bs} element(s) (one per batch "
+                             f"item) or 1, got {c}")
+    _nsir_noise_shape(noise, bs, num_samples, num_bandpass_taps)
+    dev = _nsir_device(plist)
+    like = torch.empty(0, device=dev)
+    packed = torch.stack([_param(p, bs, like, f"noise_shaped_impulse_response parameter {i}", allow_broadcast=True)
+                          for i, p in enumerate(plist)], dim=1).contiguous()
+    return _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, _nsir_dtype(plist))
+
+
+def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tensor, num_samples: int = 65536,
+                                         num_bandpass_taps: int = 1023, *, noise: Optional[torch.Tensor] = None):
+    """``noise_shaped_impulse_response`` with its 24 parameters stacked as ``(bs, 24)`` (12 gains, 12 decays)."""
+    _nsir_checks(sample_rate, num_samples, num_bandpass_taps)
+    if not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != 24:
+        raise ValueError(f"params: expected a (bs, 24) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
+    _nsir_noise_shape(noise, params.shape[0], num_samples, num_bandpass_taps)
+    dev = _nsir_device([params])
+    dt = params.dtype if params.is_floating_point() else torch.float32
+    return _nsir_run(params.to(device=dev, dtype=torch.float32).contiguous(), noise, sample_rate, num_samples,
+                     num_bandpass_taps, dt)
 
 
 # --------------------------------------------------------------------------------------

@@ -213,6 +213,26 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
 /* host-only: the 12 x taps fp32 filter bank (scipy.signal.firwin restated; no GPU needed) */
 int dasp_reverb_filterbank(int64_t taps, double sample_rate, float* out);
 
+/* ---- noise_shaped_impulse_response: the reverb's IR synthesis on its own      (reference functional.py:547-567) ----
+ * params is [bs][24] = 12 band gains, 12 band decays (the reverb's first 24); ir_out is (bs, 2, num_samples):
+ *   IR[b][c][t] = (1/12) sum_k gain_k exp(-(10 decay_k + 1) tt(t)) f[b][c][k][t],  tt = torch.linspace(0, 1, L)
+ * for every t < num_samples (num_samples >= 1; tt = 0 at num_samples 1).  noise / seed_dev as in dasp_reverb_fwd; the
+ * synthesis variants, their test hooks (dasp_debug_reverb_path, dasp_debug_reverb_last_path,
+ * dasp_debug_reverb_flat_filterbank) and the Philox keys are the reverb's, with leff = num_samples.  So with the same
+ * seed word the taps are the bits the reverb convolves when n >= num_samples.
+ * The geometry is the reverb's struct: leff = num_samples, rpp and f_floats as dasp_reverb_geometry at n = num_samples
+ * (num_samples >= 2), x_blocks = xspec_c64 = irspec_c64 = 0.  f_save (geom.f_floats floats, or NULL when no backward
+ * follows) keeps the band-filtered noise for the backward.  Backward: gir is dL/dIR (bs, 2, num_samples), gparams
+ * [bs][24]; device_noise is 1 iff the forward ran with noise == NULL.  workspace: geom.fwd_workspace_bytes /
+ * geom.bwd_workspace_bytes.  A geometry query with bs = 0 needs no GPU. */
+int dasp_nsir_geometry(int64_t bs, int64_t num_samples, int64_t taps, int64_t chunk_items, dasp_reverb_geom* out);
+int dasp_nsir_fwd(const float* params, const float* noise, const uint64_t* seed_dev, float* ir_out,
+                  float* f_save /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
+                  int64_t num_samples, int64_t taps, int64_t chunk_items, float sample_rate, void* stream);
+int dasp_nsir_bwd(const float* gir, const float* params, const float* f_save, float* gparams, void* workspace,
+                  int64_t workspace_bytes, int64_t bs, int64_t num_samples, int64_t taps, int64_t chunk_items,
+                  int64_t device_noise, void* stream);
+
 /* ---- convolution_reverberation: the reverb's apply stage with a caller-supplied impulse response
  *      (reference functional.py:569-575: y = (1 - mix) x + mix (x * IR), causal, cropped to n) --------------
  * x is (bs, in_chs, n), ir is (bs, ir_chs, ir_len) with in_chs 1 or 2 and ir_chs 1, 2 or 4 (mono is used for both

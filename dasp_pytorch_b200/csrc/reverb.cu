@@ -37,10 +37,11 @@
 // true-stereo IR (ir_chs 4) is two partition sets per IR (ConvGeom::sets), multiplied by the TS variants of the MAC
 // kernels.
 //
-// noise_shaped_impulse_response (dasp_nsir_*) is the IR synthesis without the convolution: every synthesis variant takes
-// its output sink as a template parameter (PartitionSink: the convolution's partition slots; PlanarSink: the caller's
-// (bs, 2, L) rows), with the geometry of the reverb at n = L.  Its backward packs the planar dL/dIR with ir_pack_kernel
-// and runs the reverb's band contraction (ir_grad_pp_kernel / ir_grad_pairs_kernel, reverb_param_grad_kernel).
+// noise_shaped_impulse_response (dasp_nsir_*) is the IR synthesis without the convolution, with the geometry of the
+// reverb at n = L.  Every synthesis kernel is a template on its output sink (PartitionSink: the convolution's partition
+// slots; PlanarSink: the caller's (bs, 2, L) rows), and both ops run one host-side synthesis stage: choose_synth (the
+// variant and its filter bank, once per call) and synth_chunk (one chunk).  The backward of the IR op packs the planar
+// dL/dIR with ir_pack_kernel and runs the reverb's band contraction, ir_grad_chunk, and reverb_param_grad_kernel.
 //
 // Steps that several kernels share are written once: FftSmem (the shared-memory layout of the FFT kernels and their
 // double-buffered bulk-copy input), fft8192_in_smem (the four passes), shape_band / store_ir_taps (the epilogue of both
@@ -53,7 +54,6 @@
 #include <map>
 #include <mutex>
 #include <tuple>
-#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -514,9 +514,8 @@ struct PlanarSink {
 // nothing else).
 // grid = (nbk, items): CTA (b, item) produces samples [b*hop, (b+1)*hop).
 template <class Sink>
-__device__ __forceinline__ void shape_ir_pairs(const float2* __restrict__ C, const float* __restrict__ params,
-                                               const Sink& out, int64_t L, int64_t leff, int nbk, int nb, int hop,
-                                               int P) {
+__global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params /* chunk x 25 */,
+                                      Sink out, int64_t L, int64_t leff, int nbk, int nb, int hop, int P) {
   const int b = blockIdx.x;
   const int64_t il = blockIdx.y;
   __shared__ float gk[kBands], rk[kBands];
@@ -542,21 +541,12 @@ __device__ __forceinline__ void shape_ir_pairs(const float2* __restrict__ C, con
     out(il, t, al, ar);
   }
 }
-__global__ void shape_ir_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params /* chunk x 25 */,
-                                      float2* __restrict__ Hb, int64_t L, int64_t leff, int jb, int nbk, int nb,
-                                      int hop, int P) {
-  shape_ir_pairs(C, params, PartitionSink{Hb, jb}, L, leff, nbk, nb, hop, P);
-}
-__global__ void nsir_shape_pairs_kernel(const float2* __restrict__ C, const float* __restrict__ params,
-                                        PlanarSink out, int64_t L, int64_t leff, int nbk, int nb, int hop, int P) {
-  shape_ir_pairs(C, params, out, L, leff, nbk, nb, hop, P);
-}
 
 // polyphase layout variant, threads in TIME order (coalesced IR stores; the 12 band loads of a thread are
 // issued together).  grid = (ceil(leff / 256), items)
 template <class Sink>
-__device__ __forceinline__ void shape_ir_pp(const float2* __restrict__ C, const float* __restrict__ params,
-                                            const Sink& out, int64_t L, int64_t leff, int R, int nb) {
+__global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __restrict__ params, Sink out, int64_t L,
+                                   int64_t leff, int R, int nb) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t il = blockIdx.y;
   __shared__ float gk[kBands], rk[kBands];
@@ -580,14 +570,6 @@ __device__ __forceinline__ void shape_ir_pp(const float2* __restrict__ C, const 
     ar = fmaf(e, v[k].y, ar);
   }
   out(il, t, al, ar);
-}
-__global__ void shape_ir_pp_kernel(const float2* __restrict__ C, const float* __restrict__ params, float2* __restrict__ Hb,
-                                   int64_t L, int64_t leff, int jb, int R, int nb) {
-  shape_ir_pp(C, params, PartitionSink{Hb, jb}, L, leff, R, nb);
-}
-__global__ void nsir_shape_pp_kernel(const float2* __restrict__ C, const float* __restrict__ params, PlanarSink out,
-                                     int64_t L, int64_t leff, int R, int nb) {
-  shape_ir_pp(C, params, out, L, leff, R, nb);
 }
 
 // ---- the in-shared-memory FFT of fft8192.cuh as the kernels below use it ---------------------------------------
@@ -695,9 +677,9 @@ __device__ __forceinline__ void store_ir_taps(const Sink& out, int64_t il, int R
 // filtered noise f is written back (over the consumed spectrum block, as (left, right) pairs) only when the
 // backward needs it.  grid = (R, items): CTA (c, item) owns polyphase class c, i.e. the IR taps R a + c.
 template <class Sink>
-__device__ __forceinline__ void ifft_shape(float* __restrict__ Cpl, const float* __restrict__ twiddles,
-                                           const float* __restrict__ params, const Sink& out, int save_f, int L,
-                                           int leff, int R) {
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params, Sink out,
+                  int save_f, int L, int leff, int R) {
   constexpr int nb = fft8k::kN;
   extern __shared__ __align__(128) float sm[];
   FftSmem s(sm);
@@ -732,16 +714,6 @@ __device__ __forceinline__ void ifft_shape(float* __restrict__ Cpl, const float*
     // (Y is next written by pass 2 of the following band, behind the barrier after its pass 1)
   }
   store_ir_taps(out, il, R, c, leff, t, accr, acci);
-}
-__global__ void __launch_bounds__(kFusedThreads, 1)
-ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params,
-                  float2* __restrict__ Hb, int save_f, int L, int leff, int jb, int R) {
-  ifft_shape(Cpl, twiddles, params, PartitionSink{Hb, jb}, save_f, L, leff, R);
-}
-__global__ void __launch_bounds__(kFusedThreads, 1)
-nsir_ifft_shape_kernel(float* __restrict__ Cpl, const float* __restrict__ twiddles, const float* __restrict__ params,
-                       PlanarSink out, int save_f, int L, int leff, int R) {
-  ifft_shape(Cpl, twiddles, params, out, save_f, L, leff, R);
 }
 
 // ---- block transforms of the audio convolution on the same in-shared-memory FFT ---------------------------
@@ -1210,10 +1182,10 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
   } while (!done);
 }
 template <int R, class Sink>
-__device__ __forceinline__ void ir_synth_cluster(const float2* __restrict__ H1, const float* __restrict__ twiddles,
-                                                 const float* __restrict__ params, const Sink& out,
-                                                 float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
-                                                 const unsigned long long* seed) {
+__global__ void __launch_bounds__(kSynthThreads, 1)
+ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles, const float* __restrict__ params,
+                        Sink out, float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
+                        const unsigned long long* seed) {
   constexpr int nb = fft8k::kN, U = nb / 2 + 1, NG = kSynthGen, NT = kSynthThreads;
   constexpr int CT = R * NG, total = kBands * U;
   constexpr uint32_t kBandBytes = 2u * nb * 4u;    // one class spectrum, planar re / im
@@ -1312,20 +1284,6 @@ __device__ __forceinline__ void ir_synth_cluster(const float2* __restrict__ H1, 
   // no CTA may leave while a remote store or arrive could still target it
   cluster_arrive();
   cluster_wait();
-}
-template <int R>
-__global__ void __launch_bounds__(kSynthThreads, 1)
-ir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles, const float* __restrict__ params,
-                        float2* __restrict__ Hb, float2* __restrict__ Csave, int64_t item0, int items, int L, int leff,
-                        int jb, const unsigned long long* seed) {
-  ir_synth_cluster<R>(H1, twiddles, params, PartitionSink{Hb, jb}, Csave, item0, items, L, leff, seed);
-}
-template <int R>
-__global__ void __launch_bounds__(kSynthThreads, 1)
-nsir_synth_cluster_kernel(const float2* __restrict__ H1, const float* __restrict__ twiddles,
-                          const float* __restrict__ params, PlanarSink out, float2* __restrict__ Csave, int64_t item0,
-                          int items, int L, int leff, const unsigned long long* seed) {
-  ir_synth_cluster<R>(H1, twiddles, params, out, Csave, item0, items, L, leff, seed);
 }
 
 // part[((item*nparts + blockIdx.x)*12 + k)*2 + {0,1}], nparts = gridDim.x; threads stride over time
@@ -1928,53 +1886,20 @@ __global__ void conv_mix_grad_kernel(const float* __restrict__ mix_part, float* 
   gmix[item0 + il] = (float)s;
 }
 
-// device-resident band spectra H_k: 12 x nb complex (full spectrum of the real taps), scaled by 1/nb;
-// built once per (device, taps, sr, nb)
-int get_filterbank(const Geom& g, double sr, cudaStream_t st, const float2** out) {
+// Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
+// spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
+// transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
+// the nb-point grid of the overlap-save blocks, 12 x nb complex, scaled 1/nb.
+int get_filterbank(const Geom& g, double sr, bool half, cudaStream_t st, const float2** out) {
   int dev = 0;
   DASP_CUDA_OK(cudaGetDevice(&dev));
-  const bool flat = debug_flat_filterbank();        // test hook: H_k = 1 -> the blocks keep the white noise itself
-  FbKey key{dev, flat ? -g.taps : g.taps, g.nb, sr};
+  const int64_t n = half ? g.n1() : g.nb, nc = half ? g.n1c() : g.nb;
+  const bool flat = debug_flat_filterbank();        // test hook: H_k = 1 -> the filtered noise is the white noise itself
+  FbKey key{dev, flat ? -g.taps : g.taps, half ? -n : n, sr};
   auto it = g_fb.find(key);
   if (it != g_fb.end()) { *out = reinterpret_cast<const float2*>(it->second); return DASP_OK; }
   DASP_REQUIRE(sr / 2.0 > 18000.0, "sample_rate %.1f too low: the filter bank needs 18 kHz < sr/2 (signal.py:84)", sr);
-  std::vector<float> taps;
-  octave_filterbank((int)g.taps, sr, taps);
-  if (flat) {
-    taps.assign(taps.size(), 0.f);
-    for (int k = 0; k < kBands; ++k) taps[(size_t)k * g.taps] = 1.0f;      // unit impulse at lag 0
-  }
-  std::vector<float2> padded((size_t)kBands * g.nb, make_float2(0.f, 0.f));
-  const float inv = 1.0f / (float)g.nb;
-  for (int k = 0; k < kBands; ++k)
-    for (int64_t i = 0; i < g.taps; ++i) padded[(size_t)k * g.nb + i].x = taps[(size_t)k * g.taps + i] * inv;
-  cufftComplex* d_buf = nullptr;
-  void* d_work = nullptr;
-  DASP_CUDA_OK(cudaMalloc(&d_buf, sizeof(cufftComplex) * padded.size()));
-  DASP_CUDA_OK(cudaMemcpyAsync(d_buf, padded.data(), sizeof(float2) * padded.size(), cudaMemcpyHostToDevice, st));
-  PlanVal pv;
-  int rc = get_plan(2, g.nb, kBands, g.nb, g.nb, pv);
-  if (rc != DASP_OK) return rc;
-  DASP_CUDA_OK(cudaMalloc(&d_work, pv.work > 0 ? pv.work : 16));
-  if ((rc = exec_c2c(pv, d_work, d_buf, CUFFT_FORWARD, st)) != DASP_OK) return rc;
-  DASP_CUDA_OK(cudaStreamSynchronize(st));   // one-off (cache fill): host vector and temp buffers die here
-  cudaFree(d_work);
-  g_fb[key] = d_buf;
-  *out = reinterpret_cast<const float2*>(d_buf);
-  return DASP_OK;
-}
-
-// half spectrum of the taps on the n1-point grid of the spectral synthesis: 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1
-int get_filterbank_n1(const Geom& g, double sr, cudaStream_t st, const float2** out) {
-  int dev = 0;
-  DASP_CUDA_OK(cudaGetDevice(&dev));
-  const int64_t n1 = g.n1(), n1c = g.n1c();
-  const bool flat = debug_flat_filterbank();        // test hook: H_k = 1 -> f_k is the white periodic sequence itself
-  FbKey key{dev, flat ? -g.taps : g.taps, -n1, sr};
-  auto it = g_fb.find(key);
-  if (it != g_fb.end()) { *out = reinterpret_cast<const float2*>(it->second); return DASP_OK; }
-  DASP_REQUIRE(sr / 2.0 > 18000.0, "sample_rate %.1f too low: the filter bank needs 18 kHz < sr/2 (signal.py:84)", sr);
-  {
+  if (half) {
     float2 roots[17][16];
     for (int r = 0; r <= 16; ++r)
       for (int m = 0; m < 16; ++m) {
@@ -1990,26 +1915,28 @@ int get_filterbank_n1(const Geom& g, double sr, cudaStream_t st, const float2** 
     taps.assign(taps.size(), 0.f);
     for (int k = 0; k < kBands; ++k) taps[(size_t)k * g.taps] = 1.0f;      // unit impulse at lag 0
   }
-  std::vector<float> padded((size_t)kBands * n1, 0.f);
-  // 1/n1 of the inverse transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) are folded in
-  const float inv = (float)(sqrt(0.5 * (double)n1) / (double)n1);
+  const float inv = half ? (float)(sqrt(0.5 * (double)n) / (double)n) : 1.0f / (float)n;
+  const int64_t w = half ? 1 : 2;                   // floats per input sample: real (R2C) or complex (in-place C2C)
+  std::vector<float> padded((size_t)(kBands * n * w), 0.f);
   for (int k = 0; k < kBands; ++k)
-    for (int64_t i = 0; i < g.taps; ++i) padded[(size_t)k * n1 + i] = taps[(size_t)k * g.taps + i] * inv;
+    for (int64_t i = 0; i < g.taps; ++i) padded[(size_t)((k * n + i) * w)] = taps[(size_t)k * g.taps + i] * inv;
   float* d_in = nullptr;
   cufftComplex* d_out = nullptr;
   void* d_work = nullptr;
   DASP_CUDA_OK(cudaMalloc(&d_in, sizeof(float) * padded.size()));
-  DASP_CUDA_OK(cudaMalloc(&d_out, sizeof(cufftComplex) * kBands * n1c));
   DASP_CUDA_OK(cudaMemcpyAsync(d_in, padded.data(), sizeof(float) * padded.size(), cudaMemcpyHostToDevice, st));
+  if (half) DASP_CUDA_OK(cudaMalloc(&d_out, sizeof(cufftComplex) * kBands * nc));
+  else      d_out = reinterpret_cast<cufftComplex*>(d_in);
   PlanVal pv;
-  int rc = get_plan(0, n1, kBands, n1, n1c, pv);
+  int rc = get_plan(half ? 0 : 2, n, kBands, n, nc, pv);
   if (rc != DASP_OK) return rc;
   DASP_CUDA_OK(cudaMalloc(&d_work, pv.work > 0 ? pv.work : 16));
   DASP_CUFFT_OK(cufftSetStream(pv.h, st));
   DASP_CUFFT_OK(cufftSetWorkArea(pv.h, d_work));
-  DASP_CUFFT_OK(cufftExecR2C(pv.h, d_in, d_out));
-  DASP_CUDA_OK(cudaStreamSynchronize(st));   // one-off cache fill
-  cudaFree(d_in);
+  if (half) DASP_CUFFT_OK(cufftExecR2C(pv.h, d_in, d_out));
+  else      DASP_CUFFT_OK(cufftExecC2C(pv.h, d_out, d_out, CUFFT_FORWARD));
+  DASP_CUDA_OK(cudaStreamSynchronize(st));   // one-off (cache fill): host vector and temp buffers die here
+  if (half) cudaFree(d_in);
   cudaFree(d_work);
   g_fb[key] = d_out;
   *out = reinterpret_cast<const float2*>(d_out);
@@ -2051,6 +1978,10 @@ bool dispatch_spectral(int R, float2* C, const float2* H1, int64_t item0, int64_
   }
 }
 constexpr int kMaxSpectralR = 16;
+
+// the layout of the filtered noise f (f_save): polyphase (the spectral synthesis, device noise up to kMaxSpectralR) or
+// overlap-save blocks
+bool polyphase_f(const Geom& g, bool device_noise) { return device_noise && g.rpp <= kMaxSpectralR; }
 
 // twiddle tables of fft8192.cuh (fp64 on the host, once per device)
 std::map<int, float*> g_fft_tab;
@@ -2103,7 +2034,7 @@ int get_side_streams(SideStreams** out) {
 }
 
 int configure_fft_kernels();
-// generator output -> ifft_shape_kernel (or its planar-sink twin) for the items of a chunk
+// generator output -> ifft_shape_kernel for the items of a chunk
 template <class Sink>
 int launch_ifft_shape(float2* C, const float* tw, const float* params, const Sink& out, bool save_f, int64_t items,
                       const Geom& g, cudaStream_t st, const int* prio) {
@@ -2116,13 +2047,8 @@ int launch_ifft_shape(float2* C, const float* tw, const float* params, const Sin
   cfg.dynamicSmemBytes = kFftSmemBytes;
   cfg.stream = st;
   add_priority(cfg, at, prio);
-  if constexpr (std::is_same<Sink, PartitionSink>::value) {
-    cudaLaunchKernelEx(&cfg, ifft_shape_kernel, reinterpret_cast<float*>(C), tw, params, out.Hb, save_f ? 1 : 0,
-                       (int)g.L, (int)g.leff, out.jb, (int)g.rpp);
-  } else {
-    cudaLaunchKernelEx(&cfg, nsir_ifft_shape_kernel, reinterpret_cast<float*>(C), tw, params, out, save_f ? 1 : 0,
-                       (int)g.L, (int)g.leff, (int)g.rpp);
-  }
+  cudaLaunchKernelEx(&cfg, ifft_shape_kernel<Sink>, reinterpret_cast<float*>(C), tw, params, out, save_f ? 1 : 0,
+                     (int)g.L, (int)g.leff, (int)g.rpp);
   DASP_LAUNCH_OK("ifft_shape_kernel");
   return DASP_OK;
 }
@@ -2135,11 +2061,7 @@ template <int R, class Sink>
 bool launch_fused(const float2* H1, const float* tw, const float* params, const Sink& out, float2* Csave, int64_t item0,
                   int64_t items, int64_t L, int64_t leff, const unsigned long long* seed, cudaStream_t st,
                   const int* prio) {
-  constexpr bool part = std::is_same<Sink, PartitionSink>::value;
-  auto kern = [] {
-    if constexpr (part) return ir_synth_cluster_kernel<R>;
-    else return nsir_synth_cluster_kernel<R>;
-  }();
+  auto kern = ir_synth_cluster_kernel<R, Sink>;
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(kSynthThreads, 1, 1);
   cfg.dynamicSmemBytes = kSynthSmemBytes;
@@ -2166,8 +2088,7 @@ bool launch_fused(const float2* H1, const float* tw, const float* params, const 
   const int64_t clusters = items < it->second ? items : it->second;
   cfg.gridDim = dim3(R, (unsigned)clusters, 1);
   add_priority(cfg, at, prio);
-  if constexpr (part) cudaLaunchKernelEx(&cfg, kern, H1, tw, params, out.Hb, Csave, item0, (int)items, (int)L, (int)leff, out.jb, seed);
-  else                cudaLaunchKernelEx(&cfg, kern, H1, tw, params, out, Csave, item0, (int)items, (int)L, (int)leff, seed);
+  cudaLaunchKernelEx(&cfg, kern, H1, tw, params, out, Csave, item0, (int)items, (int)L, (int)leff, seed);
   return true;
 }
 template <class Sink>
@@ -2218,6 +2139,15 @@ void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs&
 // the extra regions.  With g.shared also ir1: the J partitions of the one IR (forward) and of its summed gradient.
 // Every IR plan transforms g.sets partition sets of J partitions per IR.
 struct Plans { PlanVal xi, hj, blk, pp; };
+// blk / pp for a chunk of `items`; work: raised to their largest work area
+int synth_plans(const Geom& g, int64_t items, Plans& p, size_t& work) {
+  int rc;
+  if ((rc = get_plan(2, g.nb, items * kBands * g.nbk, g.nb, g.nb, p.blk)) != DASP_OK) return rc;
+  if ((rc = get_plan(2, g.nb, items * kBands * g.rpp, g.nb, g.nb, p.pp)) != DASP_OK) return rc;
+  if (p.blk.work > work) work = p.blk.work;
+  if (p.pp.work > work) work = p.pp.work;
+  return DASP_OK;
+}
 struct Setup { Plans full, rem; PlanVal ir1; FwdWs fwd; BwdWs bwd; };
 int conv_setup(const ConvGeom& g, const Geom* synth, Setup& s) {
   int rc;
@@ -2233,12 +2163,7 @@ int conv_setup(const ConvGeom& g, const Geom* synth, Setup& s) {
     if ((rc = get_plan(2, kNbA, items * g.sets * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
     if (p.xi.work > work) work = p.xi.work;
     if (p.hj.work > work) work = p.hj.work;
-    if (synth) {
-      if ((rc = get_plan(2, synth->nb, items * kBands * synth->nbk, synth->nb, synth->nb, p.blk)) != DASP_OK) return rc;
-      if ((rc = get_plan(2, synth->nb, items * kBands * synth->rpp, synth->nb, synth->nb, p.pp)) != DASP_OK) return rc;
-      if (p.blk.work > work) work = p.blk.work;
-      if (p.pp.work > work) work = p.pp.work;
-    }
+    if (synth && (rc = synth_plans(*synth, items, p, work)) != DASP_OK) return rc;
   }
   size_t fwd_extra = 0, bwd_extra = 0;
   if (synth) {
@@ -2294,8 +2219,9 @@ int configure_fft_kernels() {
   int dev = 0;
   DASP_CUDA_OK(cudaGetDevice(&dev));
   if (!configured[dev]) {
-    DASP_CUDA_OK(cudaFuncSetAttribute(ifft_shape_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
-    DASP_CUDA_OK(cudaFuncSetAttribute(nsir_ifft_shape_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    DASP_CUDA_OK(cudaFuncSetAttribute(ifft_shape_kernel<PartitionSink>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(ifft_shape_kernel<PlanarSink>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(x_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_mix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
@@ -2461,6 +2387,96 @@ int conv_bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const
   return DASP_OK;
 }
 
+// ---- the IR synthesis of one chunk and its band contraction, for the reverb and noise_shaped_impulse_response ----
+// The variant of a forward call (every variant draws the same Philox stream; the two own-FFT ones are bit-identical):
+//   path 2 (default, device noise, nb == 8192): ir_synth_cluster_kernel for R <= kMaxClusterR, generator ->
+//     ifft_shape_kernel for larger R or when the device cannot co-schedule the cluster;
+//   path 1 (dasp_debug_reverb_path(2), R <= kMaxHookR): generator -> ifft_shape_kernel;
+//   path 0: device noise up to kMaxSpectralR (dasp_debug_reverb_path(1), and any other nb): generator -> batched cuFFT
+//     -> shape_ir_pp_kernel; the caller's noise tensor (parity mode) or a longer IR: time-domain noise in overlap-save
+//     blocks -> C2C -> cmul_filter_pairs_kernel -> inverse C2C -> shape_ir_pairs_kernel.
+struct Synth {
+  int path;
+  bool spectral;                  // polyphase_f: the filtered spectrum is drawn directly (paths 2, 1 and the first 0)
+  const float2* H;                // the filter bank of that variant: half spectrum on the n1 grid, or the blocks' spectrum
+  const float* tw;                // the FFT tables (paths 2 and 1)
+  const float* noise;             // the caller's noise rows of length lp, or null (Philox keyed by *seed)
+  const unsigned long long* seed;
+  int64_t lp;
+};
+// L: the true IR length of the noise rows (g.L is 2 for noise_shaped_impulse_response at L = 1)
+int choose_synth(const Geom& g, int64_t L, const float* noise, const unsigned long long* seed, double sr,
+                 cudaStream_t st, Synth& sy) {
+  sy = Synth{0, polyphase_f(g, noise == nullptr), nullptr, nullptr, noise, seed, L + g.P};
+  int rc = get_filterbank(g, sr, sy.spectral, st, &sy.H);
+  if (rc != DASP_OK) return rc;
+  if (sy.spectral && g.nb == fft8k::kN && g.L < (int64_t)1 << 31 && debug_reverb_path() != 1)
+    sy.path = debug_reverb_path() == 2 && g.rpp <= kMaxHookR ? 1 : 2;
+  if (sy.path != 0 && (rc = get_fft_tables(st, &sy.tw)) != DASP_OK) return rc;
+  return DASP_OK;
+}
+
+// Taps t < leff of the chunk's items to the sink (the reverb: partition slots; noise_shaped_impulse_response: planar
+// rows).  params: the chunk's 25-wide rows; C: its filtered noise, kept for the backward when keep_f; pl / cufft: the
+// cuFFT plans and work area of path 0.  st / prio: the stream and launch priority (the reverb's side stream when it
+// pipelines, which it does on paths 2 and 1 only: path 0 shares the cuFFT work area with the convolution).
+template <class Sink>
+int synth_chunk(const Geom& g, const Synth& sy, const Sink& out, const float* params, float2* C, bool keep_f,
+                const Plans& pl, void* cufft, int64_t item0, int64_t items, cudaStream_t st, const int* prio) {
+  g_last_fused = sy.path;
+  const int nbk = (int)g.nbk, nb = (int)g.nb, R = (int)g.rpp;
+  int rc;
+  if (sy.path != 0) {
+    if (sy.path == 2 && g.rpp <= kMaxClusterR &&
+        dispatch_fused(R, sy.H, sy.tw, params, out, keep_f ? C : nullptr, item0, items, g.L, g.leff, sy.seed, st, prio)) {
+      DASP_LAUNCH_OK("ir_synth_cluster_kernel");
+      return DASP_OK;
+    }
+    dispatch_spectral(R, C, sy.H, item0, items, nb, sy.seed, /*planar=*/true, st, prio);
+    DASP_LAUNCH_OK("spectral_gen_kernel");
+    return launch_ifft_shape(C, sy.tw, params, out, keep_f, items, g, st, prio);
+  }
+  if (sy.spectral) {
+    // one inverse transform of the drawn spectrum (polyphase layout)
+    dispatch_spectral(R, C, sy.H, item0, items, nb, sy.seed, /*planar=*/false, st, nullptr);
+    DASP_LAUNCH_OK("spectral_gen_kernel");
+    if ((rc = exec_c2c(pl.pp, cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
+    shape_ir_pp_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(C, params, out, g.L,
+                                                                                              g.leff, R, nb);
+    DASP_LAUNCH_OK("shape_ir_pp_kernel");
+    return DASP_OK;
+  }
+  const dim3 gblk((unsigned)nbk, kBands, (unsigned)items);
+  if (sy.noise) noise_pairs_layout_kernel<<<gblk, 256, 0, st>>>(sy.noise, C, item0, nbk, nb, (int)g.hop, sy.lp);
+  else          noise_pairs_philox_kernel<<<gblk, 256, 0, st>>>(C, item0, nbk, nb, (int)g.hop, sy.seed);
+  DASP_LAUNCH_OK("reverb noise kernel");
+  if ((rc = exec_c2c(pl.blk, cufft, C, CUFFT_FORWARD, st)) != DASP_OK) return rc;
+  cmul_filter_pairs_kernel<<<gblk, 256, 0, st>>>(C, sy.H, nbk, nb);
+  DASP_LAUNCH_OK("cmul_filter_pairs_kernel");
+  if ((rc = exec_c2c(pl.blk, cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
+  shape_ir_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, params, out, g.L, g.leff, nbk, nb,
+                                                                           (int)g.hop, (int)g.P);
+  DASP_LAUNCH_OK("shape_ir_pairs_kernel");
+  return DASP_OK;
+}
+
+// The band contraction of the backward on the chunk's dL/dIR Et (partition layout) and its filtered noise C (layout
+// polyphase_f): nparts partials of the 24 band-parameter gradients per item into part, for reverb_param_grad_kernel
+int ir_grad_chunk(const Geom& g, bool polyphase, const float2* Et, const float2* C, const float* params, float* part,
+                  int64_t items, cudaStream_t st, int& nparts) {
+  const int J = (int)g.jb, nb = (int)g.nb;
+  nparts = (int)(polyphase ? g.nparts_pp() : g.nbk);
+  if (polyphase) {
+    ir_grad_pp_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(Et, C, params, part, g.L, g.leff, J,
+                                                                              (int)g.rpp, nb);
+  } else {
+    ir_grad_pairs_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(Et, C, params, part, g.L, g.leff, J,
+                                                                                 nparts, nb, (int)g.hop, (int)g.P);
+  }
+  DASP_LAUNCH_OK("ir_grad kernel");
+  return DASP_OK;
+}
+
 }  // namespace
 
 void reverb_shutdown() {
@@ -2525,29 +2541,15 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
   const unsigned long long* seed = reinterpret_cast<const unsigned long long*>(seed_dev);
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
-  const float2 *H = nullptr, *H1 = nullptr;
-  const bool spectral = (noise == nullptr) && g.rpp <= kMaxSpectralR;
-  if (spectral) { if ((rc = get_filterbank_n1(g, (double)sample_rate, st, &H1)) != DASP_OK) return rc; }
-  else          { if ((rc = get_filterbank(g, (double)sample_rate, st, &H)) != DASP_OK) return rc; }
+  Synth sy;
+  if ((rc = choose_synth(g, g.L, noise, seed, (double)sample_rate, st, sy)) != DASP_OK) return rc;
   Setup s{};
   if ((rc = conv_setup(g, &g, s)) != DASP_OK) return rc;
   if ((rc = check_workspace("reverb fwd", s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
   const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
-  void* ws_cufft = base + w.cufft;
-  const int64_t lp = g.L + g.P;
-  const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P, I = (int)g.ib, J = (int)g.jb;
+  const int I = (int)g.ib, J = (int)g.jb;
 
-  // device-noise IR synthesis (every variant draws the same Philox stream; the two own-FFT ones are bit-identical):
-  //   default, nb == 8192: ir_synth_cluster_kernel for R <= 6, generator -> ifft_shape_kernel for 7 <= R <= 16 or
-  //     when the device cannot co-schedule the cluster (last path 2);
-  //   dasp_debug_reverb_path(2), R <= 8: generator -> ifft_shape_kernel (last path 1);
-  //   dasp_debug_reverb_path(1), and any other nb: generator -> batched cuFFT -> shape_ir_pp_kernel (last path 0).
-  int synth = 0;
-  const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
-  const bool two_kernel_hook = debug_reverb_path() == 2 && g.rpp <= kMaxHookR;
-  if (own_fft && debug_reverb_path() != 1) synth = two_kernel_hook ? 1 : 2;
-  g_last_fused = synth;
   // Pipeline: chunk k + 1's synthesis runs on a side stream while chunk k's convolution runs on st.  The synthesis holds
   // only the SMs its clusters fit on (17 clusters of 6 = 102 of 132 on an H100 SXM), the convolution fills the rest.
   // Chunk k's synthesis goes to side[k % 2] (the next chunk's clusters are queued behind the running ones and take each
@@ -2556,7 +2558,7 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
   // so nothing outlives the call, and under stream capture the fork and join are graph edges.  This needs the chunks'
   // slots disjoint: the synthesis writes only f_save / irspec_save slots (kept when a backward follows; otherwise they
   // share one workspace slot), and neither side uses the shared cuFFT work area (own-FFT synthesis and convolution).
-  const bool pipelined = synth != 0 && f_save && irspec_save && own_fft_rows(n, x, irspec_save);
+  const bool pipelined = sy.path != 0 && f_save && irspec_save && own_fft_rows(n, x, irspec_save);
   SideStreams* side = nullptr;
   if (pipelined) {
     if ((rc = get_side_streams(&side)) != DASP_OK) return rc;
@@ -2574,49 +2576,16 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
                        : reinterpret_cast<float2*>(base + w.extra);
     float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? (float2*)irspec_save + item0 * J * (int64_t)kNbA : (float2*)(base + w.hsp);
-    const dim3 gblk((unsigned)nbk, kBands, (unsigned)items);
     const bool own_conv = own_fft_rows(n, x, hs);
-
-    // ---- IR synthesis: taps t < leff land as (left, right) pairs in the first half of partition t / kB of hs ----
-    // x_fft_kernel reads nothing else of hs; the cuFFT transform of the partitions reads whole slots, so they are
-    // zero-filled first
-    if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
     const float* tw = nullptr;
-    if ((synth != 0 || own_conv) && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    bool clustered = false;
-    if (synth == 2 && g.rpp <= kMaxClusterR) {
-      clustered = dispatch_fused((int)g.rpp, H1, tw, params + item0 * 25, PartitionSink{hs, J}, f_save ? C : nullptr,
-                                 item0, items, g.L, g.leff, seed, sst, prio);
-      if (clustered) DASP_LAUNCH_OK("ir_synth_cluster_kernel");
-    }
-    if (clustered) {
-    } else if (synth != 0) {
-      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, sst, prio);
-      DASP_LAUNCH_OK("spectral_gen_kernel");
-      if ((rc = launch_ifft_shape(C, tw, params + item0 * 25, PartitionSink{hs, J}, f_save != nullptr, items, g, sst,
-                                  prio)) != DASP_OK)
-        return rc;
-    } else if (spectral) {
-      // device noise: draw the filtered spectrum directly, one inverse transform (polyphase layout)
-      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st, nullptr);
-      DASP_LAUNCH_OK("spectral_gen_kernel");
-      if ((rc = exec_c2c(pl.pp, ws_cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
-      shape_ir_pp_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(
-          C, params + item0 * 25, hs, g.L, g.leff, J, (int)g.rpp, nb);
-      DASP_LAUNCH_OK("shape_ir_pp_kernel");
-    } else {
-      // parity mode (caller's noise tensor) or very long IR: time-domain noise, overlap-save blocks
-      if (noise) noise_pairs_layout_kernel<<<gblk, 256, 0, st>>>(noise, C, item0, nbk, nb, hop, lp);
-      else       noise_pairs_philox_kernel<<<gblk, 256, 0, st>>>(C, item0, nbk, nb, hop, seed);
-      DASP_LAUNCH_OK("reverb noise kernel");
-      if ((rc = exec_c2c(pl.blk, ws_cufft, C, CUFFT_FORWARD, st)) != DASP_OK) return rc;
-      cmul_filter_pairs_kernel<<<gblk, 256, 0, st>>>(C, H, nbk, nb);
-      DASP_LAUNCH_OK("cmul_filter_pairs_kernel");
-      if ((rc = exec_c2c(pl.blk, ws_cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
-      shape_ir_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, params + item0 * 25, hs, g.L, g.leff,
-                                                                               J, nbk, nb, hop, P);
-      DASP_LAUNCH_OK("shape_ir_pairs_kernel");
-    }
+    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+
+    // IR taps t < leff land as (left, right) pairs in the first half of partition t / kB of hs.  x_fft_kernel reads
+    // nothing else of hs; the cuFFT transform of the partitions reads whole slots, so they are zero-filled first
+    if (!own_conv) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * J * kNbA, st));
+    if ((rc = synth_chunk(g, sy, PartitionSink{hs, J}, params + item0 * 25, C, f_save != nullptr, pl, base + w.cufft,
+                          item0, items, sst, prio)) != DASP_OK)
+      return rc;
     if (pipelined) {
       DASP_CUDA_OK(cudaEventRecord(side->done[k & 1], sst));
       DASP_CUDA_OK(cudaStreamWaitEvent(st, side->done[k & 1], 0));
@@ -2637,7 +2606,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
   if (rc != DASP_OK) return rc;
   DASP_REQUIRE(in_chs == 1 || in_chs == 2, "only mono/stereo signals are supported");
   if (bs == 0) return DASP_OK;
-  const bool polyphase = device_noise != 0 && g.rpp <= kMaxSpectralR;   // layout the forward left in f_save
+  const bool polyphase = polyphase_f(g, device_noise != 0);   // the layout the forward left in f_save
   DASP_REQUIRE(gy && x && params && f_save && xspec_save && irspec_save && gx && gparams && workspace,
                "reverb bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -2650,7 +2619,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
   const float2* ws_es = (const float2*)(base + w.es);
   float* ws_irpart = (float*)(base + w.extra);
   const float* ws_mixpart = (const float*)(base + w.mixpart);
-  const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P, I = (int)g.ib, J = (int)g.jb;
+  const int I = (int)g.ib, J = (int)g.jb;
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
@@ -2661,7 +2630,7 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
 
     const bool own_conv = own_fft_rows(n, gy, nullptr);
     // dL/dIR through the band parameters on the own FFT needs the polyphase f_save at nb = 8192
-    const bool own_irgrad = own_conv && polyphase && nb == fft8k::kN && g.L < (int64_t)1 << 31;
+    const bool own_irgrad = own_conv && polyphase && g.nb == fft8k::kN && g.L < (int64_t)1 << 31;
     const float* tw = nullptr;
     if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
     if ((rc = conv_bwd_chunk(g, pl, own_conv, own_irgrad ? IrGrad::kPlanar : IrGrad::kTime, tw, gy, x, (int)in_chs, xs,
@@ -2675,17 +2644,9 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
                                                                         params + item0 * 25, ws_irpart, (int)g.L,
                                                                         (int)g.leff, J, (int)g.rpp, nunits);
       DASP_LAUNCH_OK("ifft_irgrad_kernel");
-    } else {
-      if (polyphase) {
-        nparts = (int)g.nparts_pp();
-        ir_grad_pp_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(ws_es, C, params + item0 * 25, ws_irpart,
-                                                                                  g.L, g.leff, J, (int)g.rpp, nb);
-      } else {
-        nparts = nbk;
-        ir_grad_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(ws_es, C, params + item0 * 25, ws_irpart,
-                                                                                    g.L, g.leff, J, nbk, nb, hop, P);
-      }
-      DASP_LAUNCH_OK("ir_grad kernel");
+    } else if ((rc = ir_grad_chunk(g, polyphase, ws_es, C, params + item0 * 25, ws_irpart, items, st, nparts)) !=
+               DASP_OK) {
+      return rc;
     }
     reverb_param_grad_kernel<<<(unsigned)((items * 25 + 127) / 128), 128, 0, st>>>(ws_irpart, ws_mixpart, params, gparams,
                                                                                    item0, items, nparts, I);
@@ -2921,11 +2882,7 @@ int nsir_setup(const Geom& g, NsirWs& w) {
   size_t work = 0;
   for (int64_t items : {g.bs > 0 ? g.chunk : 0, g.bs % g.chunk}) {
     if (items == 0) continue;
-    Plans& p = items == g.chunk ? w.full : w.rem;
-    if ((rc = get_plan(2, g.nb, items * kBands * g.nbk, g.nb, g.nb, p.blk)) != DASP_OK) return rc;
-    if ((rc = get_plan(2, g.nb, items * kBands * g.rpp, g.nb, g.nb, p.pp)) != DASP_OK) return rc;
-    if (p.blk.work > work) work = p.blk.work;
-    if (p.pp.work > work) work = p.pp.work;
+    if ((rc = synth_plans(g, items, items == g.chunk ? w.full : w.rem, work)) != DASP_OK) return rc;
   }
   size_t o = 0;
   w.p25 = o;  o += align256(sizeof(float) * (size_t)(g.chunk * 25));
@@ -2971,67 +2928,24 @@ int dasp_nsir_fwd(const float* params, const float* noise, const uint64_t* seed_
   const unsigned long long* seed = reinterpret_cast<const unsigned long long*>(seed_dev);
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
-  const float2 *H = nullptr, *H1 = nullptr;
-  const bool spectral = (noise == nullptr) && g.rpp <= kMaxSpectralR;
-  if (spectral) { if ((rc = get_filterbank_n1(g, (double)sample_rate, st, &H1)) != DASP_OK) return rc; }
-  else          { if ((rc = get_filterbank(g, (double)sample_rate, st, &H)) != DASP_OK) return rc; }
+  Synth sy;
+  if ((rc = choose_synth(g, num_samples, noise, seed, (double)sample_rate, st, sy)) != DASP_OK) return rc;
   NsirWs w{};
   if ((rc = nsir_setup(g, w)) != DASP_OK) return rc;
   if ((rc = check_workspace("impulse response fwd", w.fwd_total, workspace_bytes)) != DASP_OK) return rc;
   unsigned char* base = (unsigned char*)workspace;
   float* p25 = (float*)(base + w.p25);
-  const int64_t lp = num_samples + g.P;
-  const int nbk = (int)g.nbk, nb = (int)g.nb, hop = (int)g.hop, P = (int)g.P;
-
-  // the reverb's choice of synthesis variant (dasp_reverb_fwd), with the same test hooks and last-path values
-  int synth = 0;
-  const bool own_fft = spectral && nb == fft8k::kN && g.L < (int64_t)1 << 31;
-  const bool two_kernel_hook = debug_reverb_path() == 2 && g.rpp <= kMaxHookR;
-  if (own_fft && debug_reverb_path() != 1) synth = two_kernel_hook ? 1 : 2;
-  g_last_fused = synth;
-  const float* tw = nullptr;
-  if (synth != 0 && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? w.full : w.rem;
     float2* C = f_save ? reinterpret_cast<float2*>(f_save) + item0 * kBands * g.pair_c64()
                        : reinterpret_cast<float2*>(base + w.f);
-    const PlanarSink out{ir_out + item0 * 2 * num_samples, num_samples};
-    const dim3 gblk((unsigned)nbk, kBands, (unsigned)items);
     nsir_params_kernel<<<(unsigned)((items * 25 + 255) / 256), 256, 0, st>>>(params + item0 * 24, p25, items);
     DASP_LAUNCH_OK("nsir_params_kernel");
-
-    bool clustered = false;
-    if (synth == 2 && g.rpp <= kMaxClusterR) {
-      clustered = dispatch_fused((int)g.rpp, H1, tw, p25, out, f_save ? C : nullptr, item0, items, g.L, g.leff, seed,
-                                 st, nullptr);
-      if (clustered) DASP_LAUNCH_OK("nsir_synth_cluster_kernel");
-    }
-    if (clustered) {
-    } else if (synth != 0) {
-      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/true, st, nullptr);
-      DASP_LAUNCH_OK("spectral_gen_kernel");
-      if ((rc = launch_ifft_shape(C, tw, p25, out, f_save != nullptr, items, g, st, nullptr)) != DASP_OK) return rc;
-    } else if (spectral) {
-      dispatch_spectral((int)g.rpp, C, H1, item0, items, nb, seed, /*planar=*/false, st, nullptr);
-      DASP_LAUNCH_OK("spectral_gen_kernel");
-      if ((rc = exec_c2c(pl.pp, base + w.cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
-      nsir_shape_pp_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items), 256, 0, st>>>(
-          C, p25, out, g.L, g.leff, (int)g.rpp, nb);
-      DASP_LAUNCH_OK("nsir_shape_pp_kernel");
-    } else {
-      if (noise) noise_pairs_layout_kernel<<<gblk, 256, 0, st>>>(noise, C, item0, nbk, nb, hop, lp);
-      else       noise_pairs_philox_kernel<<<gblk, 256, 0, st>>>(C, item0, nbk, nb, hop, seed);
-      DASP_LAUNCH_OK("reverb noise kernel");
-      if ((rc = exec_c2c(pl.blk, base + w.cufft, C, CUFFT_FORWARD, st)) != DASP_OK) return rc;
-      cmul_filter_pairs_kernel<<<gblk, 256, 0, st>>>(C, H, nbk, nb);
-      DASP_LAUNCH_OK("cmul_filter_pairs_kernel");
-      if ((rc = exec_c2c(pl.blk, base + w.cufft, C, CUFFT_INVERSE, st)) != DASP_OK) return rc;
-      nsir_shape_pairs_kernel<<<dim3((unsigned)nbk, (unsigned)items), 256, 0, st>>>(C, p25, out, g.L, g.leff, nbk, nb,
-                                                                                   hop, P);
-      DASP_LAUNCH_OK("nsir_shape_pairs_kernel");
-    }
+    if ((rc = synth_chunk(g, sy, PlanarSink{ir_out + item0 * 2 * num_samples, num_samples}, p25, C, f_save != nullptr,
+                          pl, base + w.cufft, item0, items, st, nullptr)) != DASP_OK)
+      return rc;
   }
   return DASP_OK;
 }
@@ -3044,7 +2958,7 @@ int dasp_nsir_bwd(const float* gir, const float* params, const float* f_save, fl
   if (rc != DASP_OK) return rc;
   if (bs == 0) return DASP_OK;
   DASP_REQUIRE(gir && params && f_save && gparams && workspace, "impulse response bwd: null pointer");
-  const bool polyphase = device_noise != 0 && g.rpp <= kMaxSpectralR;   // layout the forward left in f_save
+  const bool polyphase = polyphase_f(g, device_noise != 0);   // the layout the forward left in f_save
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
   NsirWs w{};
@@ -3056,7 +2970,6 @@ int dasp_nsir_bwd(const float* gir, const float* params, const float* f_save, fl
   float2* et = (float2*)(base + w.et);
   float* part = (float*)(base + w.part);
   const int J = (int)g.jb;
-  const int nparts = (int)(polyphase ? g.nparts_pp() : g.nbk);
 
   for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
@@ -3066,14 +2979,8 @@ int dasp_nsir_bwd(const float* gir, const float* params, const float* f_save, fl
     ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, 1), 256, 0, st>>>(gir, et, item0, J,
                                                                                               num_samples, g.leff, 2);
     DASP_LAUNCH_OK("ir_pack_kernel");
-    if (polyphase) {
-      ir_grad_pp_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(et, C, p25, part, g.L, g.leff, J,
-                                                                                 (int)g.rpp, (int)g.nb);
-    } else {
-      ir_grad_pairs_kernel<<<dim3((unsigned)nparts, (unsigned)items), 256, 0, st>>>(
-          et, C, p25, part, g.L, g.leff, J, (int)g.nbk, (int)g.nb, (int)g.hop, (int)g.P);
-    }
-    DASP_LAUNCH_OK("ir_grad kernel");
+    int nparts;
+    if ((rc = ir_grad_chunk(g, polyphase, et, C, p25, part, items, st, nparts)) != DASP_OK) return rc;
     // mix_blocks 0: the mix column of g25 is 0 and is not copied out
     reverb_param_grad_kernel<<<(unsigned)((items * 25 + 127) / 128), 128, 0, st>>>(part, nullptr, p25, g25, 0, items,
                                                                                    nparts, 0);

@@ -656,6 +656,13 @@ def reverb_chunk_items(device) -> int:
     return 2 * int(torch.cuda.get_device_properties(device).multi_processor_count)
 
 
+def _check_noise_shape(noise, bs, num_samples, num_bandpass_taps):
+    if noise is not None:
+        expect = (bs * 2, 12, num_samples + num_bandpass_taps - 1)
+        if tuple(noise.shape) != expect:
+            raise ValueError(f"noise must have shape {expect}, got {tuple(noise.shape)}")
+
+
 def _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps):
     """parity mode: validate the caller's noise tensor; default mode: draw the 64-bit Philox key ON THE DEVICE.
 
@@ -664,10 +671,8 @@ def _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps):
     the in-kernel generator is therefore one ``random_()`` word of torch's CUDA generator, left in device memory
     and read by the kernels when they run: no host round trip, same reproducibility, and a captured graph
     re-draws it on every replay (torch registers the generator's Philox offset with the graph)."""
+    _check_noise_shape(noise, bs, num_samples, num_bandpass_taps)
     if noise is not None:
-        expect = (bs * 2, 12, num_samples + num_bandpass_taps - 1)
-        if tuple(noise.shape) != expect:
-            raise ValueError(f"noise must have shape {expect}, got {tuple(noise.shape)}")
         return noise.to(device=xf.device, dtype=torch.float32).contiguous(), None
     return None, torch.empty(1, dtype=torch.int64, device=xf.device).random_()
 
@@ -883,13 +888,6 @@ def _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, dt):
     return ir.to(dt)
 
 
-def _nsir_noise_shape(noise, bs, num_samples, num_bandpass_taps):
-    if noise is not None:
-        expect = (bs * 2, 12, num_samples + num_bandpass_taps - 1)
-        if tuple(noise.shape) != expect:
-            raise ValueError(f"noise must have shape {expect}, got {tuple(noise.shape)}")
-
-
 def noise_shaped_impulse_response(
     sample_rate: float,
     band0_gain: torch.Tensor,
@@ -959,7 +957,7 @@ def noise_shaped_impulse_response(
         if c not in (1, bs):
             raise ValueError(f"noise_shaped_impulse_response parameter {i}: expected {bs} element(s) (one per batch "
                              f"item) or 1, got {c}")
-    _nsir_noise_shape(noise, bs, num_samples, num_bandpass_taps)
+    _check_noise_shape(noise, bs, num_samples, num_bandpass_taps)
     dev = _nsir_device(plist)
     like = torch.empty(0, device=dev)
     packed = torch.stack([_param(p, bs, like, f"noise_shaped_impulse_response parameter {i}", allow_broadcast=True)
@@ -973,7 +971,7 @@ def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tenso
     _nsir_checks(sample_rate, num_samples, num_bandpass_taps)
     if not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != 24:
         raise ValueError(f"params: expected a (bs, 24) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
-    _nsir_noise_shape(noise, params.shape[0], num_samples, num_bandpass_taps)
+    _check_noise_shape(noise, params.shape[0], num_samples, num_bandpass_taps)
     dev = _nsir_device([params])
     dt = params.dtype if params.is_floating_point() else torch.float32
     return _nsir_run(params.to(device=dev, dtype=torch.float32).contiguous(), noise, sample_rate, num_samples,

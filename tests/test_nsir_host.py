@@ -107,7 +107,7 @@ def test_nsir_geometry_rejects_bad_shapes(lib):
     assert lib.dasp_nsir_geometry(0, 100, 1023, 1, None) == -1
 
 
-def test_nsir_kernels_in_library(lib):
+def test_ir_synthesis_kernels_in_library(lib):
     from dasp_pytorch_b200 import _abi
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
@@ -116,10 +116,12 @@ def test_nsir_kernels_in_library(lib):
     entries = set(re.findall(r"STO_ENTRY\s+(\S+)", out))
     def has(pat):
         return any(re.search(pat, e) for e in entries)
-    for r in range(1, 7):
-        assert has(rf"nsir_synth_cluster_kernelILi{r}E"), r
-        assert has(rf"\dir_synth_cluster_kernelILi{r}E"), r              # the reverb's own stays
-    for name in ("nsir_ifft_shape_kernel", "nsir_shape_pp_kernel", "nsir_shape_pairs_kernel", "nsir_params_kernel",
-                 "ifft_shape_kernel", "shape_ir_pp_kernel", "shape_ir_pairs_kernel", "ir_pack_kernel",
-                 "ir_grad_pp_kernel", "ir_grad_pairs_kernel", "reverb_param_grad_kernel"):
+    # every IR-synthesis kernel in both instantiations: the reverb's partition sink and the IR op's planar sink
+    for sink in ("13PartitionSink", "10PlanarSink"):
+        for r in range(1, 7):
+            assert has(rf"\dir_synth_cluster_kernelILi{r}ENS0_{sink}EE"), (r, sink)
+        for name in ("ifft_shape_kernel", "shape_ir_pp_kernel", "shape_ir_pairs_kernel"):
+            assert has(rf"\d{name}INS0_{sink}EE"), (name, sink)
+    for name in ("nsir_params_kernel", "ir_pack_kernel", "ir_grad_pp_kernel", "ir_grad_pairs_kernel",
+                 "reverb_param_grad_kernel"):
         assert has(rf"\d{name}E"), name

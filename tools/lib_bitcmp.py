@@ -8,8 +8,12 @@ A build is chosen when the package loads it (DASP_LIB_PATH), so each library run
 what its calls computed to DIR/a/<case>.npy and DIR/b/<case>.npy; then the files are compared.  The cases reach the
 paths bench.py does not: the cuFFT pipeline and the two-kernel IR synthesis (dasp_debug_reverb_path 1 and 2), R = 9
 (two-kernel synthesis by default) and R = 17 (time-domain overlap-save), parity mode with a noise tensor, 2047 taps
-(nb = 16384: cuFFT polyphase synthesis), n % 4 != 0 (cuFFT convolution), mono input, and convolution_reverberation with
-per-item and shared impulse responses.  The dynamics cases run both curves at every warps-per-item W the library can be
+(nb = 16384: cuFFT polyphase synthesis), n % 4 != 0 (cuFFT convolution), mono input, a forward without a backward (the
+filtered noise and the spectra in the workspace), several chunks and a remainder (the forward's synthesis alternates
+between its two side streams), and convolution_reverberation with per-item and shared impulse responses.  The
+noise_shaped_impulse_response cases run the same synthesis paths with the planar sink (the cluster kernel, hooks 2 and
+1, R = 12, R = 17, parity noise, 2047 taps, L = 1, chunks, a forward without a backward) and save the IR, dL/dparams
+and the last path.  The dynamics cases run both curves at every warps-per-item W the library can be
 pinned to (dasp_debug_force_warps), at lengths where that W fits: without a key mono (the generic channel loop), stereo
 (the stereo kernels), stereo through the generic loop (DASP_DYN_GENERIC=1) and a look-ahead; with a key a mono key, a
 stereo key, a look-ahead and a key that needs no gradient.  Refactors that must keep the bits use it; it needs a CUDA
@@ -27,7 +31,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SR = 44100
 
-# name: (kind, bs, in_chs, n, L or ir_len, taps | ir_chs, debug path | shared IR, parity noise)
+# name: (kind, bs, in_chs, n, L or ir_len, taps | ir_chs, debug path | shared IR, parity noise[, options]); options:
+# "grad": False (a forward only), "chunk": items per pass (REVERB_CHUNK_ITEMS)
 CASES = {
     "reverb_cluster_R6": ("reverb", 3, 2, 48000, 96000, 1023, 0, False),
     "reverb_two_kernel_R6": ("reverb", 3, 2, 48000, 96000, 1023, 2, False),
@@ -43,6 +48,22 @@ CASES = {
     "conv_item_n_odd": ("conv", 3, 2, 48001, 30000, 2, False, False),
     "conv_shared": ("conv", 4, 2, 48000, 30000, 2, True, False),
     "conv_shared_n_odd": ("conv", 4, 1, 48003, 20000, 1, True, False),
+    "reverb_fwd_only": ("reverb", 3, 2, 48000, 96000, 1023, 0, False, {"grad": False}),
+    "reverb_chunks": ("reverb", 5, 2, 48000, 96000, 1023, 0, False, {"chunk": 2}),
+}
+
+# noise_shaped_impulse_response: name: (bs, L, taps, debug path, parity noise, options as above)
+NSIR_CASES = {
+    "nsir_cluster_R6": (3, 48000, 1023, 0, False, {}),
+    "nsir_two_kernel_R6": (3, 48000, 1023, 2, False, {}),
+    "nsir_cufft_R6": (3, 48000, 1023, 1, False, {}),
+    "nsir_R12": (2, 96000, 1023, 0, False, {}),
+    "nsir_R17": (2, 132000, 1023, 0, False, {}),
+    "nsir_parity": (2, 20000, 1023, 0, True, {}),
+    "nsir_taps2047": (2, 30000, 2047, 0, False, {}),
+    "nsir_L1": (3, 1, 1023, 0, False, {}),
+    "nsir_fwd_only": (3, 48000, 1023, 0, False, {"grad": False}),
+    "nsir_chunks": (5, 48000, 1023, 0, False, {"chunk": 2}),
 }
 
 # dynamics: name: (x channels, key channels (0: no key), look-ahead, DASP_DYN_GENERIC, key gradient); each runs for
@@ -71,26 +92,33 @@ def run_cases(out_dir):
 
     lib = _abi.lib()
     dev = torch.device("cuda:0")
+    chunk0 = D.functional.REVERB_CHUNK_ITEMS
     os.makedirs(out_dir, exist_ok=True)
-    for ci, (name, (kind, bs, in_chs, n, L, c5, c6, parity)) in enumerate(CASES.items()):
+    for ci, (name, (kind, bs, in_chs, n, L, c5, c6, parity, *opt)) in enumerate(CASES.items()):
+        opt = opt[0] if opt else {}
+        grad = opt.get("grad", True)
         g = torch.Generator().manual_seed(1000 + ci)
-        x = ((torch.rand(bs, in_chs, n, generator=g) * 2 - 1) * 0.5).to(dev).requires_grad_(True)
+        x = ((torch.rand(bs, in_chs, n, generator=g) * 2 - 1) * 0.5).to(dev).requires_grad_(grad)
         gy = (torch.rand(bs, 2, n, generator=g) * 2 - 1).to(dev)
         res = {}
         if kind == "reverb":
             taps, path = c5, c6
-            params = torch.rand(bs, 25, generator=g).to(dev).requires_grad_(True)
+            params = torch.rand(bs, 25, generator=g).to(dev).requires_grad_(grad)
             noise = torch.randn(bs * 2, 12, L + taps - 1, generator=g).to(dev) if parity else None
             torch.manual_seed(77 + ci)                 # the device-noise key is drawn from torch's CUDA generator
             lib.dasp_debug_reverb_path(path)
+            D.functional.REVERB_CHUNK_ITEMS = opt.get("chunk", chunk0)
             try:
                 y = D.functional.noise_shaped_reverberation_packed(x, SR, params, num_samples=L, num_bandpass_taps=taps,
                                                                    noise=noise)
                 res["last_path"] = np.array([lib.dasp_debug_reverb_last_path()], dtype=np.int32)
-                y.backward(gy)
+                if grad:
+                    y.backward(gy)
             finally:
                 lib.dasp_debug_reverb_path(0)
-            res["params_grad"] = params.grad
+                D.functional.REVERB_CHUNK_ITEMS = chunk0
+            if grad:
+                res["params_grad"] = params.grad
         else:
             ir_chs, shared = c5, c6
             ir = (torch.randn(1 if shared else bs, ir_chs, L, generator=g) * 0.05).to(dev).requires_grad_(True)
@@ -101,12 +129,55 @@ def run_cases(out_dir):
             res["last_path_bwd"] = np.array([lib.dasp_debug_conv_last_path(1)], dtype=np.int32)
             res["ir_grad"], res["mix_grad"] = ir.grad, mix.grad
         torch.cuda.synchronize(dev)
-        res["y"], res["x_grad"] = y, x.grad
-        for k, v in res.items():
-            a = v.detach().cpu().numpy() if torch.is_tensor(v) else v
-            np.save(os.path.join(out_dir, f"{name}.{k}.npy"), a)
-        print(f"{name}: done", flush=True)
+        res["y"] = y
+        if grad:
+            res["x_grad"] = x.grad
+        save(out_dir, name, res)
+    run_nsir_cases(out_dir)
     run_dynamics_cases(out_dir)
+
+
+def save(out_dir, name, res):
+    """one .npy per result of case `name` (tensors or numpy arrays)"""
+    import torch
+
+    for k, v in res.items():
+        a = v.detach().cpu().numpy() if torch.is_tensor(v) else v
+        np.save(os.path.join(out_dir, f"{name}.{k}.npy"), a)
+    print(f"{name}: done", flush=True)
+
+
+def run_nsir_cases(out_dir):
+    """the noise_shaped_impulse_response cases: the IR, dL/dparams and the last synthesis path of each"""
+    import torch
+
+    import dasp_pytorch_b200 as D
+    from dasp_pytorch_b200 import _abi
+
+    lib = _abi.lib()
+    dev = torch.device("cuda:0")
+    chunk0 = D.functional.REVERB_CHUNK_ITEMS
+    for ci, (name, (bs, L, taps, path, parity, opt)) in enumerate(NSIR_CASES.items()):
+        grad = opt.get("grad", True)
+        g = torch.Generator().manual_seed(3000 + ci)
+        params = torch.rand(bs, 24, generator=g).to(dev).requires_grad_(grad)
+        gir = torch.randn(bs, 2, L, generator=g).to(dev)
+        noise = torch.randn(bs * 2, 12, L + taps - 1, generator=g).to(dev) if parity else None
+        torch.manual_seed(177 + ci)
+        lib.dasp_debug_reverb_path(path)
+        D.functional.REVERB_CHUNK_ITEMS = opt.get("chunk", chunk0)
+        try:
+            ir = D.functional.noise_shaped_impulse_response_packed(SR, params, num_samples=L, num_bandpass_taps=taps,
+                                                                   noise=noise)
+            res = {"ir": ir, "last_path": np.array([lib.dasp_debug_reverb_last_path()], dtype=np.int32)}
+            if grad:
+                ir.backward(gir)
+                res["params_grad"] = params.grad
+        finally:
+            lib.dasp_debug_reverb_path(0)
+            D.functional.REVERB_CHUNK_ITEMS = chunk0
+        torch.cuda.synchronize(dev)
+        save(out_dir, name, res)
 
 
 def run_dynamics_cases(out_dir):

@@ -5,7 +5,9 @@ path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_sha
 ``Processor`` classes, ``stereo_bus``, ``stereo_panner``, ``stereo_widener`` -- plus ``expander`` (stubbed upstream)
 ``convolution_reverberation`` (the reverb's convolution with a caller-supplied impulse response) and
 ``sidechain_compressor`` / ``sidechain_expander`` (the detector on an external key signal) and
-``noise_shaped_impulse_response`` (the reverb's impulse response on its own, with gradients to its band parameters).
+``noise_shaped_impulse_response`` (the reverb's impulse response on its own, with gradients to its band parameters) and
+``parametric_eq_frequency_response`` (the EQ's complex transfer function at chosen frequencies, with gradients to its
+18 parameters).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
@@ -18,6 +20,8 @@ from dasp_pytorch_b200.functional import (  # noqa: F401
     noise_shaped_impulse_response_packed,
     noise_shaped_reverberation,
     parametric_eq,
+    parametric_eq_frequency_response,
+    parametric_eq_frequency_response_packed,
     sidechain_compressor,
     sidechain_expander,
     stereo_bus,

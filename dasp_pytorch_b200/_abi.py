@@ -73,6 +73,9 @@ _SIGNATURES = {
     "dasp_eq_bwd_workspace_floats": (I64, [I64, I64]),
     "dasp_eq_fwd": (c_int, [P, P, P, P, I64, I64, I64, c_float, P]),
     "dasp_eq_bwd": (c_int, [P, P, P, P, P, P, P, I64, I64, I64, I64, c_float, P]),
+    "dasp_eq_response_workspace_floats": (I64, [I64, I64]),
+    "dasp_eq_response_fwd": (c_int, [P, P, P, P, I64, I64, I64, c_float, P]),
+    "dasp_eq_response_bwd": (c_int, [P, P, P, P, P, I64, I64, I64, c_float, P]),
     "dasp_reverb_geometry": (c_int, [I64, I64, I64, I64, I64, ctypes.POINTER(ReverbGeom)]),
     "dasp_reverb_fwd": (c_int, [P, I64, P, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, c_float, P]),
     "dasp_reverb_bwd": (c_int, [P, P, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),

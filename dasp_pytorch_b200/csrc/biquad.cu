@@ -804,6 +804,208 @@ __global__ void eq_param_grad_kernel(const float* __restrict__ partial, const fl
   }
 }
 
+// =============================================================================== frequency response
+// H(e^{jw}) = prod_k H_k evaluated directly on a caller's frequency grid (the reference samples the same product on
+// its n_fft grid with fp32 rfft of the coefficients, signal.py:7-32).  In the sigma form (state matrix [[sg,1],[q,sg]],
+// input (be1, B2), output s1 + b0 u) a section's transfer function is
+//       H_k = b0 + N / D,   N = be1 u + B2,   D = u^2 - q,   u = e^{jw} - sg = (d - v) + j s
+// with d = 1 - sg rounded once from fp64 and v = 2 sin^2(w/2), s = sin w rounded once from fp64 per frequency: the small
+// quantities (d, v, q) are stored directly, never formed as differences of O(1) numbers, which is where the direct form
+// B(e^{-jw}) / A(e^{-jw}) loses everything for the low sections in fp32 (1 + a1 + a2 ~ 1e-5).
+//
+// Workspace (floats): [pair partials, 60 * bs * chunks when chunks > 1 (fp64)] [vs: 2 * nfreq] [coef: 30 * bs]
+// [partial: 30 * bs].  The forward needs the vs and coef tables only.
+constexpr int kRespThreads = 256;
+constexpr int kRespItems = 4;            // items per forward thread: one (v, s) load serves kRespItems bins
+constexpr int64_t kRespMinBlocks = 512;  // backward: split an item's frequencies until the grid has about this many CTAs
+constexpr int64_t kRespMinBins = 1024;   // ... but never below this many bins per CTA
+
+struct RespLayout {
+  int64_t chunks, dbl_floats, vs, coef, partial, fwd_floats, total;
+};
+__host__ __device__ inline RespLayout resp_layout(int64_t bs, int64_t nfreq) {
+  RespLayout l;
+  const int64_t by_bins = (nfreq + kRespMinBins - 1) / kRespMinBins;
+  const int64_t by_grid = bs > 0 ? (kRespMinBlocks + bs - 1) / bs : 1;
+  l.chunks = by_bins < by_grid ? by_bins : by_grid;
+  if (l.chunks < 1) l.chunks = 1;
+  l.dbl_floats = l.chunks > 1 ? 2 * 30 * bs * l.chunks : 0;
+  l.vs = l.dbl_floats;
+  l.coef = l.vs + 2 * nfreq;
+  l.partial = l.coef + 30 * bs;
+  l.fwd_floats = l.partial;
+  l.total = l.partial + 30 * bs;
+  return l;
+}
+
+// one thread per frequency: (v, s) in fp64, rounded once; one thread per (item, section): (d, q, be1, B2, b0)
+__global__ void eq_resp_prep_kernel(const double* __restrict__ freqs, const float* __restrict__ params,
+                                     float2* __restrict__ vs, float* __restrict__ coef, int64_t nfreq, int64_t bs,
+                                     float sample_rate) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx < nfreq) {
+    const double r = freqs[idx] / (double)sample_rate;          // cycles per sample; H is periodic in r
+    const double rr = r - rint(r);                              // [-1/2, 1/2]: w = 2 pi rr
+    const double h = sinpi(rr);                                 // sin(w / 2)
+    vs[idx] = make_float2((float)(2.0 * h * h), (float)sinpi(2.0 * rr));
+  }
+  if (idx < bs * kSections) {
+    const int64_t item = idx / kSections;
+    const int k = (int)(idx - item * kSections);
+    const float* pp = params + item * 18 + 3 * k;
+    const SigmaCoef sc = design_section((double)pp[0], (double)pp[1], (double)pp[2], (double)sample_rate,
+                                        section_kind(k));
+    float* c = coef + item * 30 + k * 5;
+    c[0] = (float)(1.0 - sc.c[0].v);
+    c[1] = (float)sc.c[1].v;
+    c[2] = (float)sc.c[2].v;
+    c[3] = (float)sc.c[3].v;
+    c[4] = (float)sc.c[4].v;
+  }
+}
+
+struct Cx { float r, i; };
+__device__ __forceinline__ Cx cmul(Cx a, Cx b) { return {a.r * b.r - a.i * b.i, a.r * b.i + a.i * b.r}; }
+
+// one section at one frequency: u, 1/D and N/D; H_k = b0 + N/D
+struct SecEval { Cx u, inv_d, nd; };
+__device__ __forceinline__ SecEval eval_section(const float* c, float v, float s) {
+  SecEval e;
+  e.u = {c[0] - v, s};
+  const Cx D = {e.u.r * e.u.r - s * s - c[1], 2.f * e.u.r * s};
+  const float m = __frcp_rn(D.r * D.r + D.i * D.i);
+  e.inv_d = {D.r * m, -D.i * m};
+  e.nd = cmul({c[2] * e.u.r + c[3], c[2] * s}, e.inv_d);
+  return e;
+}
+
+// forward: CTA (frequency tile, group of kRespItems items); h is (bs, nfreq) interleaved (re, im)
+__global__ void __launch_bounds__(kRespThreads) eq_resp_fwd_kernel(const float2* __restrict__ vs,
+                                                                    const float* __restrict__ coef,
+                                                                    float2* __restrict__ h, int64_t nfreq,
+                                                                    int64_t bs) {
+  __shared__ float cs[kRespItems * 30];
+  const int64_t f = (int64_t)blockIdx.x * kRespThreads + threadIdx.x;
+  const int64_t groups = (bs + kRespItems - 1) / kRespItems;
+  const float2 t = f < nfreq ? vs[f] : make_float2(0.f, 0.f);
+  for (int64_t g = blockIdx.y; g < groups; g += gridDim.y) {
+    const int64_t b0 = g * kRespItems;
+    const int nit = (int)(bs - b0 < kRespItems ? bs - b0 : kRespItems);
+    __syncthreads();                                            // the previous group's coefficients are consumed
+    for (int e = threadIdx.x; e < nit * 30; e += kRespThreads) cs[e] = coef[b0 * 30 + e];
+    __syncthreads();
+    if (f >= nfreq) continue;
+#pragma unroll
+    for (int it = 0; it < kRespItems; ++it) {
+      if (it < nit) {
+        Cx H = {1.f, 0.f};
+#pragma unroll
+        for (int k = 0; k < kSections; ++k) {
+          const float* c = cs + it * 30 + k * 5;
+          const SecEval e = eval_section(c, t.x, t.y);
+          H = cmul(H, {c[4] + e.nd.r, e.nd.i});
+        }
+        h[(b0 + it) * nfreq + f] = make_float2(H.r, H.i);
+      }
+    }
+  }
+}
+
+// backward: CTA (item, frequency chunk).  Per bin and section, with G = dL/dRe H + i dL/dIm H and P_k the product of
+// the other five sections, Re(conj(G) P_k dH_k/dc) for c = (sg, q, be1, B2, b0):
+//   dH/dsg = (2u N/D - be1) / D,  dH/dq = (N/D) / D,  dH/dbe1 = u / D,  dH/dB2 = 1 / D,  dH/db0 = 1.
+// Each thread sums its bins in fp64; the CTA then sums its threads in a fixed order.  One chunk per item writes the 30
+// sums (fp32) straight into the row eq_param_grad_kernel reads; several write fp64 pair partials for
+// eq_resp_sum_kernel.
+__global__ void __launch_bounds__(kRespThreads, 2) eq_resp_bwd_kernel(const float2* __restrict__ gh,
+                                                                    const float2* __restrict__ vs,
+                                                                    const float* __restrict__ coef,
+                                                                    float* __restrict__ partial,
+                                                                    double* __restrict__ dpart, int64_t nfreq,
+                                                                    int64_t chunks) {
+  constexpr int kWarps = kRespThreads / 32;
+  __shared__ double red[kWarps][30];
+  const int64_t item = blockIdx.x;
+  const int64_t chunk = blockIdx.y;
+  const int64_t per = (nfreq + chunks - 1) / chunks;
+  const int64_t f0 = chunk * per, f1 = (f0 + per < nfreq) ? f0 + per : nfreq;
+  __shared__ float c[30];                          // the item's sections: broadcast reads keep the registers free
+  if (threadIdx.x < 30) c[threadIdx.x] = coef[item * 30 + threadIdx.x];
+  __syncthreads();
+  double acc[30];
+#pragma unroll
+  for (int e = 0; e < 30; ++e) acc[e] = 0.0;
+  const float2* grow = gh + item * nfreq;
+
+  for (int64_t f = f0 + threadIdx.x; f < f1; f += kRespThreads) {
+    const float2 t = vs[f];
+    const float2 g = grow[f];
+    SecEval se[kSections];
+    Cx Hk[kSections];
+#pragma unroll
+    for (int k = 0; k < kSections; ++k) {
+      se[k] = eval_section(c + k * 5, t.x, t.y);
+      Hk[k] = {c[k * 5 + 4] + se[k].nd.r, se[k].nd.i};
+    }
+    // conj(G) times the product of the other sections: prefix products from the left, suffix from the right
+    Cx pre[kSections];
+    pre[0] = {g.x, -g.y};
+#pragma unroll
+    for (int k = 1; k < kSections; ++k) pre[k] = cmul(pre[k - 1], Hk[k - 1]);
+    Cx suf = {1.f, 0.f};
+#pragma unroll
+    for (int k = kSections - 1; k >= 0; --k) {
+      const Cx w = cmul(pre[k], suf);
+      const SecEval& e = se[k];
+      const float be1 = c[k * 5 + 2];
+      const Cx wd = cmul(w, e.inv_d);                         // w / D
+      const Cx two_u_nd = cmul({2.f * e.u.r, 2.f * e.u.i}, e.nd);
+      acc[k * 5 + 0] += (double)(cmul(wd, {two_u_nd.r - be1, two_u_nd.i}).r);
+      acc[k * 5 + 1] += (double)(cmul(wd, e.nd).r);
+      acc[k * 5 + 2] += (double)(cmul(wd, e.u).r);
+      acc[k * 5 + 3] += (double)wd.r;
+      acc[k * 5 + 4] += (double)w.r;
+      suf = cmul(suf, Hk[k]);
+    }
+  }
+
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int e = 0; e < 30; ++e) {
+    const double s = warp_sum(acc[e]);
+    if (lane == 0) red[warp][e] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < 30) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) s += red[w][threadIdx.x];
+    if (chunks == 1) partial[item * 30 + threadIdx.x] = (float)s;
+    else dpart[(item * chunks + chunk) * 30 + threadIdx.x] = s;
+  }
+}
+
+// the chunks of an item, added in chunk order: one thread per (item, sum)
+__global__ void eq_resp_sum_kernel(const double* __restrict__ dpart, float* __restrict__ partial, int64_t bs,
+                                   int64_t chunks) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= bs * 30) return;
+  const int64_t item = idx / 30;
+  const int e = (int)(idx - item * 30);
+  double s = 0.0;
+  for (int64_t j = 0; j < chunks; ++j) s += dpart[(item * chunks + j) * 30 + e];
+  partial[idx] = (float)s;
+}
+
+int resp_prep(const double* freqs, const float* params, const RespLayout& l, float* ws, int64_t bs, int64_t nfreq,
+              float sample_rate, cudaStream_t st) {
+  const int64_t n = nfreq > bs * kSections ? nfreq : bs * kSections;
+  eq_resp_prep_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      freqs, params, reinterpret_cast<float2*>(ws + l.vs), ws + l.coef, nfreq, bs, sample_rate);
+  DASP_LAUNCH_OK("eq_resp_prep_kernel");
+  return DASP_OK;
+}
+
 // ---- host side -----------------------------------------------------------------------------
 // experiment knobs (read once): DASP_EQ_FWD_W / DASP_EQ_BWD_W = warps per row pair, DASP_EQ_FWD_S / DASP_EQ_BWD_S =
 // load stages per warp.  0 / unset = automatic.
@@ -980,6 +1182,70 @@ int dasp_eq_bwd(const float* gy, const float* x, const float* params, const floa
   if (rc != DASP_OK) return rc;
   const int64_t tot = bs * kSections;
   eq_param_grad_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, st>>>(ws, params, gparams, bs, (int)chs, sample_rate);
+  DASP_LAUNCH_OK("eq_param_grad_kernel");
+  return DASP_OK;
+}
+
+int64_t dasp_eq_response_workspace_floats(int64_t bs, int64_t nfreq) {
+  if (bs < 0 || nfreq < 0) return 0;
+  return resp_layout(bs, nfreq).total;
+}
+
+int dasp_eq_response_fwd(const float* params, const double* freqs_hz, float* h, float* ws, int64_t ws_floats,
+                         int64_t bs, int64_t nfreq, float sample_rate, void* stream) {
+  DASP_REQUIRE(bs >= 0 && nfreq >= 0, "eq response fwd: bad shape bs=%lld nfreq=%lld", (long long)bs,
+               (long long)nfreq);
+  if (bs == 0 || nfreq == 0) return DASP_OK;
+  DASP_REQUIRE(params && freqs_hz && h, "eq response fwd: null pointer");
+  DASP_REQUIRE(sample_rate > 0.f, "eq response fwd: sample_rate must be positive");
+  const RespLayout l = resp_layout(bs, nfreq);
+  if (ws == nullptr || ws_floats < l.fwd_floats) {
+    set_error("eq response fwd: workspace needs %lld floats, got %lld", (long long)l.fwd_floats, (long long)ws_floats);
+    return DASP_ERR_WORKSPACE;
+  }
+  const int64_t ftiles = (nfreq + kRespThreads - 1) / kRespThreads;
+  DASP_REQUIRE(ftiles < (1ll << 31), "eq response fwd: too many frequencies");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = resp_prep(freqs_hz, params, l, ws, bs, nfreq, sample_rate, st);
+  if (rc != DASP_OK) return rc;
+  const int64_t groups = (bs + kRespItems - 1) / kRespItems;
+  const dim3 grid((unsigned)ftiles, (unsigned)(groups < 65535 ? groups : 65535));
+  eq_resp_fwd_kernel<<<grid, kRespThreads, 0, st>>>(reinterpret_cast<const float2*>(ws + l.vs), ws + l.coef,
+                                                    reinterpret_cast<float2*>(h), nfreq, bs);
+  DASP_LAUNCH_OK("eq_resp_fwd_kernel");
+  return DASP_OK;
+}
+
+int dasp_eq_response_bwd(const float* gh, const float* params, const double* freqs_hz, float* gparams, float* ws,
+                         int64_t ws_floats, int64_t bs, int64_t nfreq, float sample_rate, void* stream) {
+  DASP_REQUIRE(bs >= 0 && nfreq >= 0, "eq response bwd: bad shape bs=%lld nfreq=%lld", (long long)bs,
+               (long long)nfreq);
+  if (bs == 0) return DASP_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  DASP_REQUIRE(gparams != nullptr, "eq response bwd: null gparams");
+  if (nfreq == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 18 * bs, st)); return DASP_OK; }
+  DASP_REQUIRE(gh && params && freqs_hz, "eq response bwd: null pointer");
+  DASP_REQUIRE(sample_rate > 0.f, "eq response bwd: sample_rate must be positive");
+  DASP_REQUIRE(bs < (1ll << 31), "eq response bwd: too many items");
+  const RespLayout l = resp_layout(bs, nfreq);
+  if (ws == nullptr || ws_floats < l.total) {
+    set_error("eq response bwd: workspace needs %lld floats, got %lld", (long long)l.total, (long long)ws_floats);
+    return DASP_ERR_WORKSPACE;
+  }
+  int rc = resp_prep(freqs_hz, params, l, ws, bs, nfreq, sample_rate, st);
+  if (rc != DASP_OK) return rc;
+  double* dpart = reinterpret_cast<double*>(ws);
+  eq_resp_bwd_kernel<<<dim3((unsigned)bs, (unsigned)l.chunks), kRespThreads, 0, st>>>(
+      reinterpret_cast<const float2*>(gh), reinterpret_cast<const float2*>(ws + l.vs), ws + l.coef, ws + l.partial,
+      dpart, nfreq, l.chunks);
+  DASP_LAUNCH_OK("eq_resp_bwd_kernel");
+  if (l.chunks > 1) {
+    eq_resp_sum_kernel<<<(unsigned)((bs * 30 + 255) / 256), 256, 0, st>>>(dpart, ws + l.partial, bs, l.chunks);
+    DASP_LAUNCH_OK("eq_resp_sum_kernel");
+  }
+  const int64_t tot = bs * kSections;
+  eq_param_grad_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, st>>>(ws + l.partial, params, gparams, bs, 1,
+                                                                      sample_rate);
   DASP_LAUNCH_OK("eq_param_grad_kernel");
   return DASP_OK;
 }

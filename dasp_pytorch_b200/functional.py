@@ -36,6 +36,8 @@ __all__ = [
     "convolution_reverberation",
     "noise_shaped_impulse_response",
     "noise_shaped_impulse_response_packed",
+    "parametric_eq_frequency_response",
+    "parametric_eq_frequency_response_packed",
 ]
 
 
@@ -84,6 +86,26 @@ def _param(p, n_expected: int, like: torch.Tensor, name: str, allow_broadcast: b
 
 def _ws(n_floats: int, device) -> torch.Tensor:
     return torch.empty(max(int(n_floats), 1), dtype=torch.float32, device=device)
+
+
+def _params_device(tensors, what):
+    """the one CUDA device of an op's parameter tensors (plain numbers have none)"""
+    devs = {t.device for t in tensors if torch.is_tensor(t)}
+    if len(devs) > 1:
+        raise DaspError(f"{what}: parameters on several devices {sorted(map(str, devs))}")
+    dev = next(iter(devs)) if devs else torch.device("cpu")
+    if dev.type != "cuda":
+        raise DaspError(f"{what}: parameters are on {dev}: dasp_pytorch_b200 only runs on CUDA "
+                        "(H100) tensors and has no CPU path")
+    return dev
+
+
+def _promoted_dtype(tensors):
+    dts = [t.dtype for t in tensors if torch.is_tensor(t) and t.is_floating_point()]
+    out = dts[0] if dts else torch.float32
+    for d in dts[1:]:
+        out = torch.promote_types(out, d)
+    return out
 
 
 # bench.py sets this to a list to collect (stage, start_event, end_event) around every C-ABI call
@@ -634,6 +656,149 @@ def parametric_eq_packed(x: torch.Tensor, sample_rate: float, params: torch.Tens
 
 
 # --------------------------------------------------------------------------------------
+# the parametric EQ's frequency response
+# --------------------------------------------------------------------------------------
+
+
+class _EqResponseFn(torch.autograd.Function):
+    """params (bs, 18), frequencies (F,) fp64 -> H (bs, F) complex64.  Only params and the frequencies are saved; the
+    backward recomputes the sections from them."""
+
+    @staticmethod
+    def forward(ctx, params, freqs, sample_rate):
+        lib = _abi.lib()
+        bs, nf = params.shape[0], freqs.shape[0]
+        dev = params.device
+        h = torch.empty(bs, nf, 2, dtype=torch.float32, device=dev)
+        nws = lib.dasp_eq_response_workspace_floats(bs, nf)
+        with torch.cuda.device(dev):
+            ws = _ws(nws, dev)
+            with _timed("eq_response_fwd", dev):
+                check(lib.dasp_eq_response_fwd(ptr(params), ptr(freqs), ptr(h), ptr(ws), nws, bs, nf,
+                                               float(sample_rate), stream_ptr(dev)), "dasp_eq_response_fwd")
+        if ctx.needs_input_grad[0]:
+            ctx.save_for_backward(params, freqs)
+        ctx.sample_rate = float(sample_rate)
+        return torch.view_as_complex(h)
+
+    @staticmethod
+    def backward(ctx, gh):
+        lib = _abi.lib()
+        params, freqs = ctx.saved_tensors
+        bs, nf = params.shape[0], freqs.shape[0]
+        dev = params.device
+        g = torch.view_as_real(gh.to(torch.complex64).resolve_conj().contiguous()) if gh.numel() else None
+        gp = torch.empty_like(params)
+        nws = lib.dasp_eq_response_workspace_floats(bs, nf)
+        with torch.cuda.device(dev):
+            ws = _ws(nws, dev)
+            with _timed("eq_response_bwd", dev):
+                check(lib.dasp_eq_response_bwd(ptr(g), ptr(params), ptr(freqs), ptr(gp), ptr(ws), nws, bs, nf,
+                                               ctx.sample_rate, stream_ptr(dev)), "dasp_eq_response_bwd")
+        return gp, None, None
+
+
+def _eq_response_checks(sample_rate, frequencies):
+    if not float(sample_rate) > 0.0:
+        raise ValueError(f"sample_rate must be positive, got {sample_rate}")
+    if not torch.is_tensor(frequencies) or frequencies.dim() != 1:
+        raise ValueError("frequencies must be a 1-D tensor of frequencies in Hz, got "
+                         f"{tuple(frequencies.shape) if torch.is_tensor(frequencies) else type(frequencies).__name__}")
+    if frequencies.requires_grad:
+        raise ValueError("frequencies must not require a gradient: the response is differentiated with respect to the "
+                         "18 EQ parameters only")
+
+
+def _eq_response_run(packed, frequencies, sample_rate, dt):
+    dev = packed.device
+    if frequencies.device.type != "cpu" and frequencies.device != dev:
+        raise DaspError(f"frequencies are on {frequencies.device}; they must be on the CPU or on {dev}")
+    freqs = frequencies.to(device=dev, dtype=torch.float64).contiguous()
+    h = _EqResponseFn.apply(packed, freqs, sample_rate)
+    return h.to(torch.complex128) if dt == torch.float64 else h
+
+
+def parametric_eq_frequency_response(
+    sample_rate: float,
+    low_shelf_gain_db: torch.Tensor,
+    low_shelf_cutoff_freq: torch.Tensor,
+    low_shelf_q_factor: torch.Tensor,
+    band0_gain_db: torch.Tensor,
+    band0_cutoff_freq: torch.Tensor,
+    band0_q_factor: torch.Tensor,
+    band1_gain_db: torch.Tensor,
+    band1_cutoff_freq: torch.Tensor,
+    band1_q_factor: torch.Tensor,
+    band2_gain_db: torch.Tensor,
+    band2_cutoff_freq: torch.Tensor,
+    band2_q_factor: torch.Tensor,
+    band3_gain_db: torch.Tensor,
+    band3_cutoff_freq: torch.Tensor,
+    band3_q_factor: torch.Tensor,
+    high_shelf_gain_db: torch.Tensor,
+    high_shelf_cutoff_freq: torch.Tensor,
+    high_shelf_q_factor: torch.Tensor,
+    frequencies: torch.Tensor,
+):
+    """The complex frequency response of the filter ``parametric_eq`` runs, at chosen frequencies::
+
+        H[b, f] = prod_k H_k(exp(j 2 pi frequencies[f] / sample_rate))
+
+    over the six RBJ sections low shelf, band0..band3 (peaking), high shelf.  With
+    ``frequencies = torch.fft.rfftfreq(n_fft, 1 / sample_rate)`` this is the reference's
+    ``signal.fft_sosfreqz(sos, n_fft)``; at ``n_fft = 2**ceil(log2(2n - 1))`` it is the ``H`` the reference's
+    ``parametric_eq`` multiplies into the spectrum of an ``n``-sample signal.  Losses on the curve (a target magnitude
+    in dB on a log-frequency grid, a penalty on boosts) need no audio and no recursion.
+
+    Args:
+        sample_rate: positive.
+        low_shelf_gain_db ... high_shelf_q_factor: the 18 parameters of ``parametric_eq``, in its order.  Each holds
+            ``bs`` elements in any shape or one element that is broadcast; bs is the largest element count.  The
+            parameters' device must be CUDA.
+        frequencies: 1-D tensor of F >= 0 frequencies in Hz, on the CPU or on the parameters' device; converted to
+            fp64, so an fp64 ``rfftfreq`` grid is taken exactly.  Any finite value (H is periodic in sample_rate).
+            It receives no gradient and must not require one.
+
+    Returns ``(bs, F)`` complex64, or complex128 when the parameters' promoted dtype is fp64.  The coefficients are
+    designed in fp64 and H is evaluated in fp32 in the sigma form of ``parametric_eq``'s sections (DESIGN.md 4.3):
+    within about 1e-5 of fp64 at every bin, where the reference's fp32 ``rfft`` of the coefficients is off by up to
+    tens of percent near low shelves.  Gradients flow to all 18 parameters (torch's convention for complex outputs);
+    only the packed parameters and the fp64 frequencies are kept for the backward.
+    """
+    plist = (
+        low_shelf_gain_db, low_shelf_cutoff_freq, low_shelf_q_factor,
+        band0_gain_db, band0_cutoff_freq, band0_q_factor,
+        band1_gain_db, band1_cutoff_freq, band1_q_factor,
+        band2_gain_db, band2_cutoff_freq, band2_q_factor,
+        band3_gain_db, band3_cutoff_freq, band3_q_factor,
+        high_shelf_gain_db, high_shelf_cutoff_freq, high_shelf_q_factor,
+    )
+    counts = [p.numel() if torch.is_tensor(p) else torch.as_tensor(p).numel() for p in plist]
+    bs = max(counts)
+    for i, c in enumerate(counts):
+        if c not in (1, bs):
+            raise ValueError(f"parametric_eq_frequency_response parameter {i}: expected {bs} element(s) (one per batch "
+                             f"item) or 1, got {c}")
+    _eq_response_checks(sample_rate, frequencies)
+    dev = _params_device(plist, "parametric_eq_frequency_response")
+    like = torch.empty(0, device=dev)
+    packed = torch.stack([_param(p, bs, like, f"parametric_eq_frequency_response parameter {i}", allow_broadcast=True)
+                          for i, p in enumerate(plist)], dim=1).contiguous()
+    return _eq_response_run(packed, frequencies, sample_rate, _promoted_dtype(plist))
+
+
+def parametric_eq_frequency_response_packed(sample_rate: float, params: torch.Tensor, frequencies: torch.Tensor):
+    """``parametric_eq_frequency_response`` with its 18 parameters stacked as ``(bs, 18)`` in signature order
+    (physical units), as ``parametric_eq_packed`` takes them.  Used by ``modules.ParametricEQ.frequency_response``."""
+    if not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != 18:
+        raise ValueError(f"params: expected a (bs, 18) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
+    _eq_response_checks(sample_rate, frequencies)
+    dev = _params_device([params], "parametric_eq_frequency_response")
+    dt = params.dtype if params.is_floating_point() else torch.float32
+    return _eq_response_run(params.to(device=dev, dtype=torch.float32).contiguous(), frequencies, sample_rate, dt)
+
+
+# --------------------------------------------------------------------------------------
 # noise-shaped reverberation
 # --------------------------------------------------------------------------------------
 
@@ -861,25 +1026,6 @@ def _nsir_checks(sample_rate, num_samples, num_bandpass_taps):
         raise ValueError(f"sample_rate {sample_rate} too low: the filter bank's 18 kHz high-pass needs sample_rate > 36000")
 
 
-def _nsir_device(tensors):
-    devs = {t.device for t in tensors if torch.is_tensor(t)}
-    if len(devs) > 1:
-        raise DaspError(f"noise_shaped_impulse_response: parameters on several devices {sorted(map(str, devs))}")
-    dev = next(iter(devs)) if devs else torch.device("cpu")
-    if dev.type != "cuda":
-        raise DaspError(f"noise_shaped_impulse_response: parameters are on {dev}: dasp_pytorch_b200 only runs on CUDA "
-                        "(H100) tensors and has no CPU path")
-    return dev
-
-
-def _nsir_dtype(tensors):
-    dts = [t.dtype for t in tensors if torch.is_tensor(t) and t.is_floating_point()]
-    out = dts[0] if dts else torch.float32
-    for d in dts[1:]:
-        out = torch.promote_types(out, d)
-    return out
-
-
 def _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, dt):
     bs = packed.shape[0]
     noise, seed = _noise_or_seed(noise, packed, bs, num_samples, num_bandpass_taps)
@@ -958,11 +1104,11 @@ def noise_shaped_impulse_response(
             raise ValueError(f"noise_shaped_impulse_response parameter {i}: expected {bs} element(s) (one per batch "
                              f"item) or 1, got {c}")
     _check_noise_shape(noise, bs, num_samples, num_bandpass_taps)
-    dev = _nsir_device(plist)
+    dev = _params_device(plist, "noise_shaped_impulse_response")
     like = torch.empty(0, device=dev)
     packed = torch.stack([_param(p, bs, like, f"noise_shaped_impulse_response parameter {i}", allow_broadcast=True)
                           for i, p in enumerate(plist)], dim=1).contiguous()
-    return _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, _nsir_dtype(plist))
+    return _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, _promoted_dtype(plist))
 
 
 def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tensor, num_samples: int = 65536,
@@ -972,7 +1118,7 @@ def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tenso
     if not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != 24:
         raise ValueError(f"params: expected a (bs, 24) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
     _check_noise_shape(noise, params.shape[0], num_samples, num_bandpass_taps)
-    dev = _nsir_device([params])
+    dev = _params_device([params], "noise_shaped_impulse_response")
     dt = params.dtype if params.is_floating_point() else torch.float32
     return _nsir_run(params.to(device=dev, dtype=torch.float32).contiguous(), noise, sample_rate, num_samples,
                      num_bandpass_taps, dt)

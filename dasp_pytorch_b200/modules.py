@@ -118,22 +118,27 @@ class Processor:
         """process_normalized; ``fn_kw`` (keyword arguments beyond the parameters) goes to either path's call, and
         ``by_name`` (default ``process_fn``) is the function the by-name path calls"""
         if self._packed_path is not None and self.process_fn is self._packed_path[1] and param_tensor.is_cuda:
-            if param_tensor.dim() != 2 or param_tensor.shape[1] != len(self.param_ranges):
-                raise ValueError(
-                    f"Parameter tensor has {param_tensor.shape[1] if param_tensor.dim() == 2 else '?'} parameters, "
-                    f"but processor has {len(self.param_ranges)} parameters."
-                )
-            scale, offset = self._affine(param_tensor.device)
-            flag = self._flag(param_tensor.device)
-            phys = _DenormFn.apply(param_tensor, offset, scale, flag)
-            if self.strict_range_check and not torch.cuda.is_current_stream_capturing():
-                if int(flag.item()) != 0:
-                    flag.zero_()
-                    self.denormalize_param_dict(self.extract_param_dict(param_tensor))      # raises with the name
-            return self._packed_path[0](x, self.sample_rate, phys, **fn_kw)
+            return self._packed_path[0](x, self.sample_rate, self._denormalize_packed(param_tensor), **fn_kw)
         param_dict = self.extract_param_dict(param_tensor)
         denorm = self.denormalize_param_dict(param_dict, _checked=self._range_check(param_tensor))
         return (by_name or self.process_fn)(x, self.sample_rate, **denorm, **fn_kw)
+
+    def _denormalize_packed(self, param_tensor: torch.Tensor) -> torch.Tensor:
+        """(batch, P) in [0, 1] on a CUDA device -> physical units: one ``dasp_denormalize`` kernel, and outside
+        graph capture (with ``strict_range_check``) the reference's ``ValueError`` naming an out-of-range parameter"""
+        if param_tensor.dim() != 2 or param_tensor.shape[1] != len(self.param_ranges):
+            raise ValueError(
+                f"Parameter tensor has {param_tensor.shape[1] if param_tensor.dim() == 2 else '?'} parameters, "
+                f"but processor has {len(self.param_ranges)} parameters."
+            )
+        scale, offset = self._affine(param_tensor.device)
+        flag = self._flag(param_tensor.device)
+        phys = _DenormFn.apply(param_tensor, offset, scale, flag)
+        if self.strict_range_check and not torch.cuda.is_current_stream_capturing():
+            if int(flag.item()) != 0:
+                flag.zero_()
+                self.denormalize_param_dict(self.extract_param_dict(param_tensor))      # raises with the name
+        return phys
 
     def _affine(self, device):
         key = (str(device), tuple(self.param_ranges.values()))
@@ -234,6 +239,17 @@ class ParametricEQ(Processor):
             self.param_ranges[f"{sec}_gain_db"] = g
             self.param_ranges[f"{sec}_cutoff_freq"] = fr
             self.param_ranges[f"{sec}_q_factor"] = q
+
+    def frequency_response(self, param_tensor: torch.Tensor, frequencies: torch.Tensor) -> torch.Tensor:
+        """The complex response ``(batch, F)`` of the EQ that ``process_normalized(x, param_tensor)`` applies, at
+        ``frequencies`` in Hz (see ``functional.parametric_eq_frequency_response``).  ``param_tensor`` is
+        ``(batch, 18)`` in [0, 1] on a CUDA device, mapped and range-checked exactly as ``process_normalized`` does;
+        gradients flow back to it."""
+        if not torch.is_tensor(param_tensor) or not param_tensor.is_cuda:
+            raise _F.DaspError("ParametricEQ.frequency_response: param_tensor must be a CUDA tensor; "
+                               "dasp_pytorch_b200 has no CPU path")
+        phys = self._denormalize_packed(param_tensor)
+        return _F.parametric_eq_frequency_response_packed(self.sample_rate, phys, frequencies)
 
 
 class _Dynamics(Processor):

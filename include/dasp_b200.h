@@ -173,7 +173,25 @@ int dasp_eq_bwd(const float* gy, const float* x, const float* params, const floa
                 float* gparams, float* ws, int64_t ws_floats, int64_t bs, int64_t chs, int64_t n,
                 float sample_rate, void* stream);
 
-/* ---- noise_shaped_reverberation          (reference functional.py:406-577, filter bank
+/* ---- parametric_eq_frequency_response: the EQ's transfer function on a caller's frequency grid
+ *      (reference signal.fft_sosfreqz signal.py:14-32, on any grid instead of rfft bins) ----------------------------
+ * params is [bs][18] as for dasp_eq_fwd; freqs_hz is [nfreq] frequencies in Hz (any finite value: H is periodic in
+ * sample_rate).  h is (bs, nfreq) complex, interleaved (re, im):
+ *   h[b][f] = prod_k H_k(exp(j 2 pi freqs_hz[f] / sample_rate)),  the six sections dasp_eq_fwd runs,
+ * evaluated in fp32 in the sigma form of the recursion with coefficients designed in fp64.  Backward: gh is the
+ * gradient (dL/dRe h, dL/dIm h) in the same layout, gparams [bs][18] receives
+ *   dL/dtheta = sum_f Re(conj(gh[b][f]) dh[b][f]/dtheta)
+ * (per-item sums in fp64, fixed order: two backward calls give the same bits).  Both recompute what they need from
+ * params and freqs_hz; ws is dasp_eq_response_workspace_floats(bs, nfreq) floats (8-byte aligned) for either
+ * direction.  bs = 0, and a forward with nfreq = 0, return 0 without touching the device; a backward with nfreq = 0
+ * only zeroes gparams on `stream`. */
+int64_t dasp_eq_response_workspace_floats(int64_t bs, int64_t nfreq);
+int dasp_eq_response_fwd(const float* params, const double* freqs_hz, float* h, float* ws, int64_t ws_floats,
+                         int64_t bs, int64_t nfreq, float sample_rate, void* stream);
+int dasp_eq_response_bwd(const float* gh, const float* params, const double* freqs_hz, float* gparams, float* ws,
+                         int64_t ws_floats, int64_t bs, int64_t nfreq, float sample_rate, void* stream);
+
+/* ---- noise_shaped_reverberation         (reference functional.py:406-577, filter bank
  *      signal.octave_band_filterbank signal.py:42-92) --------------------------------------
  * params is [bs][25] = 12 band gains, 12 band decays, mix (signature order).  x is (bs, in_chs, n)
  * with in_chs 1 or 2; y is always (bs, 2, n) (mono is duplicated, functional.py:493-495).

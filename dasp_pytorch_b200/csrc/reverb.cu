@@ -2008,24 +2008,22 @@ int get_fft_tables(cudaStream_t st, const float** out) {
   *out = it->second;
   return DASP_OK;
 }
-// Side streams of the forward's IR synthesis (see dasp_reverb_fwd), created once per device at the greatest stream
-// priority.  fork is recorded on the caller's stream before the first synthesis, done[k % 2] after chunk k's synthesis
-// on side[k % 2].  Reusing the events across chunks and calls is safe: cudaStreamWaitEvent takes the state of the
-// event at the time of the call, and a later record does not change what an earlier wait waits for.
-struct SideStreams { cudaStream_t side[2]; cudaEvent_t fork, done[2]; int prio; };
-std::map<int, SideStreams> g_side;                  // guarded by g_mu
-int get_side_streams(SideStreams** out) {
+// Side stream of the forward's IR synthesis (see dasp_reverb_fwd), created once per device at the greatest stream
+// priority.  fork is recorded on the caller's stream before the first synthesis, done after each chunk's synthesis on
+// side.  Reusing the events across chunks and calls is safe: cudaStreamWaitEvent takes the state of the event at the
+// time of the call, and a later record does not change what an earlier wait waits for.
+struct SideStream { cudaStream_t side; cudaEvent_t fork, done; int prio; };
+std::map<int, SideStream> g_side;                   // guarded by g_mu
+int get_side_stream(SideStream** out) {
   int dev = 0;
   DASP_CUDA_OK(cudaGetDevice(&dev));
   auto it = g_side.find(dev);
   if (it == g_side.end()) {
-    SideStreams s{};
+    SideStream s{};
     int least = 0;
     DASP_CUDA_OK(cudaDeviceGetStreamPriorityRange(&least, &s.prio));
-    for (int i = 0; i < 2; ++i) {
-      DASP_CUDA_OK(cudaStreamCreateWithPriority(&s.side[i], cudaStreamNonBlocking, s.prio));
-      DASP_CUDA_OK(cudaEventCreateWithFlags(&s.done[i], cudaEventDisableTiming));
-    }
+    DASP_CUDA_OK(cudaStreamCreateWithPriority(&s.side, cudaStreamNonBlocking, s.prio));
+    DASP_CUDA_OK(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
     DASP_CUDA_OK(cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming));
     it = g_side.emplace(dev, s).first;
   }
@@ -2278,9 +2276,10 @@ int conv_shared_ir_spectra(const ConvGeom& g, const PlanVal& ir1, bool own, cons
 // both on the own FFT with the tables tw; otherwise cuFFT C2C does.  h_stride: item stride of hs in complex elements,
 // g.sets J kNbA; 0 for one IR shared by the batch, whose partitions conv_shared_ir_spectra has transformed already.
 // g.sets == 2 (a true-stereo IR): hs holds set A then set B per IR, and the product is partition_mac_kernel<TS 1>.
+// xs_ready (own only): the caller has already transformed the chunk's windows into xs.
 int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, int in_chs, float2* xs,
                    float2* hs, int64_t h_stride, const float* mix, int mix_stride, float* y, unsigned char* ws,
-                   const FwdWs& w, int64_t item0, int64_t items, cudaStream_t st) {
+                   const FwdWs& w, int64_t item0, int64_t items, cudaStream_t st, bool xs_ready = false) {
   float2* ys = (float2*)(ws + w.ys);
   const int I = (int)g.ib, J = (int)g.jb;
   const int nblk = (int)(items * I);
@@ -2289,10 +2288,13 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
     if (rc != DASP_OK) return rc;
     // one work list: the items*I audio windows, then the items*sets*J IR partitions (transformed in place in hs; the
     // zero padding of a partition depends on its index within its set, slot mod J)
-    const int nunits = (int)(items * (I + (h_stride != 0 ? g.sets * J : 0)));
-    x_fft_kernel<<<(unsigned)((nunits + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nblk,
-                                                                nunits);
-    DASP_LAUNCH_OK("x_fft_kernel");
+    const int nwin = xs_ready ? 0 : nblk;
+    const int nunits = nwin + (int)(h_stride != 0 ? items * g.sets * J : 0);
+    if (nunits > 0) {
+      x_fft_kernel<<<(unsigned)((nunits + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
+          x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nwin, nunits);
+      DASP_LAUNCH_OK("x_fft_kernel");
+    }
     if (g.sets == 2) launch_mac<false, true, 1>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
     else             launch_mac<false, true>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
@@ -2488,10 +2490,8 @@ void reverb_shutdown() {
   for (auto& kv : g_fft_tab) cudaFree(kv.second);
   g_fft_tab.clear();
   for (auto& kv : g_side) {
-    for (int i = 0; i < 2; ++i) {
-      cudaStreamDestroy(kv.second.side[i]);
-      cudaEventDestroy(kv.second.done[i]);
-    }
+    cudaStreamDestroy(kv.second.side);
+    cudaEventDestroy(kv.second.done);
     cudaEventDestroy(kv.second.fork);
   }
   g_side.clear();
@@ -2552,25 +2552,33 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
 
   // Pipeline: chunk k + 1's synthesis runs on a side stream while chunk k's convolution runs on st.  The synthesis holds
   // only the SMs its clusters fit on (17 clusters of 6 = 102 of 132 on an H100 SXM), the convolution fills the rest.
-  // Chunk k's synthesis goes to side[k % 2] (the next chunk's clusters are queued behind the running ones and take each
-  // slot as it frees), at the greatest priority so that pending clusters are dispatched before convolution CTAs, and
-  // st waits for it before chunk k's convolution; the last of these waits joins every side-stream launch back into st,
+  // Every chunk's synthesis goes to the one side stream, at the greatest priority so that its clusters are dispatched
+  // before convolution CTAs, and st waits for it before chunk k's convolution; the last of these waits joins every
+  // side-stream launch back into st,
   // so nothing outlives the call, and under stream capture the fork and join are graph edges.  This needs the chunks'
   // slots disjoint: the synthesis writes only f_save / irspec_save slots (kept when a backward follows; otherwise they
   // share one workspace slot), and neither side uses the shared cuFFT work area (own-FFT synthesis and convolution).
+  // One side stream, not one per chunk: a cluster launch queued behind a running one stays pending for the whole chunk,
+  // and while it was pending the convolution ran at about 12 of the 30 free SMs' worth of its full rate (H100 SXM; the
+  // block scheduler appears to hold SMs back for the pending cluster).  With one stream, the next chunk's clusters are
+  // launched only when the running chunk ends, and the convolution gets the free SMs (DESIGN.md §0).
   const bool pipelined = sy.path != 0 && f_save && irspec_save && own_fft_rows(n, x, irspec_save);
-  SideStreams* side = nullptr;
+  SideStream* side = nullptr;
   if (pipelined) {
-    if ((rc = get_side_streams(&side)) != DASP_OK) return rc;
+    if ((rc = get_side_stream(&side)) != DASP_OK) return rc;
     DASP_CUDA_OK(cudaEventRecord(side->fork, st));   // the seed word and the parameters are written on st
-    for (int i = 0; i < 2; ++i) DASP_CUDA_OK(cudaStreamWaitEvent(side->side[i], side->fork, 0));
+    DASP_CUDA_OK(cudaStreamWaitEvent(side->side, side->fork, 0));
   }
   const int* prio = pipelined ? &side->prio : nullptr;
+  // The audio windows do not depend on the IR: when every item has its xspec_save slot, the whole batch's windows are
+  // transformed on st right after chunk 0's synthesis is launched, so they run on the SMs its clusters leave free
+  // instead of waiting behind it.  The chunks' convolutions then transform only their IR partitions.
+  const bool windows_first = pipelined && xspec_save != nullptr;
 
   for (int64_t item0 = 0, k = 0; item0 < bs; item0 += g.chunk, ++k) {
     const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? s.full : s.rem;
-    const cudaStream_t sst = pipelined ? side->side[k & 1] : st;      // the stream of this chunk's synthesis
+    const cudaStream_t sst = pipelined ? side->side : st;      // the stream of this chunk's synthesis
     // kept for the backward when the caller passes *_save buffers, transient workspace otherwise
     float2* C = f_save ? reinterpret_cast<float2*>(f_save) + item0 * kBands * g.pair_c64()
                        : reinterpret_cast<float2*>(base + w.extra);
@@ -2586,12 +2594,19 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     if ((rc = synth_chunk(g, sy, PartitionSink{hs, J}, params + item0 * 25, C, f_save != nullptr, pl, base + w.cufft,
                           item0, items, sst, prio)) != DASP_OK)
       return rc;
+    if (windows_first && k == 0) {
+      if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
+      const int nwin = (int)(bs * I);
+      x_fft_kernel<<<(unsigned)((nwin + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
+          x, (float2*)xspec_save, nullptr, tw, 0, I, J, g.n, g.leff, (int)in_chs, nwin, nwin);
+      DASP_LAUNCH_OK("x_fft_kernel");
+    }
     if (pipelined) {
-      DASP_CUDA_OK(cudaEventRecord(side->done[k & 1], sst));
-      DASP_CUDA_OK(cudaStreamWaitEvent(st, side->done[k & 1], 0));
+      DASP_CUDA_OK(cudaEventRecord(side->done, sst));
+      DASP_CUDA_OK(cudaStreamWaitEvent(st, side->done, 0));
     }
     if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, J * (int64_t)kNbA, params + 24, 25, y, base,
-                             w, item0, items, st)) != DASP_OK)
+                             w, item0, items, st, windows_first)) != DASP_OK)
       return rc;
   }
   return DASP_OK;

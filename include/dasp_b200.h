@@ -14,10 +14,10 @@
  *   - `stream` is a cudaStream_t; all work is enqueued on it, nothing synchronises -- with ONE documented
  *     exception: the first call on a device for a new (taps, sample_rate, geometry) builds library-owned caches
  *     (cuFFT plans, filter-bank spectra, FFT twiddle tables: cudaMalloc + one cudaStreamSynchronize; for the
- *     reverb forward also two side streams at the greatest priority and three events).  Warm the shapes up once
+ *     reverb forward also a side stream at the greatest priority and two events).  Warm the shapes up once
  *     before capturing a CUDA graph -- the first call should not be under capture; later calls are pure enqueues.
- *     dasp_reverb_fwd with f_save and irspec_save (a backward follows) runs each chunk's IR synthesis on those side
- *     streams, forked from `stream` by an event recorded on it at the start of the call and joined back into it
+ *     dasp_reverb_fwd with f_save and irspec_save (a backward follows) runs each chunk's IR synthesis on that side
+ *     stream, forked from `stream` by an event recorded on it at the start of the call and joined back into it
  *     before the call returns (event waits, which stream capture turns into graph edges), so the caller still sees
  *     one stream;
  *   - return value 0 = ok, negative = error (see DASP_ERR_*); the message is available

@@ -9,8 +9,8 @@ what its calls computed to DIR/a/<case>.npy and DIR/b/<case>.npy; then the files
 paths bench.py does not: the cuFFT pipeline and the two-kernel IR synthesis (dasp_debug_reverb_path 1 and 2), R = 9
 (two-kernel synthesis by default) and R = 17 (time-domain overlap-save), parity mode with a noise tensor, 2047 taps
 (nb = 16384: cuFFT polyphase synthesis), n % 4 != 0 (cuFFT convolution), mono input, a forward without a backward (the
-filtered noise and the spectra in the workspace), several chunks and a remainder (the forward's synthesis alternates
-between its two side streams), and convolution_reverberation with per-item and shared impulse responses.  The
+filtered noise and the spectra in the workspace), several chunks and a remainder (the forward's synthesis runs on its
+side stream), and convolution_reverberation with per-item and shared impulse responses.  The
 noise_shaped_impulse_response cases run the same synthesis paths with the planar sink (the cluster kernel, hooks 2 and
 1, R = 12, R = 17, parity noise, 2047 taps, L = 1, chunks, a forward without a backward) and save the IR, dL/dparams
 and the last path.  The dynamics cases run both curves at every warps-per-item W the library can be

@@ -7,14 +7,17 @@ path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_sha
 ``sidechain_compressor`` / ``sidechain_expander`` (the detector on an external key signal) and
 ``noise_shaped_impulse_response`` (the reverb's impulse response on its own, with gradients to its band parameters) and
 ``parametric_eq_frequency_response`` (the EQ's complex transfer function at chosen frequencies, with gradients to its
-18 parameters).
+18 parameters) and ``compressor_gain`` / ``expander_gain`` (the time-varying gain the compressor / expander multiplies
+into the audio, linear or in dB, with gradients to the detector input and the parameters).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
     compressor,
+    compressor_gain,
     convolution_reverberation,
     distortion,
     expander,
+    expander_gain,
     gain,
     noise_shaped_impulse_response,
     noise_shaped_impulse_response_packed,

@@ -100,6 +100,9 @@ _SIGNATURES = {
                                             I64, P]),
     "dasp_dynamics_sidechain_bwd": (c_int, [c_int, P, P, P, I64, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, c_float,
                                             c_float, I64, P]),
+    "dasp_dynamics_gain_fwd": (c_int, [c_int, P, I64, P, P, P, P, P, P, P, I64, I64, c_float, c_float, c_int, P]),
+    "dasp_dynamics_gain_bwd": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, c_int,
+                                       P]),
 }
 
 

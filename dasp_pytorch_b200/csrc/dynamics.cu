@@ -25,6 +25,11 @@
 // They differ in three places only: which stage buffers the detector sums (x from buffer 0, or the
 // key from buffer C, 2C in the backward); what the backward writes to the dL/dx buffers (plain:
 // gy G + the detector term; keyed: gy G); and where dL/dside goes (into x's rows, or into the key's).
+//
+// The gain curve on its own (dynamics_gain_fwd_kernel / dynamics_gain_bwd_kernel, GAIN): the same bodies with the
+// detector on x and no audio path.  The forward overwrites stage buffer 0 with G (or its dB value s + M) and stores
+// that one row; the backward reads dL/dG from buffer C instead of forming sum_c gy x, and writes dL/dside there.  With
+// the compressor's tile geometry the gain is bit-identical to the G the compressor multiplies into x.
 #include <math.h>
 #include <stdlib.h>
 
@@ -113,22 +118,45 @@ struct ScBwdRows {        // [0,C) = x (read only), [C,2C) = gy (in) -> gx (out)
   }
 };
 
-// the stage-buffer rows of one item, without (ChannelRows / BwdRows) or with a key (ScFwdRows / ScBwdRows)
-template <bool KEY>
+// the gain op's arguments: d.x is the detector input (bs, C, N).  Forward: d.y = G, or s + M in dB (bs, 1, N).
+// Backward: d.gy = dL/dG, or dL/d(dB) (bs, 1, N) in; d.y = dL/dside (bs, 1, N) out
+struct GainParams {
+  DynParams d;
+  int db;                // a runtime flag: one uniform branch per sample instead of twice the instantiations
+};
+struct GainFwdRows {      // buffers [0,C) = x (read only); buffer 0 is overwritten with the gain -> g
+  const float* x0; float* g0; int64_t n;
+  __device__ __forceinline__ const float* src(int b) const { return x0 + (int64_t)b * n; }
+  __device__ __forceinline__ float* dst(int b) const { return b == 0 ? g0 : nullptr; }
+};
+struct GainBwdRows {      // [0,C) = x (read only), C = dL/dG (in) -> dL/dside (out)
+  const float* x0; const float* gg0; float* gs0; int64_t n; int chs;
+  __device__ __forceinline__ const float* src(int b) const { return b < chs ? x0 + (int64_t)b * n : gg0; }
+  __device__ __forceinline__ float* dst(int b) const { return b < chs ? nullptr : gs0; }
+};
+
+// the stage-buffer rows of one item, without (ChannelRows / BwdRows) or with a key (ScFwdRows / ScBwdRows), or of
+// the gain op (GainFwdRows / GainBwdRows)
+template <bool KEY, bool GAIN = false>
 __device__ __forceinline__ auto fwd_rows(const DynParams& p, const float* key, int K, int item) {
   const int C = p.chs;
-  if constexpr (KEY) {
+  static_assert(!(KEY && GAIN), "the gain op has no key");
+  if constexpr (GAIN) {
+    return GainFwdRows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * p.n, p.n};
+  } else if constexpr (KEY) {
     return ScFwdRows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, key + (int64_t)item * K * p.n, p.n,
                      C};
   } else {
     return ChannelRows{p.x + (int64_t)item * C * p.n, p.y + (int64_t)item * C * p.n, p.n};
   }
 }
-template <bool KEY>
+template <bool KEY, bool GAIN = false>
 __device__ __forceinline__ auto bwd_rows(const DynParams& p, const float* key, float* gkey, int K, int item) {
   const int C = p.chs;
   const int64_t base = (int64_t)item * C * p.n;
-  if constexpr (KEY) {
+  if constexpr (GAIN) {
+    return GainBwdRows{p.x + base, p.gy + (int64_t)item * p.n, p.y + (int64_t)item * p.n, p.n, C};
+  } else if constexpr (KEY) {
     const int64_t kbase = (int64_t)item * K * p.n;
     return ScBwdRows{p.x + base, p.gy + base, p.y + base, key + kbase, gkey ? gkey + kbase : nullptr, p.n, C};
   } else {
@@ -342,8 +370,9 @@ constexpr size_t kSmemHeader = 512;
 // look-ahead): the two channel values of a sample stay in registers between the side-chain sum and the gain application
 // instead of being read from shared memory twice (round 2: the scan kernels are bound by the shared-memory pipe).
 // KEY: the detector sums the K key buffers that follow x's C (K = 0 without a key); ST is for the plain path only.
-template <Curve CV, int W, bool LA, bool ST, bool KEY>
-__device__ __forceinline__ void dynamics_fwd(const DynParams p, const float* key, int K) {
+// GAIN: buffer 0 receives G, or s + M when db, instead of the audio being scaled.
+template <Curve CV, int W, bool LA, bool ST, bool KEY, bool GAIN = false>
+__device__ __forceinline__ void dynamics_fwd(const DynParams p, const float* key, int K, bool db = false) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem<W> sm(smem_raw);
   const int item = blockIdx.x;
@@ -357,7 +386,7 @@ __device__ __forceinline__ void dynamics_fwd(const DynParams p, const float* key
   make_tables(tb, p.attack_ms[item], p.sample_rate, lane);
 
   TileGeom g{p.n, tile_len, p.ntiles, false};
-  auto rows = fwd_rows<KEY>(p, key, K, item);
+  auto rows = fwd_rows<KEY, GAIN>(p, key, K, item);
   TilePipe<kStages> pipe;
   pipe.init(sm.bars, sm.stages, KEY ? C + K : C, tile_len, p.bulk != 0);
   pipe.prologue(g, rows);
@@ -398,7 +427,11 @@ __device__ __forceinline__ void dynamics_fwd(const DynParams p, const float* key
     float G[kE];
 #pragma unroll
     for (int j = 0; j < kE; ++j) G[j] = exp2f((fmaf(tb.apow[j], c_in, s[j]) + M) * kLog2Of10Over20);
-    if (ST) {
+    if (GAIN) {
+      float* gb = pipe.buf(st, 0) + off;
+#pragma unroll
+      for (int j = 0; j < kE; ++j) gb[j] = db ? fmaf(tb.apow[j], c_in, s[j]) + M : G[j];
+    } else if (ST) {
       float* xa = pipe.buf(st, 0) + off;
       float* xb = pipe.buf(st, 1) + off;
 #pragma unroll
@@ -437,6 +470,11 @@ __global__ void __launch_bounds__(W * 32) dynamics_sc_fwd_kernel(ScParams sp) {
   dynamics_fwd<CV, W, LA, false, true>(sp.d, sp.key, sp.key_chs);
 }
 
+template <Curve CV, int W>
+__global__ void __launch_bounds__(W * 32) dynamics_gain_fwd_kernel(GainParams gp) {
+  dynamics_fwd<CV, W, false, false, false, true>(gp.d, nullptr, 0, gp.db != 0);
+}
+
 // =============================================================================== backward
 // block reduction of the five per-thread sums, chain rule to the user parameters, written to gparams[item][0..5]
 template <int W>
@@ -471,8 +509,9 @@ __device__ __forceinline__ void param_grads(float (&red)[5][W], float acc_m, flo
 }
 
 // KEY: the detector sums the K key buffers that follow x's C and dL/dy's C; gkey (may be null) receives dL/dside
-template <Curve CV, int W, bool LA, bool ST, bool KEY>
-__device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key, float* gkey, int K) {
+// GAIN: buffer C holds dL/dG (dL/d(s + M) when db) in place of dL/dy's C buffers, and receives dL/dside
+template <Curve CV, int W, bool LA, bool ST, bool KEY, bool GAIN = false>
+__device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key, float* gkey, int K, bool db = false) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem<W> sm(smem_raw);
   __shared__ float red[5][W];
@@ -493,9 +532,9 @@ __device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key
   const float rlane_pow = tr.lane_pow;
 
   TileGeom g{p.n, tile_len, p.ntiles, true};
-  auto rows = bwd_rows<KEY>(p, key, gkey, K, item);
+  auto rows = bwd_rows<KEY, GAIN>(p, key, gkey, K, item);
   TilePipe<kStages> pipe;
-  pipe.init(sm.bars, sm.stages, KEY ? 2 * C + K : 2 * C, tile_len, p.bulk != 0);
+  pipe.init(sm.bars, sm.stages, GAIN ? C + 1 : (KEY ? 2 * C + K : 2 * C), tile_len, p.bulk != 0);
   pipe.prologue(g, rows);
 
   float w_tile = 0.f;                                 // adjoint state w[first sample of the next tile]
@@ -545,7 +584,12 @@ __device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key
       float dG[kE];
 #pragma unroll
       for (int j = 0; j < kE; ++j) dG[j] = ST ? fmaf(g0[ST ? j : 0], x0[ST ? j : 0], g1[ST ? j : 0] * x1[ST ? j : 0]) : 0.f;
-      for (int c = 0; c < (ST ? 0 : C); ++c) {
+      if (GAIN) {
+        const float* gg = pipe.buf(st, C) + off;
+#pragma unroll
+        for (int j = 0; j < kE; ++j) dG[j] = gg[j];
+      }
+      for (int c = 0; c < (ST || GAIN ? 0 : C); ++c) {
         const float* xb = pipe.buf(st, c) + off;
         const float* gb = pipe.buf(st, C + c) + off;
         if (!LA) {
@@ -565,7 +609,7 @@ __device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key
       for (int j = kE - 1; j >= 0; --j) {
         const bool valid = (n0 + j < p.n);
         G[j] = exp2f((s[j] + M) * kLog2Of10Over20);
-        const float ds = valid ? dG[j] * G[j] * kLn10Over20 : 0.f;
+        const float ds = valid ? ((GAIN && db) ? dG[j] : dG[j] * G[j] * kLn10Over20) : 0.f;
         acc_m += ds;
         run = fmaf(tb.alpha, run, ds);
         wv[j] = run;
@@ -592,8 +636,12 @@ __device__ __forceinline__ void dynamics_bwd(const DynParams p, const float* key
       }
       dxs[j] = dx;
     }
-    // dL/dx = gy G, plus dL/dside on the plain path (x is the detector's input there)
-    if (ST) {
+    // dL/dx = gy G, plus dL/dside on the plain path (x is the detector's input there); the gain op returns dL/dside
+    if (GAIN) {
+      float* gs = pipe.buf(st, C) + off;
+#pragma unroll
+      for (int j = 0; j < kE; ++j) gs[j] = dxs[j];
+    } else if (ST) {
       float* ga = pipe.buf(st, 2) + off;
       float* gb = pipe.buf(st, 3) + off;
 #pragma unroll
@@ -640,6 +688,12 @@ template <Curve CV, int W, bool LA>
 __global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1))
     dynamics_sc_bwd_kernel(ScParams sp) {
   dynamics_bwd<CV, W, LA, false, true>(sp.d, sp.key, sp.gkey, sp.key_chs);
+}
+
+template <Curve CV, int W>
+__global__ void __launch_bounds__(W * 32, (W <= 4) ? (4 * DASP_DYN_BWD_MINB) / W : (W == 8 ? 2 : 1))
+    dynamics_gain_bwd_kernel(GainParams gp) {
+  dynamics_bwd<CV, W, false, false, false, true>(gp.d, nullptr, nullptr, 0, gp.db != 0);
 }
 
 // lookahead > 0 only: gx[b,c,m] += gy[b,c,m+la] * G[b,m+la]
@@ -723,8 +777,15 @@ int launch_w(bool bwd, const ScParams& sp, int64_t bs, cudaStream_t st) {
   const bool stereo = sp.key_chs == 0 && sp.d.chs == 2 && !debug_generic_channels();
   return stereo ? launch_variant<CV, W, false, true>(bwd, sp, bs, st) : launch_variant<CV, W, false, false>(bwd, sp, bs, st);
 }
-template <Curve CV>
-int dispatch(bool bwd, int w, const ScParams& sp, int64_t bs, cudaStream_t st) {
+// the gain op: x's C buffers, and in the backward one more for dL/dG -> dL/dside
+template <Curve CV, int W>
+int launch_w(bool bwd, const GainParams& gp, int64_t bs, cudaStream_t st) {
+  const int nbuf = gp.d.chs + (bwd ? 1 : 0);
+  return bwd ? launch<dynamics_gain_bwd_kernel<CV, W>>("dynamics_gain_bwd_kernel", gp, W, nbuf, bs, st)
+             : launch<dynamics_gain_fwd_kernel<CV, W>>("dynamics_gain_fwd_kernel", gp, W, nbuf, bs, st);
+}
+template <Curve CV, class Args>
+int dispatch(bool bwd, int w, const Args& sp, int64_t bs, cudaStream_t st) {
   switch (w) {
     case 1: return launch_w<CV, 1>(bwd, sp, bs, st);
     case 2: return launch_w<CV, 2>(bwd, sp, bs, st);
@@ -816,6 +877,35 @@ int dyn_bwd(int kind, const float* gy, const float* x, const float* key, int64_t
   return DASP_OK;
 }
 
+// the gain op, after the entry points' argument checks.  Its tiles are the compressor's (dyn_warps without a key), so
+// that G is bit-identical to the gain the compressor applies; the backward's C + 1 buffers fit wherever 2C do.
+int dyn_gain_fwd(int kind, const float* x, const float* ps[5], float* g, float* ckpt, int64_t bs, int64_t chs,
+                 int64_t n, float sample_rate, float eps, int db, cudaStream_t st) {
+  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics gain: kind must be 0 (compressor) or 1 (expander)");
+  if (bs == 0 || n == 0) return DASP_OK;
+  DASP_REQUIRE(g != nullptr, "dynamics gain fwd: null g");
+  const int w = dyn_warps(bs, chs, 0);
+  GainParams gp{dyn_params(w, x, nullptr, 0, ps, chs, n, sample_rate, eps, 0).d, db != 0};
+  gp.d.y = g; gp.d.ckpt = ckpt;
+  gp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(g);
+  return kind == 0 ? dispatch<Curve::Compress>(false, w, gp, bs, st) : dispatch<Curve::Expand>(false, w, gp, bs, st);
+}
+
+int dyn_gain_bwd(int kind, const float* gg, const float* x, const float* ps[5], const float* ckpt, float* gside,
+                 float* gparams, int64_t bs, int64_t chs, int64_t n, float sample_rate, float eps, int db,
+                 cudaStream_t st) {
+  DASP_REQUIRE(kind == 0 || kind == 1, "dynamics gain: kind must be 0 (compressor) or 1 (expander)");
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(gparams != nullptr, "dynamics gain bwd: null gparams");
+  if (n == 0) { DASP_CUDA_OK(cudaMemsetAsync(gparams, 0, sizeof(float) * 6 * bs, st)); return DASP_OK; }
+  DASP_REQUIRE(gg && gside && ckpt, "dynamics gain bwd: null pointer");
+  const int w = dyn_warps(bs, chs, 0);
+  GainParams gp{dyn_params(w, x, nullptr, 0, ps, chs, n, sample_rate, eps, 0).d, db != 0};
+  gp.d.gy = gg; gp.d.y = gside; gp.d.ckpt = const_cast<float*>(ckpt); gp.d.gparams = gparams;
+  gp.d.bulk = (n % 4 == 0) && aligned16(x) && aligned16(gg) && aligned16(gside);
+  return kind == 0 ? dispatch<Curve::Compress>(true, w, gp, bs, st) : dispatch<Curve::Expand>(true, w, gp, bs, st);
+}
+
 }  // namespace
 }  // namespace dasp
 
@@ -878,6 +968,26 @@ int dasp_dynamics_sidechain_bwd(int kind, const float* gy, const float* x, const
   if (rc != DASP_OK) return rc;
   return dyn_bwd(kind, gy, x, key, key_chs, ps, ckpt, gx, gkey, gparams, g_scratch, bs, chs, n, sample_rate, eps,
                  lookahead, (cudaStream_t)stream);
+}
+
+// ---- the gain curve on its own ----
+int dasp_dynamics_gain_fwd(int kind, const float* x, int64_t chs, const float* threshold_db, const float* ratio,
+                           const float* attack_ms, const float* knee_db, const float* makeup_db, float* g, float* ckpt,
+                           int64_t bs, int64_t n, float sample_rate, float eps, int db, void* stream) {
+  const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
+  int rc = check_common(x, ps, bs, chs, n, 0);
+  if (rc != DASP_OK) return rc;
+  return dyn_gain_fwd(kind, x, ps, g, ckpt, bs, chs, n, sample_rate, eps, db, (cudaStream_t)stream);
+}
+
+int dasp_dynamics_gain_bwd(int kind, const float* gg, const float* x, const float* threshold_db, const float* ratio,
+                           const float* attack_ms, const float* knee_db, const float* makeup_db, const float* ckpt,
+                           float* gside, float* gparams, int64_t bs, int64_t chs, int64_t n, float sample_rate,
+                           float eps, int db, void* stream) {
+  const float* ps[5] = {threshold_db, ratio, attack_ms, knee_db, makeup_db};
+  int rc = check_common(x, ps, bs, chs, n, 0);
+  if (rc != DASP_OK) return rc;
+  return dyn_gain_bwd(kind, gg, x, ps, ckpt, gside, gparams, bs, chs, n, sample_rate, eps, db, (cudaStream_t)stream);
 }
 
 }  // extern "C"

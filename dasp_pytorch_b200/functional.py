@@ -32,6 +32,8 @@ __all__ = [
     "expander",
     "sidechain_compressor",
     "sidechain_expander",
+    "compressor_gain",
+    "expander_gain",
     "noise_shaped_reverberation",
     "convolution_reverberation",
     "noise_shaped_impulse_response",
@@ -543,6 +545,150 @@ def sidechain_expander(
     the compressor: gating one track from another."""
     return _dynamics(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
                      lookahead_samples, sidechain)
+
+
+# --------------------------------------------------------------------------------------
+# the compressor's / expander's gain curve
+# --------------------------------------------------------------------------------------
+
+
+DYNAMICS_MAX_CHANNELS = 32
+
+
+class _DynamicsGainFn(torch.autograd.Function):
+    """Detector input x (bs, C, n) -> the gain (bs, 1, n): G, or s + M in dB when ``db``.  kind 0 = compressor,
+    1 = expander.  The backward writes dL/dside once per item and hands it to every channel as an expanded view."""
+
+    @staticmethod
+    def forward(ctx, x, threshold, ratio, attack, knee, makeup, kind, sample_rate, eps, db):
+        lib = _abi.lib()
+        bs, chs, n = x.shape
+        g = torch.empty(bs, 1, n, dtype=torch.float32, device=x.device)
+        need_bwd = any(ctx.needs_input_grad[:6])
+        ckpt = None
+        with torch.cuda.device(x.device):
+            if need_bwd:
+                tile = lib.dasp_dynamics_tile_len(bs, chs)           # the compressor's tiles for (bs, chs)
+                if tile <= 0:
+                    raise DaspError(f"dynamics gain: unsupported channel count {chs}")
+                ckpt = torch.empty(bs * max(1, -(-n // tile)), dtype=torch.float32, device=x.device)
+            with _timed("dyn_gain_fwd", x.device):
+                check(lib.dasp_dynamics_gain_fwd(kind, ptr(x), chs, ptr(threshold), ptr(ratio), ptr(attack), ptr(knee),
+                                                 ptr(makeup), ptr(g), ptr(ckpt), bs, n, float(sample_rate), float(eps),
+                                                 int(db), stream_ptr(x.device)), "dasp_dynamics_gain_fwd")
+        if need_bwd:
+            ctx.save_for_backward(x, threshold, ratio, attack, knee, makeup, ckpt)
+        ctx.cfg = (kind, float(sample_rate), float(eps), int(db))
+        return g
+
+    @staticmethod
+    def backward(ctx, gg):
+        lib = _abi.lib()
+        x, threshold, ratio, attack, knee, makeup, ckpt = ctx.saved_tensors
+        kind, sample_rate, eps, db = ctx.cfg
+        bs, chs, n = x.shape
+        gg = gg.contiguous()
+        gside = torch.empty(bs, 1, n, dtype=torch.float32, device=x.device)
+        gp = torch.empty(bs, 6, dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device), _timed("dyn_gain_bwd", x.device):
+            check(lib.dasp_dynamics_gain_bwd(kind, ptr(gg), ptr(x), ptr(threshold), ptr(ratio), ptr(attack), ptr(knee),
+                                             ptr(makeup), ptr(ckpt), ptr(gside), ptr(gp), bs, chs, n, sample_rate, eps,
+                                             db, stream_ptr(x.device)), "dasp_dynamics_gain_bwd")
+        gx = gside.expand(bs, chs, n) if ctx.needs_input_grad[0] else None
+        return gx, gp[:, 0], gp[:, 1], gp[:, 2], gp[:, 4], gp[:, 5], None, None, None, None
+
+
+def _gain_input(x):
+    """rank and channel count of the detector input, checked before anything touches a device"""
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, channels, samples)")
+    if not 1 <= x.shape[1] <= DYNAMICS_MAX_CHANNELS:
+        raise ValueError(f"x: 1 to {DYNAMICS_MAX_CHANNELS} channels are supported, got {x.shape[1]}")
+
+
+def _dynamics_gain(kind, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
+                   db):
+    _gain_input(x)
+    bs = x.shape[0]
+    ps = [
+        _param(p, bs, x, name, allow_broadcast=True).contiguous()
+        for p, name in (
+            (threshold_db, "threshold_db"),
+            (ratio, "ratio"),
+            (attack_ms, "attack_ms"),
+            (knee_db, "knee_db"),
+            (makeup_gain_db, "makeup_gain_db"),
+        )
+    ]
+    _param(release_ms, bs, x, "release_ms", allow_broadcast=True)         # shape only, as in compressor
+    xf, dt = _audio(x)
+    return _DynamicsGainFn.apply(xf, *ps, kind, sample_rate, eps, bool(db)).to(dt)
+
+
+def dynamics_gain_packed(kind: int, x: torch.Tensor, sample_rate: float, params: torch.Tensor, eps: float = 1e-8, *,
+                         db: bool = False):
+    """``compressor_gain`` (kind 0) / ``expander_gain`` (kind 1) with the six parameters stacked as ``(bs, 6)`` in
+    signature order (threshold, ratio, attack, release, knee, makeup)."""
+    _gain_input(x)
+    pt = _packed(params, x.shape[0], 6, x, "params").t().contiguous()        # (6, bs): rows are contiguous
+    xf, dt = _audio(x)
+    return _DynamicsGainFn.apply(xf, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, bool(db)).to(dt)
+
+
+def compressor_gain(
+    x: torch.Tensor,
+    sample_rate: float,
+    threshold_db: torch.Tensor,
+    ratio: torch.Tensor,
+    attack_ms: torch.Tensor,
+    release_ms: torch.Tensor,
+    knee_db: torch.Tensor,
+    makeup_gain_db: torch.Tensor,
+    eps: float = 1e-8,
+    *,
+    db: bool = False,
+):
+    """The time-varying gain ``G`` that ``compressor`` multiplies into the audio, as an op of its own: ``(bs, 1, n)``,
+    broadcasting against any ``(bs, C', n)``.
+
+    ``x`` is the detector input ``(bs, C, n)``, ``1 <= C <= 32``: the audio itself, or a key of any channel count.  The
+    detector is the compressor's: ``side = x.sum(dim=1)`` (accumulated in fp64, rounded once), ``level =
+    20 log10(max(|side|, eps))``, the static curve, the zero-state one-pole attack smoother ``s`` and the makeup ``M``.
+    The result is ``G = 10^((s + M) / 20)``, or ``s + M`` in dB with ``db=True`` (finite where the linear gain
+    underflows, e.g. an expander at a high ratio on silence).  Computed in fp32, returned in x's dtype.  Parameters
+    broadcast as in ``compressor``; ``release_ms`` is validated for shape and gets no gradient.  There is no look-ahead:
+    it delays the audio path, never the gain, so for every C and look-ahead ``la``
+
+        ``compressor(x, ..., lookahead_samples=la)[b, c, t] == x[b, c, t - la] * compressor_gain(x, ...)[b, 0, t]``
+
+    bit for bit (0 for ``t < la``).  ``sidechain_compressor(x, sidechain=k)`` agrees with
+    ``delay(x) * compressor_gain(k)`` to rounding, not bit for bit: its tiles depend on x's channels too.
+
+    Gradients: every channel of x receives the same ``dL/dside``, which carries ``1/side`` and is 0 where
+    ``|side| < eps`` (returned as an expanded view of one row per item); the five other parameters as in ``compressor``.
+    Without a gradient to compute, no smoother checkpoint is kept.
+    """
+    return _dynamics_gain(0, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
+                          db)
+
+
+def expander_gain(
+    x: torch.Tensor,
+    sample_rate: float,
+    threshold_db: torch.Tensor,
+    ratio: torch.Tensor,
+    attack_ms: torch.Tensor,
+    release_ms: torch.Tensor,
+    knee_db: torch.Tensor,
+    makeup_gain_db: torch.Tensor,
+    eps: float = 1e-8,
+    *,
+    db: bool = False,
+):
+    """The gain ``expander`` applies, exactly as ``compressor_gain`` is the compressor's: the expander's static curve,
+    the same detector, smoother and makeup, the same bit-for-bit contract with ``expander``."""
+    return _dynamics_gain(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
+                          db)
 
 
 # --------------------------------------------------------------------------------------

@@ -281,12 +281,26 @@ class _Dynamics(Processor):
         by_name = self._sidechain_fn if self.process_fn is self._packed_path[1] else None
         return self._process_normalized(x, param_tensor, by_name, sidechain=sidechain)
 
+    _kind = None          # 0: compressor, 1: expander
+
+    def gain_curve(self, x: torch.Tensor, param_tensor: torch.Tensor, *, db: bool = False) -> torch.Tensor:
+        """The gain ``(batch, 1, n)`` that ``process_normalized(x, param_tensor)`` multiplies into the audio, with the
+        detector on ``x`` (see ``functional.compressor_gain``); ``db=True`` returns it in dB.  ``param_tensor`` is
+        ``(batch, 6)`` in [0, 1] on a CUDA device, mapped and range-checked exactly as ``process_normalized`` does;
+        gradients flow back to it and to x."""
+        if not torch.is_tensor(param_tensor) or not param_tensor.is_cuda:
+            raise _F.DaspError(f"{type(self).__name__}.gain_curve: param_tensor must be a CUDA tensor; "
+                               "dasp_pytorch_b200 has no CPU path")
+        phys = self._denormalize_packed(param_tensor)
+        return _F.dynamics_gain_packed(self._kind, x, self.sample_rate, phys, db=db)
+
 
 class Compressor(_Dynamics):
     def __init__(self, sample_rate: int, **kw):
         super().__init__(sample_rate, **kw)
         self.process_fn = compressor
         self._sidechain_fn = sidechain_compressor
+        self._kind = 0
         self._packed_path = (lambda x, sr, p, **kw: _F.dynamics_packed(0, x, sr, p, **kw), compressor)
 
 
@@ -297,6 +311,7 @@ class Expander(_Dynamics):
         super().__init__(sample_rate, max_ratio=max_ratio, **kw)
         self.process_fn = expander
         self._sidechain_fn = sidechain_expander
+        self._kind = 1
         self._packed_path = (lambda x, sr, p, **kw: _F.dynamics_packed(1, x, sr, p, **kw), expander)
 
 

@@ -155,6 +155,20 @@ int dasp_dynamics_sidechain_bwd(int kind, const float* gy, const float* x, const
                                 float* gkey /* may be NULL */, float* gparams, float* g_scratch, int64_t bs,
                                 int64_t chs, int64_t n, float sample_rate, float eps, int64_t lookahead,
                                 void* stream);
+/* The gain curve on its own: the detector of dasp_dynamics_fwd on x (bs, chs, n), 1 <= chs <= 32, and no audio path.
+ * g (bs, 1, n) receives G[b,t] = 10^((s + M) / 20), or s + M in dB when db != 0 (s: the smoothed static curve,
+ * M: makeup).  The tiles are dasp_dynamics_fwd's for the same (bs, chs), so G is bit-identical to the gain that
+ * dasp_dynamics_fwd multiplies into x[b,c,t-lookahead], and ckpt holds bs * ceil(n / dasp_dynamics_tile_len(bs, chs))
+ * floats (NULL in the forward when no backward will follow).  Backward: gg (bs, 1, n) is dL/dg (dL/d(dB) when db);
+ * gside (bs, 1, n) receives dL/dside, the gradient every channel of x gets, which is 0 where |side| < eps; gparams as
+ * above.  Bad shapes and channel counts return -1 before any CUDA call. */
+int dasp_dynamics_gain_fwd(int kind, const float* x, int64_t chs, const float* threshold_db, const float* ratio,
+                           const float* attack_ms, const float* knee_db, const float* makeup_db, float* g, float* ckpt,
+                           int64_t bs, int64_t n, float sample_rate, float eps, int db, void* stream);
+int dasp_dynamics_gain_bwd(int kind, const float* gg, const float* x, const float* threshold_db, const float* ratio,
+                           const float* attack_ms, const float* knee_db, const float* makeup_db, const float* ckpt,
+                           float* gside, float* gparams, int64_t bs, int64_t chs, int64_t n, float sample_rate,
+                           float eps, int db, void* stream);
 
 /* ---- parametric_eq: six cascaded biquads   (reference functional.py:118-272 with
  *      signal.biquad signal.py:242-306 and signal.sosfilt_via_fsm signal.py:136-166) ------

@@ -8,12 +8,15 @@ path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_sha
 ``noise_shaped_impulse_response`` (the reverb's impulse response on its own, with gradients to its band parameters) and
 ``parametric_eq_frequency_response`` (the EQ's complex transfer function at chosen frequencies, with gradients to its
 18 parameters) and ``compressor_gain`` / ``expander_gain`` (the time-varying gain the compressor / expander multiplies
-into the audio, linear or in dB, with gradients to the detector input and the parameters).
+into the audio, linear or in dB, with gradients to the detector input and the parameters) and ``convolution_bus`` (any
+number of input channels, each through its own impulse responses, summed into a mono or stereo bus).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
+    CONV_BUS_MAX_INPUTS,
     compressor,
     compressor_gain,
+    convolution_bus,
     convolution_reverberation,
     distortion,
     expander,

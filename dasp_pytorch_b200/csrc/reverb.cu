@@ -37,6 +37,11 @@
 // true-stereo IR (ir_chs 4) is two partition sets per IR (ConvGeom::sets), multiplied by the TS variants of the MAC
 // kernels.
 //
+// convolution_bus (dasp_conv_bus_*) is the same partitioned convolution for S inputs summed into O = 1 or 2 outputs:
+// every signal's rows are packed two per transform (bus_fft_kernel, bus_ir_pack_kernel + x_fft_kernel's partition
+// units), bus_mac_kernel sums the untangled products over the inputs, and bus_ifft_kernel writes the outputs, dL/dx and
+// dL/dIR; a shared IR's gradient goes through irgrad_sum_kernel.
+//
 // noise_shaped_impulse_response (dasp_nsir_*) is the IR synthesis without the convolution, with the geometry of the
 // reverb at n = L.  Every synthesis kernel is a template on its output sink (PartitionSink: the convolution's partition
 // slots; PlanarSink: the caller's (bs, 2, L) rows), and both ops run one host-side synthesis stage: choose_synth (the
@@ -1886,6 +1891,352 @@ __global__ void conv_mix_grad_kernel(const float* __restrict__ mix_part, float* 
   gmix[item0 + il] = (float)s;
 }
 
+// ---- convolution_bus: S input rows, each through its own IR, summed into O = 1 or 2 output rows -----------------
+// Every signal of the bus is a group of rows (the S inputs, the O outputs, the S O IR rows s O + o): its rows are packed
+// two per complex transform, row 2k as the real and row 2k + 1 as the imaginary part, and an odd last row packs alone
+// (imaginary part 0).  So an item has P = ceil(S / 2) window spectra per block, NH = ceil(S O / 2) partition sets
+// (a stereo bus: set s = h_s0 + i h_s1; a mono bus: set k = h_2k + i h_2k+1) and one gradient spectrum per block.
+// bus_mac_kernel untangles every operand into the spectra of its real rows, so one formula serves both bus widths.
+
+// forward transforms of row pairs, runs of kConvRun units (il, k, i), il < items, k < groups, i < I:
+//   out[((il*groups + k)*I + i)*kNbA + f] = FFT of (r_2k + i r_2k+1)[(i-1) kB + m], m < kNbA, zero outside [lo, n), where
+//   the rows r are the `rows` rows of item item0 + il in src and lo = 0 (half == 0: the audio windows, as x_fft_kernel)
+//   or kB (half == 1: [zeros(kB) | g[i kB, (i+1) kB)], g_fft_kernel's block i); lo = kB for i = 0 either way.
+//   Requires n % 4 == 0 and 16-byte aligned rows (bulk copies).
+__global__ void __launch_bounds__(kFusedThreads, 1)
+bus_fft_kernel(const float* __restrict__ src, float2* __restrict__ out, const float* __restrict__ twiddles, int64_t item0,
+               int rows, int groups, int I, int64_t n, int half, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {                // all threads: zero padding; thread 0: the bulk copies
+    if (m >= m1) return;
+    const int q = m / I, i = m - q * I;            // q = il * groups + k
+    const int64_t il = q / groups;
+    const int k = q - (int)il * groups;
+    const bool two = 2 * k + 1 < rows;
+    float* re = s.buf(it);
+    float* im = re + fft8k::kPlaneG;
+    const int64_t s0 = (int64_t)(i - 1) * kB;
+    const int lo = (half || i == 0) ? kB : 0;
+    const int64_t rem = n - s0;
+    const int hi = rem < kNbA ? (int)rem : kNbA;   // valid window samples are [lo, hi), hi > lo
+    for (int e = t; e < lo; e += kFusedThreads) { re[e] = 0.f; im[e] = 0.f; }
+    for (int e = hi + t; e < kNbA; e += kFusedThreads) { re[e] = 0.f; im[e] = 0.f; }
+    if (!two) for (int e = lo + t; e < hi; e += kFusedThreads) im[e] = 0.f;
+    if (t == 0) {
+      const float* ra = src + ((item0 + il) * rows + 2 * k) * n + s0;
+      uint64_t* bar = &s.full[it & 1];
+      mbar_arrive_expect_tx(bar, (two ? 2u : 1u) * (uint32_t)(hi - lo) * 4u);
+      for (int o = lo; o < hi; o += 4096) {
+        const uint32_t bytes = (uint32_t)((hi - o < 4096 ? hi - o : 4096) * 4);
+        tma_load_1d(re + o, ra + o, bytes, bar);
+        if (two) tma_load_1d(im + o, ra + n + o, bytes, bar);
+      }
+    }
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  __syncthreads();                                 // the zero padding of the first two buffers is in place
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    float xr[16], xi[16];
+    fft8192_in_smem<false>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    float2* o = out + (int64_t)m * kNbA;
+#pragma unroll
+    for (int q = 0; q < 16; ++q) o[t + 512 * q] = make_float2(xr[q], xi[q]);
+  }
+}
+
+// IR taps t < leff of row pairs (2k, 2k + 1) of the (rows, L) rows of item item0 + il -> (re, im) pairs in the first
+// half of partition slot t / kB of set k (an odd last row packs with 0).  grid = (ceil(leff / 256), items, NH sets)
+__global__ void bus_ir_pack_kernel(const float* __restrict__ ir, float2* __restrict__ Hb, int64_t item0, int rows, int J,
+                                   int64_t L, int64_t leff) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t il = blockIdx.y;
+  const int k = blockIdx.z;
+  if (t >= leff) return;
+  const float* ra = ir + ((item0 + il) * rows + 2 * k) * L;
+  Hb[ir_slot(il * gridDim.z + k, J, t)] = make_float2(ra[t], 2 * k + 1 < rows ? ra[L + t] : 0.f);
+}
+
+// The products of the bus on the block spectra, per bin pair (f, kNbA - f) and item.  Every operand is untangled into
+// the spectra of its real rows (X_s: input s, H_so: IR row s O + o, G_o: output gradient o), and every result is stored
+// packed two real rows per block, planar, scaled by `scale`:
+//   BUS_FWD: Y_o[i] = sum_s sum_j X_s[i - j] H_so[j]                       out: I blocks (Y_0 + i Y_1)
+//   BUS_DX:  D_s[i] = sum_o sum_j G_o[i + j] conj(H_so[j]),  stored as W_s[i] = D_s[i] + (-1)^f D_s[i + 1]: the inverse
+//            of W_s[i] has, in its second half, the second half of D_s[i]'s inverse plus the first half of D_s[i + 1]'s
+//            (a circular shift by kB is the factor (-1)^f), i.e. dL/dx_s on samples [i kB, (i+1) kB) with the
+//            overlap-add already done                                   out: P I blocks (W_2p + i W_2p+1)
+//   BUS_DIR: E_so[j] = sum_i G_o[j + i] conj(X_s[i])                         out: NH J blocks (set k: rows 2k, 2k + 1)
+// X: P I blocks per item; H: NH J blocks per IR at item stride hstride (0: one IR for the batch); G: I blocks per item.
+// MAXB > 0 caches the block operands of one input in registers (I, J <= MAXB) and loops over the inputs with the
+// accumulators held; MAXB == 0 reads every operand from L2.
+enum BusMac { BUS_FWD, BUS_DX, BUS_DIR };
+template <int MAXB, int MODE, int O>
+__global__ void __launch_bounds__(128) bus_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                      int64_t hstride, const float2* __restrict__ G,
+                                                      float2* __restrict__ Out, int S, int I, int J, float scale) {
+  constexpr int M = MAXB > 0 ? MAXB : 1;
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int64_t il = blockIdx.y;
+  const int P = (S + 1) / 2, NH = (S * O + 1) / 2;
+  const float2* x = X + il * (int64_t)P * I * kNbA;
+  const float2* h = H + il * hstride;
+  const float2* g = G + il * (int64_t)I * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  // input s at block i
+  auto xin = [&](int s, int i) -> float2 {
+    float2 a, b;
+    pair(x, (int64_t)(s >> 1) * I + i, a, b);
+    return (s & 1) ? b : a;
+  };
+  // IR rows (s, 0) and (s, 1) (O == 2), or row s (O == 1) at partition j
+  auto hin = [&](int s, int j, float2& h0, float2& h1) {
+    if (O == 2) { pair(h, (int64_t)s * J + j, h0, h1); }
+    else { float2 a, b; pair(h, (int64_t)(s >> 1) * J + j, a, b); h0 = (s & 1) ? b : a; h1 = zero; }
+  };
+  auto gin = [&](int i, float2& g0, float2& g1) { pair(g, i, g0, g1); };
+  // packed planar store of real rows (a, b) into block `slot` of Out (item-local index `slot` of the item's blocks)
+  auto emit = [&](int64_t slot, float2 a, float2 b) {
+    a.x *= scale; a.y *= scale; b.x *= scale; b.y *= scale;
+    float* pl = reinterpret_cast<float*>(Out + slot * kNbA);
+    pl[f] = a.x - b.y; pl[kNbA + f] = a.y + b.x;
+    if (fm != f) { pl[fm] = a.x + b.y; pl[kNbA + fm] = b.x - a.y; }
+  };
+  const float sgn = (f & 1) ? -1.f : 1.f;
+  auto axpy = [&](float2 acc, float2 v) { return make_float2(fmaf(sgn, v.x, acc.x), fmaf(sgn, v.y, acc.y)); };
+
+  if constexpr (MODE == BUS_FWD) {
+    const int64_t ob = il * (int64_t)I;
+    if constexpr (MAXB > 0) {
+      float2 y0[M], y1[M];
+#pragma unroll
+      for (int o = 0; o < M; ++o) y0[o] = y1[o] = zero;
+      for (int s = 0; s < S; ++s) {
+        float2 xv[M], h0[M], h1[M];
+#pragma unroll
+        for (int i = 0; i < M; ++i) {
+          xv[i] = h0[i] = h1[i] = zero;                // operands beyond I / J are zero
+          if (i < I) xv[i] = xin(s, i);
+          if (i < J) hin(s, i, h0[i], h1[i]);
+        }
+#pragma unroll
+        for (int o = 0; o < M; ++o) {
+#pragma unroll
+          for (int j = 0; j <= o; ++j) {
+            cfma(y0[o], xv[o - j], h0[j]);
+            if (O == 2) cfma(y1[o], xv[o - j], h1[j]);
+          }
+        }
+      }
+#pragma unroll
+      for (int o = 0; o < M; ++o)
+        if (o < I) emit(ob + o, y0[o], y1[o]);
+    } else {
+      for (int o = 0; o < I; ++o) {
+        float2 y0 = zero, y1 = zero;
+        for (int s = 0; s < S; ++s) {
+          for (int j = 0; j <= o && j < J; ++j) {
+            float2 h0, h1;
+            hin(s, j, h0, h1);
+            const float2 xv = xin(s, o - j);
+            cfma(y0, xv, h0);
+            if (O == 2) cfma(y1, xv, h1);
+          }
+        }
+        emit(ob + o, y0, y1);
+      }
+    }
+  } else if constexpr (MODE == BUS_DX) {
+    const int64_t ob = il * (int64_t)P * I;
+    if constexpr (MAXB > 0) {
+      float2 g0[M], g1[M];
+#pragma unroll
+      for (int i = 0; i < M; ++i) {
+        g0[i] = g1[i] = zero;
+        if (i < I) gin(i, g0[i], g1[i]);
+      }
+      for (int p = 0; p < P; ++p) {
+        // source 2p: W into wa (folded in place, ascending); source 2p + 1: D in descending order, W emitted with wa
+        float2 wa[M], h0[M], h1[M];
+#pragma unroll
+        for (int j = 0; j < M; ++j) {
+          h0[j] = h1[j] = zero;
+          if (j < J) hin(2 * p, j, h0[j], h1[j]);
+        }
+#pragma unroll
+        for (int i = 0; i < M; ++i) {
+          wa[i] = zero;
+#pragma unroll
+          for (int j = 0; i + j < M; ++j) {
+            cfma_conj(wa[i], g0[i + j], h0[j]);
+            if (O == 2) cfma_conj(wa[i], g1[i + j], h1[j]);
+          }
+        }
+#pragma unroll
+        for (int i = 0; i + 1 < M; ++i) wa[i] = axpy(wa[i], wa[i + 1]);
+        const bool two = 2 * p + 1 < S;
+#pragma unroll
+        for (int j = 0; j < M; ++j) {
+          h0[j] = h1[j] = zero;
+          if (two && j < J) hin(2 * p + 1, j, h0[j], h1[j]);
+        }
+        float2 next = zero;                            // D_b[i + 1]
+#pragma unroll
+        for (int i = M - 1; i >= 0; --i) {
+          float2 d = zero;
+#pragma unroll
+          for (int j = 0; i + j < M; ++j) {
+            cfma_conj(d, g0[i + j], h0[j]);
+            if (O == 2) cfma_conj(d, g1[i + j], h1[j]);
+          }
+          if (i < I) emit(ob + (int64_t)p * I + i, wa[i], axpy(d, next));
+          next = d;
+        }
+      }
+    } else {
+      for (int p = 0; p < P; ++p) {
+        for (int i = 0; i < I; ++i) {
+          float2 w[2] = {zero, zero};
+          for (int c = 0; c < 2 && 2 * p + c < S; ++c) {
+            for (int q = i; q < i + 2 && q < I; ++q) {   // D_s[i] + (-1)^f D_s[i + 1]
+              float2 d = zero;
+              for (int j = 0; j < J && q + j < I; ++j) {
+                float2 g0v, g1v, h0, h1;
+                gin(q + j, g0v, g1v);
+                hin(2 * p + c, j, h0, h1);
+                cfma_conj(d, g0v, h0);
+                if (O == 2) cfma_conj(d, g1v, h1);
+              }
+              w[c] = q == i ? d : axpy(w[c], d);
+            }
+          }
+          emit(ob + (int64_t)p * I + i, w[0], w[1]);
+        }
+      }
+    }
+  } else {
+    static_assert(MODE == BUS_DIR, "bus_mac_kernel: unknown mode");
+    const int64_t ob = il * (int64_t)NH * J;
+    if constexpr (MAXB > 0) {
+      float2 g0[M], g1[M];
+#pragma unroll
+      for (int i = 0; i < M; ++i) {
+        g0[i] = g1[i] = zero;
+        if (i < I) gin(i, g0[i], g1[i]);
+      }
+      for (int p = 0; p < P; ++p) {
+        float2 xa[M], xb[M];
+#pragma unroll
+        for (int i = 0; i < M; ++i) {
+          xa[i] = xb[i] = zero;
+          if (i < I) pair(x, (int64_t)p * I + i, xa[i], xb[i]);
+        }
+        const bool two = 2 * p + 1 < S;
+#pragma unroll
+        for (int j = 0; j < M; ++j) {
+          if (j < J) {
+            float2 e00 = zero, e01 = zero, e10 = zero, e11 = zero;   // E_{2p+c, o} = e_co
+#pragma unroll
+            for (int i = 0; i + j < M; ++i) {
+              cfma_conj(e00, g0[j + i], xa[i]);
+              cfma_conj(e10, g0[j + i], xb[i]);
+              if (O == 2) { cfma_conj(e01, g1[j + i], xa[i]); cfma_conj(e11, g1[j + i], xb[i]); }
+            }
+            if (O == 2) {
+              emit(ob + (int64_t)(2 * p) * J + j, e00, e01);
+              if (two) emit(ob + (int64_t)(2 * p + 1) * J + j, e10, e11);
+            } else {
+              emit(ob + (int64_t)p * J + j, e00, two ? e10 : zero);
+            }
+          }
+        }
+      }
+    } else {
+      for (int p = 0; p < P; ++p) {
+        const bool two = 2 * p + 1 < S;
+        for (int j = 0; j < J; ++j) {
+          float2 e00 = zero, e01 = zero, e10 = zero, e11 = zero;
+          for (int i = 0; i + j < I; ++i) {
+            float2 g0v, g1v, xa, xb;
+            gin(j + i, g0v, g1v);
+            pair(x, (int64_t)p * I + i, xa, xb);
+            cfma_conj(e00, g0v, xa);
+            cfma_conj(e10, g0v, xb);
+            if (O == 2) { cfma_conj(e01, g1v, xa); cfma_conj(e11, g1v, xb); }
+          }
+          if (O == 2) {
+            emit(ob + (int64_t)(2 * p) * J + j, e00, e01);
+            if (two) emit(ob + (int64_t)(2 * p + 1) * J + j, e10, e11);
+          } else {
+            emit(ob + (int64_t)p * J + j, e00, two ? e10 : zero);
+          }
+        }
+      }
+    }
+  }
+}
+
+// inverse transforms of packed planar block spectra into row pairs, runs of kConvRun units (il, k, q), il < items,
+// k < groups, q < nblk: half `half` (0: the first, 1: the second kB outputs) of IFFT(Spl[unit]) is written as samples
+// [q kB, (q+1) kB) ∩ [0, lim) of rows 2k (real part) and 2k + 1 (imaginary part, if 2k + 1 < rows) of the `rows` rows
+// of length len of item item0 + il in dst.  The bus output and dL/dx (half 1, lim = len = n) and dL/dIR (half 0,
+// lim = leff, len = L).
+__global__ void __launch_bounds__(kFusedThreads, 1)
+bus_ifft_kernel(const float* __restrict__ Spl, const float* __restrict__ twiddles, float* __restrict__ dst, int64_t item0,
+                int rows, int groups, int nblk, int64_t len, int64_t lim, int half, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {
+    if (t == 0 && m < m1) s.load_planar(it, Spl + (int64_t)m * 2 * kNbA);
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    float xr[16], xi[16];
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    const int u = m / nblk, q = m - u * nblk;      // u = il * groups + k
+    const int64_t il = u / groups;
+    const int k = u - (int)il * groups;
+    const bool two = 2 * k + 1 < rows;
+    float* ra = dst + ((item0 + il) * rows + 2 * k) * len;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const int64_t tg = (int64_t)q * kB + t + 512 * c;
+      if (tg < lim) {
+        const float vr = half ? xr[c + 8] : xr[c], vi = half ? xi[c + 8] : xi[c];
+        ra[tg] = vr;
+        if (two) ra[len + tg] = vi;
+      }
+    }
+  }
+}
+
+__global__ void bus_ones_kernel(float* __restrict__ v, int64_t count) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < count) v[e] = 1.f;
+}
+
 // Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
 // spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
 // transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
@@ -2873,6 +3224,267 @@ int dasp_conv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_
                          int64_t chunk_items, void* stream) {
   return conv_op_bwd(true, gy, x, in_chs, ir_chs, ir_len, mix, xspec_save, irspec_save, gx, gir, gmix, workspace,
                      workspace_bytes, bs, n, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ convolution_bus
+// y[:, o] = sum_s x[:, s] * h[:, s, o] on the partitioned convolution of convolution_reverberation: the same blocks and
+// partitions, the same partition transform (x_fft_kernel on packed taps), the same fp64 sum of a shared IR's gradient
+// (irgrad_sum_kernel); the row-pair transforms, the products and the inverse transforms are the bus kernels above.
+namespace {
+int g_bus_last_path[2] = {0, 0};                     // test hook: dispatch of the last bus forward / backward
+
+struct BusGeom : ConvGeom {
+  int S, O;                     // input rows, output rows
+  int P, NH;                    // window spectra per block (ceil(S / 2)), IR partition sets (ceil(S O / 2))
+};
+struct BusWs { size_t ys, xsp, hsp, fwd_total; size_t gs, ds, es, ones, acc, bwd_total; };
+
+int make_bus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t S, int64_t O, int64_t chunk, BusGeom& g) {
+  DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "conv bus: 1 to %d inputs are supported, got %lld",
+               DASP_CONV_BUS_MAX_INPUTS, (long long)S);
+  DASP_REQUIRE(O == 1 || O == 2, "conv bus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
+  int rc = make_conv_geom(bs, n, L, chunk, g);
+  if (rc != DASP_OK) return rc;
+  g.shared = shared;
+  g.S = (int)S; g.O = (int)O;
+  g.P = (g.S + 1) / 2; g.NH = (g.S * g.O + 1) / 2;
+  return DASP_OK;
+}
+
+// every region is chunk-sized except the saved spectra (the caller's xspec_save / irspec_save when a backward follows)
+// and, shared, the per-item factors of irgrad_sum_kernel (ones, bs floats) and its fp64 sum
+void bus_layout(const BusGeom& g, BusWs& w) {
+  const size_t blk = sizeof(float2) * (size_t)kNbA;
+  const size_t c = (size_t)g.chunk, I = (size_t)g.ib, J = (size_t)g.jb;
+  size_t o = 0;
+  w.ys = o;  o += align256(blk * c * I);
+  w.xsp = o; o += align256(blk * c * g.P * I);
+  w.hsp = o; o += align256(blk * (g.shared ? 1 : c) * g.NH * J);
+  w.fwd_total = o;
+  o = 0;
+  w.gs = o;   o += align256(blk * c * I);
+  w.ds = o;   o += align256(blk * c * g.P * I);
+  w.es = o;   o += align256(blk * c * g.NH * J);
+  w.ones = o; o += align256(g.shared ? sizeof(float) * (size_t)g.bs : 0);
+  w.acc = o;  o += align256(g.shared ? sizeof(double2) * (size_t)kNbA * g.NH * J : 0);
+  w.bwd_total = o;
+}
+
+// register-cached products when both operand lists fit (MAXB 12 / 16), else from L2 (templates: C++ linkage)
+extern "C++" {
+template <int MODE, int O>
+void launch_bus_mac_o(const BusGeom& g, const float2* X, const float2* H, int64_t hstride, const float2* G, float2* Out,
+                      int64_t items, cudaStream_t st) {
+  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+  const int I = (int)g.ib, J = (int)g.jb, m = I > J ? I : J;
+  const float inv = 1.0f / (float)kNbA;
+  if (m <= 12)      bus_mac_kernel<12, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, g.S, I, J, inv);
+  else if (m <= 16) bus_mac_kernel<16, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, g.S, I, J, inv);
+  else              bus_mac_kernel<0, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, g.S, I, J, inv);
+}
+template <int MODE>
+int launch_bus_mac(const BusGeom& g, const float2* X, const float2* H, int64_t hstride, const float2* G, float2* Out,
+                   int64_t items, cudaStream_t st) {
+  if (g.O == 2) launch_bus_mac_o<MODE, 2>(g, X, H, hstride, G, Out, items, st);
+  else          launch_bus_mac_o<MODE, 1>(g, X, H, hstride, G, Out, items, st);
+  DASP_LAUNCH_OK("bus_mac_kernel");
+  return DASP_OK;
+}
+}  // extern "C++"
+bool bus_mac_cached(const BusGeom& g) { return (g.ib > g.jb ? g.ib : g.jb) <= 16; }
+
+int configure_bus_kernels() {
+  static std::map<int, bool> configured;
+  int rc = configure_fft_kernels();                  // x_fft_kernel transforms the partitions
+  if (rc != DASP_OK) return rc;
+  int dev = 0;
+  DASP_CUDA_OK(cudaGetDevice(&dev));
+  if (!configured[dev]) {
+    DASP_CUDA_OK(cudaFuncSetAttribute(bus_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(bus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    configured[dev] = true;
+  }
+  return DASP_OK;
+}
+
+unsigned runs(int64_t units) { return (unsigned)((units + kConvRun - 1) / kConvRun); }
+
+int conv_bus_geometry(bool shared, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O, int64_t chunk_items,
+                      dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "conv bus geometry: null out");
+  BusGeom g;
+  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  BusWs w;
+  bus_layout(g, w);
+  out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
+  out->xspec_c64 = g.bs * g.P * g.ib * kNbA;
+  out->irspec_c64 = (shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.NH * g.jb * kNbA;
+  out->fwd_workspace_bytes = (int64_t)w.fwd_total;
+  out->bwd_workspace_bytes = (int64_t)w.bwd_total;
+  return DASP_OK;
+}
+
+// The rows must allow the bulk copies of bus_fft_kernel: n % 4 == 0 and 16-byte aligned x / gy (the Python op pads).
+int conv_bus_fwd(bool shared, const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O,
+                 int64_t chunk_items, void* stream) {
+  BusGeom g;
+  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(x && ir && y && workspace, "conv bus fwd: null pointer");
+  DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "conv bus fwd: pass both *_save buffers or neither");
+  DASP_REQUIRE(n % 4 == 0 && aligned16(x), "conv bus fwd: x needs n %% 4 == 0 and 16-byte aligned rows, got n=%lld",
+               (long long)n);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  BusWs w;
+  bus_layout(g, w);
+  if ((rc = check_workspace("conv bus fwd", w.fwd_total, workspace_bytes)) != DASP_OK) return rc;
+  if ((rc = configure_bus_kernels()) != DASP_OK) return rc;
+  const float* tw = nullptr;
+  if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+  unsigned char* base = (unsigned char*)workspace;
+  float2* ys = (float2*)(base + w.ys);
+  const int I = (int)g.ib, J = (int)g.jb;
+  const int64_t h_stride = shared ? 0 : g.NH * J * (int64_t)kNbA;
+  float2* const hs0 = irspec_save ? (float2*)irspec_save : (float2*)(base + w.hsp);
+
+  // the IR partition spectra of IRs [item0, item0 + items) in hs: taps packed by row pairs, then transformed in place
+  auto fill_ir = [&](float2* hs, int64_t item0, int64_t items) -> int {
+    bus_ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, (unsigned)g.NH), 256, 0, st>>>(
+        ir, hs, item0, g.S * g.O, J, g.L, g.leff);
+    DASP_LAUNCH_OK("bus_ir_pack_kernel");
+    const int nparts = (int)(items * g.NH * J);
+    x_fft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(nullptr, nullptr, hs, tw, 0, I, J, g.n, g.leff, 1,
+                                                                     0, nparts);
+    DASP_LAUNCH_OK("x_fft_kernel");
+    return DASP_OK;
+  };
+  g_bus_last_path[0] = 1 | (shared ? 2 : 0) | (bus_mac_cached(g) ? 4 : 0);
+  if (shared && (rc = fill_ir(hs0, 0, 1)) != DASP_OK) return rc;
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    float2* xs = xspec_save ? (float2*)xspec_save + item0 * g.P * I * (int64_t)kNbA : (float2*)(base + w.xsp);
+    float2* hs = (irspec_save && !shared) ? hs0 + item0 * h_stride : hs0;
+    if (!shared && (rc = fill_ir(hs, item0, items)) != DASP_OK) return rc;
+    const int nwin = (int)(items * g.P * I), nblk = (int)(items * I);
+    bus_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, g.S, g.P, I, g.n, 0, nwin);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    if ((rc = launch_bus_mac<BUS_FWD>(g, xs, hs, h_stride, nullptr, ys, items, st)) != DASP_OK) return rc;
+    bus_ifft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y, item0,
+                                                                      g.O, 1, I, g.n, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+  }
+  return DASP_OK;
+}
+
+int conv_bus_bwd(bool shared, const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O,
+                 int64_t chunk_items, void* stream) {
+  BusGeom g;
+  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  if (bs == 0) return DASP_OK;
+  DASP_REQUIRE(gy && xspec_save && irspec_save && gx && workspace, "conv bus bwd: null pointer");
+  DASP_REQUIRE(n % 4 == 0 && aligned16(gy), "conv bus bwd: gy needs n %% 4 == 0 and 16-byte aligned rows, got n=%lld",
+               (long long)n);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  BusWs w;
+  bus_layout(g, w);
+  if ((rc = check_workspace("conv bus bwd", w.bwd_total, workspace_bytes)) != DASP_OK) return rc;
+  if ((rc = configure_bus_kernels()) != DASP_OK) return rc;
+  const float* tw = nullptr;
+  if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+  unsigned char* base = (unsigned char*)workspace;
+  float2* gs = (float2*)(base + w.gs);
+  float2* ds = (float2*)(base + w.ds);
+  float2* es = (float2*)(base + w.es);
+  float* ones = (float*)(base + w.ones);
+  double2* acc = (double2*)(base + w.acc);
+  const int I = (int)g.ib, J = (int)g.jb, R = g.S * g.O;
+  const int64_t h_stride = shared ? 0 : g.NH * J * (int64_t)kNbA;
+  const int64_t per_ir = g.NH * J * (int64_t)kNbA;
+  // bit 0: own FFT, bit 1: register-cached products, bit 2: dL/dIR computed, bit 3: one IR shared by the batch
+  g_bus_last_path[1] = 1 | (bus_mac_cached(g) ? 2 : 0) | (gir ? 4 : 0) | (shared ? 8 : 0);
+  if (shared && gir) {
+    bus_ones_kernel<<<(unsigned)((bs + 255) / 256), 256, 0, st>>>(ones, bs);
+    DASP_LAUNCH_OK("bus_ones_kernel");
+  }
+  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
+    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+    const float2* xs = (const float2*)xspec_save + item0 * g.P * I * (int64_t)kNbA;
+    const float2* hs = (const float2*)irspec_save + item0 * h_stride;
+    const int nblk = (int)(items * I), nwin = (int)(items * g.P * I);
+    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, g.O, 1, I, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    if ((rc = launch_bus_mac<BUS_DX>(g, xs, hs, h_stride, gs, ds, items, st)) != DASP_OK) return rc;
+    bus_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx, item0,
+                                                                      g.S, g.P, I, g.n, g.n, 1, nwin);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    if (!gir) continue;                              // a fixed IR: no dL/dIR work at all
+    if ((rc = launch_bus_mac<BUS_DIR>(g, xs, hs, 0, gs, es, items, st)) != DASP_OK) return rc;
+    if (shared) {
+      irgrad_sum_kernel<<<(unsigned)((per_ir + 255) / 256), 256, 0, st>>>(es, ones, acc, item0, (int)items, per_ir,
+                                                                          item0 + items == bs);
+      DASP_LAUNCH_OK("irgrad_sum_kernel");
+    } else {
+      const int nparts = (int)(items * g.NH * J);
+      bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir,
+                                                                          item0, R, g.NH, J, g.L, g.leff, 0, nparts);
+      DASP_LAUNCH_OK("bus_ifft_kernel");
+    }
+  }
+  if (!gir) return DASP_OK;
+  if (shared) {                                      // the summed spectra, in item 0's slots of es
+    const int nparts = (int)(g.NH * J);
+    bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir, 0,
+                                                                        R, g.NH, J, g.L, g.leff, 0, nparts);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+  }
+  if (g.L > g.leff) {                                // taps that reach no output sample
+    DASP_CUDA_OK(cudaMemset2DAsync(gir + g.leff, sizeof(float) * g.L, 0, sizeof(float) * (g.L - g.leff),
+                                   (size_t)((shared ? 1 : bs) * R), st));
+  }
+  return DASP_OK;
+}
+}  // namespace
+
+int dasp_debug_conv_bus_last_path(int which) { return g_bus_last_path[which ? 1 : 0]; }
+
+int dasp_conv_bus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t shared,
+                           int64_t chunk_items, dasp_conv_geom* out) {
+  return conv_bus_geometry(shared != 0, bs, n, ir_len, inputs, outputs, chunk_items, out);
+}
+
+int dasp_conv_bus_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                      int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs,
+                      int64_t chunk_items, void* stream) {
+  return conv_bus_fwd(false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, inputs,
+                      outputs, chunk_items, stream);
+}
+
+int dasp_conv_bus_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                      void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs,
+                      int64_t outputs, int64_t chunk_items, void* stream) {
+  return conv_bus_bwd(false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, inputs,
+                      outputs, chunk_items, stream);
+}
+
+int dasp_conv_bus_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                             int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
+  return conv_bus_fwd(true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, inputs,
+                      outputs, chunk_items, stream);
+}
+
+int dasp_conv_bus_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                             int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
+  return conv_bus_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, inputs,
+                      outputs, chunk_items, stream);
 }
 
 // ------------------------------------------------------------------ noise_shaped_impulse_response

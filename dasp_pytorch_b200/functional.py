@@ -36,6 +36,7 @@ __all__ = [
     "expander_gain",
     "noise_shaped_reverberation",
     "convolution_reverberation",
+    "convolution_bus",
     "noise_shaped_impulse_response",
     "noise_shaped_impulse_response_packed",
     "parametric_eq_frequency_response",
@@ -1381,3 +1382,136 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
     m = _param(mix, bs, xf, "mix", allow_broadcast=True).contiguous()
     y = _ConvReverbFn.apply(xf, irf, m, reverb_chunk_items(xf.device))
     return y.to(dt)
+
+
+# --------------------------------------------------------------------------------------
+# convolution_bus
+# --------------------------------------------------------------------------------------
+
+CONV_BUS_MAX_INPUTS = 32      # DASP_CONV_BUS_MAX_INPUTS in include/dasp_b200.h
+
+
+class _ConvBusFn(torch.autograd.Function):
+    """x (bs, S, n), ir (bs | 1, S, O, L) -> y (bs, O, n).  n % 4 == 0 and 16-byte aligned rows (convolution_bus pads).
+    An ir of batch 1 with bs > 1 runs the dasp_conv_bus_shared_* entry points; its gradient is the sum over the items."""
+
+    @staticmethod
+    def forward(ctx, x, ir, chunk):
+        lib = _abi.lib()
+        bs, S, n = x.shape
+        ir_bs, _, O, ir_len = ir.shape
+        shared = ir_bs == 1 and bs > 1
+        kind = "conv_bus_shared" if shared else "conv_bus"
+        dev = x.device
+        y = torch.empty(bs, O, n, dtype=torch.float32, device=dev)
+        need_bwd = any(ctx.needs_input_grad[:2])
+        geom = _abi.ConvGeom()
+        with torch.cuda.device(dev):
+            check(lib.dasp_conv_bus_geometry(bs, n, ir_len, S, O, int(shared), chunk, geom), "dasp_conv_bus_geometry")
+            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
+            xspec = irspec = None
+            if need_bwd:
+                xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
+                irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
+            with _timed("conv_bus_fwd", dev):
+                check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), ptr(ir), ptr(y), ptr(xspec), ptr(irspec), ptr(ws),
+                                                       ws.numel(), bs, n, ir_len, S, O, chunk, stream_ptr(dev)),
+                      f"dasp_{kind}_fwd")
+        if need_bwd:
+            ctx.save_for_backward(xspec, irspec)
+        ctx.cfg = (kind, bs, S, O, n, ir.shape, chunk, geom.bwd_workspace_bytes)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _abi.lib()
+        xspec, irspec = ctx.saved_tensors
+        kind, bs, S, O, n, ir_shape, chunk, bwd_bytes = ctx.cfg
+        dev = gy.device
+        gy = gy.contiguous()
+        if gy.data_ptr() % 16:
+            gy = gy.clone()
+        gx = torch.empty(bs, S, n, dtype=torch.float32, device=dev)
+        # a fixed IR (measured rooms, a fixed downmix) skips every dL/dIR kernel
+        gir = torch.empty(ir_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev), _timed("conv_bus_bwd", dev):
+            check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(xspec), ptr(irspec), ptr(gx), ptr(gir), ptr(ws),
+                                                   ws.numel(), bs, n, ir_shape[3], S, O, chunk, stream_ptr(dev)),
+                  f"dasp_{kind}_bwd")
+        return gx, gir, None
+
+
+def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor):
+    """Any number of input channels, each convolved with its own impulse responses and summed into one mono or stereo
+    bus::
+
+        y[:, o] = sum_s (x[:, s] * h[:, s, o])[:n]
+
+    (``*`` the causal convolution cropped to ``n``, exactly as ``convolution_reverberation`` defines its wet signal).
+    Uses: reverberant multi-source mixtures (each speaker or noise source through the room impulse response of its
+    own position), binaural or stereo downmixes of 5.1 / 7.1 audio through one set of BRIRs shared by the batch,
+    multitrack mixing with a room per stem, and a learnable S-input FIR trained through its taps.
+
+    Args:
+        x: audio ``(bs, S, n)``, ``1 <= S <= CONV_BUS_MAX_INPUTS`` input channels (sources, stems, speaker feeds).
+        sample_rate: unused (kept for the common processor signature).
+        impulse_response: ``(bs, S, O, L)``, one IR set per item, or ``(1, S, O, L)``, one set shared by the batch;
+            ``O`` is 1 (mono bus) or 2 (stereo bus), any ``L >= 1``.  Row ``(s, o)`` is the path from input ``s`` to
+            output ``o``.
+
+    Returns ``(bs, O, n)`` in x's dtype, computed in fp32.  There is no dry/wet mix: the inputs and the outputs differ
+    in number, so no dry signal is defined; a caller who wants one adds it to the result.
+
+    Identities (held to fp32 rounding):
+
+    1. ``S = 2, O = 2``: ``convolution_reverberation(x, sr, h.reshape(bs, 4, L), mix=1)``, whose true-stereo row
+       order ``2 i + o`` is this layout.
+    2. ``S = 1, O = 2``: ``convolution_reverberation(x, sr, h[:, 0], mix=1)``.
+    3. Any ``S``: the sum over ``s`` of ``convolution_bus(x[:, s:s+1], sr, h[:, s:s+1])``.
+
+    Gradients flow to ``x`` (every input) and to every IR row; taps at or beyond ``n`` reach no output and get exactly
+    0.  The gradient of a shared ``(1, S, O, L)`` IR has that shape and is the sum over the items, accumulated in fp64
+    in item order, so it does not depend on ``REVERB_CHUNK_ITEMS``.  When the IR does not require a gradient, the
+    backward skips all dL/dIR work.  The convolution is ``convolution_reverberation``'s (4096-sample partitions, the
+    in-shared-memory 8192-point FFT) with the rows of every signal packed two per transform: one window transform per
+    pair of inputs and block, and one inverse transform per block for the whole bus.  Rows whose length is not a
+    multiple of 4 are zero-padded to one (the transforms bulk-copy 16-byte rows); a padding sample reaches no output
+    sample below ``n``.
+    """
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
+    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 4:
+        raise ValueError("impulse_response must be a tensor of shape (batch, inputs, outputs, taps)")
+    bs, S, n = x.shape
+    if not 1 <= S <= CONV_BUS_MAX_INPUTS:
+        raise ValueError(f"convolution_bus: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, got {S}")
+    ir_bs, ir_s, O, L = impulse_response.shape
+    if ir_s != S:
+        raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
+    if O not in (1, 2):
+        raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
+    if ir_bs != bs and not (ir_bs == 1 and bs > 1):
+        raise ValueError(f"impulse_response has batch {ir_bs}, x has batch {bs} (expected {bs} or 1)")
+    if L < 1:
+        raise ValueError("impulse_response needs at least one tap")
+    if n < 1:
+        raise ValueError("x needs at least one sample")
+    xf, dt = _audio(x)
+    if not impulse_response.is_cuda:
+        raise DaspError(f"impulse_response is on {impulse_response.device}: dasp_pytorch_b200 only runs on CUDA (H100) "
+                        "tensors and has no CPU path")
+    if impulse_response.device != xf.device:
+        raise DaspError(f"impulse_response is on {impulse_response.device} but x is on {xf.device}")
+    if not impulse_response.is_floating_point():
+        raise DaspError(f"impulse_response must be a floating-point tensor, got {impulse_response.dtype}")
+    irf = impulse_response.to(torch.float32).contiguous()
+    n4 = (n + 3) // 4 * 4
+    if n4 != n:
+        xf = torch.nn.functional.pad(xf, (0, n4 - n))
+        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
+            irf = irf[..., :n].contiguous()
+    elif xf.data_ptr() % 16:
+        xf = xf.clone()
+    y = _ConvBusFn.apply(xf, irf, reverb_chunk_items(xf.device))
+    return (y[..., :n] if n4 != n else y).to(dt)

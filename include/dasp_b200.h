@@ -320,6 +320,40 @@ int dasp_conv_shared_ts_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t 
    bit 1 = fused correlation kernel, bit 2 = dL/dIR computed, bit 3 = shared IR, bit 4 = true-stereo IR */
 int dasp_debug_conv_last_path(int which);
 
+/* ---- convolution_bus: S input rows, each through its own impulse responses, summed into a mono or stereo bus ------
+ * x is (bs, S, n), ir is (bs, S, O, ir_len) (or ONE (S, O, ir_len) IR set for the whole batch: the *_shared_* entry
+ * points), y is (bs, O, n), with 1 <= S <= DASP_CONV_BUS_MAX_INPUTS inputs and O = 1 or 2 outputs:
+ *   y[b, o] = sum_s (x[b, s] * ir[b, s, o])[:n]   (* the causal convolution, as convolution_reverberation's wet signal)
+ * There is no dry/wet mix: inputs and outputs differ in number, so no dry signal is defined.
+ * The convolution is convolution_reverberation's (conv_block-sample partitions, the same FFT), with the rows of every
+ * signal packed two per transform: ceil(S / 2) window spectra per block, ceil(S O / 2) partition sets per IR.
+ * n % 4 == 0 and 16-byte aligned x / gy rows are required (the transforms bulk-copy them).
+ * Buffers kept for the backward (NULL for both when no backward follows): xspec_save geom.xspec_c64 and irspec_save
+ * geom.irspec_c64 complex64.  Backward: gx (bs, S, n); gir (bs, S, O, ir_len) (shared: (S, O, ir_len), the sum over
+ * the items in fp64 in item order, the same bits for every chunk_items), or NULL, which skips all dL/dIR work; taps
+ * >= leff = min(ir_len, n) get 0.  Workspace sizes come from dasp_conv_bus_geometry (shared != 0 for the shared entry
+ * points), which needs no GPU.  Bad S, O or shapes are rejected before any CUDA call. */
+#define DASP_CONV_BUS_MAX_INPUTS 32
+int dasp_conv_bus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t shared,
+                           int64_t chunk_items, dasp_conv_geom* out);
+int dasp_conv_bus_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                      int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs,
+                      int64_t chunk_items, void* stream);
+int dasp_conv_bus_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                      float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                      int64_t ir_len, int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream);
+int dasp_conv_bus_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                             int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream);
+int dasp_conv_bus_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                             float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
+                             int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t chunk_items,
+                             void* stream);
+/* test hook: dispatch of the most recent bus call.  which = 0 (forward): bit 0 = own in-shared-memory FFT (always),
+   bit 1 = shared IR, bit 2 = register-cached products.  which = 1 (backward): bit 0 = own FFT (always), bit 1 =
+   register-cached products, bit 2 = dL/dIR computed, bit 3 = shared IR */
+int dasp_debug_conv_bus_last_path(int which);
+
 #ifdef __cplusplus
 }
 #endif

@@ -32,15 +32,17 @@
 // convolution_reverberation is the audio convolution with the caller's IR (ir_pack_kernel fills the partitions).  The
 // convolution is written once on the host: conv_fwd_chunk / conv_bwd_chunk run a chunk for both ops, on one ConvGeom,
 // one plan set (conv_setup) and one workspace layout per direction; each op adds only its IR fill, its mix stride and
-// its dL/dIR consumer.  One IR for the whole batch (dasp_conv_shared_*) is the item stride 0 of the IR spectra: they
-// are transformed once, and irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.  A
-// true-stereo IR (ir_chs 4) is two partition sets per IR (ConvGeom::sets), multiplied by the TS variants of the MAC
-// kernels.
+// its dL/dIR consumer.  A true-stereo IR (ir_chs 4) is two partition sets per IR (ConvGeom::sets), multiplied by the TS
+// variants of the MAC kernels.
 //
 // convolution_bus (dasp_conv_bus_*) is the same partitioned convolution for S inputs summed into O = 1 or 2 outputs:
-// every signal's rows are packed two per transform (bus_fft_kernel, bus_ir_pack_kernel + x_fft_kernel's partition
-// units), bus_mac_kernel sums the untangled products over the inputs, and bus_ifft_kernel writes the outputs, dL/dx and
-// dL/dIR; a shared IR's gradient goes through irgrad_sum_kernel.
+// every signal's rows are packed two per transform (bus_fft_kernel, ir_pack_kernel + x_fft_kernel's partition units),
+// bus_mac_kernel sums the untangled products over the inputs, and bus_ifft_kernel writes the outputs, dL/dx and dL/dIR.
+//
+// Both ops whose IR the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd: checks,
+// workspace, IR packing, chunk loop, zeros of the unreachable dL/dIR taps).  One IR for the whole batch
+// (dasp_conv_shared_*, dasp_conv_bus_shared_*) is the item stride 0 of the IR spectra: they are transformed once, and
+// irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.
 //
 // noise_shaped_impulse_response (dasp_nsir_*) is the IR synthesis without the convolution, with the geometry of the
 // reverb at n = L.  Every synthesis kernel is a template on its output sink (PartitionSink: the convolution's partition
@@ -125,14 +127,17 @@ void octave_filterbank(int taps, double sr, std::vector<float>& out) {
 }
 
 // ------------------------------------------------------------------ geometry
-// the partitioned audio convolution, shared by the reverb and convolution_reverberation
+// the partitioned audio convolution, shared by the reverb, convolution_reverberation and convolution_bus
 struct ConvGeom {
   int64_t bs, n, L;
   int64_t leff;                 // min(L, n): the only IR taps that can reach the output
   int64_t ib, jb;               // output/input blocks of kB samples, IR partitions of kB taps
   int64_t chunk;
-  bool shared = false;          // one impulse response for the whole batch (convolution_reverberation only)
-  int sets = 1;                 // partition sets per IR: 2 for a true-stereo IR (convolution_reverberation only)
+  bool shared = false;          // one impulse response for the whole batch (the ops whose IR the caller supplies)
+  int p = 1;                    // window spectra per block: ceil(S / 2) for the bus
+  int sets = 1;                 // partition sets per IR: 2 for a true-stereo IR, ceil(S O / 2) for the bus
+  bool has_mix = true;          // a dry/wet mix, and with it the dL/dmix partials region (not the bus)
+  bool own_only = false;        // the own FFT only: no cuFFT plans or work area, no dasp_debug_reverb_path(1) (the bus)
 };
 
 int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
@@ -1773,19 +1778,21 @@ __global__ void nsir_params_kernel(const float* __restrict__ p24, float* __restr
 // ifft_dx_kernel as in the reverb; dL/dIR partition j = mix * first half of IFFT(sum_p G[j+p] conj(X[p])), unpacked into
 // the caller's rows by ifft_irtaps_kernel (or irtaps_unpack_kernel after the cuFFT inverse).
 
-// taps t < leff of the planar (bs, ir_chs, L) rows -> (left, right) pairs in the first half of partition slot t / kB
-// (a mono IR feeds both channels).  A true-stereo IR (ir_chs 4, rows L->L, L->R, R->L, R->R) fills two partition sets
-// per item: set s = gridDim.z index packs rows 2s and 2s + 1 into the slots of (il * 2 + s).
-// grid = (ceil(leff / 256), items, 1 or 2 sets)
+// taps t < leff of the planar (bs, rows, L) rows -> (row 2s, row 2s + 1) pairs in the first half of partition slot
+// t / kB of set s = gridDim.z index, i.e. of slot (il * sets + s).  An odd last row pairs with itself when odd_self (a
+// mono IR of convolution_reverberation feeds both channels), else with 0 (the bus).  A true-stereo IR (rows L->L, L->R,
+// R->L, R->R) fills two sets per item.  grid = (ceil(leff / 256), items, sets)
 __global__ void ir_pack_kernel(const float* __restrict__ ir, float2* __restrict__ Hb, int64_t item0, int J, int64_t L,
-                               int64_t leff, int ir_chs) {
+                               int64_t leff, int rows, bool odd_self) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t il = blockIdx.y;
   const int s = blockIdx.z;
   if (t >= leff) return;
-  const float* rl = ir + ((item0 + il) * ir_chs + 2 * s) * L;
-  const float* rr = ir_chs == 1 ? rl : rl + L;
-  Hb[ir_slot(il * gridDim.z + s, J, t)] = make_float2(rl[t], rr[t]);
+  const bool pair = 2 * s + 1 < rows;
+  const float* ra = ir + ((item0 + il) * rows + 2 * s) * L;
+  const float* rb = pair ? ra + L : ra;
+  const float im = rb[t];                          // loaded either way: both loads issue together
+  Hb[ir_slot(il * gridDim.z + s, J, t)] = make_float2(ra[t], pair || odd_self ? im : 0.f);
 }
 
 // unit m = (il*sets + s)*J + j: dL/dIR taps [j kB, (j+1) kB) ∩ [0, leff) = mix * first half of IFFT(Epl[m]) (left,
@@ -1828,33 +1835,29 @@ ifft_irtaps_kernel(const float* __restrict__ Epl, const float* __restrict__ twid
   }
 }
 
-// dL/dIR taps [t0, L) of the caller's rows: mix * Et (inverse-transformed partitions, pairs in the first half of each
-// slot) below leff, 0 from leff on (those taps cannot reach an output).  t0 = leff writes only the zeros.  A null mix is
-// a factor of 1.  Partition set s (gridDim.z = 2 for a true-stereo IR) goes to rows 2s, 2s + 1.
-// grid = (ceil((L - t0) / 256), items, 1 or 2 sets)
+// dL/dIR taps [0, leff) of the caller's rows: mix * Et (inverse-transformed partitions, pairs in the first half of each
+// slot).  A null mix is a factor of 1.  Partition set s (gridDim.z = 2 for a true-stereo IR) goes to rows 2s, 2s + 1.
+// grid = (ceil(leff / 256), items, 1 or 2 sets)
 __global__ void irtaps_unpack_kernel(const float2* __restrict__ Et, const float* __restrict__ mix, float* __restrict__ gir,
-                                     int64_t item0, int J, int64_t L, int64_t leff, int ir_chs, int64_t t0) {
-  const int64_t t = t0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+                                     int64_t item0, int J, int64_t L, int64_t leff, int ir_chs) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t il = blockIdx.y, b = item0 + il;
   const int s = blockIdx.z;
-  if (t >= L) return;
-  float2 v = make_float2(0.f, 0.f);
-  float mx = 0.f;
-  if (t < leff) {
-    v = Et[ir_slot(il * gridDim.z + s, J, t)];
-    mx = mix ? mix[b] : 1.f;
-  }
+  if (t >= leff) return;
+  const float2 v = Et[ir_slot(il * gridDim.z + s, J, t)];
+  const float mx = mix ? mix[b] : 1.f;
   float* row = gir + (b * ir_chs + 2 * s) * L;
   if (ir_chs == 1) row[t] = mx * (v.x + v.y);
   else { row[t] = mx * v.x; row[L + t] = mx * v.y; }
 }
 
-// dL/dIR of one impulse response shared by the batch: the sum over items b of mix[b] E_b, taken on the partition spectra
-// E_b of the es region before any inverse transform (the inverse is linear).  Element by element in fp64 and in absolute
-// item order: a product of two floats is exact in fp64, so every element goes through the same sequence of additions
-// however the batch is cut into chunks, and the result is the same bits for every chunk size.  Item 0 writes acc instead
-// of adding to it (the workspace is never cleared); the chunk that holds the last item writes the sum, rounded to fp32,
-// over item 0's slot of Et instead, for the inverse transforms (thread e alone reads and writes element e of every slot).
+// dL/dIR of one impulse response shared by the batch: the sum over items b of mix[b] E_b (a null mix: factors of 1),
+// taken on the partition spectra E_b of the es region before any inverse transform (the inverse is linear).  Element by
+// element in fp64 and in absolute item order: a product of two floats is exact in fp64, so every element goes through
+// the same sequence of additions however the batch is cut into chunks, and the result is the same bits for every chunk
+// size.  Item 0 writes acc instead of adding to it (the workspace is never cleared); the chunk that holds the last item
+// writes the sum, rounded to fp32, over item 0's slot of Et instead, for the inverse transforms (thread e alone reads
+// and writes element e of every slot).
 // Element-wise, so it serves the planar (own FFT) and the interleaved (cuFFT) spectra alike.
 // grid = ceil(sets J kNbA / 256), one complex element of the sets * J partitions per thread
 __global__ void irgrad_sum_kernel(float2* Et, const float* __restrict__ mix, double2* __restrict__ acc, int64_t item0,
@@ -1867,13 +1870,13 @@ __global__ void irgrad_sum_kernel(float2* Et, const float* __restrict__ mix, dou
     a = acc[e];
   } else {                                         // item 0: written, not added
     const float2 v = Et[e];
-    const double m = (double)mix[0];
+    const double m = mix ? (double)mix[0] : 1.0;
     a = make_double2(m * (double)v.x, m * (double)v.y);
     il = 1;
   }
   for (; il < items; ++il) {
     const float2 v = Et[il * per_item + e];
-    const double m = (double)mix[item0 + il];
+    const double m = mix ? (double)mix[item0 + il] : 1.0;
     a.x += m * (double)v.x;
     a.y += m * (double)v.y;
   }
@@ -1952,18 +1955,6 @@ bus_fft_kernel(const float* __restrict__ src, float2* __restrict__ out, const fl
 #pragma unroll
     for (int q = 0; q < 16; ++q) o[t + 512 * q] = make_float2(xr[q], xi[q]);
   }
-}
-
-// IR taps t < leff of row pairs (2k, 2k + 1) of the (rows, L) rows of item item0 + il -> (re, im) pairs in the first
-// half of partition slot t / kB of set k (an odd last row packs with 0).  grid = (ceil(leff / 256), items, NH sets)
-__global__ void bus_ir_pack_kernel(const float* __restrict__ ir, float2* __restrict__ Hb, int64_t item0, int rows, int J,
-                                   int64_t L, int64_t leff) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t il = blockIdx.y;
-  const int k = blockIdx.z;
-  if (t >= leff) return;
-  const float* ra = ir + ((item0 + il) * rows + 2 * k) * L;
-  Hb[ir_slot(il * gridDim.z + k, J, t)] = make_float2(ra[t], 2 * k + 1 < rows ? ra[L + t] : 0.f);
 }
 
 // The products of the bus on the block spectra, per bin pair (f, kNbA - f) and item.  Every operand is untangled into
@@ -2232,11 +2223,6 @@ bus_ifft_kernel(const float* __restrict__ Spl, const float* __restrict__ twiddle
   }
 }
 
-__global__ void bus_ones_kernel(float* __restrict__ v, int64_t count) {
-  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e < count) v[e] = 1.f;
-}
-
 // Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
 // spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
 // transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
@@ -2455,8 +2441,9 @@ bool dispatch_fused(int R, const float2* H1, const float* tw, const float* param
 inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // workspace carve-up shared by the geometry queries and the entry points; extra: the reverb's own region (the filtered
-// noise of a chunk when f_save is not kept / the per-partition partials of the 24 band-parameter gradients); acc: the
-// fp64 sum of a shared IR's dL/dIR partition spectra (0 bytes unless g.shared)
+// noise of a chunk when f_save is not kept / the per-partition partials of the 24 band-parameter gradients); mixpart:
+// the dL/dmix partials (0 bytes without a mix); acc: the fp64 sum of a shared IR's dL/dIR partition spectra (0 bytes
+// unless g.shared)
 struct FwdWs { size_t ys, xsp, hsp, extra, cufft, total; };
 struct BwdWs { size_t gs, ds, es, extra, mixpart, acc, cufft, total; };
 
@@ -2464,7 +2451,7 @@ void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs&
   size_t o = 0;
   w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
   // transient homes for what a forward WITHOUT a backward does not keep (null *_save pointers)
-  w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.p * g.ib * kNbA));
   w.hsp = o; o += align256(sizeof(float2) * (size_t)((g.shared ? 1 : g.chunk) * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.cufft = o; o += align256(cufft_work);
@@ -2473,10 +2460,10 @@ void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs&
 void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs& w) {
   size_t o = 0;
   w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
-  w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.p * g.ib * kNbA));
   w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
-  w.mixpart = o; o += align256(sizeof(float) * (size_t)(g.chunk * g.ib));
+  w.mixpart = o; o += align256(g.has_mix ? sizeof(float) * (size_t)(g.chunk * g.ib) : 0);
   w.acc = o; o += align256(g.shared ? sizeof(double2) * (size_t)(g.sets * g.jb * kNbA) : 0);
   w.cufft = o; o += align256(cufft_work);
   w.total = o;
@@ -2486,7 +2473,7 @@ void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs&
 // largest work area.  xi / hj: the block transforms of the convolution's cuFFT pipeline (audio / dL/dx windows, IR /
 // dL/dIR partitions).  With synth (the reverb) also blk / pp, its IR synthesis (overlap-save blocks, polyphase), and
 // the extra regions.  With g.shared also ir1: the J partitions of the one IR (forward) and of its summed gradient.
-// Every IR plan transforms g.sets partition sets of J partitions per IR.
+// Every IR plan transforms g.sets partition sets of J partitions per IR.  g.own_only: no plans and no work area.
 struct Plans { PlanVal xi, hj, blk, pp; };
 // blk / pp for a chunk of `items`; work: raised to their largest work area
 int synth_plans(const Geom& g, int64_t items, Plans& p, size_t& work) {
@@ -2501,12 +2488,12 @@ struct Setup { Plans full, rem; PlanVal ir1; FwdWs fwd; BwdWs bwd; };
 int conv_setup(const ConvGeom& g, const Geom* synth, Setup& s) {
   int rc;
   size_t work = 0;
-  if (g.shared && g.bs > 0) {
+  if (g.shared && g.bs > 0 && !g.own_only) {
     if ((rc = get_plan(2, kNbA, g.sets * g.jb, kNbA, kNbA, s.ir1)) != DASP_OK) return rc;
     work = s.ir1.work;
   }
   for (int64_t items : {g.bs > 0 ? g.chunk : 0, g.bs % g.chunk}) {
-    if (items == 0) continue;
+    if (items == 0 || g.own_only) continue;
     Plans& p = items == g.chunk ? s.full : s.rem;
     if ((rc = get_plan(2, kNbA, items * g.ib, kNbA, kNbA, p.xi)) != DASP_OK) return rc;
     if ((rc = get_plan(2, kNbA, items * g.sets * g.jb, kNbA, kNbA, p.hj)) != DASP_OK) return rc;
@@ -2541,7 +2528,7 @@ int put_conv_geometry(const ConvGeom& g, const Geom* synth, Out* out) {
   int rc = conv_setup(g, synth, s);
   if (rc != DASP_OK) return rc;
   out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
-  out->xspec_c64 = g.bs * g.ib * kNbA;
+  out->xspec_c64 = g.bs * g.p * g.ib * kNbA;
   out->irspec_c64 = (g.shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.sets * g.jb * kNbA;
   out->fwd_workspace_bytes = (int64_t)s.fwd.total;
   out->bwd_workspace_bytes = (int64_t)s.bwd.total;
@@ -2561,6 +2548,8 @@ void launch_mac(const float2* A, const float2* Bm, float2* Out, int na, int nbm,
 
 // grid of a persistent FFT kernel: one CTA per SM, at most one per unit of work
 unsigned persistent_grid(int64_t units) { return (unsigned)(units < sm_count() ? units : sm_count()); }
+// grid of an FFT kernel that gives each CTA a run of kConvRun units
+unsigned runs(int64_t units) { return (unsigned)((units + kConvRun - 1) / kConvRun); }
 
 // one-off opt-in to the large dynamic shared memory of the FFT kernels (per device, guarded by g_mu)
 int configure_fft_kernels() {
@@ -2578,6 +2567,8 @@ int configure_fft_kernels() {
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irtaps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(bus_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(bus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     configured[dev] = true;
   }
   return DASP_OK;
@@ -2605,27 +2596,23 @@ bool fused_corr(IrGrad e, int I, int J, int sets) {
   return e == IrGrad::kPlanar && (I > J ? I : J) <= (sets == 2 ? kTsFusedMaxB : 16);
 }
 
-// The partitions of an impulse response shared by the batch, transformed in place in hs once before the first chunk,
-// filled as conv_fwd_chunk expects them; own: x_fft_kernel with no audio windows, otherwise the J-batch cuFFT C2C.
-int conv_shared_ir_spectra(const ConvGeom& g, const PlanVal& ir1, bool own, const float* tw, float2* hs,
-                           unsigned char* ws, const FwdWs& w, cudaStream_t st) {
-  const int J = (int)g.jb, nparts = g.sets * J;
-  if (own) {
-    int rc = configure_fft_kernels();
-    if (rc != DASP_OK) return rc;
-    x_fft_kernel<<<(unsigned)((nparts + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
-        nullptr, nullptr, hs, tw, 0, (int)g.ib, J, g.n, g.leff, 1, 0, nparts);
-    DASP_LAUNCH_OK("x_fft_kernel");
-    return DASP_OK;
-  }
-  return exec_c2c(ir1, ws + w.cufft, hs, CUFFT_FORWARD, st);
+// The partitions of `irs` impulse responses in hs (g.sets J per IR), transformed in place on the own FFT: x_fft_kernel
+// with no audio windows.  A shared IR's before the first chunk; the bus's per chunk, in a launch of their own.
+int ir_partition_spectra(const ConvGeom& g, const float* tw, float2* hs, int64_t irs, cudaStream_t st) {
+  int rc = configure_fft_kernels();
+  if (rc != DASP_OK) return rc;
+  const int nparts = (int)(irs * g.sets * g.jb);
+  x_fft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(nullptr, nullptr, hs, tw, 0, (int)g.ib, (int)g.jb,
+                                                                   g.n, g.leff, 1, 0, nparts);
+  DASP_LAUNCH_OK("x_fft_kernel");
+  return DASP_OK;
 }
 
 // y = (1 - mix) x + mix (x * IR), mix of item b at mix[b * mix_stride].  The caller has written IR taps t < leff as
 // (left, right) pairs into the first half of partition slot t / kB of hs, and on the cuFFT pipeline zero-filled the
 // slots first.  xs / hs receive the window / partition spectra.  own (own_fft_rows of x and hs): x_fft_kernel transforms
 // both on the own FFT with the tables tw; otherwise cuFFT C2C does.  h_stride: item stride of hs in complex elements,
-// g.sets J kNbA; 0 for one IR shared by the batch, whose partitions conv_shared_ir_spectra has transformed already.
+// g.sets J kNbA; 0 for one IR shared by the batch, whose partitions the caller has transformed already.
 // g.sets == 2 (a true-stereo IR): hs holds set A then set B per IR, and the product is partition_mac_kernel<TS 1>.
 // xs_ready (own only): the caller has already transformed the chunk's windows into xs.
 int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, int in_chs, float2* xs,
@@ -2642,15 +2629,15 @@ int conv_fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw
     const int nwin = xs_ready ? 0 : nblk;
     const int nunits = nwin + (int)(h_stride != 0 ? items * g.sets * J : 0);
     if (nunits > 0) {
-      x_fft_kernel<<<(unsigned)((nunits + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
-          x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs, nwin, nunits);
+      x_fft_kernel<<<runs(nunits), kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs,
+                                                                        nwin, nunits);
       DASP_LAUNCH_OK("x_fft_kernel");
     }
     if (g.sets == 2) launch_mac<false, true, 1>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
     else             launch_mac<false, true>(xs, hs, ys, I, J, h_stride != 0, I, items, 1.0f / (float)kNbA, st);
     DASP_LAUNCH_OK("partition_mac_kernel");
-    ifft_mix_kernel<<<(unsigned)((nblk + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
-                                                                   mix_stride, y, item0, I, g.n, in_chs, nblk);
+    ifft_mix_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix,
+                                                                     mix_stride, y, item0, I, g.n, in_chs, nblk);
     DASP_LAUNCH_OK("ifft_mix_kernel");
     return DASP_OK;
   }
@@ -2948,8 +2935,8 @@ int dasp_reverb_fwd(const float* x, int64_t in_chs, const float* params, const f
     if (windows_first && k == 0) {
       if ((rc = configure_fft_kernels()) != DASP_OK) return rc;
       const int nwin = (int)(bs * I);
-      x_fft_kernel<<<(unsigned)((nwin + kConvRun - 1) / kConvRun), kFusedThreads, kFftSmemBytes, st>>>(
-          x, (float2*)xspec_save, nullptr, tw, 0, I, J, g.n, g.leff, (int)in_chs, nwin, nwin);
+      x_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, (float2*)xspec_save, nullptr, tw, 0, I, J, g.n,
+                                                                     g.leff, (int)in_chs, nwin, nwin);
       DASP_LAUNCH_OK("x_fft_kernel");
     }
     if (pipelined) {
@@ -3021,161 +3008,220 @@ int dasp_reverb_bwd(const float* gy, const float* x, int64_t in_chs, const float
   return DASP_OK;
 }
 
-// ------------------------------------------------------------------ convolution_reverberation
+// ------------------------------------------------------------------ convolution_reverberation and convolution_bus
+// The ops whose impulse response the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd):
+// the argument checks, the lock, the workspace, the *_save buffers or their transient workspace slots, the IR taps
+// packed into their partition slots (ir_pack_kernel), and the chunk loop.  One IR for the whole batch (g.shared) is the
+// item stride 0 of the IR spectra: packed and transformed once before the first chunk; in the backward,
+// irgrad_sum_kernel sums the items' dL/dIR partition spectra in fp64 (factor mix[b], or 1 without a mix) and the sum is
+// transformed once after the last chunk.  dL/dIR taps [leff, L) reach no output and get their zeros from one memset
+// after the chunk loop.  The op (ConvOp, BusOp) supplies only its IR rows (ir_rows per item, packed two per partition
+// set; kOddSelf: an odd last row pairs with itself, else with 0), its products per chunk (fwd_chunk; bwd_chunk, which
+// leaves the dL/dIR partitions in the es region in the form e) and the inverse transform of those partitions into the
+// caller's rows (ir_taps, with the factor mix[b] or none).
 namespace {
 int g_conv_last_path[2] = {0, 0};                    // test hook: dispatch of the last conv forward / backward
+int g_bus_last_path[2] = {0, 0};                     // test hook: dispatch of the last bus forward / backward
 
-// The bodies of dasp_conv_* (one IR per item) and dasp_conv_shared_* (one IR for the whole batch).  Shared, the IR's
-// partitions are filled and transformed once before the first chunk and every item reads the same spectra (item stride
-// 0); the backward sums mix[b] times each item's dL/dIR partition spectra in fp64 (irgrad_sum_kernel) and transforms
-// the sum once after the last chunk.  A true-stereo IR (ir_chs 4) is two partition sets per IR (g.sets = 2), carried
-// through the same routines.
-int conv_op_geometry(bool shared, int sets, int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items,
-                     dasp_conv_geom* out) {
-  DASP_REQUIRE(out != nullptr, "conv geometry: null out");
-  ConvGeom g;
-  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
-  if (rc != DASP_OK) return rc;
-  g.shared = shared;
-  g.sets = sets;
-  return put_conv_geometry(g, nullptr, out);
-}
-int ir_sets(int64_t ir_chs) { return ir_chs == 4 ? 2 : 1; }
-
-int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,
-                const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
-                int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
-  ConvGeom g;
-  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
-  if (rc != DASP_OK) return rc;
-  g.shared = shared;
-  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2 || ir_chs == 4),
-               "conv: only mono/stereo signals and mono/stereo/true-stereo IRs");
-  g.sets = ir_sets(ir_chs);
-  if (bs == 0) return DASP_OK;
-  DASP_REQUIRE(x && ir && mix && y && workspace, "conv fwd: null pointer");
-  DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "conv fwd: pass both *_save buffers or neither");
+extern "C++" {
+template <class Op>
+int caller_ir_fwd(const Op& op, const ConvGeom& g, const float* x, const float* ir, const float* mix, float* y,
+                  void* xspec_save, void* irspec_save, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (g.bs == 0) return DASP_OK;
+  DASP_REQUIRE(x && ir && (mix || !g.has_mix) && y && workspace, "%s: null pointer", Op::kFwd);
+  DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "%s: pass both *_save buffers or neither",
+               Op::kFwd);
+  DASP_REQUIRE(!g.own_only || (g.n % 4 == 0 && aligned16(x)),
+               "%s: x needs n %% 4 == 0 and 16-byte aligned rows, got n=%lld", Op::kFwd, (long long)g.n);
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> lk(g_mu);
   Setup s{};
-  if ((rc = conv_setup(g, nullptr, s)) != DASP_OK) return rc;
-  if ((rc = check_workspace("conv fwd", s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
+  int rc = conv_setup(g, nullptr, s);
+  if (rc != DASP_OK) return rc;
+  if ((rc = check_workspace(Op::kFwd, s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
   const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
-  const int I = (int)g.ib, J = (int)g.jb, S = g.sets;
-  const int64_t h_stride = shared ? 0 : S * J * (int64_t)kNbA;
+  const int I = (int)g.ib, J = (int)g.jb;
+  const int64_t h_stride = g.shared ? 0 : g.sets * J * (int64_t)kNbA;
   float2* const hs0 = irspec_save ? (float2*)irspec_save : (float2*)(base + w.hsp);
   const float* tw = nullptr;
 
   // IR taps t < leff of items [item0, item0 + items) into their partition slots; the cuFFT transform of the partitions
   // reads whole slots, x_fft_kernel only the taps ir_pack_kernel writes
   auto fill_ir = [&](float2* hs, bool own, int64_t item0, int64_t items) -> int {
-    if (!own) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * S * J * kNbA, st));
-    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, (unsigned)S), 256, 0, st>>>(
-        ir, hs, item0, J, g.L, g.leff, (int)ir_chs);
+    if (!own) DASP_CUDA_OK(cudaMemsetAsync(hs, 0, sizeof(float2) * items * g.sets * J * kNbA, st));
+    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, (unsigned)g.sets), 256, 0, st>>>(
+        ir, hs, item0, J, g.L, g.leff, op.ir_rows, Op::kOddSelf);
     DASP_LAUNCH_OK("ir_pack_kernel");
     return DASP_OK;
   };
-  if (shared) {
-    const bool own = own_fft_rows(n, x, hs0);
+  if (g.shared) {
+    const bool own = g.own_only || own_fft_rows(g.n, x, hs0);
     if ((rc = fill_ir(hs0, own, 0, 1)) != DASP_OK) return rc;
     if (own && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    if ((rc = conv_shared_ir_spectra(g, s.ir1, own, tw, hs0, base, w, st)) != DASP_OK) return rc;
+    rc = own ? ir_partition_spectra(g, tw, hs0, 1, st) : exec_c2c(s.ir1, base + w.cufft, hs0, CUFFT_FORWARD, st);
+    if (rc != DASP_OK) return rc;
   }
-  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
-    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
+  for (int64_t item0 = 0; item0 < g.bs; item0 += g.chunk) {
+    const int64_t items = (g.bs - item0 < g.chunk) ? g.bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? s.full : s.rem;
-    float2* xs = xspec_save ? (float2*)xspec_save + item0 * I * (int64_t)kNbA : (float2*)(base + w.xsp);
+    float2* xs = xspec_save ? (float2*)xspec_save + item0 * g.p * I * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? hs0 + item0 * h_stride : hs0;
-    const bool own_conv = own_fft_rows(n, x, hs);
-    g_conv_last_path[0] = (own_conv ? 1 : 0) | (shared ? 2 : 0) | (S == 2 ? 4 : 0);
-    if (!shared && (rc = fill_ir(hs, own_conv, item0, items)) != DASP_OK) return rc;
-    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    if ((rc = conv_fwd_chunk(g, pl, own_conv, tw, x, (int)in_chs, xs, hs, h_stride, mix, 1, y, base, w, item0, items,
-                             st)) != DASP_OK)
+    const bool own = g.own_only || own_fft_rows(g.n, x, hs);
+    if (!g.shared && (rc = fill_ir(hs, own, item0, items)) != DASP_OK) return rc;
+    if (own && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    if ((rc = op.fwd_chunk(g, pl, own, tw, x, mix, xs, hs, h_stride, y, base, w, item0, items, st)) != DASP_OK)
       return rc;
   }
   return DASP_OK;
+}
+
+// x and mix (and gmix) only with g.has_mix: the backward needs x for the dL/dmix partials alone
+template <class Op>
+int caller_ir_bwd(const Op& op, const ConvGeom& g, const float* gy, const float* x, const float* mix,
+                  const void* xspec_save, const void* irspec_save, float* gx, float* gir, float* gmix, void* workspace,
+                  int64_t workspace_bytes, void* stream) {
+  if (g.bs == 0) return DASP_OK;
+  DASP_REQUIRE(gy && xspec_save && irspec_save && gx && workspace && (!g.has_mix || (x && mix && gmix)),
+               "%s: null pointer", Op::kBwd);
+  DASP_REQUIRE(!g.own_only || (g.n % 4 == 0 && aligned16(gy)),
+               "%s: gy needs n %% 4 == 0 and 16-byte aligned rows, got n=%lld", Op::kBwd, (long long)g.n);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(g_mu);
+  Setup s{};
+  int rc = conv_setup(g, nullptr, s);
+  if (rc != DASP_OK) return rc;
+  if ((rc = check_workspace(Op::kBwd, s.bwd.total, workspace_bytes)) != DASP_OK) return rc;
+  const BwdWs& w = s.bwd;
+  unsigned char* base = (unsigned char*)workspace;
+  float2* ws_es = (float2*)(base + w.es);
+  const float* ws_mixpart = (const float*)(base + w.mixpart);
+  double2* ws_acc = (double2*)(base + w.acc);
+  const int I = (int)g.ib, J = (int)g.jb;
+  const int64_t per_ir = g.sets * J * (int64_t)kNbA;
+  const int64_t h_stride = g.shared ? 0 : per_ir;
+  const float* tw = nullptr;
+  bool own = false;
+
+  for (int64_t item0 = 0; item0 < g.bs; item0 += g.chunk) {
+    const int64_t items = (g.bs - item0 < g.chunk) ? g.bs - item0 : g.chunk;
+    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
+    const float2* xs = (const float2*)xspec_save + item0 * g.p * I * (int64_t)kNbA;
+    const float2* hs = (const float2*)irspec_save + item0 * h_stride;
+    own = g.own_only || own_fft_rows(g.n, gy, nullptr);
+    const IrGrad e = gir == nullptr ? IrGrad::kNone
+                                    : (own ? IrGrad::kPlanar : (g.shared ? IrGrad::kSpectra : IrGrad::kTime));
+    if (own && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
+    rc = op.bwd_chunk(g, pl, own, e, tw, gy, x, mix, xs, hs, h_stride, gx, base, w, item0, items, st);
+    if (rc != DASP_OK) return rc;
+    if (e != IrGrad::kNone && g.shared) {
+      irgrad_sum_kernel<<<(unsigned)((per_ir + 255) / 256), 256, 0, st>>>(ws_es, mix, ws_acc, item0, (int)items,
+                                                                          per_ir, item0 + items == g.bs);
+      DASP_LAUNCH_OK("irgrad_sum_kernel");
+    } else if (e != IrGrad::kNone && (rc = op.ir_taps(g, own, tw, ws_es, mix, gir, item0, items, st)) != DASP_OK) {
+      return rc;
+    }
+    if (g.has_mix) {
+      conv_mix_grad_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(ws_mixpart, gmix, item0, items, I);
+      DASP_LAUNCH_OK("conv_mix_grad_kernel");
+    }
+  }
+  if (!gir) return DASP_OK;
+  if (g.shared) {
+    // the summed partition spectra, rounded to fp32 in item 0's slots of es: sets J inverse transforms for the one IR
+    if (!own && (rc = exec_c2c(s.ir1, base + w.cufft, ws_es, CUFFT_INVERSE, st)) != DASP_OK) return rc;
+    if ((rc = op.ir_taps(g, own, tw, ws_es, nullptr, gir, 0, 1, st)) != DASP_OK) return rc;
+  }
+  if (g.L > g.leff) {
+    DASP_CUDA_OK(cudaMemset2DAsync(gir + g.leff, sizeof(float) * g.L, 0, sizeof(float) * (g.L - g.leff),
+                                   (size_t)((g.shared ? 1 : g.bs) * op.ir_rows), st));
+  }
+  return DASP_OK;
+}
+}  // extern "C++"
+
+// convolution_reverberation: y = (1 - mix) x + mix (x * IR) on conv_fwd_chunk / conv_bwd_chunk.  x is mono or stereo;
+// the IR mono (feeding both channels), stereo, or true-stereo (ir_chs 4: two partition sets per IR, g.sets = 2).
+struct ConvOp {
+  static constexpr const char* kFwd = "conv fwd";
+  static constexpr const char* kBwd = "conv bwd";
+  static constexpr bool kOddSelf = true;
+  int in_chs, ir_rows;
+  int fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, const float* mix,
+                float2* xs, float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    g_conv_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (g.sets == 2 ? 4 : 0);
+    return conv_fwd_chunk(g, pl, own, tw, x, in_chs, xs, hs, h_stride, mix, 1, y, ws, w, item0, items, st);
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const float* tw, const float* gy,
+                const float* x, const float* mix, const float2* xs, const float2* hs, int64_t h_stride, float* gx,
+                unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed, bit 3: one IR shared by the batch, bit 4: a
+    // true-stereo IR
+    g_conv_last_path[1] = (own ? 1 : 0) | (fused_corr(e, (int)g.ib, (int)g.jb, g.sets) ? 2 : 0) |
+                          (e != IrGrad::kNone ? 4 : 0) | (g.shared ? 8 : 0) | (g.sets == 2 ? 16 : 0);
+    return conv_bwd_chunk(g, pl, own, e, tw, gy, x, in_chs, xs, hs, h_stride, mix, 1, gx, ws, w, item0, items, st);
+  }
+  // dL/dIR taps [0, leff) of IRs [item0, item0 + items) from their partitions in es: planar spectra (own), or
+  // time-domain pairs after the inverse cuFFT
+  int ir_taps(const ConvGeom& g, bool own, const float* tw, const float2* es, const float* mix, float* gir,
+              int64_t item0, int64_t items, cudaStream_t st) const {
+    const int J = (int)g.jb;
+    if (own) {
+      const int nunits = (int)(items * g.sets * J);
+      ifft_irtaps_kernel<<<persistent_grid(nunits), kFusedThreads, kFftSmemBytes, st>>>(
+          reinterpret_cast<const float*>(es), tw, mix, gir, item0, J, g.sets, g.L, g.leff, ir_rows, nunits);
+      DASP_LAUNCH_OK("ifft_irtaps_kernel");
+    } else {
+      irtaps_unpack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, (unsigned)g.sets), 256, 0, st>>>(
+          es, mix, gir, item0, J, g.L, g.leff, ir_rows);
+      DASP_LAUNCH_OK("irtaps_unpack_kernel");
+    }
+    return DASP_OK;
+  }
+};
+
+// the geometry and argument checks of dasp_conv_* (one IR per item) and dasp_conv_shared_* (one IR for the batch)
+int ir_sets(int64_t ir_chs) { return ir_chs == 4 ? 2 : 1; }
+int conv_op_geom(bool shared, int sets, int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items, ConvGeom& g) {
+  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  g.shared = shared;
+  g.sets = sets;
+  return DASP_OK;
+}
+int conv_op_geometry(bool shared, int sets, int64_t bs, int64_t n, int64_t ir_len, int64_t chunk_items,
+                     dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "conv geometry: null out");
+  ConvGeom g;
+  int rc = conv_op_geom(shared, sets, bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
+}
+int check_conv_chs(int64_t in_chs, int64_t ir_chs) {
+  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2 || ir_chs == 4),
+               "conv: only mono/stereo signals and mono/stereo/true-stereo IRs");
+  return DASP_OK;
+}
+
+int conv_op_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len,
+                const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = conv_op_geom(shared, ir_sets(ir_chs), bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK || (rc = check_conv_chs(in_chs, ir_chs)) != DASP_OK) return rc;
+  return caller_ir_fwd(ConvOp{(int)in_chs, (int)ir_chs}, g, x, ir, mix, y, xspec_save, irspec_save, workspace,
+                       workspace_bytes, stream);
 }
 
 int conv_op_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len,
                 const float* mix, const void* xspec_save, const void* irspec_save, float* gx, float* gir, float* gmix,
                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_conv_geom(bs, n, ir_len, chunk_items, g);
-  if (rc != DASP_OK) return rc;
-  g.shared = shared;
-  DASP_REQUIRE((in_chs == 1 || in_chs == 2) && (ir_chs == 1 || ir_chs == 2 || ir_chs == 4),
-               "conv: only mono/stereo signals and mono/stereo/true-stereo IRs");
-  g.sets = ir_sets(ir_chs);
-  if (bs == 0) return DASP_OK;
-  DASP_REQUIRE(gy && x && mix && xspec_save && irspec_save && gx && gmix && workspace, "conv bwd: null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  std::lock_guard<std::mutex> lk(g_mu);
-  Setup s{};
-  if ((rc = conv_setup(g, nullptr, s)) != DASP_OK) return rc;
-  if ((rc = check_workspace("conv bwd", s.bwd.total, workspace_bytes)) != DASP_OK) return rc;
-  const BwdWs& w = s.bwd;
-  unsigned char* base = (unsigned char*)workspace;
-  float2* ws_es = (float2*)(base + w.es);
-  const float* ws_mixpart = (const float*)(base + w.mixpart);
-  double2* ws_acc = (double2*)(base + w.acc);
-  const int I = (int)g.ib, J = (int)g.jb, S = g.sets;
-  const int64_t h_stride = shared ? 0 : S * J * (int64_t)kNbA;
-  const float* tw = nullptr;
-  bool own_conv = false;
-
-  // dL/dIR taps of items [item0, item0 + items) from their partitions in the es region (planar spectra, or time-domain
-  // pairs after the inverse cuFFT), times mix[b] (a null mix: 1)
-  auto ir_taps = [&](IrGrad e, int64_t item0, int64_t items, const float* mx) -> int {
-    if (e == IrGrad::kPlanar) {
-      const int nunits = (int)(items * S * J);
-      ifft_irtaps_kernel<<<persistent_grid(nunits), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ws_es), tw, mx,
-                                                                        gir, item0, J, S, g.L, g.leff, (int)ir_chs, nunits);
-      DASP_LAUNCH_OK("ifft_irtaps_kernel");
-    }
-    // taps t0 <= t < L: the zeros from leff on after ifft_irtaps_kernel, every tap after the cuFFT inverse
-    const int64_t t0 = e == IrGrad::kPlanar ? g.leff : 0;
-    if (g.L > t0) {
-      irtaps_unpack_kernel<<<dim3((unsigned)((g.L - t0 + 255) / 256), (unsigned)items, (unsigned)S), 256, 0, st>>>(
-          ws_es, mx, gir, item0, J, g.L, g.leff, (int)ir_chs, t0);
-      DASP_LAUNCH_OK("irtaps_unpack_kernel");
-    }
-    return DASP_OK;
-  };
-  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
-    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const Plans& pl = (items == g.chunk) ? s.full : s.rem;
-    const float2* xs = (const float2*)xspec_save + item0 * I * (int64_t)kNbA;
-    const float2* hs = (const float2*)irspec_save + item0 * h_stride;
-    own_conv = own_fft_rows(n, gy, nullptr);
-    const IrGrad e = gir == nullptr ? IrGrad::kNone
-                                    : (own_conv ? IrGrad::kPlanar : (shared ? IrGrad::kSpectra : IrGrad::kTime));
-    // bit 0: own FFT, bit 1: fused correlations, bit 2: dL/dIR computed, bit 3: one IR shared by the batch, bit 4: a
-    // true-stereo IR
-    g_conv_last_path[1] = (own_conv ? 1 : 0) | (fused_corr(e, I, J, S) ? 2 : 0) | (gir ? 4 : 0) | (shared ? 8 : 0) |
-                          (S == 2 ? 16 : 0);
-    if (own_conv && (rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-    if ((rc = conv_bwd_chunk(g, pl, own_conv, e, tw, gy, x, (int)in_chs, xs, hs, h_stride, mix, 1, gx, base, w, item0,
-                             items, st)) != DASP_OK)
-      return rc;
-    if (e != IrGrad::kNone && shared) {
-      const int64_t per_item = S * J * (int64_t)kNbA;
-      irgrad_sum_kernel<<<(unsigned)((per_item + 255) / 256), 256, 0, st>>>(ws_es, mix, ws_acc, item0, (int)items,
-                                                                            per_item, item0 + items == bs);
-      DASP_LAUNCH_OK("irgrad_sum_kernel");
-    } else if (e != IrGrad::kNone && (rc = ir_taps(e, item0, items, mix)) != DASP_OK) {
-      return rc;
-    }
-    conv_mix_grad_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(ws_mixpart, gmix, item0, items, I);
-    DASP_LAUNCH_OK("conv_mix_grad_kernel");
-  }
-  if (shared && gir) {
-    // the summed partition spectra, rounded to fp32 in item 0's slots of es: S J inverse transforms for the one IR
-    if (!own_conv && (rc = exec_c2c(s.ir1, base + w.cufft, ws_es, CUFFT_INVERSE, st)) != DASP_OK) return rc;
-    if ((rc = ir_taps(own_conv ? IrGrad::kPlanar : IrGrad::kTime, 0, 1, nullptr)) != DASP_OK) return rc;
-  }
-  return DASP_OK;
+  int rc = conv_op_geom(shared, ir_sets(ir_chs), bs, n, ir_len, chunk_items, g);
+  if (rc != DASP_OK || (rc = check_conv_chs(in_chs, ir_chs)) != DASP_OK) return rc;
+  return caller_ir_bwd(ConvOp{(int)in_chs, (int)ir_chs}, g, gy, x, mix, xspec_save, irspec_save, gx, gir, gmix,
+                       workspace, workspace_bytes, stream);
 }
 }  // namespace
 
@@ -3227,228 +3273,120 @@ int dasp_conv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_
 }
 
 // ------------------------------------------------------------------ convolution_bus
-// y[:, o] = sum_s x[:, s] * h[:, s, o] on the partitioned convolution of convolution_reverberation: the same blocks and
-// partitions, the same partition transform (x_fft_kernel on packed taps), the same fp64 sum of a shared IR's gradient
-// (irgrad_sum_kernel); the row-pair transforms, the products and the inverse transforms are the bus kernels above.
+// y[:, o] = sum_s x[:, s] * h[:, s, o] through the stage above on the own FFT only: P = ceil(S / 2) window spectra per
+// block (g.p) and NH = ceil(S O / 2) partition sets per IR (g.sets), no mix.  The row-pair transforms, the products and
+// the inverse transforms are the bus kernels; the IR partitions go through x_fft_kernel's partition units.
 namespace {
-int g_bus_last_path[2] = {0, 0};                     // test hook: dispatch of the last bus forward / backward
+// register-cached products when both operand lists fit (MAXB 12 / 16), else from L2 (templates: C++ linkage)
+extern "C++" {
+template <int MODE, int O>
+void launch_bus_mac_o(const ConvGeom& g, int S, const float2* X, const float2* H, int64_t hstride, const float2* G,
+                      float2* Out, int64_t items, cudaStream_t st) {
+  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+  const int I = (int)g.ib, J = (int)g.jb, m = I > J ? I : J;
+  const float inv = 1.0f / (float)kNbA;
+  if (m <= 12)      bus_mac_kernel<12, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, inv);
+  else if (m <= 16) bus_mac_kernel<16, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, inv);
+  else              bus_mac_kernel<0, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, inv);
+}
+template <int MODE>
+int launch_bus_mac(const ConvGeom& g, int S, int O, const float2* X, const float2* H, int64_t hstride, const float2* G,
+                   float2* Out, int64_t items, cudaStream_t st) {
+  if (O == 2) launch_bus_mac_o<MODE, 2>(g, S, X, H, hstride, G, Out, items, st);
+  else        launch_bus_mac_o<MODE, 1>(g, S, X, H, hstride, G, Out, items, st);
+  DASP_LAUNCH_OK("bus_mac_kernel");
+  return DASP_OK;
+}
+}  // extern "C++"
+bool bus_mac_cached(const ConvGeom& g) { return (g.ib > g.jb ? g.ib : g.jb) <= 16; }
 
-struct BusGeom : ConvGeom {
-  int S, O;                     // input rows, output rows
-  int P, NH;                    // window spectra per block (ceil(S / 2)), IR partition sets (ceil(S O / 2))
+struct BusOp {
+  static constexpr const char* kFwd = "conv bus fwd";
+  static constexpr const char* kBwd = "conv bus bwd";
+  static constexpr bool kOddSelf = false;
+  int S, O, ir_rows;                                 // inputs, outputs, IR rows S O
+  int fwd_chunk(const ConvGeom& g, const Plans&, bool own, const float* tw, const float* x, const float*, float2* xs,
+                float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    g_bus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (bus_mac_cached(g) ? 4 : 0);
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    if (h_stride != 0 && (rc = ir_partition_spectra(g, tw, hs, items, st)) != DASP_OK) return rc;
+    float2* ys = (float2*)(ws + w.ys);
+    const int I = (int)g.ib, nwin = (int)(items * g.p * I), nblk = (int)(items * I);
+    bus_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, S, g.p, I, g.n, 0, nwin);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    if ((rc = launch_bus_mac<BUS_FWD>(g, S, O, xs, hs, h_stride, nullptr, ys, items, st)) != DASP_OK) return rc;
+    bus_ifft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y, item0,
+                                                                      O, 1, I, g.n, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    return DASP_OK;
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans&, bool own, IrGrad e, const float* tw, const float* gy, const float*,
+                const float*, const float2* xs, const float2* hs, int64_t h_stride, float* gx, unsigned char* ws,
+                const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    // bit 0: own FFT, bit 1: register-cached products, bit 2: dL/dIR computed, bit 3: one IR shared by the batch
+    g_bus_last_path[1] = (own ? 1 : 0) | (bus_mac_cached(g) ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) |
+                         (g.shared ? 8 : 0);
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* gs = (float2*)(ws + w.gs);
+    float2* ds = (float2*)(ws + w.ds);
+    const int I = (int)g.ib, nblk = (int)(items * I), nwin = (int)(items * g.p * I);
+    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, O, 1, I, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    if ((rc = launch_bus_mac<BUS_DX>(g, S, O, xs, hs, h_stride, gs, ds, items, st)) != DASP_OK) return rc;
+    bus_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx, item0,
+                                                                      S, g.p, I, g.n, g.n, 1, nwin);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    if (e == IrGrad::kNone) return DASP_OK;          // a fixed IR: no dL/dIR work at all
+    return launch_bus_mac<BUS_DIR>(g, S, O, xs, hs, 0, gs, (float2*)(ws + w.es), items, st);
+  }
+  // dL/dIR taps [0, leff) of IRs [item0, item0 + items): the first half of the inverse of each partition
+  int ir_taps(const ConvGeom& g, bool, const float* tw, const float2* es, const float*, float* gir, int64_t item0,
+              int64_t items, cudaStream_t st) const {
+    const int J = (int)g.jb, nparts = (int)(items * g.sets * J);
+    bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir,
+                                                                        item0, ir_rows, g.sets, J, g.L, g.leff, 0,
+                                                                        nparts);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    return DASP_OK;
+  }
 };
-struct BusWs { size_t ys, xsp, hsp, fwd_total; size_t gs, ds, es, ones, acc, bwd_total; };
 
-int make_bus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t S, int64_t O, int64_t chunk, BusGeom& g) {
+// the bus's argument checks, filling its geometry
+int make_bus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t S, int64_t O, int64_t chunk, ConvGeom& g) {
   DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "conv bus: 1 to %d inputs are supported, got %lld",
                DASP_CONV_BUS_MAX_INPUTS, (long long)S);
   DASP_REQUIRE(O == 1 || O == 2, "conv bus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
   int rc = make_conv_geom(bs, n, L, chunk, g);
   if (rc != DASP_OK) return rc;
   g.shared = shared;
-  g.S = (int)S; g.O = (int)O;
-  g.P = (g.S + 1) / 2; g.NH = (g.S * g.O + 1) / 2;
+  g.p = (int)(S + 1) / 2;
+  g.sets = (int)(S * O + 1) / 2;
+  g.has_mix = false;
+  g.own_only = true;
   return DASP_OK;
 }
 
-// every region is chunk-sized except the saved spectra (the caller's xspec_save / irspec_save when a backward follows)
-// and, shared, the per-item factors of irgrad_sum_kernel (ones, bs floats) and its fp64 sum
-void bus_layout(const BusGeom& g, BusWs& w) {
-  const size_t blk = sizeof(float2) * (size_t)kNbA;
-  const size_t c = (size_t)g.chunk, I = (size_t)g.ib, J = (size_t)g.jb;
-  size_t o = 0;
-  w.ys = o;  o += align256(blk * c * I);
-  w.xsp = o; o += align256(blk * c * g.P * I);
-  w.hsp = o; o += align256(blk * (g.shared ? 1 : c) * g.NH * J);
-  w.fwd_total = o;
-  o = 0;
-  w.gs = o;   o += align256(blk * c * I);
-  w.ds = o;   o += align256(blk * c * g.P * I);
-  w.es = o;   o += align256(blk * c * g.NH * J);
-  w.ones = o; o += align256(g.shared ? sizeof(float) * (size_t)g.bs : 0);
-  w.acc = o;  o += align256(g.shared ? sizeof(double2) * (size_t)kNbA * g.NH * J : 0);
-  w.bwd_total = o;
-}
-
-// register-cached products when both operand lists fit (MAXB 12 / 16), else from L2 (templates: C++ linkage)
-extern "C++" {
-template <int MODE, int O>
-void launch_bus_mac_o(const BusGeom& g, const float2* X, const float2* H, int64_t hstride, const float2* G, float2* Out,
-                      int64_t items, cudaStream_t st) {
-  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
-  const int I = (int)g.ib, J = (int)g.jb, m = I > J ? I : J;
-  const float inv = 1.0f / (float)kNbA;
-  if (m <= 12)      bus_mac_kernel<12, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, g.S, I, J, inv);
-  else if (m <= 16) bus_mac_kernel<16, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, g.S, I, J, inv);
-  else              bus_mac_kernel<0, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, g.S, I, J, inv);
-}
-template <int MODE>
-int launch_bus_mac(const BusGeom& g, const float2* X, const float2* H, int64_t hstride, const float2* G, float2* Out,
-                   int64_t items, cudaStream_t st) {
-  if (g.O == 2) launch_bus_mac_o<MODE, 2>(g, X, H, hstride, G, Out, items, st);
-  else          launch_bus_mac_o<MODE, 1>(g, X, H, hstride, G, Out, items, st);
-  DASP_LAUNCH_OK("bus_mac_kernel");
-  return DASP_OK;
-}
-}  // extern "C++"
-bool bus_mac_cached(const BusGeom& g) { return (g.ib > g.jb ? g.ib : g.jb) <= 16; }
-
-int configure_bus_kernels() {
-  static std::map<int, bool> configured;
-  int rc = configure_fft_kernels();                  // x_fft_kernel transforms the partitions
-  if (rc != DASP_OK) return rc;
-  int dev = 0;
-  DASP_CUDA_OK(cudaGetDevice(&dev));
-  if (!configured[dev]) {
-    DASP_CUDA_OK(cudaFuncSetAttribute(bus_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
-    DASP_CUDA_OK(cudaFuncSetAttribute(bus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
-    configured[dev] = true;
-  }
-  return DASP_OK;
-}
-
-unsigned runs(int64_t units) { return (unsigned)((units + kConvRun - 1) / kConvRun); }
-
-int conv_bus_geometry(bool shared, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O, int64_t chunk_items,
-                      dasp_conv_geom* out) {
-  DASP_REQUIRE(out != nullptr, "conv bus geometry: null out");
-  BusGeom g;
-  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
-  if (rc != DASP_OK) return rc;
-  BusWs w;
-  bus_layout(g, w);
-  out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
-  out->xspec_c64 = g.bs * g.P * g.ib * kNbA;
-  out->irspec_c64 = (shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.NH * g.jb * kNbA;
-  out->fwd_workspace_bytes = (int64_t)w.fwd_total;
-  out->bwd_workspace_bytes = (int64_t)w.bwd_total;
-  return DASP_OK;
-}
-
-// The rows must allow the bulk copies of bus_fft_kernel: n % 4 == 0 and 16-byte aligned x / gy (the Python op pads).
 int conv_bus_fwd(bool shared, const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
                  void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O,
                  int64_t chunk_items, void* stream) {
-  BusGeom g;
+  ConvGeom g;
   int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
   if (rc != DASP_OK) return rc;
-  if (bs == 0) return DASP_OK;
-  DASP_REQUIRE(x && ir && y && workspace, "conv bus fwd: null pointer");
-  DASP_REQUIRE((xspec_save == nullptr) == (irspec_save == nullptr), "conv bus fwd: pass both *_save buffers or neither");
-  DASP_REQUIRE(n % 4 == 0 && aligned16(x), "conv bus fwd: x needs n %% 4 == 0 and 16-byte aligned rows, got n=%lld",
-               (long long)n);
-  cudaStream_t st = (cudaStream_t)stream;
-  std::lock_guard<std::mutex> lk(g_mu);
-  BusWs w;
-  bus_layout(g, w);
-  if ((rc = check_workspace("conv bus fwd", w.fwd_total, workspace_bytes)) != DASP_OK) return rc;
-  if ((rc = configure_bus_kernels()) != DASP_OK) return rc;
-  const float* tw = nullptr;
-  if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-  unsigned char* base = (unsigned char*)workspace;
-  float2* ys = (float2*)(base + w.ys);
-  const int I = (int)g.ib, J = (int)g.jb;
-  const int64_t h_stride = shared ? 0 : g.NH * J * (int64_t)kNbA;
-  float2* const hs0 = irspec_save ? (float2*)irspec_save : (float2*)(base + w.hsp);
-
-  // the IR partition spectra of IRs [item0, item0 + items) in hs: taps packed by row pairs, then transformed in place
-  auto fill_ir = [&](float2* hs, int64_t item0, int64_t items) -> int {
-    bus_ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, (unsigned)g.NH), 256, 0, st>>>(
-        ir, hs, item0, g.S * g.O, J, g.L, g.leff);
-    DASP_LAUNCH_OK("bus_ir_pack_kernel");
-    const int nparts = (int)(items * g.NH * J);
-    x_fft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(nullptr, nullptr, hs, tw, 0, I, J, g.n, g.leff, 1,
-                                                                     0, nparts);
-    DASP_LAUNCH_OK("x_fft_kernel");
-    return DASP_OK;
-  };
-  g_bus_last_path[0] = 1 | (shared ? 2 : 0) | (bus_mac_cached(g) ? 4 : 0);
-  if (shared && (rc = fill_ir(hs0, 0, 1)) != DASP_OK) return rc;
-  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
-    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    float2* xs = xspec_save ? (float2*)xspec_save + item0 * g.P * I * (int64_t)kNbA : (float2*)(base + w.xsp);
-    float2* hs = (irspec_save && !shared) ? hs0 + item0 * h_stride : hs0;
-    if (!shared && (rc = fill_ir(hs, item0, items)) != DASP_OK) return rc;
-    const int nwin = (int)(items * g.P * I), nblk = (int)(items * I);
-    bus_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, g.S, g.P, I, g.n, 0, nwin);
-    DASP_LAUNCH_OK("bus_fft_kernel");
-    if ((rc = launch_bus_mac<BUS_FWD>(g, xs, hs, h_stride, nullptr, ys, items, st)) != DASP_OK) return rc;
-    bus_ifft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y, item0,
-                                                                      g.O, 1, I, g.n, g.n, 1, nblk);
-    DASP_LAUNCH_OK("bus_ifft_kernel");
-  }
-  return DASP_OK;
+  return caller_ir_fwd(BusOp{(int)S, (int)O, (int)(S * O)}, g, x, ir, nullptr, y, xspec_save, irspec_save, workspace,
+                       workspace_bytes, stream);
 }
 
 int conv_bus_bwd(bool shared, const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
                  void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O,
                  int64_t chunk_items, void* stream) {
-  BusGeom g;
+  ConvGeom g;
   int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
   if (rc != DASP_OK) return rc;
-  if (bs == 0) return DASP_OK;
-  DASP_REQUIRE(gy && xspec_save && irspec_save && gx && workspace, "conv bus bwd: null pointer");
-  DASP_REQUIRE(n % 4 == 0 && aligned16(gy), "conv bus bwd: gy needs n %% 4 == 0 and 16-byte aligned rows, got n=%lld",
-               (long long)n);
-  cudaStream_t st = (cudaStream_t)stream;
-  std::lock_guard<std::mutex> lk(g_mu);
-  BusWs w;
-  bus_layout(g, w);
-  if ((rc = check_workspace("conv bus bwd", w.bwd_total, workspace_bytes)) != DASP_OK) return rc;
-  if ((rc = configure_bus_kernels()) != DASP_OK) return rc;
-  const float* tw = nullptr;
-  if ((rc = get_fft_tables(st, &tw)) != DASP_OK) return rc;
-  unsigned char* base = (unsigned char*)workspace;
-  float2* gs = (float2*)(base + w.gs);
-  float2* ds = (float2*)(base + w.ds);
-  float2* es = (float2*)(base + w.es);
-  float* ones = (float*)(base + w.ones);
-  double2* acc = (double2*)(base + w.acc);
-  const int I = (int)g.ib, J = (int)g.jb, R = g.S * g.O;
-  const int64_t h_stride = shared ? 0 : g.NH * J * (int64_t)kNbA;
-  const int64_t per_ir = g.NH * J * (int64_t)kNbA;
-  // bit 0: own FFT, bit 1: register-cached products, bit 2: dL/dIR computed, bit 3: one IR shared by the batch
-  g_bus_last_path[1] = 1 | (bus_mac_cached(g) ? 2 : 0) | (gir ? 4 : 0) | (shared ? 8 : 0);
-  if (shared && gir) {
-    bus_ones_kernel<<<(unsigned)((bs + 255) / 256), 256, 0, st>>>(ones, bs);
-    DASP_LAUNCH_OK("bus_ones_kernel");
-  }
-  for (int64_t item0 = 0; item0 < bs; item0 += g.chunk) {
-    const int64_t items = (bs - item0 < g.chunk) ? bs - item0 : g.chunk;
-    const float2* xs = (const float2*)xspec_save + item0 * g.P * I * (int64_t)kNbA;
-    const float2* hs = (const float2*)irspec_save + item0 * h_stride;
-    const int nblk = (int)(items * I), nwin = (int)(items * g.P * I);
-    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, g.O, 1, I, g.n, 1, nblk);
-    DASP_LAUNCH_OK("bus_fft_kernel");
-    if ((rc = launch_bus_mac<BUS_DX>(g, xs, hs, h_stride, gs, ds, items, st)) != DASP_OK) return rc;
-    bus_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx, item0,
-                                                                      g.S, g.P, I, g.n, g.n, 1, nwin);
-    DASP_LAUNCH_OK("bus_ifft_kernel");
-    if (!gir) continue;                              // a fixed IR: no dL/dIR work at all
-    if ((rc = launch_bus_mac<BUS_DIR>(g, xs, hs, 0, gs, es, items, st)) != DASP_OK) return rc;
-    if (shared) {
-      irgrad_sum_kernel<<<(unsigned)((per_ir + 255) / 256), 256, 0, st>>>(es, ones, acc, item0, (int)items, per_ir,
-                                                                          item0 + items == bs);
-      DASP_LAUNCH_OK("irgrad_sum_kernel");
-    } else {
-      const int nparts = (int)(items * g.NH * J);
-      bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir,
-                                                                          item0, R, g.NH, J, g.L, g.leff, 0, nparts);
-      DASP_LAUNCH_OK("bus_ifft_kernel");
-    }
-  }
-  if (!gir) return DASP_OK;
-  if (shared) {                                      // the summed spectra, in item 0's slots of es
-    const int nparts = (int)(g.NH * J);
-    bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir, 0,
-                                                                        R, g.NH, J, g.L, g.leff, 0, nparts);
-    DASP_LAUNCH_OK("bus_ifft_kernel");
-  }
-  if (g.L > g.leff) {                                // taps that reach no output sample
-    DASP_CUDA_OK(cudaMemset2DAsync(gir + g.leff, sizeof(float) * g.L, 0, sizeof(float) * (g.L - g.leff),
-                                   (size_t)((shared ? 1 : bs) * R), st));
-  }
-  return DASP_OK;
+  return caller_ir_bwd(BusOp{(int)S, (int)O, (int)(S * O)}, g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir,
+                       nullptr, workspace, workspace_bytes, stream);
 }
 }  // namespace
 
@@ -3456,7 +3394,11 @@ int dasp_debug_conv_bus_last_path(int which) { return g_bus_last_path[which ? 1 
 
 int dasp_conv_bus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t shared,
                            int64_t chunk_items, dasp_conv_geom* out) {
-  return conv_bus_geometry(shared != 0, bs, n, ir_len, inputs, outputs, chunk_items, out);
+  DASP_REQUIRE(out != nullptr, "conv bus geometry: null out");
+  ConvGeom g;
+  int rc = make_bus_geom(shared != 0, bs, n, ir_len, inputs, outputs, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
 }
 
 int dasp_conv_bus_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
@@ -3603,8 +3545,8 @@ int dasp_nsir_bwd(const float* gir, const float* params, const float* f_save, fl
     const float2* C = reinterpret_cast<const float2*>(f_save) + item0 * kBands * g.pair_c64();
     nsir_params_kernel<<<(unsigned)((items * 25 + 255) / 256), 256, 0, st>>>(params + item0 * 24, p25, items);
     DASP_LAUNCH_OK("nsir_params_kernel");
-    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, 1), 256, 0, st>>>(gir, et, item0, J,
-                                                                                              num_samples, g.leff, 2);
+    ir_pack_kernel<<<dim3((unsigned)((g.leff + 255) / 256), (unsigned)items, 1), 256, 0, st>>>(
+        gir, et, item0, J, num_samples, g.leff, 2, false);
     DASP_LAUNCH_OK("ir_pack_kernel");
     int nparts;
     if ((rc = ir_grad_chunk(g, polyphase, et, C, p25, part, items, st, nparts)) != DASP_OK) return rc;

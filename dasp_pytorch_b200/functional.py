@@ -1276,6 +1276,19 @@ def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tenso
 # --------------------------------------------------------------------------------------
 
 
+def _conv_buffers(geom_fn, args, dev, need_bwd):
+    """the geometry query `geom_fn` (dasp_conv*_geometry, dasp_conv_bus_geometry) on `args`, the forward workspace and,
+    when a backward follows, the saved window and IR spectra; returns them and the backward's workspace bytes"""
+    geom = _abi.ConvGeom()
+    check(getattr(_abi.lib(), geom_fn)(*args, geom), geom_fn)
+    ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
+    xspec = irspec = None
+    if need_bwd:
+        xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
+        irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
+    return ws, xspec, irspec, geom.bwd_workspace_bytes
+
+
 class _ConvReverbFn(torch.autograd.Function):
     """x (bs, 1|2, n), ir (bs, 1|2|4, L), mix (bs,) -> y (bs, 2, n).  An ir of batch 1 with bs > 1 is one IR shared by
     the batch (the dasp_conv_shared_* entry points): its gradient is the sum over the items, shape (1, 1|2|4, L).  A
@@ -1292,14 +1305,8 @@ class _ConvReverbFn(torch.autograd.Function):
         dev = x.device
         y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:3])
-        geom = _abi.ConvGeom()
         with torch.cuda.device(dev):
-            check(getattr(lib, geom_fn)(bs, n, ir_len, chunk, geom), geom_fn)
-            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
-            xspec = irspec = None
-            if need_bwd:
-                xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
-                irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
+            ws, xspec, irspec, bwd_bytes = _conv_buffers(geom_fn, (bs, n, ir_len, chunk), dev, need_bwd)
             with _timed("conv_fwd", dev):
                 check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), in_chs, ptr(ir), ir_chs, ir_len, ptr(mix), ptr(y),
                                                        ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n, chunk,
@@ -1307,7 +1314,7 @@ class _ConvReverbFn(torch.autograd.Function):
                       f"dasp_{kind}_fwd")
         if need_bwd:
             ctx.save_for_backward(x, xspec, irspec, mix)
-        ctx.cfg = (kind, ir_bs, ir_chs, ir_len, chunk, geom.bwd_workspace_bytes)
+        ctx.cfg = (kind, ir_bs, ir_chs, ir_len, chunk, bwd_bytes)
         return y
 
     @staticmethod
@@ -1405,21 +1412,16 @@ class _ConvBusFn(torch.autograd.Function):
         dev = x.device
         y = torch.empty(bs, O, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:2])
-        geom = _abi.ConvGeom()
         with torch.cuda.device(dev):
-            check(lib.dasp_conv_bus_geometry(bs, n, ir_len, S, O, int(shared), chunk, geom), "dasp_conv_bus_geometry")
-            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
-            xspec = irspec = None
-            if need_bwd:
-                xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
-                irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
+            ws, xspec, irspec, bwd_bytes = _conv_buffers("dasp_conv_bus_geometry",
+                                                         (bs, n, ir_len, S, O, int(shared), chunk), dev, need_bwd)
             with _timed("conv_bus_fwd", dev):
                 check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), ptr(ir), ptr(y), ptr(xspec), ptr(irspec), ptr(ws),
                                                        ws.numel(), bs, n, ir_len, S, O, chunk, stream_ptr(dev)),
                       f"dasp_{kind}_fwd")
         if need_bwd:
             ctx.save_for_backward(xspec, irspec)
-        ctx.cfg = (kind, bs, S, O, n, ir.shape, chunk, geom.bwd_workspace_bytes)
+        ctx.cfg = (kind, bs, S, O, n, ir.shape, chunk, bwd_bytes)
         return y
 
     @staticmethod
@@ -1498,14 +1500,9 @@ def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch
     if n < 1:
         raise ValueError("x needs at least one sample")
     xf, dt = _audio(x)
-    if not impulse_response.is_cuda:
-        raise DaspError(f"impulse_response is on {impulse_response.device}: dasp_pytorch_b200 only runs on CUDA (H100) "
-                        "tensors and has no CPU path")
-    if impulse_response.device != xf.device:
-        raise DaspError(f"impulse_response is on {impulse_response.device} but x is on {xf.device}")
-    if not impulse_response.is_floating_point():
-        raise DaspError(f"impulse_response must be a floating-point tensor, got {impulse_response.dtype}")
-    irf = impulse_response.to(torch.float32).contiguous()
+    irf, _ = _audio_nd(impulse_response, 4, "impulse_response")
+    if irf.device != xf.device:
+        raise DaspError(f"impulse_response is on {irf.device} but x is on {xf.device}")
     n4 = (n + 3) // 4 * 4
     if n4 != n:
         xf = torch.nn.functional.pad(xf, (0, n4 - n))

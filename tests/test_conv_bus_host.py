@@ -67,10 +67,9 @@ GEOMS = [(48000, 48000, 8, 2, 48000, 12), (48000, 96000, 3, 1, 48000, 12), (4800
          (6000, 4097, 5, 1, 4097, 2), (70000, 66000, 16, 2, 66000, 17), (1001, 500, 2, 2, 500, 1)]
 
 
-@pytest.mark.parametrize("shared", [0, 1])
-@pytest.mark.parametrize("n,L,S,O,leff,J", GEOMS)
-def test_bus_geometry_without_gpu(lib, n, L, S, O, leff, J, shared):
-    """the sizes follow from the pair packing: ceil(S / 2) window spectra per block, ceil(S O / 2) partition sets"""
+def _check_bus_geometry(lib, n, L, S, O, leff, J, shared):
+    """the sizes follow from the pair packing: ceil(S / 2) window spectra per block, ceil(S O / 2) partition sets; a
+    shared IR adds the fp64 sum of its dL/dIR spectra to the backward workspace"""
     from dasp_pytorch_b200 import _abi
     I, P, NH = -(-n // KB), (S + 1) // 2, (S * O + 1) // 2
     for bs, chunk in ((0, 7), (10, 4)):
@@ -84,8 +83,22 @@ def test_bus_geometry_without_gpu(lib, n, L, S, O, leff, J, shared):
         blk = 8 * NFFT
         fwd = _align(blk * c * I) + _align(blk * c * P * I) + _align(blk * (1 if shared else c) * NH * J)
         bwd = (_align(blk * c * I) + _align(blk * c * P * I) + _align(blk * c * NH * J)
-               + (_align(4 * bs) + _align(16 * NFFT * NH * J) if shared else 0))
+               + (_align(16 * NFFT * NH * J) if shared else 0))
         assert (g.fwd_workspace_bytes, g.bwd_workspace_bytes) == (fwd, bwd)
+
+
+@pytest.mark.parametrize("shared", [0])
+@pytest.mark.parametrize("n,L,S,O,leff,J", GEOMS)
+def test_bus_geometry_without_gpu(lib, n, L, S, O, leff, J, shared):
+    """one IR set per item"""
+    _check_bus_geometry(lib, n, L, S, O, leff, J, shared)
+
+
+@pytest.mark.parametrize("n,L,S,O,leff,J", GEOMS)
+def test_bus_shared_geometry_without_gpu(lib, n, L, S, O, leff, J):
+    """one IR set for the batch: its partition spectra once, and no per-item factors in the backward workspace (the
+    fp64 sum of a shared IR's gradient takes a null factor as 1)"""
+    _check_bus_geometry(lib, n, L, S, O, leff, J, 1)
 
 
 def test_bus_memory_at_1024_items_of_8_inputs(lib):

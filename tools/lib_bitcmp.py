@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Run seeded forward + backward calls of the reverbs and of the compressor / expander through two builds of the library
-and compare every result byte for byte.
+"""Run seeded forward + backward calls of the reverbs, convolution_bus and the compressor / expander through two builds of
+the library and compare every result byte for byte.
 
     python tools/lib_bitcmp.py LIB_A LIB_B --out DIR
 
@@ -10,7 +10,10 @@ paths bench.py does not: the cuFFT pipeline and the two-kernel IR synthesis (das
 (two-kernel synthesis by default) and R = 17 (time-domain overlap-save), parity mode with a noise tensor, 2047 taps
 (nb = 16384: cuFFT polyphase synthesis), n % 4 != 0 (cuFFT convolution), mono input, a forward without a backward (the
 filtered noise and the spectra in the workspace), several chunks and a remainder (the forward's synthesis runs on its
-side stream), and convolution_reverberation with per-item and shared impulse responses.  The
+side stream), and convolution_reverberation with per-item and shared impulse responses: stereo, mono and true-stereo
+(per item on both pipelines, shared, and shared over several chunks with mono x), and a fixed IR (no dL/dIR).  The
+convolution_bus cases cover a mono bus per item, a stereo bus with a shared IR over several chunks, n % 4 != 0 (the
+padded rows) and a fixed IR.  Every convolution case saves its last-path hooks.  The
 noise_shaped_impulse_response cases run the same synthesis paths with the planar sink (the cluster kernel, hooks 2 and
 1, R = 12, R = 17, parity noise, 2047 taps, L = 1, chunks, a forward without a backward) and save the IR, dL/dparams
 and the last path.  The dynamics cases run both curves at every warps-per-item W the library can be
@@ -32,7 +35,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SR = 44100
 
 # name: (kind, bs, in_chs, n, L or ir_len, taps | ir_chs, debug path | shared IR, parity noise[, options]); options:
-# "grad": False (a forward only), "chunk": items per pass (REVERB_CHUNK_ITEMS)
+# "grad": False (a forward only), "chunk": items per pass (REVERB_CHUNK_ITEMS), "ir_grad": False (a fixed IR).  A bus
+# case reads in_chs as its S inputs and ir_chs as its O outputs.
 CASES = {
     "reverb_cluster_R6": ("reverb", 3, 2, 48000, 96000, 1023, 0, False),
     "reverb_two_kernel_R6": ("reverb", 3, 2, 48000, 96000, 1023, 2, False),
@@ -50,6 +54,15 @@ CASES = {
     "conv_shared_n_odd": ("conv", 4, 1, 48003, 20000, 1, True, False),
     "reverb_fwd_only": ("reverb", 3, 2, 48000, 96000, 1023, 0, False, {"grad": False}),
     "reverb_chunks": ("reverb", 5, 2, 48000, 96000, 1023, 0, False, {"chunk": 2}),
+    "conv_ts_item": ("conv", 3, 2, 48000, 30000, 4, False, False),
+    "conv_ts_item_n_odd": ("conv", 3, 2, 48001, 30000, 4, False, False),
+    "conv_ts_shared": ("conv", 4, 2, 48000, 50000, 4, True, False),
+    "conv_ts_shared_chunks_mono_x": ("conv", 5, 1, 48000, 30000, 4, True, False, {"chunk": 2}),
+    "conv_fixed_ir": ("conv", 3, 2, 48000, 30000, 2, False, False, {"ir_grad": False}),
+    "bus_S3_O1_item": ("bus", 3, 3, 48000, 30000, 1, False, False),
+    "bus_S8_O2_shared_chunks": ("bus", 5, 8, 48000, 50000, 2, True, False, {"chunk": 2}),
+    "bus_S5_O2_n_odd": ("bus", 3, 5, 48003, 20000, 2, False, False),
+    "bus_fixed_ir": ("bus", 3, 4, 48000, 30000, 2, False, False, {"ir_grad": False}),
 }
 
 # noise_shaped_impulse_response: name: (bs, L, taps, debug path, parity noise, options as above)
@@ -99,7 +112,7 @@ def run_cases(out_dir):
         grad = opt.get("grad", True)
         g = torch.Generator().manual_seed(1000 + ci)
         x = ((torch.rand(bs, in_chs, n, generator=g) * 2 - 1) * 0.5).to(dev).requires_grad_(grad)
-        gy = (torch.rand(bs, 2, n, generator=g) * 2 - 1).to(dev)
+        gy = (torch.rand(bs, c5 if kind == "bus" else 2, n, generator=g) * 2 - 1).to(dev)
         res = {}
         if kind == "reverb":
             taps, path = c5, c6
@@ -120,14 +133,27 @@ def run_cases(out_dir):
             if grad:
                 res["params_grad"] = params.grad
         else:
-            ir_chs, shared = c5, c6
-            ir = (torch.randn(1 if shared else bs, ir_chs, L, generator=g) * 0.05).to(dev).requires_grad_(True)
-            mix = torch.rand(bs, generator=g).to(dev).requires_grad_(True)
-            y = D.functional.convolution_reverberation(x, SR, ir, mix)
-            res["last_path_fwd"] = np.array([lib.dasp_debug_conv_last_path(0)], dtype=np.int32)
-            y.backward(gy)
-            res["last_path_bwd"] = np.array([lib.dasp_debug_conv_last_path(1)], dtype=np.int32)
-            res["ir_grad"], res["mix_grad"] = ir.grad, mix.grad
+            shared, ir_grad = c6, opt.get("ir_grad", True)
+            bus = kind == "bus"
+            shape = (in_chs, c5, L) if bus else (c5, L)
+            ir = (torch.randn(1 if shared else bs, *shape, generator=g) * 0.05).to(dev).requires_grad_(ir_grad)
+            hook = lib.dasp_debug_conv_bus_last_path if bus else lib.dasp_debug_conv_last_path
+            D.functional.REVERB_CHUNK_ITEMS = opt.get("chunk", chunk0)
+            try:
+                if bus:
+                    y = D.functional.convolution_bus(x, SR, ir)
+                else:
+                    mix = torch.rand(bs, generator=g).to(dev).requires_grad_(True)
+                    y = D.functional.convolution_reverberation(x, SR, ir, mix)
+                res["last_path_fwd"] = np.array([hook(0)], dtype=np.int32)
+                y.backward(gy)
+                res["last_path_bwd"] = np.array([hook(1)], dtype=np.int32)
+            finally:
+                D.functional.REVERB_CHUNK_ITEMS = chunk0
+            if ir_grad:
+                res["ir_grad"] = ir.grad
+            if not bus:
+                res["mix_grad"] = mix.grad
         torch.cuda.synchronize(dev)
         res["y"] = y
         if grad:

@@ -49,10 +49,11 @@ __all__ = [
 # --------------------------------------------------------------------------------------
 
 
-def _audio(x: torch.Tensor, name: str = "x"):
-    """validate the (bs, chs, n) audio tensor -> (fp32 contiguous tensor, original dtype)"""
-    if not torch.is_tensor(x) or x.dim() != 3:
-        raise ValueError(f"{name} must be a tensor of shape (batch, channels, samples)")
+def _audio(x: torch.Tensor, name: str = "x", rank: Optional[int] = None):
+    """validate the (bs, chs, n) audio tensor, or one of rank ``rank`` -> (fp32 contiguous tensor, original dtype)"""
+    if not torch.is_tensor(x) or x.dim() != (3 if rank is None else rank):
+        raise ValueError(f"{name} must be a tensor of shape (batch, channels, samples)" if rank is None else
+                         f"{name} must be a {rank}-dimensional tensor")
     if not x.is_cuda:
         raise DaspError(
             f"{name} is on {x.device}: dasp_pytorch_b200 only runs on CUDA (H100) tensors and has no CPU path"
@@ -87,8 +88,34 @@ def _param(p, n_expected: int, like: torch.Tensor, name: str, allow_broadcast: b
     return p
 
 
+def _stack_params(plist, bs: int, like: torch.Tensor, what: str) -> torch.Tensor:
+    """the parameters ``plist`` of op ``what``, each ``bs`` elements or one broadcast, as fp32 ``(bs, P)``"""
+    return torch.stack([_param(p, bs, like, f"{what} parameter {i}", allow_broadcast=True)
+                        for i, p in enumerate(plist)], dim=1).contiguous()
+
+
+def _packed_shape(params, ncol: int, bs: Optional[int] = None):
+    """packed parameters must be a ``(bs, ncol)`` tensor; without ``bs`` (the parameter-only ops) any batch"""
+    if (not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != ncol
+            or bs is not None and params.shape[0] != bs):
+        raise ValueError(f"params: expected a ({'bs' if bs is None else bs}, {ncol}) parameter tensor, got "
+                         f"{tuple(getattr(params, 'shape', ()))}")
+
+
+def _packed(params, ncol: int, like: torch.Tensor) -> torch.Tensor:
+    """the ``(bs, ncol)`` packed parameters of an op on x = ``like``, as fp32 contiguous"""
+    _packed_shape(params, ncol, like.shape[0])
+    if params.device != like.device:
+        raise DaspError(f"params is on {params.device} but x is on {like.device}")
+    return params.to(torch.float32).contiguous()
+
+
 def _ws(n_floats: int, device) -> torch.Tensor:
     return torch.empty(max(int(n_floats), 1), dtype=torch.float32, device=device)
+
+
+def _ws_bytes(n_bytes: int, device) -> torch.Tensor:
+    return torch.empty(max(int(n_bytes), 16), dtype=torch.uint8, device=device)
 
 
 def _params_device(tensors, what):
@@ -109,6 +136,29 @@ def _promoted_dtype(tensors):
     for d in dts[1:]:
         out = torch.promote_types(out, d)
     return out
+
+
+def _params_batch(plist, what: str) -> int:
+    """the batch of a parameter-only op: the largest element count, which every parameter holds, or one element"""
+    counts = [p.numel() if torch.is_tensor(p) else torch.as_tensor(p).numel() for p in plist]
+    bs = max(counts)
+    for i, c in enumerate(counts):
+        if c not in (1, bs):
+            raise ValueError(f"{what} parameter {i}: expected {bs} element(s) (one per batch item) or 1, got {c}")
+    return bs
+
+
+def _params_stacked(plist, bs: int, what: str):
+    """a parameter-only op's parameters -> (fp32 ``(bs, P)`` on their one CUDA device, their promoted dtype)"""
+    dev = _params_device(plist, what)
+    return _stack_params(plist, bs, torch.empty(0, device=dev), what), _promoted_dtype(plist)
+
+
+def _packed_params(params, what: str):
+    """a parameter-only op's ``(bs, P)`` packed parameters -> (fp32 contiguous on their CUDA device, their dtype)"""
+    dev = _params_device([params], what)
+    dt = params.dtype if params.is_floating_point() else torch.float32
+    return params.to(device=dev, dtype=torch.float32).contiguous(), dt
 
 
 # bench.py sets this to a list to collect (stage, start_event, end_event) around every C-ABI call
@@ -267,23 +317,13 @@ class _StereoFn(torch.autograd.Function):
         return gx, gp, None
 
 
-def _audio_nd(x, ndim, name="x"):
-    if not torch.is_tensor(x) or x.dim() != ndim:
-        raise ValueError(f"{name} must be a {ndim}-dimensional tensor")
-    if not x.is_cuda:
-        raise DaspError(f"{name} is on {x.device}: dasp_pytorch_b200 only runs on CUDA (H100) tensors and has no CPU path")
-    if not x.is_floating_point():
-        raise DaspError(f"{name} must be a floating-point tensor, got {x.dtype}")
-    return x.to(torch.float32).contiguous(), x.dtype
-
-
 def stereo_widener(x: torch.Tensor, sample_rate: float, width: torch.Tensor):
     """Mid/side stereo widener (reference ``functional.py:580-604``).
 
     ``x`` is ``(bs, 2, seq_len)``, ``width`` holds ``bs`` elements (0 = mono sum, 0.5 = unchanged,
     1 = side only).  mid = (L+R)/sqrt2 scaled by 2(1-width), side = (L-R)/sqrt2 scaled by 2 width.
     """
-    xf, dt = _audio_nd(x, 3)
+    xf, dt = _audio(x, rank=3)
     bs, chs, _ = xf.shape
     assert chs == 2, "Input tensor must have shape (bs, 2, seq_len)"
     w = _param(width, bs, xf, "width").contiguous()
@@ -297,7 +337,7 @@ def stereo_panner(x: torch.Tensor, sample_rate: float, pan: torch.Tensor):
     ``(bs, 2, num_tracks, seq_len)`` -- the layout the reference's code produces (its docstring says
     ``(bs, num_tracks, 2, seq_len)``, its ``unsqueeze(1).repeat(1, 2, 1, 1)`` does not).
     """
-    xf, dt = _audio_nd(x, 3)
+    xf, dt = _audio(x, rank=3)
     bs, tracks, _ = xf.shape
     pn = _param(pan, bs * tracks, xf, "pan").contiguous()
     return _StereoFn.apply(xf, pn, "panner").to(dt)
@@ -308,7 +348,7 @@ def stereo_bus(x: torch.Tensor, sample_rate: int, send_db: torch.Tensor):
 
     ``x`` is ``(bs, 2, tracks, seq_len)``, ``send_db`` holds ``bs*tracks`` elements; returns ``(bs, 2, seq_len)``.
     """
-    xf, dt = _audio_nd(x, 4)
+    xf, dt = _audio(x, rank=4)
     bs, chs, tracks, _ = xf.shape
     assert chs == 2, "Input tensor must have shape (bs, 2, tracks, seq_len)"
     sd = _param(send_db, bs * tracks, xf, "send_db").contiguous()
@@ -320,7 +360,9 @@ def stereo_bus(x: torch.Tensor, sample_rate: int, send_db: torch.Tensor):
 # --------------------------------------------------------------------------------------
 
 
-SIDECHAIN_MAX_CHANNELS = 32
+# the detector's channel limit (kMaxChs in dynamics.cu): x's channels for the gain ops, the key's for the side chain
+DYNAMICS_MAX_CHANNELS = 32
+SIDECHAIN_MAX_CHANNELS = DYNAMICS_MAX_CHANNELS
 # the backward streams x, dL/dy and the key through shared memory: 2 * channels + key channels tiles per stage
 SIDECHAIN_MAX_BUFFERS = 76
 
@@ -406,25 +448,40 @@ def _sidechain(sidechain, x):
     return _audio(sidechain, "sidechain")
 
 
-def _dynamics(kind, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-              lookahead_samples, sidechain=None):
+def _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db):
+    """-> ``pack(x)``: the five ``(bs,)`` columns the dynamics kernels read, kept apart (a stack would add a launch)"""
+    def pack(like):
+        bs = like.shape[0]
+        ps = [
+            _param(p, bs, like, name, allow_broadcast=True).contiguous()
+            for p, name in (
+                (threshold_db, "threshold_db"),
+                (ratio, "ratio"),
+                (attack_ms, "attack_ms"),
+                (knee_db, "knee_db"),
+                (makeup_gain_db, "makeup_gain_db"),
+            )
+        ]
+        # release_ms is validated for shape only: the reference accepts and ignores it
+        # (functional.py:333,343-344), so it receives no gradient here either.
+        _param(release_ms, bs, like, "release_ms", allow_broadcast=True)
+        return ps
+    return pack
+
+
+def _dynamics_params_packed(params):
+    """``(bs, 6)`` packed dynamics parameters -> ``pack(x)``: the same five columns, rows of one transpose"""
+    def pack(like):
+        pt = _packed(params, 6, like).t().contiguous()        # (6, bs): rows are contiguous
+        return pt[0], pt[1], pt[2], pt[4], pt[5]
+    return pack
+
+
+def _dynamics(kind, x, sample_rate, pack, eps, lookahead_samples, sidechain=None):
+    """the body of the compressor / expander ops and dynamics_packed; ``pack(xf)`` checks and packs the parameters"""
     key = _sidechain(sidechain, x)[0] if sidechain is not None else None
     xf, dt = _audio(x)
-    bs = xf.shape[0]
-    ps = [
-        _param(p, bs, xf, name, allow_broadcast=True).contiguous()
-        for p, name in (
-            (threshold_db, "threshold_db"),
-            (ratio, "ratio"),
-            (attack_ms, "attack_ms"),
-            (knee_db, "knee_db"),
-            (makeup_gain_db, "makeup_gain_db"),
-        )
-    ]
-    # release_ms is validated for shape only: the reference accepts and ignores it
-    # (functional.py:333,343-344), so it receives no gradient here either.
-    _param(release_ms, bs, xf, "release_ms", allow_broadcast=True)
-    y = _DynamicsFn.apply(xf, key, *ps, kind, sample_rate, eps, int(lookahead_samples))
+    y = _DynamicsFn.apply(xf, key, *pack(xf), kind, sample_rate, eps, int(lookahead_samples))
     return y.to(dt)
 
 
@@ -433,11 +490,7 @@ def dynamics_packed(kind: int, x: torch.Tensor, sample_rate: float, params: torc
     """compressor (kind 0) / expander (kind 1) with the six parameters stacked as ``(bs, 6)`` in signature order
     (threshold, ratio, attack, release, knee, makeup).  One transpose instead of six column copies.  ``sidechain``:
     ``None`` for ``compressor`` / ``expander``, a key tensor for ``sidechain_compressor`` / ``sidechain_expander``."""
-    key = _sidechain(sidechain, x)[0] if sidechain is not None else None
-    xf, dt = _audio(x)
-    pt = _packed(params, xf.shape[0], 6, xf, "params").t().contiguous()        # (6, bs): rows are contiguous
-    y = _DynamicsFn.apply(xf, key, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, int(lookahead_samples))
-    return y.to(dt)
+    return _dynamics(kind, x, sample_rate, _dynamics_params_packed(params), eps, lookahead_samples, sidechain)
 
 
 def compressor(
@@ -465,8 +518,8 @@ def compressor(
     (``tests/test_gpu_dynamics.py::test_compressor_gap_to_the_frequency_sampling_reference``
     tracks the gap).
     """
-    return _dynamics(0, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                     lookahead_samples)
+    pack = _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db)
+    return _dynamics(0, x, sample_rate, pack, eps, lookahead_samples)
 
 
 def expander(
@@ -489,8 +542,8 @@ def expander(
     knee, quadratic knee of width ``knee_db``, unity above -- followed by the compressor's
     attack smoother and makeup gain.  Pinned to ``oracle.expander``.
     """
-    return _dynamics(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                     lookahead_samples)
+    pack = _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db)
+    return _dynamics(1, x, sample_rate, pack, eps, lookahead_samples)
 
 
 def sidechain_compressor(
@@ -524,8 +577,8 @@ def sidechain_compressor(
     dtype); a key that does not require a gradient gets none written.  ``sidechain=x`` gives the same ``y`` as
     ``compressor``; x's gradient is then the sum of both paths.
     """
-    return _dynamics(0, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                     lookahead_samples, sidechain)
+    pack = _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db)
+    return _dynamics(0, x, sample_rate, pack, eps, lookahead_samples, sidechain)
 
 
 def sidechain_expander(
@@ -544,16 +597,13 @@ def sidechain_expander(
 ):
     """``expander`` whose detector listens to the key ``sidechain``, exactly as ``sidechain_compressor`` does for
     the compressor: gating one track from another."""
-    return _dynamics(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                     lookahead_samples, sidechain)
+    pack = _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db)
+    return _dynamics(1, x, sample_rate, pack, eps, lookahead_samples, sidechain)
 
 
 # --------------------------------------------------------------------------------------
 # the compressor's / expander's gain curve
 # --------------------------------------------------------------------------------------
-
-
-DYNAMICS_MAX_CHANNELS = 32
 
 
 class _DynamicsGainFn(torch.autograd.Function):
@@ -607,21 +657,10 @@ def _gain_input(x):
         raise ValueError(f"x: 1 to {DYNAMICS_MAX_CHANNELS} channels are supported, got {x.shape[1]}")
 
 
-def _dynamics_gain(kind, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                   db):
+def _dynamics_gain(kind, x, sample_rate, pack, eps, db):
+    """the body of compressor_gain, expander_gain and dynamics_gain_packed; ``pack(x)`` runs before x's device check"""
     _gain_input(x)
-    bs = x.shape[0]
-    ps = [
-        _param(p, bs, x, name, allow_broadcast=True).contiguous()
-        for p, name in (
-            (threshold_db, "threshold_db"),
-            (ratio, "ratio"),
-            (attack_ms, "attack_ms"),
-            (knee_db, "knee_db"),
-            (makeup_gain_db, "makeup_gain_db"),
-        )
-    ]
-    _param(release_ms, bs, x, "release_ms", allow_broadcast=True)         # shape only, as in compressor
+    ps = pack(x)
     xf, dt = _audio(x)
     return _DynamicsGainFn.apply(xf, *ps, kind, sample_rate, eps, bool(db)).to(dt)
 
@@ -630,10 +669,7 @@ def dynamics_gain_packed(kind: int, x: torch.Tensor, sample_rate: float, params:
                          db: bool = False):
     """``compressor_gain`` (kind 0) / ``expander_gain`` (kind 1) with the six parameters stacked as ``(bs, 6)`` in
     signature order (threshold, ratio, attack, release, knee, makeup)."""
-    _gain_input(x)
-    pt = _packed(params, x.shape[0], 6, x, "params").t().contiguous()        # (6, bs): rows are contiguous
-    xf, dt = _audio(x)
-    return _DynamicsGainFn.apply(xf, pt[0], pt[1], pt[2], pt[4], pt[5], kind, sample_rate, eps, bool(db)).to(dt)
+    return _dynamics_gain(kind, x, sample_rate, _dynamics_params_packed(params), eps, db)
 
 
 def compressor_gain(
@@ -669,8 +705,8 @@ def compressor_gain(
     ``|side| < eps`` (returned as an expanded view of one row per item); the five other parameters as in ``compressor``.
     Without a gradient to compute, no smoother checkpoint is kept.
     """
-    return _dynamics_gain(0, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                          db)
+    pack = _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db)
+    return _dynamics_gain(0, x, sample_rate, pack, eps, db)
 
 
 def expander_gain(
@@ -688,8 +724,8 @@ def expander_gain(
 ):
     """The gain ``expander`` applies, exactly as ``compressor_gain`` is the compressor's: the expander's static curve,
     the same detector, smoother and makeup, the same bit-for-bit contract with ``expander``."""
-    return _dynamics_gain(1, x, sample_rate, threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db, eps,
-                          db)
+    pack = _dynamics_params(threshold_db, ratio, attack_ms, release_ms, knee_db, makeup_gain_db)
+    return _dynamics_gain(1, x, sample_rate, pack, eps, db)
 
 
 # --------------------------------------------------------------------------------------
@@ -770,8 +806,6 @@ def parametric_eq(
     of the ``ParametricEQ`` ranges at n = 48000, but up to 3 % for a 20 Hz shelf at n = 4096
     (item 0 of ``tests/golden/parametric_eq.npz`` keeps such a case; DESIGN.md section 2).
     """
-    xf, dt = _audio(x)
-    bs = xf.shape[0]
     plist = (
         low_shelf_gain_db, low_shelf_cutoff_freq, low_shelf_q_factor,
         band0_gain_db, band0_cutoff_freq, band0_q_factor,
@@ -780,26 +814,21 @@ def parametric_eq(
         band3_gain_db, band3_cutoff_freq, band3_q_factor,
         high_shelf_gain_db, high_shelf_cutoff_freq, high_shelf_q_factor,
     )
-    packed = torch.stack([_param(p, bs, xf, f"parametric_eq parameter {i}", allow_broadcast=True)
-                          for i, p in enumerate(plist)], dim=1).contiguous()
-    y = _ParametricEqFn.apply(xf, packed, sample_rate)
+    return _parametric_eq(x, sample_rate, lambda xf: _stack_params(plist, xf.shape[0], xf, "parametric_eq"))
+
+
+def _parametric_eq(x, sample_rate, pack):
+    """the body of parametric_eq and parametric_eq_packed; ``pack(xf)`` checks and packs the parameters"""
+    xf, dt = _audio(x)
+    y = _ParametricEqFn.apply(xf, pack(xf), sample_rate)
     return y.to(dt)
-
-
-def _packed(params, bs: int, ncol: int, like: torch.Tensor, name: str) -> torch.Tensor:
-    if not torch.is_tensor(params) or params.dim() != 2 or tuple(params.shape) != (bs, ncol):
-        raise ValueError(f"{name}: expected a ({bs}, {ncol}) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
-    if params.device != like.device:
-        raise DaspError(f"{name} is on {params.device} but x is on {like.device}")
-    return params.to(torch.float32).contiguous()
 
 
 def parametric_eq_packed(x: torch.Tensor, sample_rate: float, params: torch.Tensor):
     """``parametric_eq`` with its 18 parameters already stacked as ``(bs, 18)`` in signature order (physical
     units).  Used by ``modules.ParametricEQ.process_normalized`` so that the whole normalised-parameter path is
     one affine kernel + the EQ kernels (SURVEY.md 8f rank 1); gradients flow to ``params``."""
-    xf, dt = _audio(x)
-    return _ParametricEqFn.apply(xf, _packed(params, xf.shape[0], 18, xf, "params"), sample_rate).to(dt)
+    return _parametric_eq(x, sample_rate, lambda xf: _packed(params, 18, xf))
 
 
 # --------------------------------------------------------------------------------------
@@ -856,7 +885,7 @@ def _eq_response_checks(sample_rate, frequencies):
                          "18 EQ parameters only")
 
 
-def _eq_response_run(packed, frequencies, sample_rate, dt):
+def _eq_response_run(packed, dt, frequencies, sample_rate):
     dev = packed.device
     if frequencies.device.type != "cpu" and frequencies.device != dev:
         raise DaspError(f"frequencies are on {frequencies.device}; they must be on the CPU or on {dev}")
@@ -920,29 +949,17 @@ def parametric_eq_frequency_response(
         band3_gain_db, band3_cutoff_freq, band3_q_factor,
         high_shelf_gain_db, high_shelf_cutoff_freq, high_shelf_q_factor,
     )
-    counts = [p.numel() if torch.is_tensor(p) else torch.as_tensor(p).numel() for p in plist]
-    bs = max(counts)
-    for i, c in enumerate(counts):
-        if c not in (1, bs):
-            raise ValueError(f"parametric_eq_frequency_response parameter {i}: expected {bs} element(s) (one per batch "
-                             f"item) or 1, got {c}")
+    bs = _params_batch(plist, "parametric_eq_frequency_response")
     _eq_response_checks(sample_rate, frequencies)
-    dev = _params_device(plist, "parametric_eq_frequency_response")
-    like = torch.empty(0, device=dev)
-    packed = torch.stack([_param(p, bs, like, f"parametric_eq_frequency_response parameter {i}", allow_broadcast=True)
-                          for i, p in enumerate(plist)], dim=1).contiguous()
-    return _eq_response_run(packed, frequencies, sample_rate, _promoted_dtype(plist))
+    return _eq_response_run(*_params_stacked(plist, bs, "parametric_eq_frequency_response"), frequencies, sample_rate)
 
 
 def parametric_eq_frequency_response_packed(sample_rate: float, params: torch.Tensor, frequencies: torch.Tensor):
     """``parametric_eq_frequency_response`` with its 18 parameters stacked as ``(bs, 18)`` in signature order
     (physical units), as ``parametric_eq_packed`` takes them.  Used by ``modules.ParametricEQ.frequency_response``."""
-    if not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != 18:
-        raise ValueError(f"params: expected a (bs, 18) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
+    _packed_shape(params, 18)
     _eq_response_checks(sample_rate, frequencies)
-    dev = _params_device([params], "parametric_eq_frequency_response")
-    dt = params.dtype if params.is_floating_point() else torch.float32
-    return _eq_response_run(params.to(device=dev, dtype=torch.float32).contiguous(), frequencies, sample_rate, dt)
+    return _eq_response_run(*_packed_params(params, "parametric_eq_frequency_response"), frequencies, sample_rate)
 
 
 # --------------------------------------------------------------------------------------
@@ -989,6 +1006,17 @@ def _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps):
     return None, torch.empty(1, dtype=torch.int64, device=xf.device).random_()
 
 
+def _geom_buffers(geom, geom_fn, args, dev, need_bwd, saved=("xspec_c64", "irspec_c64")):
+    """the geometry query `geom_fn` (dasp_*_geometry) on `args` into `geom` (ReverbGeom or ConvGeom), the forward
+    workspace and, when a backward follows, the buffers kept for it, one per size field in `saved` (``*_c64``:
+    complex64, ``f_floats``: fp32); returns them and the backward's workspace bytes"""
+    check(getattr(_abi.lib(), geom_fn)(*args, geom), geom_fn)
+    ws = _ws_bytes(geom.fwd_workspace_bytes, dev)
+    bufs = [torch.empty(getattr(geom, f), dtype=torch.complex64 if f.endswith("_c64") else torch.float32, device=dev)
+            if need_bwd else None for f in saved]
+    return ws, bufs, geom.bwd_workspace_bytes
+
+
 class _ReverbFn(torch.autograd.Function):
     """x (bs, 1|2, n), params (bs, 25) -> y (bs, 2, n)."""
 
@@ -999,15 +1027,10 @@ class _ReverbFn(torch.autograd.Function):
         dev = x.device
         y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:2])
-        geom = _abi.ReverbGeom()
         with torch.cuda.device(dev):
-            check(lib.dasp_reverb_geometry(bs, n, num_samples, taps, chunk, geom), "dasp_reverb_geometry")
-            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
-            fsave = xspec = irspec = None
-            if need_bwd:
-                fsave = torch.empty(geom.f_floats, dtype=torch.float32, device=dev)
-                xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
-                irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
+            ws, (fsave, xspec, irspec), bwd_bytes = _geom_buffers(
+                _abi.ReverbGeom(), "dasp_reverb_geometry", (bs, n, num_samples, taps, chunk), dev, need_bwd,
+                ("f_floats", "xspec_c64", "irspec_c64"))
             with _timed("reverb_fwd", dev):
                 check(lib.dasp_reverb_fwd(ptr(x), in_chs, ptr(params), ptr(noise), ptr(seed), ptr(y), ptr(fsave),
                                           ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n, num_samples, taps, chunk,
@@ -1016,7 +1039,7 @@ class _ReverbFn(torch.autograd.Function):
             # slot 2 (the wet signal, which the backward no longer needs) stays empty so that callers that inspect
             # grad_fn.saved_tensors keep the layout (x, params, -, f, X spectra, IR spectra)
             ctx.save_for_backward(x, params, None, fsave, xspec, irspec)
-        ctx.cfg = (num_samples, taps, chunk, geom.bwd_workspace_bytes, 1 if noise is None else 0)
+        ctx.cfg = (num_samples, taps, chunk, bwd_bytes, 1 if noise is None else 0)
         return y
 
     @staticmethod
@@ -1029,7 +1052,7 @@ class _ReverbFn(torch.autograd.Function):
         gy = gy.contiguous()
         gx = torch.empty_like(x)
         gp = torch.empty_like(params)
-        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        ws = _ws_bytes(bwd_bytes, dev)
         with torch.cuda.device(dev), _timed("reverb_bwd", dev):
             check(lib.dasp_reverb_bwd(ptr(gy), ptr(x), in_chs, ptr(params), ptr(fsave), ptr(xspec), ptr(irspec),
                                       ptr(gx), ptr(gp), ptr(ws), ws.numel(), bs, n, num_samples, taps, chunk,
@@ -1086,10 +1109,6 @@ def noise_shaped_reverberation(
     memory (``torch.manual_seed`` makes the call reproducible; a captured CUDA graph draws fresh
     noise on every replay, like the reference's ``torch.randn`` would).
     """
-    assert num_bandpass_taps % 2 == 1, "num_bandpass_taps must be odd"
-    xf, dt = _audio(x)
-    bs, chs, n = xf.shape
-    assert chs <= 2, "only mono/stereo signals are supported"
     plist = (
         band0_gain, band1_gain, band2_gain, band3_gain, band4_gain, band5_gain,
         band6_gain, band7_gain, band8_gain, band9_gain, band10_gain, band11_gain,
@@ -1097,8 +1116,17 @@ def noise_shaped_reverberation(
         band6_decay, band7_decay, band8_decay, band9_decay, band10_decay, band11_decay,
         mix,
     )
-    packed = torch.stack([_param(p, bs, xf, f"noise_shaped_reverberation parameter {i}", allow_broadcast=True)
-                          for i, p in enumerate(plist)], dim=1).contiguous()
+    return _reverb(x, sample_rate, lambda xf: _stack_params(plist, xf.shape[0], xf, "noise_shaped_reverberation"),
+                   num_samples, num_bandpass_taps, noise)
+
+
+def _reverb(x, sample_rate, pack, num_samples, num_bandpass_taps, noise):
+    """the body of noise_shaped_reverberation and its packed twin; ``pack(xf)`` checks and packs the parameters"""
+    assert num_bandpass_taps % 2 == 1, "num_bandpass_taps must be odd"
+    xf, dt = _audio(x)
+    bs, chs, _ = xf.shape
+    assert chs <= 2, "only mono/stereo signals are supported"
+    packed = pack(xf)
     noise, seed = _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps)
     y = _ReverbFn.apply(xf, packed, noise, seed, sample_rate, int(num_samples), int(num_bandpass_taps),
                         reverb_chunk_items(xf.device))
@@ -1108,15 +1136,7 @@ def noise_shaped_reverberation(
 def noise_shaped_reverberation_packed(x: torch.Tensor, sample_rate: float, params: torch.Tensor, num_samples: int = 65536,
                                       num_bandpass_taps: int = 1023, *, noise: Optional[torch.Tensor] = None):
     """``noise_shaped_reverberation`` with its 25 parameters stacked as ``(bs, 25)`` (12 gains, 12 decays, mix)."""
-    assert num_bandpass_taps % 2 == 1, "num_bandpass_taps must be odd"
-    xf, dt = _audio(x)
-    bs, chs, _ = xf.shape
-    assert chs <= 2, "only mono/stereo signals are supported"
-    packed = _packed(params, bs, 25, xf, "params")
-    noise, seed = _noise_or_seed(noise, xf, bs, num_samples, num_bandpass_taps)
-    y = _ReverbFn.apply(xf, packed, noise, seed, sample_rate, int(num_samples), int(num_bandpass_taps),
-                        reverb_chunk_items(xf.device))
-    return y.to(dt)
+    return _reverb(x, sample_rate, lambda xf: _packed(params, 25, xf), num_samples, num_bandpass_taps, noise)
 
 
 # --------------------------------------------------------------------------------------
@@ -1134,18 +1154,16 @@ class _NsirFn(torch.autograd.Function):
         dev = params.device
         ir = torch.empty(bs, 2, num_samples, dtype=torch.float32, device=dev)
         need_bwd = ctx.needs_input_grad[0]
-        geom = _abi.ReverbGeom()
         with torch.cuda.device(dev):
-            check(lib.dasp_nsir_geometry(bs, num_samples, taps, chunk, geom), "dasp_nsir_geometry")
-            ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
-            fsave = torch.empty(geom.f_floats, dtype=torch.float32, device=dev) if need_bwd else None
+            ws, (fsave,), bwd_bytes = _geom_buffers(_abi.ReverbGeom(), "dasp_nsir_geometry",
+                                                    (bs, num_samples, taps, chunk), dev, need_bwd, ("f_floats",))
             with _timed("nsir_fwd", dev):
                 check(lib.dasp_nsir_fwd(ptr(params), ptr(noise), ptr(seed), ptr(ir), ptr(fsave), ptr(ws), ws.numel(),
                                         bs, num_samples, taps, chunk, float(sample_rate), stream_ptr(dev)),
                       "dasp_nsir_fwd")
         if need_bwd:
             ctx.save_for_backward(params, fsave)
-        ctx.cfg = (num_samples, taps, chunk, geom.bwd_workspace_bytes, 1 if noise is None else 0)
+        ctx.cfg = (num_samples, taps, chunk, bwd_bytes, 1 if noise is None else 0)
         return ir
 
     @staticmethod
@@ -1157,7 +1175,7 @@ class _NsirFn(torch.autograd.Function):
         dev = params.device
         gir = gir.to(torch.float32).contiguous()
         gp = torch.empty_like(params)
-        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        ws = _ws_bytes(bwd_bytes, dev)
         with torch.cuda.device(dev), _timed("nsir_bwd", dev):
             check(lib.dasp_nsir_bwd(ptr(gir), ptr(params), ptr(fsave), ptr(gp), ptr(ws), ws.numel(), bs, num_samples,
                                     taps, chunk, device_noise, stream_ptr(dev)), "dasp_nsir_bwd")
@@ -1173,7 +1191,7 @@ def _nsir_checks(sample_rate, num_samples, num_bandpass_taps):
         raise ValueError(f"sample_rate {sample_rate} too low: the filter bank's 18 kHz high-pass needs sample_rate > 36000")
 
 
-def _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, dt):
+def _nsir_run(packed, dt, noise, sample_rate, num_samples, num_bandpass_taps):
     bs = packed.shape[0]
     noise, seed = _noise_or_seed(noise, packed, bs, num_samples, num_bandpass_taps)
     ir = _NsirFn.apply(packed, noise, seed, sample_rate, int(num_samples), int(num_bandpass_taps),
@@ -1244,31 +1262,20 @@ def noise_shaped_impulse_response(
         band0_decay, band1_decay, band2_decay, band3_decay, band4_decay, band5_decay,
         band6_decay, band7_decay, band8_decay, band9_decay, band10_decay, band11_decay,
     )
-    counts = [p.numel() if torch.is_tensor(p) else torch.as_tensor(p).numel() for p in plist]
-    bs = max(counts)
-    for i, c in enumerate(counts):
-        if c not in (1, bs):
-            raise ValueError(f"noise_shaped_impulse_response parameter {i}: expected {bs} element(s) (one per batch "
-                             f"item) or 1, got {c}")
+    bs = _params_batch(plist, "noise_shaped_impulse_response")
     _check_noise_shape(noise, bs, num_samples, num_bandpass_taps)
-    dev = _params_device(plist, "noise_shaped_impulse_response")
-    like = torch.empty(0, device=dev)
-    packed = torch.stack([_param(p, bs, like, f"noise_shaped_impulse_response parameter {i}", allow_broadcast=True)
-                          for i, p in enumerate(plist)], dim=1).contiguous()
-    return _nsir_run(packed, noise, sample_rate, num_samples, num_bandpass_taps, _promoted_dtype(plist))
+    return _nsir_run(*_params_stacked(plist, bs, "noise_shaped_impulse_response"), noise, sample_rate, num_samples,
+                     num_bandpass_taps)
 
 
 def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tensor, num_samples: int = 65536,
                                          num_bandpass_taps: int = 1023, *, noise: Optional[torch.Tensor] = None):
     """``noise_shaped_impulse_response`` with its 24 parameters stacked as ``(bs, 24)`` (12 gains, 12 decays)."""
     _nsir_checks(sample_rate, num_samples, num_bandpass_taps)
-    if not torch.is_tensor(params) or params.dim() != 2 or params.shape[1] != 24:
-        raise ValueError(f"params: expected a (bs, 24) parameter tensor, got {tuple(getattr(params, 'shape', ()))}")
+    _packed_shape(params, 24)
     _check_noise_shape(noise, params.shape[0], num_samples, num_bandpass_taps)
-    dev = _params_device([params], "noise_shaped_impulse_response")
-    dt = params.dtype if params.is_floating_point() else torch.float32
-    return _nsir_run(params.to(device=dev, dtype=torch.float32).contiguous(), noise, sample_rate, num_samples,
-                     num_bandpass_taps, dt)
+    return _nsir_run(*_packed_params(params, "noise_shaped_impulse_response"), noise, sample_rate, num_samples,
+                     num_bandpass_taps)
 
 
 # --------------------------------------------------------------------------------------
@@ -1276,17 +1283,21 @@ def noise_shaped_impulse_response_packed(sample_rate: float, params: torch.Tenso
 # --------------------------------------------------------------------------------------
 
 
-def _conv_buffers(geom_fn, args, dev, need_bwd):
-    """the geometry query `geom_fn` (dasp_conv*_geometry, dasp_conv_bus_geometry) on `args`, the forward workspace and,
-    when a backward follows, the saved window and IR spectra; returns them and the backward's workspace bytes"""
-    geom = _abi.ConvGeom()
-    check(getattr(_abi.lib(), geom_fn)(*args, geom), geom_fn)
-    ws = torch.empty(max(geom.fwd_workspace_bytes, 16), dtype=torch.uint8, device=dev)
-    xspec = irspec = None
-    if need_bwd:
-        xspec = torch.empty(geom.xspec_c64, dtype=torch.complex64, device=dev)
-        irspec = torch.empty(geom.irspec_c64, dtype=torch.complex64, device=dev)
-    return ws, xspec, irspec, geom.bwd_workspace_bytes
+def _caller_ir_shape(impulse_response, bs: int):
+    """a caller's IR, taps last, against x's batch: one IR per item, or one shared by a batch of more than one"""
+    ir_bs = impulse_response.shape[0]
+    if ir_bs != bs and not (ir_bs == 1 and bs > 1):
+        raise ValueError(f"impulse_response has batch {ir_bs}, x has batch {bs} (expected {bs} or 1)")
+    if impulse_response.shape[-1] < 1:
+        raise ValueError("impulse_response needs at least one tap")
+
+
+def _caller_ir(impulse_response, xf, rank=None):
+    """a caller's IR (rank 3, or ``rank``) as fp32 contiguous on x's device"""
+    irf, _ = _audio(impulse_response, "impulse_response", rank)
+    if irf.device != xf.device:
+        raise DaspError(f"impulse_response is on {irf.device} but x is on {xf.device}")
+    return irf
 
 
 class _ConvReverbFn(torch.autograd.Function):
@@ -1306,7 +1317,8 @@ class _ConvReverbFn(torch.autograd.Function):
         y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:3])
         with torch.cuda.device(dev):
-            ws, xspec, irspec, bwd_bytes = _conv_buffers(geom_fn, (bs, n, ir_len, chunk), dev, need_bwd)
+            ws, (xspec, irspec), bwd_bytes = _geom_buffers(_abi.ConvGeom(), geom_fn, (bs, n, ir_len, chunk), dev,
+                                                           need_bwd)
             with _timed("conv_fwd", dev):
                 check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), in_chs, ptr(ir), ir_chs, ir_len, ptr(mix), ptr(y),
                                                        ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n, chunk,
@@ -1329,7 +1341,7 @@ class _ConvReverbFn(torch.autograd.Function):
         # a fixed IR (data augmentation with measured rooms) skips every dL/dIR kernel
         gir = torch.empty(ir_bs, ir_chs, ir_len, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
         gmix = torch.empty_like(mix)
-        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        ws = _ws_bytes(bwd_bytes, dev)
         with torch.cuda.device(dev), _timed("conv_bwd", dev):
             check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(x), in_chs, ir_chs, ir_len, ptr(mix), ptr(xspec),
                                                    ptr(irspec), ptr(gx), ptr(gir), ptr(gmix), ptr(ws), ws.numel(), bs,
@@ -1375,17 +1387,12 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
         if t.shape[1] not in chans:
             raise ValueError(f"{name}: only {what} is supported, got {t.shape[1]} channels")
     bs = x.shape[0]
-    if impulse_response.shape[0] != bs and not (impulse_response.shape[0] == 1 and bs > 1):
-        raise ValueError(f"impulse_response has batch {impulse_response.shape[0]}, x has batch {bs} (expected {bs} or 1)")
-    if impulse_response.shape[2] < 1:
-        raise ValueError("impulse_response needs at least one tap")
+    _caller_ir_shape(impulse_response, bs)
     nmix = mix.numel() if torch.is_tensor(mix) else torch.as_tensor(mix).numel()
     if nmix not in (1, bs):
         raise ValueError(f"mix: expected {bs} element(s) (one per batch item) or 1, got {nmix}")
     xf, dt = _audio(x)
-    irf, _ = _audio(impulse_response, "impulse_response")
-    if irf.device != xf.device:
-        raise DaspError(f"impulse_response is on {irf.device} but x is on {xf.device}")
+    irf = _caller_ir(impulse_response, xf)
     m = _param(mix, bs, xf, "mix", allow_broadcast=True).contiguous()
     y = _ConvReverbFn.apply(xf, irf, m, reverb_chunk_items(xf.device))
     return y.to(dt)
@@ -1413,8 +1420,8 @@ class _ConvBusFn(torch.autograd.Function):
         y = torch.empty(bs, O, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:2])
         with torch.cuda.device(dev):
-            ws, xspec, irspec, bwd_bytes = _conv_buffers("dasp_conv_bus_geometry",
-                                                         (bs, n, ir_len, S, O, int(shared), chunk), dev, need_bwd)
+            ws, (xspec, irspec), bwd_bytes = _geom_buffers(_abi.ConvGeom(), "dasp_conv_bus_geometry",
+                                                           (bs, n, ir_len, S, O, int(shared), chunk), dev, need_bwd)
             with _timed("conv_bus_fwd", dev):
                 check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), ptr(ir), ptr(y), ptr(xspec), ptr(irspec), ptr(ws),
                                                        ws.numel(), bs, n, ir_len, S, O, chunk, stream_ptr(dev)),
@@ -1436,7 +1443,7 @@ class _ConvBusFn(torch.autograd.Function):
         gx = torch.empty(bs, S, n, dtype=torch.float32, device=dev)
         # a fixed IR (measured rooms, a fixed downmix) skips every dL/dIR kernel
         gir = torch.empty(ir_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
-        ws = torch.empty(max(bwd_bytes, 16), dtype=torch.uint8, device=dev)
+        ws = _ws_bytes(bwd_bytes, dev)
         with torch.cuda.device(dev), _timed("conv_bus_bwd", dev):
             check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(xspec), ptr(irspec), ptr(gx), ptr(gir), ptr(ws),
                                                    ws.numel(), bs, n, ir_shape[3], S, O, chunk, stream_ptr(dev)),
@@ -1488,21 +1495,16 @@ def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch
     bs, S, n = x.shape
     if not 1 <= S <= CONV_BUS_MAX_INPUTS:
         raise ValueError(f"convolution_bus: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, got {S}")
-    ir_bs, ir_s, O, L = impulse_response.shape
+    _, ir_s, O, L = impulse_response.shape
     if ir_s != S:
         raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
     if O not in (1, 2):
         raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
-    if ir_bs != bs and not (ir_bs == 1 and bs > 1):
-        raise ValueError(f"impulse_response has batch {ir_bs}, x has batch {bs} (expected {bs} or 1)")
-    if L < 1:
-        raise ValueError("impulse_response needs at least one tap")
+    _caller_ir_shape(impulse_response, bs)
     if n < 1:
         raise ValueError("x needs at least one sample")
     xf, dt = _audio(x)
-    irf, _ = _audio_nd(impulse_response, 4, "impulse_response")
-    if irf.device != xf.device:
-        raise DaspError(f"impulse_response is on {irf.device} but x is on {xf.device}")
+    irf = _caller_ir(impulse_response, xf, 4)
     n4 = (n + 3) // 4 * 4
     if n4 != n:
         xf = torch.nn.functional.pad(xf, (0, n4 - n))

@@ -21,6 +21,7 @@ Differences, all on the host side:
 """
 from __future__ import annotations
 
+import functools
 from typing import Dict
 
 import torch
@@ -140,6 +141,12 @@ class Processor:
                 self.denormalize_param_dict(self.extract_param_dict(param_tensor))      # raises with the name
         return phys
 
+    def _denormalize_cuda(self, param_tensor, caller: str) -> torch.Tensor:
+        """``_denormalize_packed`` for the methods that have only the packed path: ``param_tensor`` must be on CUDA"""
+        if not torch.is_tensor(param_tensor) or not param_tensor.is_cuda:
+            raise _F.DaspError(f"{caller}: param_tensor must be a CUDA tensor; dasp_pytorch_b200 has no CPU path")
+        return self._denormalize_packed(param_tensor)
+
     def _affine(self, device):
         key = (str(device), tuple(self.param_ranges.values()))
         cache = self.__dict__.setdefault("_affine_cache", {})
@@ -245,20 +252,22 @@ class ParametricEQ(Processor):
         ``frequencies`` in Hz (see ``functional.parametric_eq_frequency_response``).  ``param_tensor`` is
         ``(batch, 18)`` in [0, 1] on a CUDA device, mapped and range-checked exactly as ``process_normalized`` does;
         gradients flow back to it."""
-        if not torch.is_tensor(param_tensor) or not param_tensor.is_cuda:
-            raise _F.DaspError("ParametricEQ.frequency_response: param_tensor must be a CUDA tensor; "
-                               "dasp_pytorch_b200 has no CPU path")
-        phys = self._denormalize_packed(param_tensor)
+        phys = self._denormalize_cuda(param_tensor, "ParametricEQ.frequency_response")
         return _F.parametric_eq_frequency_response_packed(self.sample_rate, phys, frequencies)
 
 
 class _Dynamics(Processor):
-    def __init__(self, sample_rate: int, min_threshold_db: float = -60.0, max_threshold_db: float = 0.0,
-                 min_ratio: float = 1.0, max_ratio: float = 20.0, min_attack_ms: float = 5.0,
-                 max_attack_ms: float = 100.0, min_release_ms: float = 5.0, max_release_ms: float = 100.0,
-                 min_knee_db: float = 0.0, max_knee_db: float = 12.0, min_makeup_gain_db: float = 0.0,
-                 max_makeup_gain_db: float = 12.0):
+    def __init__(self, kind: int, process_fn, sidechain_fn, sample_rate: int, min_threshold_db: float = -60.0,
+                 max_threshold_db: float = 0.0, min_ratio: float = 1.0, max_ratio: float = 20.0,
+                 min_attack_ms: float = 5.0, max_attack_ms: float = 100.0, min_release_ms: float = 5.0,
+                 max_release_ms: float = 100.0, min_knee_db: float = 0.0, max_knee_db: float = 12.0,
+                 min_makeup_gain_db: float = 0.0, max_makeup_gain_db: float = 12.0):
         self.sample_rate = sample_rate
+        self.process_fn = process_fn
+        # the side-chain counterpart of the package's process_fn (functional.sidechain_compressor / _expander)
+        self._sidechain_fn = sidechain_fn
+        self._kind = kind          # 0: compressor, 1: expander
+        self._packed_path = (functools.partial(_F.dynamics_packed, self._kind), process_fn)
         self.param_ranges = {
             "threshold_db": (min_threshold_db, max_threshold_db),
             "ratio": (min_ratio, max_ratio),
@@ -267,9 +276,6 @@ class _Dynamics(Processor):
             "knee_db": (min_knee_db, max_knee_db),
             "makeup_gain_db": (min_makeup_gain_db, max_makeup_gain_db),
         }
-
-    # the side-chain counterpart of the package's process_fn (functional.sidechain_compressor / _expander)
-    _sidechain_fn = None
 
     def process_normalized(self, x: torch.Tensor, param_tensor: torch.Tensor, sidechain=None):
         """``Processor.process_normalized`` with an optional key: ``sidechain`` (bs, K, n) drives the detector
@@ -281,38 +287,25 @@ class _Dynamics(Processor):
         by_name = self._sidechain_fn if self.process_fn is self._packed_path[1] else None
         return self._process_normalized(x, param_tensor, by_name, sidechain=sidechain)
 
-    _kind = None          # 0: compressor, 1: expander
-
     def gain_curve(self, x: torch.Tensor, param_tensor: torch.Tensor, *, db: bool = False) -> torch.Tensor:
         """The gain ``(batch, 1, n)`` that ``process_normalized(x, param_tensor)`` multiplies into the audio, with the
         detector on ``x`` (see ``functional.compressor_gain``); ``db=True`` returns it in dB.  ``param_tensor`` is
         ``(batch, 6)`` in [0, 1] on a CUDA device, mapped and range-checked exactly as ``process_normalized`` does;
         gradients flow back to it and to x."""
-        if not torch.is_tensor(param_tensor) or not param_tensor.is_cuda:
-            raise _F.DaspError(f"{type(self).__name__}.gain_curve: param_tensor must be a CUDA tensor; "
-                               "dasp_pytorch_b200 has no CPU path")
-        phys = self._denormalize_packed(param_tensor)
+        phys = self._denormalize_cuda(param_tensor, f"{type(self).__name__}.gain_curve")
         return _F.dynamics_gain_packed(self._kind, x, self.sample_rate, phys, db=db)
 
 
 class Compressor(_Dynamics):
     def __init__(self, sample_rate: int, **kw):
-        super().__init__(sample_rate, **kw)
-        self.process_fn = compressor
-        self._sidechain_fn = sidechain_compressor
-        self._kind = 0
-        self._packed_path = (lambda x, sr, p, **kw: _F.dynamics_packed(0, x, sr, p, **kw), compressor)
+        super().__init__(0, compressor, sidechain_compressor, sample_rate, **kw)
 
 
 class Expander(_Dynamics):
     """New: the reference advertises an expander but only stubs it (functional.py:402-403)."""
 
     def __init__(self, sample_rate: int, max_ratio: float = 4.0, **kw):
-        super().__init__(sample_rate, max_ratio=max_ratio, **kw)
-        self.process_fn = expander
-        self._sidechain_fn = sidechain_expander
-        self._kind = 1
-        self._packed_path = (lambda x, sr, p, **kw: _F.dynamics_packed(1, x, sr, p, **kw), expander)
+        super().__init__(1, expander, sidechain_expander, sample_rate, max_ratio=max_ratio, **kw)
 
 
 class NoiseShapedReverb(Processor):

@@ -44,7 +44,8 @@
 // Tiles are swept in reverse time order with the same warp/mailbox structure (the adjoint carry flows from tile
 // i+1 to tile i); per tile the six section inputs are recomputed from the checkpoint into per-warp shared memory
 // (no cross-tile dependency: every tile's incoming states are checkpointed), then sections are unwound 6 -> 1.
-// The 30 sums per row are reduced deterministically; a second tiny kernel adds the channels of an item and applies
+// The 30 sums per row run in fp32 over at most kFoldTiles tiles of a warp, are folded into fp64 and reduced
+// deterministically; a second tiny kernel adds the channels of an item and applies
 // the fp64 Jacobian d(sg,q,be1,B2,b0)/d(gain_dB, fc, Q) (forward-mode dual numbers).
 #include <math.h>
 #include <stdlib.h>
@@ -61,6 +62,7 @@ constexpr int kE = DASP_EQ_E;    // samples per lane per tile (odd: conflict-fre
 static_assert(kE % 2 == 1, "E must be odd");
 constexpr int kTile = 32 * kE;   // samples per tile (one warp)
 constexpr int kSections = 6;
+constexpr int kFoldTiles = 16;   // backward: tiles of a warp between folds of the fp32 gradient sums into fp64
 constexpr size_t kSmemPerSm = 227 * 1024;     // usable shared memory of one SM / one CTA
 
 // ------------------------------------------------------------------ coefficient design (fp64)
@@ -600,6 +602,21 @@ __global__ void __launch_bounds__(W * 32) eq_bwd_kernel(EqParams p) {
 #pragma unroll
     for (int q = 0; q < 5; ++q) acc[k][q] = zero2();
   }
+  // Every kFoldTiles tiles of the warp the lanes' fp32 sums are reduced across the warp and added to the warp's fp64
+  // totals, which lane e (< 30) holds for sum e of rows A and B; the fp32 sums then restart.  A lane's fp32 sum thus
+  // covers at most kFoldTiles * kE samples however long the row is.
+  double tot_a = 0.0, tot_b = 0.0;
+  auto fold = [&]() {
+#pragma unroll
+    for (int k = 0; k < kSections; ++k) {
+#pragma unroll
+      for (int q = 0; q < 5; ++q) {
+        const double sa = warp_sum((double)acc[k][q].x), sb = warp_sum((double)acc[k][q].y);
+        if (lane == k * 5 + q) { tot_a += sa; tot_b += sb; }
+        acc[k][q] = zero2();
+      }
+    }
+  };
 
   auto load_seq = [&](int seq, int stage) {        // x and dL/dy tiles of sequence number seq complete on ONE barrier
     const int tile = p.ntiles - 1 - seq;
@@ -757,18 +774,13 @@ __global__ void __launch_bounds__(W * 32) eq_bwd_kernel(EqParams p) {
 #pragma unroll
     for (int j = 0; j < kE; ++j) { gu[off + j] = gq[j].x; gu[kTile + off + j] = gq[j].y; }
     warp_store(gu, oa, ob, tile, rp, lane);
+    if (jt % kFoldTiles == kFoldTiles - 1) fold();
   }
   if (rp.bulk && lane == 0) tma_store_wait_all<0>();
 
   // ---- deterministic block reduction of the 2 x 30 sums (fp64), one partial row per row of the pair ----
-#pragma unroll
-  for (int k = 0; k < kSections; ++k) {
-#pragma unroll
-    for (int q = 0; q < 5; ++q) {
-      const double sa = warp_sum((double)acc[k][q].x), sb = warp_sum((double)acc[k][q].y);
-      if (lane == 0) { red[warp][k * 5 + q][0] = sa; red[warp][k * 5 + q][1] = sb; }
-    }
-  }
+  fold();
+  if (lane < kSections * 5) { red[warp][lane][0] = tot_a; red[warp][lane][1] = tot_b; }
   __syncthreads();
   for (int o = threadIdx.x; o < kSections * 5 * 2; o += W * 32) {      // W = 1 has fewer threads than outputs
     const int h = o / (kSections * 5), e = o - h * (kSections * 5);

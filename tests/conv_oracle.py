@@ -35,10 +35,10 @@ def reverb_ir(sample_rate, params, noise, num_samples, num_bandpass_taps, dtype=
     bs = params[0].numel()
     gains = torch.stack([p.reshape(bs) for p in params[0:12]], dim=1).reshape(bs, 1, 12, 1).to(dtype)
     decays = torch.stack([p.reshape(bs) for p in params[12:24]], dim=1).reshape(bs, 1, 12, 1).to(dtype)
-    fb = oracle.octave_filterbank(num_bandpass_taps, sample_rate).to(dtype)
+    fb = oracle.octave_filterbank(num_bandpass_taps, sample_rate).to(device=noise.device, dtype=dtype)
     m = 1 << math.ceil(math.log2(noise.shape[-1] + num_bandpass_taps - 1))
     full = torch.fft.irfft(torch.fft.rfft(noise.to(dtype), m) * torch.fft.rfft(torch.flip(fb, dims=[-1]), m), m)
     shaped = full[..., num_bandpass_taps - 1: noise.shape[-1]].reshape(bs, 2, 12, num_samples)
-    t = torch.linspace(0, 1, steps=num_samples, dtype=torch.float32).to(dtype)
+    t = torch.linspace(0, 1, steps=num_samples, dtype=torch.float32).to(device=noise.device, dtype=dtype)
     env = torch.exp(-(decays * 10.0 + 1.0) * t.reshape(1, 1, 1, -1))
     return (shaped * env * gains).mean(dim=2)

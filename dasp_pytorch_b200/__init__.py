@@ -9,11 +9,14 @@ path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_sha
 ``parametric_eq_frequency_response`` (the EQ's complex transfer function at chosen frequencies, with gradients to its
 18 parameters) and ``compressor_gain`` / ``expander_gain`` (the time-varying gain the compressor / expander multiplies
 into the audio, linear or in dB, with gradients to the detector input and the parameters) and ``convolution_bus`` (any
-number of input channels, each through its own impulse responses, summed into a mono or stereo bus).
+number of input channels, each through its own impulse responses, summed into a mono or stereo bus) and
+``time_varying_convolution_reverberation`` (a trajectory of impulse responses crossfaded along the output, for moving
+sources and listeners).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
     CONV_BUS_MAX_INPUTS,
+    CONV_PARTITION_SAMPLES,
     compressor,
     compressor_gain,
     convolution_bus,
@@ -33,6 +36,7 @@ from dasp_pytorch_b200.functional import (  # noqa: F401
     stereo_bus,
     stereo_panner,
     stereo_widener,
+    time_varying_convolution_reverberation,
 )
 from dasp_pytorch_b200.modules import (  # noqa: F401
     Compressor,

@@ -39,7 +39,12 @@
 // every signal's rows are packed two per transform (bus_fft_kernel, ir_pack_kernel + x_fft_kernel's partition units),
 // bus_mac_kernel sums the untangled products over the inputs, and bus_ifft_kernel writes the outputs, dL/dx and dL/dIR.
 //
-// Both ops whose IR the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd: checks,
+// time_varying_convolution_reverberation (dasp_tvconv_*) is the same convolution with K IRs crossfaded along the
+// output: the audio windows of a static convolution, the products of the two IRs of each block (tv_mac_kernel), and
+// the crossfade in the epilogue of the inverse (tv_ifft_kernel) and in the prologue of the gradient transform
+// (tv_fft_kernel).
+//
+// The ops whose IR the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd: checks,
 // workspace, IR packing, chunk loop, zeros of the unreachable dL/dIR taps).  One IR for the whole batch
 // (dasp_conv_shared_*, dasp_conv_bus_shared_*) is the item stride 0 of the IR spectra: they are transformed once, and
 // irgrad_sum_kernel sums the items' dL/dIR spectra in fp64 before one inverse transform.
@@ -138,6 +143,8 @@ struct ConvGeom {
   int sets = 1;                 // partition sets per IR: 2 for a true-stereo IR, ceil(S O / 2) for the bus
   bool has_mix = true;          // a dry/wet mix, and with it the dL/dmix partials region (not the bus)
   bool own_only = false;        // the own FFT only: no cuFFT plans or work area, no dasp_debug_reverb_path(1) (the bus)
+  int64_t ex = 0;               // product / gradient spectra per item beyond ib: the crossfaded blocks of the
+                                // time-varying convolution, which carry two IRs' products
 };
 
 int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
@@ -2223,6 +2230,272 @@ bus_ifft_kernel(const float* __restrict__ Spl, const float* __restrict__ twiddle
   }
 }
 
+// ---- time_varying_convolution_reverberation: K IRs, IR k anchored at k hop, crossfaded linearly along the output ----
+// hop = H kB, so output block i lies in anchor interval k = i / H.  Blocks i < nX = min(I, (K - 1) H) are crossfaded
+// between IRs k and k + 1 with a = (t - k hop) / hop; later blocks carry IR K - 1 alone.  An item's product (forward)
+// and gradient (backward) spectra are U = I + nX blocks:
+//   forward  slot 2i + c (i < nX):  (Y_k,c[i], Y_k+1,c[i]) packed as real + i imag: one inverse gives output channel c
+//                                   as (1 - a) real + a imag
+//            slot nX + i (i >= nX): (Y_K-1,0[i], Y_K-1,1[i]): one inverse gives both channels, as ifft_mix_kernel
+//   backward slot 2i (i < nX):      Ga[i] = FFT of [0 | (1 - a) g block i]  (L + i R)
+//            slot 2i + 1:           Gb[i] = FFT of [0 | a g block i]
+//            slot nX + i (i >= nX): G[i]  = FFT of [0 | g block i]
+// The IR rows of an item are r = k C + c (C = 1 or 2 IR channels; a mono IR feeds both), packed two per partition set
+// by ir_pack_kernel: set s = rows (2s, 2s + 1), an odd last row with 0.
+__device__ __forceinline__ int tv_slot(int i, int nX) { return i < nX ? 2 * i : nX + i; }
+// crossfade weight a of IR k + 1 at sample t of block i (t = i kB + u)
+__device__ __forceinline__ float tv_a(int i, int H, int u, int64_t hop) {
+  return (float)((int64_t)(i - (i / H) * H) * kB + u) / (float)hop;
+}
+
+// gradient transforms, runs of kConvRun units m = il U + s: bus_fft_kernel's half == 1 path (one gradient pair per
+// unit) with the crossfade weight applied to the block in shared memory before the transform.  n % 4 == 0 and
+// 16-byte aligned rows.
+__global__ void __launch_bounds__(kFusedThreads, 1)
+tv_fft_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, const float* __restrict__ twiddles, int64_t item0,
+              int I, int nX, int H, int64_t hop, int64_t n, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int U = I + nX;
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto block = [&](int m, int& i, int& part) {     // part 0: 1 - a, 1: a, 2: no weight
+    const int u = m - (m / U) * U;
+    if (u < 2 * nX) { i = u >> 1; part = u & 1; }
+    else { i = u - nX; part = 2; }
+  };
+  auto fetch = [&](int it, int m) {                // all threads: zero padding; thread 0: the bulk copies
+    if (m >= m1) return;
+    const int64_t il = m / U;
+    int i, part;
+    block(m, i, part);
+    float* re = s.buf(it);
+    float* im = re + fft8k::kPlaneG;
+    const int64_t s0 = (int64_t)i * kB;
+    const int64_t rem = n - s0;
+    const int len = rem < kB ? (int)rem : kB;
+    for (int e = t; e < kB; e += kFusedThreads) { re[e] = 0.f; im[e] = 0.f; }
+    for (int e = kB + len + t; e < kNbA; e += kFusedThreads) { re[e] = 0.f; im[e] = 0.f; }
+    if (t == 0) {
+      const float* gl = gy + ((item0 + il) * 2) * n + s0;
+      uint64_t* bar = &s.full[it & 1];
+      mbar_arrive_expect_tx(bar, 2u * (uint32_t)len * 4u);
+      tma_load_1d(re + kB, gl, (uint32_t)len * 4u, bar);
+      tma_load_1d(im + kB, gl + n, (uint32_t)len * 4u, bar);
+    }
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  __syncthreads();
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    float* gi = gr + fft8k::kPlaneG;
+    int i, part;
+    block(m, i, part);
+    if (part < 2) {                                // uniform over the CTA
+      for (int e = t; e < kB; e += kFusedThreads) {
+        const float a = tv_a(i, H, e, hop);
+        const float w = part ? a : 1.0f - a;
+        gr[kB + e] *= w;
+        gi[kB + e] *= w;
+      }
+      __syncthreads();
+    }
+    float xr[16], xi[16];
+    fft8192_in_smem<false>(gr, gi, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    float2* out = Gb + (int64_t)m * kNbA;
+#pragma unroll
+    for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(xr[q], xi[q]);
+  }
+}
+
+// inverse transforms of the product slots, runs of kConvRun units m = il U + s, with ifft_mix_kernel's crop and
+// dry/wet mix and the crossfade in the epilogue: y_c = (1 - mix) x_c + mix wet_c on samples [i kB, (i+1) kB) ∩ [0, n).
+__global__ void __launch_bounds__(kFusedThreads, 1)
+tv_ifft_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddles, const float* __restrict__ x,
+               const float* __restrict__ mix_p, float* __restrict__ y, int64_t item0, int I, int nX, int H, int64_t hop,
+               int64_t n, int in_chs, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int U = I + nX;
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {
+    if (t == 0 && m < m1) s.load_planar(it, Ypl + (int64_t)m * 2 * kNbA);
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    const int64_t il = m / U, b = item0 + il;
+    const int u = m - (int)il * U;
+    const bool cross = u < 2 * nX;                 // uniform over the CTA
+    const int i = cross ? u >> 1 : u - nX, c = cross ? u & 1 : 0;
+    const float mix = mix_p[b];
+    const float* xl = x + (b * in_chs) * n;
+    const float* xrr = in_chs == 1 ? xl : xl + n;
+    float a0[8], a1[8];                            // the dry samples of this thread's 8 outputs
+    float xr[16], xi[16];
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2); },
+                          [&] {
+#pragma unroll
+                            for (int q = 0; q < 8; ++q) {
+                              const int64_t tg = (int64_t)i * kB + (t + 512 * q);
+                              a0[q] = tg < n ? xl[tg] : 0.f;
+                              a1[q] = tg < n ? xrr[tg] : 0.f;
+                            }
+                          },
+                          xr, xi);
+#pragma unroll
+    for (int q = 8; q < 16; ++q) {                 // outputs kB .. 2 kB - 1 of the transform
+      const int e = t + 512 * q - kB;
+      const int64_t tg = (int64_t)i * kB + e;
+      if (tg < n) {
+        if (cross) {
+          const float a = tv_a(i, H, e, hop);
+          const float wet = fmaf(a, xi[q], (1.0f - a) * xr[q]);
+          const float dry = c ? a1[q - 8] : a0[q - 8];
+          y[(b * 2 + c) * n + tg] = fmaf(mix, wet - dry, dry);
+        } else {
+          y[(b * 2 + 0) * n + tg] = fmaf(mix, xr[q] - a0[q - 8], a0[q - 8]);
+          y[(b * 2 + 1) * n + tg] = fmaf(mix, xi[q] - a1[q - 8], a1[q - 8]);
+        }
+      }
+    }
+  }
+}
+
+// The products of the time-varying convolution per bin pair (f, kNbA - f) and item, every operand untangled into the
+// spectra of its real rows (X_c: audio channel c, H_k,c: IR k's channel c, G: the gradient slots), results packed two
+// real rows per block, planar, scaled by 1 / kNbA; all operands from L2.
+//   TV_FWD: Y_k,c[i] = sum_j X_c[i - j] H_k,c[j] for the IRs of block i          out: U slots per item (see above)
+//   TV_DX:  D_c[m] = sum_j Ga_c[m+j] conj(H_k(m+j),c[j]) + Gb_c[m+j] conj(H_k(m+j)+1,c[j])
+//                                                                                out: I blocks per item (D_0 + i D_1)
+//   TV_DIR: E_k,c[j] = sum_{i in interval k} Ga_c[i] conj(X_c[i-j]) + sum_{i in interval k-1} Gb_c[i] conj(X_c[i-j]),
+//           times mix[b] when mix is not null (a shared trajectory's factors are applied by irgrad_sum_kernel); a mono
+//           IR row k receives E_k,0 + E_k,1                                     out: sets J blocks per item
+// H: sets J partitions per trajectory at item stride hstride (0: one trajectory for the batch).
+enum TvMac { TV_FWD, TV_DX, TV_DIR };
+template <int MODE, int C>
+__global__ void __launch_bounds__(128) tv_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                     int64_t hstride, const float2* __restrict__ G,
+                                                     const float* __restrict__ mix, float2* __restrict__ Out,
+                                                     int64_t item0, int I, int J, int K, int nX, int Hb, int sets) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int64_t il = blockIdx.y;
+  const int U = I + nX;
+  const float2* x = X + il * (int64_t)I * kNbA;
+  const float2* h = H + il * hstride;
+  const float2* g = G + il * (int64_t)U * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  auto hin = [&](int k, int j, float2& h0, float2& h1) {     // IR k at partition j, channels 0 and 1
+    if (C == 2) { pair(h, (int64_t)k * J + j, h0, h1); }
+    else { float2 a, b; pair(h, (int64_t)(k >> 1) * J + j, a, b); h0 = h1 = (k & 1) ? b : a; }
+  };
+  const float scale = 1.0f / (float)kNbA;
+  auto emit = [&](int64_t slot, float2 a, float2 b, float sc) {
+    a.x *= sc; a.y *= sc; b.x *= sc; b.y *= sc;
+    float* pl = reinterpret_cast<float*>(Out + slot * kNbA);
+    pl[f] = a.x - b.y; pl[kNbA + f] = a.y + b.x;
+    if (fm != f) { pl[fm] = a.x + b.y; pl[kNbA + fm] = b.x - a.y; }
+  };
+  auto ival = [&](int i) { const int k = i / Hb; return k < K - 1 ? k : K - 1; };   // anchor interval of block i
+
+  if constexpr (MODE == TV_FWD) {
+    for (int o = 0; o < I; ++o) {
+      const int k = ival(o);
+      const bool cross = o < nX;
+      float2 y0 = zero, y1 = zero, z0 = zero, z1 = zero;    // IR k: channels 0, 1; IR k + 1: channels 0, 1
+      for (int j = 0; j <= o && j < J; ++j) {
+        float2 x0, x1, h0, h1;
+        pair(x, o - j, x0, x1);
+        hin(k, j, h0, h1);
+        cfma(y0, x0, h0);
+        cfma(y1, x1, h1);
+        if (cross) {
+          hin(k + 1, j, h0, h1);
+          cfma(z0, x0, h0);
+          cfma(z1, x1, h1);
+        }
+      }
+      const int64_t ob = il * (int64_t)U;
+      if (cross) { emit(ob + 2 * o, y0, z0, scale); emit(ob + 2 * o + 1, y1, z1, scale); }
+      else emit(ob + nX + o, y0, y1, scale);
+    }
+  } else if constexpr (MODE == TV_DX) {
+    for (int m = 0; m < I; ++m) {
+      float2 d0 = zero, d1 = zero;
+      for (int j = 0; j < J && m + j < I; ++j) {
+        const int i = m + j, k = ival(i);
+        float2 g0, g1, h0, h1;
+        pair(g, tv_slot(i, nX), g0, g1);
+        hin(k, j, h0, h1);
+        cfma_conj(d0, g0, h0);
+        cfma_conj(d1, g1, h1);
+        if (i < nX) {
+          pair(g, 2 * i + 1, g0, g1);
+          hin(k + 1, j, h0, h1);
+          cfma_conj(d0, g0, h0);
+          cfma_conj(d1, g1, h1);
+        }
+      }
+      emit(il * (int64_t)I + m, d0, d1, scale);
+    }
+  } else {
+    static_assert(MODE == TV_DIR, "tv_mac_kernel: unknown mode");
+    const float sc = mix ? mix[item0 + il] * scale : scale;
+    // E_k,c[j] over both intervals that carry IR k
+    auto ecorr = [&](int k, int j, float2& e0, float2& e1) {
+      e0 = e1 = zero;
+      for (int part = 0; part < 2; ++part) {       // 0: Ga of interval k, 1: Gb of interval k - 1
+        const int kk = k - part;
+        if (kk < 0) continue;
+        const int lo = kk * Hb, hi = kk == K - 1 ? I : ((kk + 1) * Hb < I ? (kk + 1) * Hb : I);
+        for (int i = lo > j ? lo : j; i < hi; ++i) {
+          float2 g0, g1, x0, x1;
+          pair(g, part ? 2 * i + 1 : tv_slot(i, nX), g0, g1);
+          pair(x, i - j, x0, x1);
+          cfma_conj(e0, g0, x0);
+          cfma_conj(e1, g1, x1);
+        }
+      }
+    };
+    const int64_t ob = il * (int64_t)sets * J;
+    for (int sI = 0; sI < sets; ++sI) {
+      for (int j = 0; j < J; ++j) {
+        float2 e0, e1;
+        if (C == 2) {
+          ecorr(sI, j, e0, e1);
+          emit(ob + (int64_t)sI * J + j, e0, e1, sc);
+        } else {
+          float2 p0, p1, q = zero;
+          ecorr(2 * sI, j, p0, p1);
+          if (2 * sI + 1 < K) {
+            ecorr(2 * sI + 1, j, e0, e1);
+            q = make_float2(e0.x + e1.x, e0.y + e1.y);
+          }
+          emit(ob + (int64_t)sI * J + j, make_float2(p0.x + p1.x, p0.y + p1.y), q, sc);
+        }
+      }
+    }
+  }
+}
+
 // Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
 // spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
 // transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
@@ -2449,7 +2722,7 @@ struct BwdWs { size_t gs, ds, es, extra, mixpart, acc, cufft, total; };
 
 void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs& w) {
   size_t o = 0;
-  w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * (g.ib + g.ex) * kNbA));
   // transient homes for what a forward WITHOUT a backward does not keep (null *_save pointers)
   w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.p * g.ib * kNbA));
   w.hsp = o; o += align256(sizeof(float2) * (size_t)((g.shared ? 1 : g.chunk) * g.sets * g.jb * kNbA));
@@ -2459,7 +2732,7 @@ void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs&
 }
 void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs& w) {
   size_t o = 0;
-  w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.ib * kNbA));
+  w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * (g.ib + g.ex) * kNbA));
   w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.p * g.ib * kNbA));
   w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
@@ -2569,6 +2842,8 @@ int configure_fft_kernels() {
     DASP_CUDA_OK(cudaFuncSetAttribute(ifft_irtaps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(bus_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(bus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(tv_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(tv_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     configured[dev] = true;
   }
   return DASP_OK;
@@ -3427,6 +3702,183 @@ int dasp_conv_bus_shared_bwd(const float* gy, const void* xspec_save, const void
                              int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
   return conv_bus_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, inputs,
                       outputs, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ time_varying_convolution_reverberation
+// wet = sum_k w_k(t) (x * h_k)(t), y = (1 - mix) x + mix wet, through the stage above on the own FFT only: the audio
+// windows as a static convolution (x_fft_kernel, one spectrum per block, saved the same way), K C IR rows per item
+// in ceil(K C / 2) partition sets, and the tv_* kernels for the crossfaded products, their inverse and the weighted
+// gradient transforms.  dL/dx and dL/dmix are ifft_dx_kernel's (the weighted correlation D is the gradient of the wet
+// signal with respect to x, so sum_t g wet = sum_s x c holds as for a static IR).
+namespace {
+int g_tv_last_path[2] = {0, 0};                      // test hook: dispatch of the last forward / backward
+
+extern "C++" {
+template <int MODE>
+int launch_tv_mac(int C, const float2* X, const float2* H, int64_t hstride, const float2* G, const float* mix,
+                  float2* Out, int64_t item0, int64_t items, int I, int J, int K, int nX, int Hb, int sets,
+                  cudaStream_t st) {
+  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+  if (C == 2) tv_mac_kernel<MODE, 2><<<grid, 128, 0, st>>>(X, H, hstride, G, mix, Out, item0, I, J, K, nX, Hb, sets);
+  else        tv_mac_kernel<MODE, 1><<<grid, 128, 0, st>>>(X, H, hstride, G, mix, Out, item0, I, J, K, nX, Hb, sets);
+  DASP_LAUNCH_OK("tv_mac_kernel");
+  return DASP_OK;
+}
+}  // extern "C++"
+
+struct TvConvOp {
+  static constexpr const char* kFwd = "tvconv fwd";
+  static constexpr const char* kBwd = "tvconv bwd";
+  static constexpr bool kOddSelf = false;
+  int in_chs, C, K, Hb, ir_rows;                     // x channels, IR channels, anchors, hop / kB, IR rows K C
+  int fwd_chunk(const ConvGeom& g, const Plans&, bool own, const float* tw, const float* x, const float* mix,
+                float2* xs, float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    // bit 0: own FFT (always), bit 1: one trajectory shared by the batch, bit 2: crossfaded blocks (K > 1)
+    g_tv_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (g.ex > 0 ? 4 : 0);
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* ys = (float2*)(ws + w.ys);
+    const int I = (int)g.ib, J = (int)g.jb, nX = (int)g.ex;
+    const int nwin = (int)(items * I), nunits = nwin + (int)(h_stride != 0 ? items * g.sets * J : 0);
+    x_fft_kernel<<<runs(nunits), kFusedThreads, kFftSmemBytes, st>>>(x, xs, hs, tw, item0, I, J, g.n, g.leff, in_chs,
+                                                                      nwin, nunits);
+    DASP_LAUNCH_OK("x_fft_kernel");
+    if ((rc = launch_tv_mac<TV_FWD>(C, xs, hs, h_stride, nullptr, nullptr, ys, item0, items, I, J, K, nX, Hb, g.sets,
+                                    st)) != DASP_OK)
+      return rc;
+    const int nout = (int)(items * (I + nX));
+    tv_ifft_kernel<<<runs(nout), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, x, mix, y,
+                                                                     item0, I, nX, Hb, (int64_t)Hb * kB, g.n, in_chs,
+                                                                     nout);
+    DASP_LAUNCH_OK("tv_ifft_kernel");
+    return DASP_OK;
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans&, bool own, IrGrad e, const float* tw, const float* gy, const float* x,
+                const float* mix, const float2* xs, const float2* hs, int64_t h_stride, float* gx, unsigned char* ws,
+                const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    // bit 0: own FFT (always), bit 1: crossfaded blocks (K > 1), bit 2: dL/dIR computed, bit 3: shared trajectory
+    g_tv_last_path[1] = (own ? 1 : 0) | (g.ex > 0 ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) | (g.shared ? 8 : 0);
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* gs = (float2*)(ws + w.gs);
+    float2* ds = (float2*)(ws + w.ds);
+    const int I = (int)g.ib, J = (int)g.jb, nX = (int)g.ex;
+    const int ng = (int)(items * (I + nX));
+    tv_fft_kernel<<<runs(ng), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, I, nX, Hb, (int64_t)Hb * kB, g.n,
+                                                                  ng);
+    DASP_LAUNCH_OK("tv_fft_kernel");
+    if ((rc = launch_tv_mac<TV_DX>(C, xs, hs, h_stride, gs, nullptr, ds, item0, items, I, J, K, nX, Hb, g.sets, st)) !=
+        DASP_OK)
+      return rc;
+    ifft_dx_kernel<<<persistent_grid(items), kFusedThreads, kFftSmemBytes, st>>>(
+        reinterpret_cast<const float*>(ds), tw, gy, x, mix, 1, gx, (float*)(ws + w.mixpart), item0, (int)items, I, g.n,
+        in_chs);
+    DASP_LAUNCH_OK("ifft_dx_kernel");
+    if (e == IrGrad::kNone) return DASP_OK;          // a fixed trajectory: no dL/dIR work at all
+    // per item the factor mix[b] goes into E here; a shared trajectory's is applied by irgrad_sum_kernel
+    return launch_tv_mac<TV_DIR>(C, xs, hs, h_stride, gs, g.shared ? nullptr : mix, (float2*)(ws + w.es), item0, items,
+                                 I, J, K, nX, Hb, g.sets, st);
+  }
+  // dL/dIR taps [0, leff) of items [item0, item0 + items): the first half of the inverse of each partition (the factor
+  // mix is in the partitions already)
+  int ir_taps(const ConvGeom& g, bool, const float* tw, const float2* es, const float*, float* gir, int64_t item0,
+              int64_t items, cudaStream_t st) const {
+    const int J = (int)g.jb, nparts = (int)(items * g.sets * J);
+    bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir,
+                                                                        item0, ir_rows, g.sets, J, g.L, g.leff, 0,
+                                                                        nparts);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    return DASP_OK;
+  }
+};
+
+// the argument checks of dasp_tvconv_*, filling the geometry
+int make_tv_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t K, int64_t ir_chs, int64_t hop, int64_t chunk,
+                 ConvGeom& g) {
+  DASP_REQUIRE(K >= 1, "tvconv: K >= 1 impulse responses are needed, got %lld", (long long)K);
+  DASP_REQUIRE(ir_chs == 1 || ir_chs == 2, "tvconv: mono or stereo impulse responses only, got %lld channels",
+               (long long)ir_chs);
+  DASP_REQUIRE(hop > 0 && hop % kB == 0, "tvconv: hop must be a positive multiple of %d, got %lld", kB,
+               (long long)hop);
+  int rc = make_conv_geom(bs, n, L, chunk, g);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE(K - 1 <= (n - 1) / hop, "tvconv: anchor %lld at (K - 1) hop is at or after the end of x (n=%lld)",
+               (long long)(K - 1), (long long)n);
+  g.shared = shared;
+  g.sets = (int)((K * ir_chs + 1) / 2);
+  g.ex = (K - 1) * (hop / kB);                     // < ib: every crossfaded block is inside x
+  g.own_only = true;
+  return DASP_OK;
+}
+TvConvOp tv_op(int64_t in_chs, int64_t ir_chs, int64_t K, int64_t hop) {
+  return TvConvOp{(int)in_chs, (int)ir_chs, (int)K, (int)(hop / kB), (int)(K * ir_chs)};
+}
+
+int tvconv_fwd(bool shared, const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, int64_t K,
+               int64_t hop, const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+               int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_tv_geom(shared, bs, n, ir_len, K, ir_chs, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE(in_chs == 1 || in_chs == 2, "tvconv: only mono/stereo signals, got %lld channels", (long long)in_chs);
+  return caller_ir_fwd(tv_op(in_chs, ir_chs, K, hop), g, x, ir, mix, y, xspec_save, irspec_save, workspace,
+                       workspace_bytes, stream);
+}
+
+int tvconv_bwd(bool shared, const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, int64_t K,
+               int64_t hop, const float* mix, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+               float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items,
+               void* stream) {
+  ConvGeom g;
+  int rc = make_tv_geom(shared, bs, n, ir_len, K, ir_chs, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE(in_chs == 1 || in_chs == 2, "tvconv: only mono/stereo signals, got %lld channels", (long long)in_chs);
+  return caller_ir_bwd(tv_op(in_chs, ir_chs, K, hop), g, gy, x, mix, xspec_save, irspec_save, gx, gir, gmix, workspace,
+                       workspace_bytes, stream);
+}
+}  // namespace
+
+int dasp_debug_tvconv_last_path(int which) { return g_tv_last_path[which ? 1 : 0]; }
+
+int dasp_tvconv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t ir_chs, int64_t hop, int64_t shared,
+                         int64_t chunk_items, dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "tvconv geometry: null out");
+  ConvGeom g;
+  int rc = make_tv_geom(shared != 0, bs, n, ir_len, K, ir_chs, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
+}
+
+int dasp_tvconv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, int64_t K,
+                    int64_t hop, const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                    int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream) {
+  return tvconv_fwd(false, x, in_chs, ir, ir_chs, ir_len, K, hop, mix, y, xspec_save, irspec_save, workspace,
+                    workspace_bytes, bs, n, chunk_items, stream);
+}
+
+int dasp_tvconv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, int64_t K,
+                    int64_t hop, const float* mix, const void* xspec_save, const void* irspec_save, float* gx,
+                    float* gir, float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                    int64_t chunk_items, void* stream) {
+  return tvconv_bwd(false, gy, x, in_chs, ir_chs, ir_len, K, hop, mix, xspec_save, irspec_save, gx, gir, gmix,
+                    workspace, workspace_bytes, bs, n, chunk_items, stream);
+}
+
+int dasp_tvconv_shared_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, int64_t K,
+                           int64_t hop, const float* mix, float* y, void* xspec_save, void* irspec_save,
+                           void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items,
+                           void* stream) {
+  return tvconv_fwd(true, x, in_chs, ir, ir_chs, ir_len, K, hop, mix, y, xspec_save, irspec_save, workspace,
+                    workspace_bytes, bs, n, chunk_items, stream);
+}
+
+int dasp_tvconv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, int64_t K,
+                           int64_t hop, const float* mix, const void* xspec_save, const void* irspec_save, float* gx,
+                           float* gir, float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                           int64_t chunk_items, void* stream) {
+  return tvconv_bwd(true, gy, x, in_chs, ir_chs, ir_len, K, hop, mix, xspec_save, irspec_save, gx, gir, gmix,
+                    workspace, workspace_bytes, bs, n, chunk_items, stream);
 }
 
 // ------------------------------------------------------------------ noise_shaped_impulse_response

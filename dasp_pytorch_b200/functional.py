@@ -37,6 +37,7 @@ __all__ = [
     "noise_shaped_reverberation",
     "convolution_reverberation",
     "convolution_bus",
+    "time_varying_convolution_reverberation",
     "noise_shaped_impulse_response",
     "noise_shaped_impulse_response_packed",
     "parametric_eq_frequency_response",
@@ -1513,4 +1514,148 @@ def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch
     elif xf.data_ptr() % 16:
         xf = xf.clone()
     y = _ConvBusFn.apply(xf, irf, reverb_chunk_items(xf.device))
+    return (y[..., :n] if n4 != n else y).to(dt)
+
+
+# --------------------------------------------------------------------------------------
+# time_varying_convolution_reverberation
+# --------------------------------------------------------------------------------------
+
+CONV_PARTITION_SAMPLES = 4096      # conv_block of dasp_conv_geom: the partition length of every caller-IR convolution
+
+
+class _TvConvFn(torch.autograd.Function):
+    """x (bs, 1|2, n), ir (bs | 1, K, 1|2, L), mix (bs,) -> y (bs, 2, n).  n % 4 == 0 and 16-byte aligned rows
+    (time_varying_convolution_reverberation pads).  An ir of batch 1 with bs > 1 runs the dasp_tvconv_shared_* entry
+    points; its gradient is the sum over the items."""
+
+    @staticmethod
+    def forward(ctx, x, ir, mix, hop, chunk):
+        lib = _abi.lib()
+        bs, in_chs, n = x.shape
+        ir_bs, K, ir_chs, ir_len = ir.shape
+        shared = ir_bs == 1 and bs > 1
+        kind = "tvconv_shared" if shared else "tvconv"
+        dev = x.device
+        y = torch.empty(bs, 2, n, dtype=torch.float32, device=dev)
+        need_bwd = any(ctx.needs_input_grad[:3])
+        with torch.cuda.device(dev):
+            ws, (xspec, irspec), bwd_bytes = _geom_buffers(
+                _abi.ConvGeom(), "dasp_tvconv_geometry", (bs, n, ir_len, K, ir_chs, hop, int(shared), chunk), dev,
+                need_bwd)
+            with _timed("tvconv_fwd", dev):
+                check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), in_chs, ptr(ir), ir_chs, ir_len, K, hop, ptr(mix),
+                                                       ptr(y), ptr(xspec), ptr(irspec), ptr(ws), ws.numel(), bs, n,
+                                                       chunk, stream_ptr(dev)),
+                      f"dasp_{kind}_fwd")
+        if need_bwd:
+            ctx.save_for_backward(x, xspec, irspec, mix)
+        ctx.cfg = (kind, ir.shape, hop, chunk, bwd_bytes)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _abi.lib()
+        x, xspec, irspec, mix = ctx.saved_tensors
+        kind, ir_shape, hop, chunk, bwd_bytes = ctx.cfg
+        bs, in_chs, n = x.shape
+        dev = x.device
+        gy = gy.contiguous()
+        if gy.data_ptr() % 16:
+            gy = gy.clone()
+        gx = torch.empty_like(x)
+        # a fixed trajectory (measured or simulated rooms) skips every dL/dIR kernel
+        gir = torch.empty(ir_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        gmix = torch.empty_like(mix)
+        ws = _ws_bytes(bwd_bytes, dev)
+        with torch.cuda.device(dev), _timed("tvconv_bwd", dev):
+            check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(x), in_chs, ir_shape[2], ir_shape[3], ir_shape[1], hop,
+                                                   ptr(mix), ptr(xspec), ptr(irspec), ptr(gx), ptr(gir), ptr(gmix),
+                                                   ptr(ws), ws.numel(), bs, n, chunk, stream_ptr(dev)),
+                  f"dasp_{kind}_bwd")
+        return gx, gir, gmix, None, None
+
+
+def time_varying_convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor,
+                                           hop: int, mix: torch.Tensor):
+    """Convolution reverb with a trajectory of K impulse responses, crossfaded along the output: a talker walking past
+    a microphone, a head-tracked binaural rendering, a listener moving through a room, a door opening, an automated or
+    learnt time-varying FIR.  IR ``k`` belongs to the anchor time ``t_k = k * hop``::
+
+        wet(t) = sum_k w_k(t) (x * h_k)(t),    y = (1 - mix) x + mix wet
+
+        k hop <= t < (k+1) hop, k < K - 1:   a = (t - k hop) / hop,   w_k = 1 - a,   w_{k+1} = a,   other w = 0
+        t >= (K - 1) hop:                    w_{K-1} = 1
+
+    (``*`` the causal convolution cropped to ``n``, exactly as ``convolution_reverberation`` defines its wet signal).
+    At every anchor time, and after the last one, the output is the static convolution with that anchor's IR; between
+    two anchors it is a linear crossfade of the outputs of the two neighbouring IRs.
+
+    This is output-side (listener-side) interpolation because it is the interpolation that overlap-save supports
+    without splitting the audio windows: every output block lies inside one anchor interval, so it needs the products
+    of two IRs with the same window spectra a static convolution uses, and the crossfade is applied to the inverse
+    transform's output.  Input-side weighting, ``sum_k (w_k x) * h_k``, would need zero-padded transforms per block
+    and IR, because an overlap-save window straddles anchor boundaries.
+
+    Args:
+        x: audio ``(bs, 1|2, n)``; mono is used for both channels.
+        sample_rate: unused (kept for the common processor signature).
+        impulse_response: ``(bs, K, 1|2, L)``, one trajectory per item, or ``(1, K, 1|2, L)``, one trajectory shared by
+            the batch; ``K >= 1``, any ``L >= 1``; a mono IR feeds both channels.
+        hop: the anchor spacing in samples, a positive multiple of ``CONV_PARTITION_SAMPLES`` (4096), the partition
+            length of the convolution, so that every output block and every gradient block lies inside one anchor
+            interval; ``(K - 1) * hop < n``.
+        mix: ``bs`` elements in any shape, or one element that is broadcast over the batch.
+
+    Returns ``(bs, 2, n)`` in x's dtype, computed in fp32.  ``K = 1`` is ``convolution_reverberation(x, sr, h[:, 0],
+    mix)``, and K equal IRs are that IR's static convolution, both to fp32 rounding.  Gradients flow to ``x``, to every
+    IR of the trajectory (a mono IR receives the sum of both channel gradients; taps at or beyond ``min(L, n)`` get
+    exactly 0) and to ``mix``.  The gradient of a shared ``(1, K, C, L)`` trajectory has that shape and is the sum over
+    the items, accumulated in fp64 in item order, so it does not depend on ``REVERB_CHUNK_ITEMS``.  When the IRs do
+    not require a gradient, the backward skips all dL/dIR work.
+
+    Cost: the audio windows are transformed once, as for one static IR, and kept for the backward once; the K IRs'
+    partitions are transformed once each; a block between two anchors takes two inverse transforms (the two IRs'
+    products, one channel each), a block after the last anchor one.  K full-length ``convolution_reverberation`` calls
+    would transform and keep the audio windows K times.  Rows whose length is not a multiple of 4 are zero-padded to
+    one (the transforms bulk-copy 16-byte rows); a padding sample reaches no output sample below ``n``.
+    """
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, channels, samples)")
+    if x.shape[1] not in (1, 2):
+        raise ValueError(f"x: only mono/stereo is supported, got {x.shape[1]} channels")
+    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 4:
+        raise ValueError("impulse_response must be a tensor of shape (batch, K, channels, taps)")
+    _, K, ir_chs, L = impulse_response.shape
+    if ir_chs not in (1, 2):
+        raise ValueError(f"impulse_response: only mono/stereo is supported, got {ir_chs} channels")
+    if K < 1:
+        raise ValueError("impulse_response needs at least one impulse response (K >= 1)")
+    bs, _, n = x.shape
+    _caller_ir_shape(impulse_response, bs)
+    if n < 1:
+        raise ValueError("x needs at least one sample")
+    if isinstance(hop, bool) or not isinstance(hop, int) and not (torch.is_tensor(hop) and hop.numel() == 1
+                                                                  and not hop.is_floating_point()):
+        raise ValueError(f"hop must be an integer number of samples, got {hop!r}")
+    hop = int(hop)
+    if hop <= 0 or hop % CONV_PARTITION_SAMPLES:
+        raise ValueError(f"hop must be a positive multiple of {CONV_PARTITION_SAMPLES} samples, got {hop}")
+    if (K - 1) * hop >= n:
+        raise ValueError(f"impulse response {K - 1} is anchored at (K - 1) * hop = {(K - 1) * hop}, at or after the "
+                         f"end of x ({n} samples)")
+    nmix = mix.numel() if torch.is_tensor(mix) else torch.as_tensor(mix).numel()
+    if nmix not in (1, bs):
+        raise ValueError(f"mix: expected {bs} element(s) (one per batch item) or 1, got {nmix}")
+    xf, dt = _audio(x)
+    irf = _caller_ir(impulse_response, xf, 4)
+    m = _param(mix, bs, xf, "mix", allow_broadcast=True).contiguous()
+    n4 = (n + 3) // 4 * 4
+    if n4 != n:
+        xf = torch.nn.functional.pad(xf, (0, n4 - n))
+        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
+            irf = irf[..., :n].contiguous()
+    elif xf.data_ptr() % 16:
+        xf = xf.clone()
+    y = _TvConvFn.apply(xf, irf, m, hop, reverb_chunk_items(xf.device))
     return (y[..., :n] if n4 != n else y).to(dt)

@@ -354,6 +354,43 @@ int dasp_conv_bus_shared_bwd(const float* gy, const void* xspec_save, const void
    register-cached products, bit 2 = dL/dIR computed, bit 3 = shared IR */
 int dasp_debug_conv_bus_last_path(int which);
 
+/* ---- time_varying_convolution_reverberation: a trajectory of K impulse responses crossfaded along the output -------
+ * x is (bs, in_chs, n) with in_chs 1 or 2, ir is (bs, K, ir_chs, ir_len) with ir_chs 1 or 2 (or ONE (K, ir_chs, ir_len)
+ * trajectory for the whole batch: the *_shared_* entry points), mix has bs elements, y is (bs, 2, n).  IR k belongs to
+ * the anchor time k hop, hop a positive multiple of conv_block (4096) with (K - 1) hop < n:
+ *   wet(t) = sum_k w_k(t) (x * h_k)(t),  y = (1 - mix) x + mix wet  (* as convolution_reverberation's wet signal)
+ *   k hop <= t < (k+1) hop, k < K - 1:  a = (t - k hop) / hop,  w_k = 1 - a,  w_k+1 = a;   t >= (K-1) hop:  w_K-1 = 1
+ * A mono x or IR is used for both channels.  The audio windows are transformed once per block, as for one static IR;
+ * a block between two anchors takes the products of its two IRs, each packed with its other channel or its
+ * neighbour so that one inverse transform carries two real rows.  n % 4 == 0 and 16-byte aligned x / gy rows are
+ * required.  Buffers kept for the backward (NULL for both when no backward follows): xspec_save geom.xspec_c64 and
+ * irspec_save geom.irspec_c64 complex64.  Backward: gx (bs, in_chs, n), gmix (bs,), gir (bs, K, ir_chs, ir_len)
+ * (shared: (K, ir_chs, ir_len), the sum over the items in fp64 in item order, the same bits for every chunk_items), or
+ * NULL, which skips all dL/dIR work; a mono IR receives the sum of both channel gradients; taps >= leff =
+ * min(ir_len, n) get 0.  Workspace sizes come from dasp_tvconv_geometry (shared != 0 for the shared entry points),
+ * which needs no GPU.  Bad K, hop, channel counts or shapes are rejected before any CUDA call. */
+int dasp_tvconv_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t ir_chs, int64_t hop, int64_t shared,
+                         int64_t chunk_items, dasp_conv_geom* out);
+int dasp_tvconv_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, int64_t K,
+                    int64_t hop, const float* mix, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                    int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items, void* stream);
+int dasp_tvconv_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, int64_t K,
+                    int64_t hop, const float* mix, const void* xspec_save, const void* irspec_save, float* gx,
+                    float* gir /* may be NULL */, float* gmix, void* workspace, int64_t workspace_bytes, int64_t bs,
+                    int64_t n, int64_t chunk_items, void* stream);
+int dasp_tvconv_shared_fwd(const float* x, int64_t in_chs, const float* ir, int64_t ir_chs, int64_t ir_len, int64_t K,
+                           int64_t hop, const float* mix, float* y, void* xspec_save, void* irspec_save,
+                           void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t chunk_items,
+                           void* stream);
+int dasp_tvconv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int64_t ir_chs, int64_t ir_len, int64_t K,
+                           int64_t hop, const float* mix, const void* xspec_save, const void* irspec_save, float* gx,
+                           float* gir /* may be NULL */, float* gmix, void* workspace, int64_t workspace_bytes,
+                           int64_t bs, int64_t n, int64_t chunk_items, void* stream);
+/* test hook: dispatch of the most recent call.  which = 0 (forward): bit 0 = own in-shared-memory FFT (always),
+   bit 1 = shared trajectory, bit 2 = crossfaded blocks (K > 1).  which = 1 (backward): bit 0 = own FFT (always),
+   bit 1 = crossfaded blocks, bit 2 = dL/dIR computed, bit 3 = shared trajectory */
+int dasp_debug_tvconv_last_path(int which);
+
 #ifdef __cplusplus
 }
 #endif

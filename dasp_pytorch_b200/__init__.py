@@ -11,7 +11,8 @@ path -- ``gain``, ``distortion``, ``parametric_eq``, ``compressor``, ``noise_sha
 into the audio, linear or in dB, with gradients to the detector input and the parameters) and ``convolution_bus`` (any
 number of input channels, each through its own impulse responses, summed into a mono or stereo bus) and
 ``time_varying_convolution_reverberation`` (a trajectory of impulse responses crossfaded along the output, for moving
-sources and listeners).
+sources and listeners) and ``time_varying_convolution_bus`` (several moving sources, each with its own trajectory of
+impulse responses, crossfaded and summed into a mono or stereo bus).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
@@ -36,6 +37,7 @@ from dasp_pytorch_b200.functional import (  # noqa: F401
     stereo_bus,
     stereo_panner,
     stereo_widener,
+    time_varying_convolution_bus,
     time_varying_convolution_reverberation,
 )
 from dasp_pytorch_b200.modules import (  # noqa: F401

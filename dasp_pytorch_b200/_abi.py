@@ -104,6 +104,12 @@ _SIGNATURES = {
     "dasp_tvconv_shared_fwd": (c_int, [P, I64, P, I64, I64, I64, I64, P, P, P, P, P, I64, I64, I64, I64, P]),
     "dasp_tvconv_shared_bwd": (c_int, [P, P, I64, I64, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, P]),
     "dasp_debug_tvconv_last_path": (c_int, [c_int]),
+    "dasp_tvbus_geometry": (c_int, [I64, I64, I64, I64, I64, I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
+    "dasp_tvbus_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvbus_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvbus_shared_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvbus_shared_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_debug_tvbus_last_path": (c_int, [c_int]),
     "dasp_dynamics_tile_len": (I64, [I64, I64]),
     "dasp_dynamics_fwd": (c_int, [c_int, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),
     "dasp_dynamics_bwd": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),

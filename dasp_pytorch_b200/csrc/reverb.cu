@@ -44,6 +44,10 @@
 // the crossfade in the epilogue of the inverse (tv_ifft_kernel) and in the prologue of the gradient transform
 // (tv_fft_kernel).
 //
+// time_varying_convolution_bus (dasp_tvbus_*) combines the two: the bus's packed window spectra, IR trajectories for
+// every source-to-output path, the two IR sets' products per block summed over the sources (tvbus_mac_kernel), and one
+// crossfaded inverse per output row and block (tvbus_ifft_kernel).
+//
 // The ops whose IR the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd: checks,
 // workspace, IR packing, chunk loop, zeros of the unreachable dL/dIR taps).  One IR for the whole batch
 // (dasp_conv_shared_*, dasp_conv_bus_shared_*) is the item stride 0 of the IR spectra: they are transformed once, and
@@ -2496,6 +2500,291 @@ __global__ void __launch_bounds__(128) tv_mac_kernel(const float2* __restrict__ 
   }
 }
 
+// ---- time_varying_convolution_bus: S sources, each with its own IR trajectory, crossfaded and summed into O outputs --
+// The bus's packing (the S inputs in P = ceil(S / 2) window spectra per block, bus_fft_kernel's; the K S O IR rows
+// r = (k S + s) O + o in NH = ceil(K S O / 2) partition sets, set q = rows 2q, 2q + 1, an odd last row with 0) on the
+// time-varying op's anchor grid (hop = H kB: blocks i < nX = (K - 1) H are crossfaded between IR sets k = i / H and
+// k + 1).  Product (forward) and gradient (backward) slots per item:
+//   O = 2: U = I + nX, the time-varying op's layout (tv_slot): slot 2i + o (i < nX) holds (Y_k,o[i], Y_k+1,o[i]), slot
+//          nX + i (i >= nX) holds (Y_K-1,0[i], Y_K-1,1[i]); the gradient slots are tv_fft_kernel's.
+//   O = 1: U = I: slot i holds (Y_k[i], Y_k+1[i]) for i < nX and (Y_K-1[i], 0) after; the gradient slot i is the FFT of
+//          [0 | (1 - a) g + i a g] for i < nX and of [0 | g] after (tvbus_gfft_kernel).
+// So one inverse transform yields one crossfaded output row (O = 2) or one output block (O = 1).
+
+// gradient transforms of a mono bus, runs of kConvRun units m = il I + i: tv_fft_kernel with one gradient row, whose
+// block carries the weight 1 - a in the real and a in the imaginary plane (one transform for both IR sets of the
+// block).  n % 4 == 0 and 16-byte aligned rows.
+__global__ void __launch_bounds__(kFusedThreads, 1)
+tvbus_gfft_kernel(const float* __restrict__ gy, float2* __restrict__ Gb, const float* __restrict__ twiddles,
+                  int64_t item0, int I, int nX, int H, int64_t hop, int64_t n, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {                // all threads: zero padding and the im plane; thread 0: the copy
+    if (m >= m1) return;
+    const int64_t il = m / I;
+    const int i = m - (int)il * I;
+    float* re = s.buf(it);
+    float* im = re + fft8k::kPlaneG;
+    const int64_t s0 = (int64_t)i * kB;
+    const int64_t rem = n - s0;
+    const int len = rem < kB ? (int)rem : kB;
+    for (int e = t; e < kB; e += kFusedThreads) re[e] = 0.f;
+    for (int e = kB + len + t; e < kNbA; e += kFusedThreads) re[e] = 0.f;
+    for (int e = t; e < kNbA; e += kFusedThreads) im[e] = 0.f;
+    if (t == 0) {
+      uint64_t* bar = &s.full[it & 1];
+      mbar_arrive_expect_tx(bar, (uint32_t)len * 4u);
+      tma_load_1d(re + kB, gy + (item0 + il) * n + s0, (uint32_t)len * 4u, bar);
+    }
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  __syncthreads();
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    float* gi = gr + fft8k::kPlaneG;
+    const int i = m - (m / I) * I;
+    if (i < nX) {                                  // uniform over the CTA
+      for (int e = t; e < kB; e += kFusedThreads) {
+        const float a = tv_a(i, H, e, hop);
+        const float v = gr[kB + e];
+        gr[kB + e] = (1.0f - a) * v;
+        gi[kB + e] = a * v;
+      }
+      __syncthreads();
+    }
+    float xr[16], xi[16];
+    fft8192_in_smem<false>(gr, gi, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    float2* out = Gb + (int64_t)m * kNbA;
+#pragma unroll
+    for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(xr[q], xi[q]);
+  }
+}
+
+// inverse transforms of the bus's product slots, runs of kConvRun units m = il U + u, with the crossfade and the crop in
+// the epilogue (tv_ifft_kernel without the dry path): a crossfaded slot gives (1 - a) re + a im on samples
+// [i kB, (i+1) kB) ∩ [0, n) of output row o (O = 2: o = u & 1; O = 1: the one row); a later slot gives rows 0 and 1 as
+// re and im (O = 2) or row 0 as re (O = 1).
+__global__ void __launch_bounds__(kFusedThreads, 1)
+tvbus_ifft_kernel(const float* __restrict__ Ypl, const float* __restrict__ twiddles, float* __restrict__ y,
+                  int64_t item0, int I, int nX, int H, int64_t hop, int64_t n, int O, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int U = O == 2 ? I + nX : I;
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {
+    if (t == 0 && m < m1) s.load_planar(it, Ypl + (int64_t)m * 2 * kNbA);
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    const int64_t il = m / U, b = item0 + il;
+    const int u = m - (int)il * U;
+    const bool cross = O == 2 ? u < 2 * nX : u < nX;                  // uniform over the CTA
+    const int i = O == 2 ? (cross ? u >> 1 : u - nX) : u;
+    const int o = O == 2 && cross ? u & 1 : 0;
+    float xr[16], xi[16];
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    float* yo = y + (b * O + o) * n;
+#pragma unroll
+    for (int q = 8; q < 16; ++q) {                 // outputs kB .. 2 kB - 1 of the transform
+      const int e = t + 512 * q - kB;
+      const int64_t tg = (int64_t)i * kB + e;
+      if (tg < n) {
+        if (cross) {
+          const float a = tv_a(i, H, e, hop);
+          yo[tg] = fmaf(a, xi[q], (1.0f - a) * xr[q]);
+        } else {
+          yo[tg] = xr[q];
+          if (O == 2) yo[n + tg] = xi[q];
+        }
+      }
+    }
+  }
+}
+
+// The products of the time-varying bus per bin pair (f, kNbA - f) and item, every operand untangled into the spectra
+// of its real rows (X_s: source s, H_k,s,o: IR row (k S + s) O + o, Ga_o / Gb_o: the gradient of output o weighted
+// 1 - a / a, G_o for a block after the last anchor), results packed two real rows per block, planar, scaled by
+// 1 / kNbA; all operands from L2.
+//   TVB_FWD: Y_k,o[i] = sum_s sum_j X_s[i - j] H_k,s,o[j] for the IR sets of block i        out: U slots (see above)
+//   TVB_DX:  D_s[m] = sum_o sum_j Ga_o[m+j] conj(H_k(m+j),s,o[j]) + Gb_o[m+j] conj(H_k(m+j)+1,s,o[j]), stored as
+//            bus_mac_kernel's W_s[m] = D_s[m] + (-1)^f D_s[m + 1] (bus_ifft_kernel's half 1 then writes dL/dx_s with
+//            the overlap-add done)                                                   out: P I blocks (W_2p + i W_2p+1)
+//   TVB_DIR: E_k,s,o[j] = sum_{i in interval k} Ga_o[i] conj(X_s[i-j]) + sum_{i in interval k-1} Gb_o[i] conj(X_s[i-j])
+//                                                                                    out: NH J blocks (set q: rows 2q, 2q+1)
+// X: P I blocks per item; H: NH J partitions per trajectory set at item stride hstride (0: one set for the batch);
+// G: U slots per item.
+enum TvBusMac { TVB_FWD, TVB_DX, TVB_DIR };
+template <int MODE, int O>
+__global__ void __launch_bounds__(128) tvbus_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                        int64_t hstride, const float2* __restrict__ G,
+                                                        float2* __restrict__ Out, int S, int I, int J, int K, int nX,
+                                                        int Hb) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int64_t il = blockIdx.y;
+  const int P = (S + 1) / 2, U = O == 2 ? I + nX : I;
+  const float2* x = X + il * (int64_t)P * I * kNbA;
+  const float2* h = H + il * hstride;
+  const float2* g = G + il * (int64_t)U * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  // IR rows (k, s, 0) and (k, s, 1) (O == 2), or row (k, s) (O == 1), at partition j
+  auto hin = [&](int k, int s, int j, float2& h0, float2& h1) {
+    const int r = k * S + s;
+    if (O == 2) { pair(h, (int64_t)r * J + j, h0, h1); }
+    else { float2 a, b; pair(h, (int64_t)(r >> 1) * J + j, a, b); h0 = (r & 1) ? b : a; h1 = zero; }
+  };
+  // the gradient of block i for IR set k(i) (part 0: Ga, or G after the last anchor) or k(i) + 1 (part 1: Gb, i < nX),
+  // outputs 0 and 1
+  auto gin = [&](int i, int part, float2& g0, float2& g1) {
+    if (O == 2) { pair(g, part ? 2 * i + 1 : tv_slot(i, nX), g0, g1); }
+    else { float2 a, b; pair(g, i, a, b); g0 = part ? b : a; g1 = zero; }
+  };
+  const float scale = 1.0f / (float)kNbA;
+  auto emit = [&](int64_t slot, float2 a, float2 b) {
+    a.x *= scale; a.y *= scale; b.x *= scale; b.y *= scale;
+    float* pl = reinterpret_cast<float*>(Out + slot * kNbA);
+    pl[f] = a.x - b.y; pl[kNbA + f] = a.y + b.x;
+    if (fm != f) { pl[fm] = a.x + b.y; pl[kNbA + fm] = b.x - a.y; }
+  };
+  auto ival = [&](int i) { const int k = i / Hb; return k < K - 1 ? k : K - 1; };   // anchor interval of block i
+
+  if constexpr (MODE == TVB_FWD) {
+    const int64_t ob = il * (int64_t)U;
+    for (int o = 0; o < I; ++o) {
+      const int k = ival(o);
+      const bool cross = o < nX;
+      float2 y0 = zero, y1 = zero, z0 = zero, z1 = zero;    // IR set k: outputs 0, 1; IR set k + 1: outputs 0, 1
+      for (int p = 0; p < P; ++p) {
+        const int nc = 2 * p + 1 < S ? 2 : 1;
+        for (int j = 0; j <= o && j < J; ++j) {
+          float2 xv[2], h0, h1;
+          pair(x, (int64_t)p * I + o - j, xv[0], xv[1]);
+          for (int c = 0; c < nc; ++c) {
+            hin(k, 2 * p + c, j, h0, h1);
+            cfma(y0, xv[c], h0);
+            if (O == 2) cfma(y1, xv[c], h1);
+            if (cross) {
+              hin(k + 1, 2 * p + c, j, h0, h1);
+              cfma(z0, xv[c], h0);
+              if (O == 2) cfma(z1, xv[c], h1);
+            }
+          }
+        }
+      }
+      if (O == 2) {
+        if (cross) { emit(ob + 2 * o, y0, z0); emit(ob + 2 * o + 1, y1, z1); }
+        else emit(ob + nX + o, y0, y1);
+      } else {
+        emit(ob + o, y0, z0);                      // z0 = 0 after the last anchor
+      }
+    }
+  } else if constexpr (MODE == TVB_DX) {
+    // D_2p+c[m], c = 0, 1 (d[1] stays 0 for an odd last source)
+    auto dcorr = [&](int p, int m, float2 (&d)[2]) {
+      d[0] = d[1] = zero;
+      const int nc = 2 * p + 1 < S ? 2 : 1;
+      for (int j = 0; j < J && m + j < I; ++j) {
+        const int i = m + j, k = ival(i);
+        for (int part = 0; part < (i < nX ? 2 : 1); ++part) {
+          float2 g0, g1, h0, h1;
+          gin(i, part, g0, g1);
+          for (int c = 0; c < nc; ++c) {
+            hin(k + part, 2 * p + c, j, h0, h1);
+            cfma_conj(d[c], g0, h0);
+            if (O == 2) cfma_conj(d[c], g1, h1);
+          }
+        }
+      }
+    };
+    const float sgn = (f & 1) ? -1.f : 1.f;
+    const int64_t ob = il * (int64_t)P * I;
+    for (int p = 0; p < P; ++p) {
+      float2 next[2] = {zero, zero};               // D[m + 1]
+      for (int m = I - 1; m >= 0; --m) {
+        float2 d[2];
+        dcorr(p, m, d);
+        emit(ob + (int64_t)p * I + m, make_float2(fmaf(sgn, next[0].x, d[0].x), fmaf(sgn, next[0].y, d[0].y)),
+             make_float2(fmaf(sgn, next[1].x, d[1].x), fmaf(sgn, next[1].y, d[1].y)));
+        next[0] = d[0]; next[1] = d[1];
+      }
+    }
+  } else {
+    static_assert(MODE == TVB_DIR, "tvbus_mac_kernel: unknown mode");
+    // e[c][o] = E_k,2p+c,o[j] over both intervals that carry IR set k: each gradient and window-pair spectrum read
+    // serves both sources of the pair
+    auto ecorr = [&](int k, int p, int j, float2 (&e)[2][2]) {
+      e[0][0] = e[0][1] = e[1][0] = e[1][1] = zero;
+      for (int part = 0; part < 2; ++part) {       // 0: Ga (G) of interval k, 1: Gb of interval k - 1
+        const int kk = k - part;
+        if (kk < 0) continue;
+        const int lo = kk * Hb, hi = kk == K - 1 ? I : ((kk + 1) * Hb < I ? (kk + 1) * Hb : I);
+        for (int i = lo > j ? lo : j; i < hi; ++i) {
+          float2 g0, g1, xa, xb;
+          gin(i, part, g0, g1);
+          pair(x, (int64_t)p * I + i - j, xa, xb);
+          cfma_conj(e[0][0], g0, xa);
+          cfma_conj(e[1][0], g0, xb);
+          if (O == 2) { cfma_conj(e[0][1], g1, xa); cfma_conj(e[1][1], g1, xb); }
+        }
+      }
+    };
+    const int NH = (K * S * O + 1) / 2;
+    const int64_t ob = il * (int64_t)NH * J;
+    float2 e[2][2];
+    if (O == 2 || S % 2 == 0) {
+      // the sets of sources 2p, 2p + 1: k S + 2p + c (O = 2, rows o = 0, 1) or k S / 2 + p (O = 1, one row each)
+      for (int k = 0; k < K; ++k) {
+        for (int p = 0; p < P; ++p) {
+          for (int j = 0; j < J; ++j) {
+            ecorr(k, p, j, e);
+            if (O == 2) {
+              emit(ob + (int64_t)(k * S + 2 * p) * J + j, e[0][0], e[0][1]);
+              if (2 * p + 1 < S) emit(ob + (int64_t)(k * S + 2 * p + 1) * J + j, e[1][0], e[1][1]);
+            } else {
+              emit(ob + (int64_t)(k * S / 2 + p) * J + j, e[0][0], e[1][0]);
+            }
+          }
+        }
+      }
+    } else {
+      // a mono bus of an odd number of sources: set q holds rows r = 2q, 2q + 1 (r = k S + s), which may belong to two
+      // IR sets, so each row is formed on its own
+      for (int q = 0; q < NH; ++q) {
+        for (int j = 0; j < J; ++j) {
+          float2 a, b = zero;
+          ecorr((2 * q) / S, ((2 * q) % S) >> 1, j, e);
+          a = e[((2 * q) % S) & 1][0];
+          if (2 * q + 1 < K * S) {
+            ecorr((2 * q + 1) / S, ((2 * q + 1) % S) >> 1, j, e);
+            b = e[((2 * q + 1) % S) & 1][0];
+          }
+          emit(ob + (int64_t)q * J + j, a, b);
+        }
+      }
+    }
+  }
+}
+
 // Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
 // spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
 // transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
@@ -2844,6 +3133,8 @@ int configure_fft_kernels() {
     DASP_CUDA_OK(cudaFuncSetAttribute(bus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(tv_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(tv_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(tvbus_gfft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(tvbus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     configured[dev] = true;
   }
   return DASP_OK;
@@ -3879,6 +4170,179 @@ int dasp_tvconv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int6
                            int64_t chunk_items, void* stream) {
   return tvconv_bwd(true, gy, x, in_chs, ir_chs, ir_len, K, hop, mix, xspec_save, irspec_save, gx, gir, gmix,
                     workspace, workspace_bytes, bs, n, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ time_varying_convolution_bus
+// y[:, o] = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, o])(t) through the stage above on the own FFT only: the bus's window
+// spectra (bus_fft_kernel, P = ceil(S / 2) per block), the K S O IR rows of a trajectory set in ceil(K S O / 2)
+// partition sets, no mix.  The products are tvbus_mac_kernel's; a stereo bus has the time-varying op's slots (its
+// inverse tvbus_ifft_kernel, its gradient transforms tv_fft_kernel), a mono bus one slot per block (tvbus_ifft_kernel,
+// tvbus_gfft_kernel).  dL/dx and the dL/dIR taps are bus_ifft_kernel's, as for the bus.
+namespace {
+int g_tvbus_last_path[2] = {0, 0};                   // test hook: dispatch of the last forward / backward
+
+extern "C++" {
+template <int MODE>
+int launch_tvbus_mac(int O, const float2* X, const float2* H, int64_t hstride, const float2* G, float2* Out,
+                     int64_t items, int S, int I, int J, int K, int nX, int Hb, cudaStream_t st) {
+  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+  if (O == 2) tvbus_mac_kernel<MODE, 2><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, K, nX, Hb);
+  else        tvbus_mac_kernel<MODE, 1><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, K, nX, Hb);
+  DASP_LAUNCH_OK("tvbus_mac_kernel");
+  return DASP_OK;
+}
+}  // extern "C++"
+
+struct TvBusOp {
+  static constexpr const char* kFwd = "tvbus fwd";
+  static constexpr const char* kBwd = "tvbus bwd";
+  static constexpr bool kOddSelf = false;
+  int S, O, K, Hb, ir_rows;                          // sources, outputs, anchors, hop / kB, IR rows K S O
+  int nx() const { return (K - 1) * Hb; }            // crossfaded blocks (< ib)
+  int slots(const ConvGeom& g) const { return (int)g.ib + (int)g.ex; }   // product / gradient slots per item
+  int fwd_chunk(const ConvGeom& g, const Plans&, bool own, const float* tw, const float* x, const float*, float2* xs,
+                float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    // bit 0: own FFT (always), bit 1: one trajectory set shared by the batch, bit 2: crossfaded blocks (K > 1)
+    g_tvbus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (K > 1 ? 4 : 0);
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    if (h_stride != 0 && (rc = ir_partition_spectra(g, tw, hs, items, st)) != DASP_OK) return rc;
+    float2* ys = (float2*)(ws + w.ys);
+    const int I = (int)g.ib, J = (int)g.jb, nwin = (int)(items * g.p * I), nout = (int)(items * slots(g));
+    bus_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, S, g.p, I, g.n, 0, nwin);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    if ((rc = launch_tvbus_mac<TVB_FWD>(O, xs, hs, h_stride, nullptr, ys, items, S, I, J, K, nx(), Hb, st)) != DASP_OK)
+      return rc;
+    tvbus_ifft_kernel<<<runs(nout), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y,
+                                                                        item0, I, nx(), Hb, (int64_t)Hb * kB, g.n, O,
+                                                                        nout);
+    DASP_LAUNCH_OK("tvbus_ifft_kernel");
+    return DASP_OK;
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans&, bool own, IrGrad e, const float* tw, const float* gy, const float*,
+                const float*, const float2* xs, const float2* hs, int64_t h_stride, float* gx, unsigned char* ws,
+                const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    // bit 0: own FFT (always), bit 1: crossfaded blocks (K > 1), bit 2: dL/dIR computed, bit 3: shared trajectory set
+    g_tvbus_last_path[1] = (own ? 1 : 0) | (K > 1 ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) | (g.shared ? 8 : 0);
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* gs = (float2*)(ws + w.gs);
+    float2* ds = (float2*)(ws + w.ds);
+    const int I = (int)g.ib, J = (int)g.jb, nwin = (int)(items * g.p * I), ng = (int)(items * slots(g));
+    const int64_t hop = (int64_t)Hb * kB;
+    if (O == 2) {
+      tv_fft_kernel<<<runs(ng), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, I, nx(), Hb, hop, g.n, ng);
+      DASP_LAUNCH_OK("tv_fft_kernel");
+    } else {
+      tvbus_gfft_kernel<<<runs(ng), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, I, nx(), Hb, hop, g.n, ng);
+      DASP_LAUNCH_OK("tvbus_gfft_kernel");
+    }
+    if ((rc = launch_tvbus_mac<TVB_DX>(O, xs, hs, h_stride, gs, ds, items, S, I, J, K, nx(), Hb, st)) != DASP_OK)
+      return rc;
+    bus_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx, item0,
+                                                                      S, g.p, I, g.n, g.n, 1, nwin);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    if (e == IrGrad::kNone) return DASP_OK;          // a fixed trajectory set: no dL/dIR work at all
+    return launch_tvbus_mac<TVB_DIR>(O, xs, hs, 0, gs, (float2*)(ws + w.es), items, S, I, J, K, nx(), Hb, st);
+  }
+  // dL/dIR taps [0, leff) of items [item0, item0 + items): the first half of the inverse of each partition
+  int ir_taps(const ConvGeom& g, bool, const float* tw, const float2* es, const float*, float* gir, int64_t item0,
+              int64_t items, cudaStream_t st) const {
+    const int J = (int)g.jb, nparts = (int)(items * g.sets * J);
+    bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir,
+                                                                        item0, ir_rows, g.sets, J, g.L, g.leff, 0,
+                                                                        nparts);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    return DASP_OK;
+  }
+};
+
+// the argument checks of dasp_tvbus_*, filling the geometry
+int make_tvbus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t K, int64_t S, int64_t O, int64_t hop,
+                    int64_t chunk, ConvGeom& g) {
+  DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "tvbus: 1 to %d inputs are supported, got %lld",
+               DASP_CONV_BUS_MAX_INPUTS, (long long)S);
+  DASP_REQUIRE(O == 1 || O == 2, "tvbus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
+  DASP_REQUIRE(K >= 1, "tvbus: K >= 1 impulse-response sets are needed, got %lld", (long long)K);
+  DASP_REQUIRE(hop > 0 && hop % kB == 0, "tvbus: hop must be a positive multiple of %d, got %lld", kB, (long long)hop);
+  int rc = make_conv_geom(bs, n, L, chunk, g);
+  if (rc != DASP_OK) return rc;
+  DASP_REQUIRE(K - 1 <= (n - 1) / hop, "tvbus: anchor %lld at (K - 1) hop is at or after the end of x (n=%lld)",
+               (long long)(K - 1), (long long)n);
+  const int64_t sets = (K * S * O + 1) / 2;
+  DASP_REQUIRE(sets <= 65535, "tvbus: at most 65535 partition sets (K S O / 2) per trajectory set, got %lld",
+               (long long)sets);
+  g.shared = shared;
+  g.p = (int)(S + 1) / 2;
+  g.sets = (int)sets;
+  g.ex = O == 2 ? (K - 1) * (hop / kB) : 0;        // a mono bus packs both IR sets of a block into one slot
+  g.has_mix = false;
+  g.own_only = true;
+  return DASP_OK;
+}
+TvBusOp tvbus_op(int64_t K, int64_t S, int64_t O, int64_t hop) {
+  return TvBusOp{(int)S, (int)O, (int)K, (int)(hop / kB), (int)(K * S * O)};
+}
+
+int tvbus_fwd(bool shared, const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+              void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
+              int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_tvbus_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return caller_ir_fwd(tvbus_op(K, S, O, hop), g, x, ir, nullptr, y, xspec_save, irspec_save, workspace,
+                       workspace_bytes, stream);
+}
+
+int tvbus_bwd(bool shared, const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+              void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
+              int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_tvbus_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return caller_ir_bwd(tvbus_op(K, S, O, hop), g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir, nullptr,
+                       workspace, workspace_bytes, stream);
+}
+}  // namespace
+
+int dasp_debug_tvbus_last_path(int which) { return g_tvbus_last_path[which ? 1 : 0]; }
+
+int dasp_tvbus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                        int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "tvbus geometry: null out");
+  ConvGeom g;
+  int rc = make_tvbus_geom(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
+}
+
+int dasp_tvbus_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                   int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                   int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvbus_fwd(false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                   outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvbus_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                   void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                   int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvbus_bwd(false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                   outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvbus_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                          void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                          int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvbus_fwd(true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                   outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvbus_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                          void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                          int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvbus_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                   outputs, hop, chunk_items, stream);
 }
 
 // ------------------------------------------------------------------ noise_shaped_impulse_response

@@ -38,6 +38,7 @@ __all__ = [
     "convolution_reverberation",
     "convolution_bus",
     "time_varying_convolution_reverberation",
+    "time_varying_convolution_bus",
     "noise_shaped_impulse_response",
     "noise_shaped_impulse_response_packed",
     "parametric_eq_frequency_response",
@@ -1524,6 +1525,20 @@ def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch
 CONV_PARTITION_SAMPLES = 4096      # conv_block of dasp_conv_geom: the partition length of every caller-IR convolution
 
 
+def _anchor_hop(hop, K: int, n: int) -> int:
+    """the anchor spacing of a trajectory of K impulse responses (sets) over n samples, as an int"""
+    if isinstance(hop, bool) or not isinstance(hop, int) and not (torch.is_tensor(hop) and hop.numel() == 1
+                                                                  and not hop.is_floating_point()):
+        raise ValueError(f"hop must be an integer number of samples, got {hop!r}")
+    hop = int(hop)
+    if hop <= 0 or hop % CONV_PARTITION_SAMPLES:
+        raise ValueError(f"hop must be a positive multiple of {CONV_PARTITION_SAMPLES} samples, got {hop}")
+    if (K - 1) * hop >= n:
+        raise ValueError(f"impulse response {K - 1} is anchored at (K - 1) * hop = {(K - 1) * hop}, at or after the "
+                         f"end of x ({n} samples)")
+    return hop
+
+
 class _TvConvFn(torch.autograd.Function):
     """x (bs, 1|2, n), ir (bs | 1, K, 1|2, L), mix (bs,) -> y (bs, 2, n).  n % 4 == 0 and 16-byte aligned rows
     (time_varying_convolution_reverberation pads).  An ir of batch 1 with bs > 1 runs the dasp_tvconv_shared_* entry
@@ -1635,15 +1650,7 @@ def time_varying_convolution_reverberation(x: torch.Tensor, sample_rate: float, 
     _caller_ir_shape(impulse_response, bs)
     if n < 1:
         raise ValueError("x needs at least one sample")
-    if isinstance(hop, bool) or not isinstance(hop, int) and not (torch.is_tensor(hop) and hop.numel() == 1
-                                                                  and not hop.is_floating_point()):
-        raise ValueError(f"hop must be an integer number of samples, got {hop!r}")
-    hop = int(hop)
-    if hop <= 0 or hop % CONV_PARTITION_SAMPLES:
-        raise ValueError(f"hop must be a positive multiple of {CONV_PARTITION_SAMPLES} samples, got {hop}")
-    if (K - 1) * hop >= n:
-        raise ValueError(f"impulse response {K - 1} is anchored at (K - 1) * hop = {(K - 1) * hop}, at or after the "
-                         f"end of x ({n} samples)")
+    hop = _anchor_hop(hop, K, n)
     nmix = mix.numel() if torch.is_tensor(mix) else torch.as_tensor(mix).numel()
     if nmix not in (1, bs):
         raise ValueError(f"mix: expected {bs} element(s) (one per batch item) or 1, got {nmix}")
@@ -1658,4 +1665,141 @@ def time_varying_convolution_reverberation(x: torch.Tensor, sample_rate: float, 
     elif xf.data_ptr() % 16:
         xf = xf.clone()
     y = _TvConvFn.apply(xf, irf, m, hop, reverb_chunk_items(xf.device))
+    return (y[..., :n] if n4 != n else y).to(dt)
+
+
+# --------------------------------------------------------------------------------------
+# time_varying_convolution_bus
+# --------------------------------------------------------------------------------------
+
+class _TvBusFn(torch.autograd.Function):
+    """x (bs, S, n), ir (bs | 1, K, S, O, L) -> y (bs, O, n).  n % 4 == 0 and 16-byte aligned rows
+    (time_varying_convolution_bus pads).  An ir of batch 1 with bs > 1 runs the dasp_tvbus_shared_* entry points; its
+    gradient is the sum over the items."""
+
+    @staticmethod
+    def forward(ctx, x, ir, hop, chunk):
+        lib = _abi.lib()
+        bs, S, n = x.shape
+        ir_bs, K, _, O, ir_len = ir.shape
+        shared = ir_bs == 1 and bs > 1
+        kind = "tvbus_shared" if shared else "tvbus"
+        dev = x.device
+        y = torch.empty(bs, O, n, dtype=torch.float32, device=dev)
+        need_bwd = any(ctx.needs_input_grad[:2])
+        with torch.cuda.device(dev):
+            ws, (xspec, irspec), bwd_bytes = _geom_buffers(
+                _abi.ConvGeom(), "dasp_tvbus_geometry", (bs, n, ir_len, K, S, O, hop, int(shared), chunk), dev,
+                need_bwd)
+            with _timed("tvbus_fwd", dev):
+                check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), ptr(ir), ptr(y), ptr(xspec), ptr(irspec), ptr(ws),
+                                                       ws.numel(), bs, n, ir_len, K, S, O, hop, chunk,
+                                                       stream_ptr(dev)),
+                      f"dasp_{kind}_fwd")
+        if need_bwd:
+            ctx.save_for_backward(xspec, irspec)
+        ctx.cfg = (kind, bs, S, O, n, ir.shape, hop, chunk, bwd_bytes)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib = _abi.lib()
+        xspec, irspec = ctx.saved_tensors
+        kind, bs, S, O, n, ir_shape, hop, chunk, bwd_bytes = ctx.cfg
+        dev = gy.device
+        gy = gy.contiguous()
+        if gy.data_ptr() % 16:
+            gy = gy.clone()
+        gx = torch.empty(bs, S, n, dtype=torch.float32, device=dev)
+        # a fixed trajectory set (measured or simulated rooms) skips every dL/dIR kernel
+        gir = torch.empty(ir_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        ws = _ws_bytes(bwd_bytes, dev)
+        with torch.cuda.device(dev), _timed("tvbus_bwd", dev):
+            check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(xspec), ptr(irspec), ptr(gx), ptr(gir), ptr(ws),
+                                                   ws.numel(), bs, n, ir_shape[4], ir_shape[1], S, O, hop, chunk,
+                                                   stream_ptr(dev)),
+                  f"dasp_{kind}_bwd")
+        return gx, gir, None, None
+
+
+def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor, hop: int):
+    """Several moving sources, each through its own trajectory of impulse responses, crossfaded along the output and
+    summed into one mono or stereo bus: ``convolution_bus`` whose IR set changes over time, as
+    ``time_varying_convolution_reverberation``'s IR does.  Set ``k`` of the trajectory, ``h[:, k]``, is a complete
+    ``convolution_bus`` IR set, the scene at the anchor time ``t_k = k * hop``::
+
+        y[:, o](t) = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, o])(t)
+
+        k hop <= t < (k+1) hop, k < K - 1:   a = (t - k hop) / hop,   w_k = 1 - a,   w_{k+1} = a,   other w = 0
+        t >= (K - 1) hop:                    w_{K-1} = 1
+
+    (``*`` the causal convolution cropped to ``n``, exactly as ``convolution_reverberation`` defines its wet signal;
+    ``w_k`` are ``time_varying_convolution_reverberation``'s crossfade weights).  Uses: reverberant multi-talker
+    mixtures with moving speakers for separation and enhancement training, binaural or stereo scenes with several
+    moving objects, a stereo source moving through a room (``S = 2, O = 2`` is a time-varying true-stereo rendering),
+    and a learnable time-varying S-input FIR.
+
+    Args:
+        x: audio ``(bs, S, n)``, ``1 <= S <= CONV_BUS_MAX_INPUTS`` sources.
+        sample_rate: unused (kept for the common processor signature).
+        impulse_response: ``(bs, K, S, O, L)``, one trajectory set per item, or ``(1, K, S, O, L)``, one set shared by
+            the batch; ``K >= 1``, ``O`` is 1 (mono bus) or 2 (stereo bus), any ``L >= 1``.  Row ``(k, s, o)`` is the
+            path from source ``s`` to output ``o`` at anchor ``k``.
+        hop: the anchor spacing in samples, a positive multiple of ``CONV_PARTITION_SAMPLES`` (4096), so that every
+            output block and every gradient block lies inside one anchor interval; ``(K - 1) * hop < n``.  All
+            sources share the one anchor grid.
+
+    Returns ``(bs, O, n)`` in x's dtype, computed in fp32.  There is no dry/wet mix, as in ``convolution_bus``.
+
+    Identities (held to fp32 rounding):
+
+    1. ``K = 1``: ``convolution_bus(x, sr, h[:, 0])``; K equal sets: ``convolution_bus`` with that set.
+    2. ``S = 1, O = 2``: ``time_varying_convolution_reverberation(x, sr, h[:, :, 0], hop, mix=1)``.
+    3. Any ``S``: the sum over ``s`` of ``time_varying_convolution_bus(x[:, s:s+1], sr, h[:, :, s:s+1], hop)``.
+    4. From the last anchor on (``t >= (K - 1) hop``): ``convolution_bus(x, sr, h[:, K - 1])``.
+
+    Gradients flow to ``x`` (every source) and to every IR row; taps at or beyond ``min(L, n)`` reach no output and
+    get exactly 0.  The gradient of a shared ``(1, K, S, O, L)`` set has that shape and is the sum over the items,
+    accumulated in fp64 in item order, so it does not depend on ``REVERB_CHUNK_ITEMS``.  When the IRs do not require a
+    gradient, the backward skips all dL/dIR work.
+
+    Cost: the rows of every signal are packed two per transform, as in ``convolution_bus``: ceil(S / 2) window
+    transforms per block, transformed and kept for the backward once for all K sets; the K S O IR rows' partitions in
+    ceil(K S O / 2) transforms per partition; one product per IR set and block summed over the sources, and one inverse
+    transform per output row and crossfaded block (a mono bus: per block).  S ``time_varying_convolution_reverberation``
+    calls would transform and keep every window S times and take S sets of inverse transforms.  A source that does not
+    move repeats its IR in every set: its partitions are transformed and kept K times, and a crossfaded block multiplies
+    its windows by both copies, for the static convolution's result (a crossfade of two equal outputs).  Rows whose
+    length is not a multiple of 4 are zero-padded to one (the transforms bulk-copy 16-byte rows); a padding sample
+    reaches no output sample below ``n``.
+    """
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
+    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 5:
+        raise ValueError("impulse_response must be a tensor of shape (batch, K, inputs, outputs, taps)")
+    bs, S, n = x.shape
+    if not 1 <= S <= CONV_BUS_MAX_INPUTS:
+        raise ValueError(f"time_varying_convolution_bus: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, "
+                         f"got {S}")
+    _, K, ir_s, O, L = impulse_response.shape
+    if ir_s != S:
+        raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
+    if O not in (1, 2):
+        raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
+    if K < 1:
+        raise ValueError("impulse_response needs at least one impulse-response set (K >= 1)")
+    _caller_ir_shape(impulse_response, bs)
+    if n < 1:
+        raise ValueError("x needs at least one sample")
+    hop = _anchor_hop(hop, K, n)
+    xf, dt = _audio(x)
+    irf = _caller_ir(impulse_response, xf, 5)
+    n4 = (n + 3) // 4 * 4
+    if n4 != n:
+        xf = torch.nn.functional.pad(xf, (0, n4 - n))
+        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
+            irf = irf[..., :n].contiguous()
+    elif xf.data_ptr() % 16:
+        xf = xf.clone()
+    y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device))
     return (y[..., :n] if n4 != n else y).to(dt)

@@ -391,6 +391,41 @@ int dasp_tvconv_shared_bwd(const float* gy, const float* x, int64_t in_chs, int6
    bit 1 = crossfaded blocks, bit 2 = dL/dIR computed, bit 3 = shared trajectory */
 int dasp_debug_tvconv_last_path(int which);
 
+/* ---- time_varying_convolution_bus: S moving sources, each with its own IR trajectory, summed into one bus ----------
+ * x is (bs, inputs, n) with 1 <= inputs (S) <= DASP_CONV_BUS_MAX_INPUTS, ir is (bs, K, S, outputs, ir_len) with outputs
+ * (O) 1 or 2 (or ONE (K, S, O, ir_len) trajectory set for the whole batch: the *_shared_* entry points), y is
+ * (bs, O, n).  ir[:, k] is a complete convolution_bus IR set, the scene at the anchor time k hop; hop is a positive
+ * multiple of conv_block (4096) with (K - 1) hop < n:
+ *   y[:, o](t) = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, o])(t)   (* and w_k as in dasp_tvconv_*; no dry/wet mix)
+ * The rows of every signal are packed two per transform as for the bus: ceil(S / 2) window transforms per block, one
+ * product per IR set and block summed over the sources, and one inverse transform per output row and crossfaded block
+ * (a stereo bus) or per block (a mono bus).  n % 4 == 0 and 16-byte aligned x / gy rows are required.  Buffers kept for
+ * the backward (NULL for both when no backward follows): xspec_save geom.xspec_c64 and irspec_save geom.irspec_c64
+ * complex64.  Backward: gx (bs, S, n), gir (bs, K, S, O, ir_len) (shared: (K, S, O, ir_len), the sum over the items in
+ * fp64 in item order, the same bits for every chunk_items), or NULL, which skips all dL/dIR work; taps >= leff =
+ * min(ir_len, n) get 0.  Workspace sizes come from dasp_tvbus_geometry (shared != 0 for the shared entry points), which
+ * needs no GPU.  Bad S, O, K, hop or shapes, null pointers and unaligned rows are rejected before any CUDA call. */
+int dasp_tvbus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                        int64_t shared, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_tvbus_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                   int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                   int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvbus_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                   float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                   int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                   void* stream);
+int dasp_tvbus_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                          void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                          int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvbus_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                          float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                          int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                          void* stream);
+/* test hook: dispatch of the most recent call.  which = 0 (forward): bit 0 = own in-shared-memory FFT (always),
+   bit 1 = shared trajectory set, bit 2 = crossfaded blocks (K > 1).  which = 1 (backward): bit 0 = own FFT (always),
+   bit 1 = crossfaded blocks, bit 2 = dL/dIR computed, bit 3 = shared trajectory set */
+int dasp_debug_tvbus_last_path(int which);
+
 #ifdef __cplusplus
 }
 #endif

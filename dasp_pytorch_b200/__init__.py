@@ -12,7 +12,8 @@ into the audio, linear or in dB, with gradients to the detector input and the pa
 number of input channels, each through its own impulse responses, summed into a mono or stereo bus) and
 ``time_varying_convolution_reverberation`` (a trajectory of impulse responses crossfaded along the output, for moving
 sources and listeners) and ``time_varying_convolution_bus`` (several moving sources, each with its own trajectory of
-impulse responses, crossfaded and summed into a mono or stereo bus).
+impulse responses, crossfaded and summed into a mono or stereo bus; ``crossfade="input"`` crossfades on the source side,
+so every emitted sample keeps the impulse response of its emission time).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401

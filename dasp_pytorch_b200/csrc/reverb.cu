@@ -46,7 +46,10 @@
 //
 // time_varying_convolution_bus (dasp_tvbus_*) combines the two: the bus's packed window spectra, IR trajectories for
 // every source-to-output path, the two IR sets' products per block summed over the sources (tvbus_mac_kernel), and one
-// crossfaded inverse per output row and block (tvbus_ifft_kernel).
+// crossfaded inverse per output row and block (tvbus_ifft_kernel).  Its source-side crossfade (dasp_tvbus_in_*) weights
+// the input instead, so every sample keeps the IR sets of its emission time: zero-padded transforms of each source's
+// weighted blocks (tvbusin_fft_kernel), the products with the IR sets of each input block's interval, overlap-added on
+// the spectra (tvbusin_mac_kernel), and the crossfade of dL/dx in the epilogue of its inverse (tvbusin_ifft_kernel).
 //
 // The ops whose IR the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd: checks,
 // workspace, IR packing, chunk loop, zeros of the unreachable dL/dIR taps).  One IR for the whole batch
@@ -149,6 +152,8 @@ struct ConvGeom {
   bool own_only = false;        // the own FFT only: no cuFFT plans or work area, no dasp_debug_reverb_path(1) (the bus)
   int64_t ex = 0;               // product / gradient spectra per item beyond ib: the crossfaded blocks of the
                                 // time-varying convolution, which carry two IRs' products
+  int64_t xw = 0;               // window (and dL/dx) spectra per item when not p ib: the source-side crossfade's
+  int64_t xwin() const { return xw > 0 ? xw : p * ib; }
 };
 
 int make_conv_geom(int64_t bs, int64_t n, int64_t L, int64_t chunk, ConvGeom& g) {
@@ -2785,6 +2790,290 @@ __global__ void __launch_bounds__(128) tvbus_mac_kernel(const float2* __restrict
   }
 }
 
+// ---- time_varying_convolution_bus, source-side crossfade: y_o = sum_k sum_s ((w_k x_s) * h_k,s,o) -------------------
+// Every sample is heard through the IR sets of its emission time, its whole tail included.  Input block i lies in one
+// anchor interval k = i / H (hop = H kB), where only w_k = 1 - a and w_k+1 = a are nonzero, so its weighted pieces are
+// exact zero-padded transforms [0 | u]: no overlap-save window straddles an anchor.  The linear convolution of [0 | u]
+// with a partition [h | 0] fills both halves of the circular result, and the first half belongs to the next output
+// block, so the overlap-add is done on the spectra: W[m] = Y[m] + (-1)^f Y[m - 1] (a circular shift by kB is the factor
+// (-1)^f), and output block m is the second half of W[m]'s inverse.  Window spectra per item, XW = nX S + (I - nX) P
+// (nX = (K - 1) H crossfaded blocks, P = ceil(S / 2)):
+//   slot i S + s (i < nX):                 FFT of [0 | (1 - a) x_s,i + i a x_s,i]: both IR sets' pieces of one source
+//   slot nX S + (i - nX) P + p (i >= nX):  FFT of [0 | x_2p,i + i x_2p+1,i]: two sources, IR set K - 1
+// The dL/dx spectra use the same slots.  The product and gradient spectra are one per block, both outputs packed.
+__device__ __forceinline__ void tvin_block(int w, int S, int P, int nX, int& i, int& c) {   // slot w -> block, source|pair
+  if (w < nX * S) { i = w / S; c = w - i * S; }
+  else { const int r = w - nX * S; i = nX + r / P; c = r - (i - nX) * P; }
+}
+
+// window transforms of x, runs of kConvRun units m = il XW + w: tvbus_gfft_kernel's weighting prologue on one source's
+// block (i < nX), bus_fft_kernel's zero-padded row pair after the last anchor.  n % 4 == 0 and 16-byte aligned rows.
+__global__ void __launch_bounds__(kFusedThreads, 1)
+tvbusin_fft_kernel(const float* __restrict__ x, float2* __restrict__ Xs, const float* __restrict__ twiddles,
+                   int64_t item0, int S, int I, int nX, int H, int64_t hop, int64_t n, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int P = (S + 1) / 2, XW = nX * S + (I - nX) * P;
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {                // all threads: zero padding; thread 0: the bulk copies
+    if (m >= m1) return;
+    const int64_t il = m / XW;
+    int i, c;
+    tvin_block(m - (int)il * XW, S, P, nX, i, c);
+    const bool cross = i < nX;
+    const bool two = !cross && 2 * c + 1 < S;      // a second source in the imaginary plane
+    float* re = s.buf(it);
+    float* im = re + fft8k::kPlaneG;
+    const int64_t s0 = (int64_t)i * kB;
+    const int64_t rem = n - s0;
+    const int len = rem < kB ? (int)rem : kB;      // kB for a crossfaded block
+    for (int e = t; e < kB; e += kFusedThreads) { re[e] = 0.f; im[e] = 0.f; }
+    for (int e = kB + len + t; e < kNbA; e += kFusedThreads) { re[e] = 0.f; im[e] = 0.f; }
+    if (!cross && !two) for (int e = kB + t; e < kB + len; e += kFusedThreads) im[e] = 0.f;
+    if (t == 0) {
+      const float* ra = x + ((item0 + il) * S + (cross ? c : 2 * c)) * n + s0;
+      uint64_t* bar = &s.full[it & 1];
+      mbar_arrive_expect_tx(bar, (two ? 2u : 1u) * (uint32_t)len * 4u);
+      tma_load_1d(re + kB, ra, (uint32_t)len * 4u, bar);
+      if (two) tma_load_1d(im + kB, ra + n, (uint32_t)len * 4u, bar);
+    }
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  __syncthreads();
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    float* gi = gr + fft8k::kPlaneG;
+    const int w = m - (m / XW) * XW;
+    if (w < nX * S) {                              // uniform over the CTA: a crossfaded block, im plane written here
+      const int i = w / S;
+      for (int e = t; e < kB; e += kFusedThreads) {
+        const float a = tv_a(i, H, e, hop);
+        const float v = gr[kB + e];
+        gr[kB + e] = (1.0f - a) * v;
+        gi[kB + e] = a * v;
+      }
+      __syncthreads();
+    }
+    float xr[16], xi[16];
+    fft8192_in_smem<false>(gr, gi, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    float2* out = Xs + (int64_t)m * kNbA;
+#pragma unroll
+    for (int q = 0; q < 16; ++q) out[t + 512 * q] = make_float2(xr[q], xi[q]);
+  }
+}
+
+// inverse transforms of the dL/dx spectra, runs of kConvRun units m = il XW + w, second half only: a crossfaded slot
+// gives (1 - a) re + a im on samples [i kB, (i+1) kB) of source s, a later slot sources 2p and 2p + 1 as re and im
+__global__ void __launch_bounds__(kFusedThreads, 1)
+tvbusin_ifft_kernel(const float* __restrict__ Dpl, const float* __restrict__ twiddles, float* __restrict__ gx,
+                    int64_t item0, int S, int I, int nX, int H, int64_t hop, int64_t n, int nunits) {
+  extern __shared__ __align__(128) float sm[];
+  FftSmem s(sm);
+  const int t = threadIdx.x;
+  s.init(twiddles, t);
+  const fft8k::Tables tb = fft8k::carve_tables(s.tabf);
+  const int P = (S + 1) / 2, XW = nX * S + (I - nX) * P;
+  const int m0 = blockIdx.x * kConvRun;
+  const int m1 = nunits - m0 < kConvRun ? nunits : m0 + kConvRun;
+  auto fetch = [&](int it, int m) {
+    if (t == 0 && m < m1) s.load_planar(it, Dpl + (int64_t)m * 2 * kNbA);
+  };
+  fetch(0, m0);
+  fetch(1, m0 + 1);
+  int it = 0;
+  for (int m = m0; m < m1; ++m, ++it) {
+    s.wait(it);
+    float* gr = s.buf(it);
+    float xr[16], xi[16];
+    fft8192_in_smem<true>(gr, gr + fft8k::kPlaneG, s, tb, t, [&] { fetch(it + 2, m + 2); }, [] {}, xr, xi);
+    const int64_t il = m / XW;
+    int i, c;
+    tvin_block(m - (int)il * XW, S, P, nX, i, c);
+    const bool cross = i < nX;                     // uniform over the CTA
+    const bool two = !cross && 2 * c + 1 < S;
+    float* ra = gx + ((item0 + il) * S + (cross ? c : 2 * c)) * n;
+#pragma unroll
+    for (int q = 8; q < 16; ++q) {                 // outputs kB .. 2 kB - 1 of the transform
+      const int e = t + 512 * q - kB;
+      const int64_t tg = (int64_t)i * kB + e;
+      if (tg < n) {
+        if (cross) {
+          const float a = tv_a(i, H, e, hop);
+          ra[tg] = fmaf(a, xi[q], (1.0f - a) * xr[q]);
+        } else {
+          ra[tg] = xr[q];
+          if (two) ra[n + tg] = xi[q];
+        }
+      }
+    }
+  }
+}
+
+// The products of the source-side bus per bin pair (f, kNbA - f) and item, every operand untangled into the spectra of
+// its real rows (Za_s / Zb_s: the 1 - a / a pieces of source s in a crossfaded block, Z_s after the last anchor, Za_s
+// then; H_k,s,o: IR row (k S + s) O + o; G_o: FFT of [0 | g_o block]), results packed two real rows per block, planar,
+// scaled by 1 / kNbA; all operands from L2.  k(i) is the anchor interval of input block i.
+//   TVI_FWD: Y_o[m] = sum_s sum_j Za_s[m-j] H_k(m-j),s,o[j] + Zb_s[m-j] H_k(m-j)+1,s,o[j], stored as
+//            W_o[m] = Y_o[m] + (-1)^f Y_o[m - 1]                                      out: I blocks (W_0 + i W_1)
+//   TVI_DX:  first folds G in place, G_o[q] <- Gt_o[q] = G_o[q] + (-1)^f G_o[q + 1], the spectrum of [g_o,q+1 | g_o,q]
+//            (the gradient of Y_o[q]'s whole inverse); then Da_s[i] = sum_o sum_j Gt_o[i+j] conj(H_k(i),s,o[j]) and
+//            Db_s[i] the same with IR set k(i) + 1 (i < nX)                           out: XW slots (Da + i Db, or
+//            D_2p + i D_2p+1 after the last anchor)
+//   TVI_DIR: E_k,s,o[j] = sum_{i in interval k} Gt_o[i+j] conj(Za_s[i]) + sum_{i in interval k-1} Gt_o[i+j] conj(Zb_s[i])
+//            (reads the folded G TVI_DX left)                                          out: NH J blocks (set q: rows 2q,
+//            2q + 1)
+// X: XW slots per item; H: NH J partitions per trajectory set at item stride hstride (0: one set for the batch); G: I
+// blocks per item.
+enum TvBusInMac { TVI_FWD, TVI_DX, TVI_DIR };
+template <int MODE, int O>
+__global__ void __launch_bounds__(128) tvbusin_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                          int64_t hstride, float2* G, float2* __restrict__ Out, int S,
+                                                          int I, int J, int K, int nX, int Hb) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int64_t il = blockIdx.y;
+  const int P = (S + 1) / 2, XW = nX * S + (I - nX) * P;
+  const float2* x = X + il * (int64_t)XW * kNbA;
+  const float2* h = H + il * hstride;
+  float2* g = G + il * (int64_t)I * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  // source s of block i: (Za, Zb), or (Z, 0) after the last anchor
+  auto xin = [&](int i, int s, float2& za, float2& zb) {
+    if (i < nX) { pair(x, (int64_t)i * S + s, za, zb); return; }
+    float2 a, b;
+    pair(x, (int64_t)nX * S + (int64_t)(i - nX) * P + (s >> 1), a, b);
+    za = (s & 1) ? b : a;
+    zb = zero;
+  };
+  // IR rows (k, s, 0) and (k, s, 1) (O == 2), or row (k, s) (O == 1), at partition j
+  auto hin = [&](int k, int s, int j, float2& h0, float2& h1) {
+    const int r = k * S + s;
+    if (O == 2) { pair(h, (int64_t)r * J + j, h0, h1); }
+    else { float2 a, b; pair(h, (int64_t)(r >> 1) * J + j, a, b); h0 = (r & 1) ? b : a; h1 = zero; }
+  };
+  const float scale = 1.0f / (float)kNbA;
+  auto emit = [&](int64_t slot, float2 a, float2 b) {
+    a.x *= scale; a.y *= scale; b.x *= scale; b.y *= scale;
+    float* pl = reinterpret_cast<float*>(Out + slot * kNbA);
+    pl[f] = a.x - b.y; pl[kNbA + f] = a.y + b.x;
+    if (fm != f) { pl[fm] = a.x + b.y; pl[kNbA + fm] = b.x - a.y; }
+  };
+  const float sgn = (f & 1) ? -1.f : 1.f;          // (-1)^f, and (-1)^fm: kNbA is even
+  auto axpy = [&](float2 acc, float2 v) { return make_float2(fmaf(sgn, v.x, acc.x), fmaf(sgn, v.y, acc.y)); };
+  auto ival = [&](int i) { const int k = i / Hb; return k < K - 1 ? k : K - 1; };   // anchor interval of block i
+
+  if constexpr (MODE == TVI_FWD) {
+    const int64_t ob = il * (int64_t)I;
+    float2 p0 = zero, p1 = zero;                   // Y_0[m - 1], Y_1[m - 1]
+    for (int m = 0; m < I; ++m) {
+      float2 y0 = zero, y1 = zero;
+      for (int j = 0; j <= m && j < J; ++j) {
+        const int i = m - j, k = ival(i);
+        for (int s = 0; s < S; ++s) {
+          float2 za, zb, h0, h1;
+          xin(i, s, za, zb);
+          hin(k, s, j, h0, h1);
+          cfma(y0, za, h0);
+          if (O == 2) cfma(y1, za, h1);
+          if (i < nX) {
+            hin(k + 1, s, j, h0, h1);
+            cfma(y0, zb, h0);
+            if (O == 2) cfma(y1, zb, h1);
+          }
+        }
+      }
+      emit(ob + m, axpy(y0, p0), axpy(y1, p1));
+      p0 = y0; p1 = y1;
+    }
+  } else if constexpr (MODE == TVI_DX) {
+    // the fold, in place on this thread's own bins f and fm, which no other thread reads; Gt[I - 1] = G[I - 1]
+    for (int q = 0; q + 1 < I; ++q) {
+      float2* a = g + (int64_t)q * kNbA;
+      const float2* b = a + kNbA;
+      a[f] = axpy(a[f], b[f]);
+      if (fm != f) a[fm] = axpy(a[fm], b[fm]);
+    }
+    const int64_t ob = il * (int64_t)XW;
+    for (int i = 0; i < I; ++i) {
+      const int k = ival(i);
+      const bool cross = i < nX;
+      for (int p = 0; p < P; ++p) {
+        const int nc = 2 * p + 1 < S ? 2 : 1;
+        float2 da[2] = {zero, zero}, db[2] = {zero, zero};
+        for (int j = 0; j < J && i + j < I; ++j) {
+          float2 g0, g1, h0, h1;
+          pair(g, i + j, g0, g1);
+          for (int c = 0; c < nc; ++c) {
+            hin(k, 2 * p + c, j, h0, h1);
+            cfma_conj(da[c], g0, h0);
+            if (O == 2) cfma_conj(da[c], g1, h1);
+            if (cross) {
+              hin(k + 1, 2 * p + c, j, h0, h1);
+              cfma_conj(db[c], g0, h0);
+              if (O == 2) cfma_conj(db[c], g1, h1);
+            }
+          }
+        }
+        if (cross) {
+          for (int c = 0; c < nc; ++c) emit(ob + (int64_t)i * S + 2 * p + c, da[c], db[c]);
+        } else {
+          emit(ob + (int64_t)nX * S + (int64_t)(i - nX) * P + p, da[0], da[1]);
+        }
+      }
+    }
+  } else {
+    static_assert(MODE == TVI_DIR, "tvbusin_mac_kernel: unknown mode");
+    // e[o] = E_k,s,o[j] over both intervals that carry IR set k
+    auto ecorr = [&](int k, int s, int j, float2 (&e)[2]) {
+      e[0] = e[1] = zero;
+      for (int part = 0; part < 2; ++part) {       // 0: Za (Z) of interval k, 1: Zb of interval k - 1
+        const int kk = k - part;
+        if (kk < 0) continue;
+        const int lo = kk * Hb, hi = kk == K - 1 ? I : ((kk + 1) * Hb < I ? (kk + 1) * Hb : I);
+        for (int i = lo; i < hi && i + j < I; ++i) {
+          float2 g0, g1, za, zb;
+          pair(g, i + j, g0, g1);
+          xin(i, s, za, zb);
+          const float2 z = part ? zb : za;
+          cfma_conj(e[0], g0, z);
+          if (O == 2) cfma_conj(e[1], g1, z);
+        }
+      }
+    };
+    const int NH = (K * S * O + 1) / 2;
+    const int64_t ob = il * (int64_t)NH * J;
+    float2 e[2];
+    for (int q = 0; q < NH; ++q) {
+      for (int j = 0; j < J; ++j) {
+        if (O == 2) {                              // set q: rows (q, o = 0) and (q, o = 1), q = k S + s
+          ecorr(q / S, q % S, j, e);
+          emit(ob + (int64_t)q * J + j, e[0], e[1]);
+        } else {                                   // set q: rows 2q and 2q + 1 (r = k S + s), an odd last row with 0
+          ecorr((2 * q) / S, (2 * q) % S, j, e);
+          const float2 a = e[0];
+          float2 b = zero;
+          if (2 * q + 1 < K * S) {
+            ecorr((2 * q + 1) / S, (2 * q + 1) % S, j, e);
+            b = e[0];
+          }
+          emit(ob + (int64_t)q * J + j, a, b);
+        }
+      }
+    }
+  }
+}
+
 // Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
 // spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
 // transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
@@ -3013,7 +3302,7 @@ void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs&
   size_t o = 0;
   w.ys = o;  o += align256(sizeof(float2) * (size_t)(g.chunk * (g.ib + g.ex) * kNbA));
   // transient homes for what a forward WITHOUT a backward does not keep (null *_save pointers)
-  w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.p * g.ib * kNbA));
+  w.xsp = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.xwin() * kNbA));
   w.hsp = o; o += align256(sizeof(float2) * (size_t)((g.shared ? 1 : g.chunk) * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.cufft = o; o += align256(cufft_work);
@@ -3022,7 +3311,7 @@ void fwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, FwdWs&
 void bwd_layout(const ConvGeom& g, size_t extra_bytes, size_t cufft_work, BwdWs& w) {
   size_t o = 0;
   w.gs = o; o += align256(sizeof(float2) * (size_t)(g.chunk * (g.ib + g.ex) * kNbA));
-  w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.p * g.ib * kNbA));
+  w.ds = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.xwin() * kNbA));
   w.es = o; o += align256(sizeof(float2) * (size_t)(g.chunk * g.sets * g.jb * kNbA));
   w.extra = o; o += align256(extra_bytes);
   w.mixpart = o; o += align256(g.has_mix ? sizeof(float) * (size_t)(g.chunk * g.ib) : 0);
@@ -3090,7 +3379,7 @@ int put_conv_geometry(const ConvGeom& g, const Geom* synth, Out* out) {
   int rc = conv_setup(g, synth, s);
   if (rc != DASP_OK) return rc;
   out->leff = g.leff; out->conv_block = kB; out->x_blocks = g.ib; out->ir_partitions = g.jb; out->chunk_items = g.chunk;
-  out->xspec_c64 = g.bs * g.p * g.ib * kNbA;
+  out->xspec_c64 = g.bs * g.xwin() * kNbA;
   out->irspec_c64 = (g.shared ? (g.bs > 0 ? 1 : 0) : g.bs) * g.sets * g.jb * kNbA;
   out->fwd_workspace_bytes = (int64_t)s.fwd.total;
   out->bwd_workspace_bytes = (int64_t)s.bwd.total;
@@ -3135,6 +3424,8 @@ int configure_fft_kernels() {
     DASP_CUDA_OK(cudaFuncSetAttribute(tv_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(tvbus_gfft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     DASP_CUDA_OK(cudaFuncSetAttribute(tvbus_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(tvbusin_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
+    DASP_CUDA_OK(cudaFuncSetAttribute(tvbusin_ifft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFftSmemBytes));
     configured[dev] = true;
   }
   return DASP_OK;
@@ -3607,7 +3898,7 @@ int caller_ir_fwd(const Op& op, const ConvGeom& g, const float* x, const float* 
   if ((rc = check_workspace(Op::kFwd, s.fwd.total, workspace_bytes)) != DASP_OK) return rc;
   const FwdWs& w = s.fwd;
   unsigned char* base = (unsigned char*)workspace;
-  const int I = (int)g.ib, J = (int)g.jb;
+  const int J = (int)g.jb;
   const int64_t h_stride = g.shared ? 0 : g.sets * J * (int64_t)kNbA;
   float2* const hs0 = irspec_save ? (float2*)irspec_save : (float2*)(base + w.hsp);
   const float* tw = nullptr;
@@ -3631,7 +3922,7 @@ int caller_ir_fwd(const Op& op, const ConvGeom& g, const float* x, const float* 
   for (int64_t item0 = 0; item0 < g.bs; item0 += g.chunk) {
     const int64_t items = (g.bs - item0 < g.chunk) ? g.bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? s.full : s.rem;
-    float2* xs = xspec_save ? (float2*)xspec_save + item0 * g.p * I * (int64_t)kNbA : (float2*)(base + w.xsp);
+    float2* xs = xspec_save ? (float2*)xspec_save + item0 * g.xwin() * (int64_t)kNbA : (float2*)(base + w.xsp);
     float2* hs = irspec_save ? hs0 + item0 * h_stride : hs0;
     const bool own = g.own_only || own_fft_rows(g.n, x, hs);
     if (!g.shared && (rc = fill_ir(hs, own, item0, items)) != DASP_OK) return rc;
@@ -3672,7 +3963,7 @@ int caller_ir_bwd(const Op& op, const ConvGeom& g, const float* gy, const float*
   for (int64_t item0 = 0; item0 < g.bs; item0 += g.chunk) {
     const int64_t items = (g.bs - item0 < g.chunk) ? g.bs - item0 : g.chunk;
     const Plans& pl = (items == g.chunk) ? s.full : s.rem;
-    const float2* xs = (const float2*)xspec_save + item0 * g.p * I * (int64_t)kNbA;
+    const float2* xs = (const float2*)xspec_save + item0 * g.xwin() * (int64_t)kNbA;
     const float2* hs = (const float2*)irspec_save + item0 * h_stride;
     own = g.own_only || own_fft_rows(g.n, gy, nullptr);
     const IrGrad e = gir == nullptr ? IrGrad::kNone
@@ -4343,6 +4634,160 @@ int dasp_tvbus_shared_bwd(const float* gy, const void* xspec_save, const void* i
                           int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
   return tvbus_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
                    outputs, hop, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ time_varying_convolution_bus, source-side crossfade
+// y[:, o] = sum_k sum_s ((w_k x[:, s]) * h[:, k, s, o]) through the stage above on the own FFT only: the window spectra
+// of tvbusin_fft_kernel (XW per item, g.xw), the partition sets and IR packing of dasp_tvbus_*, one product and one
+// inverse per block (tvbus_ifft_kernel without crossfaded slots), the static bus's gradient transforms, dL/dx through
+// tvbusin_ifft_kernel, and the dL/dIR taps through bus_ifft_kernel.
+namespace {
+extern "C++" {
+template <int MODE>
+int launch_tvbusin_mac(int O, const float2* X, const float2* H, int64_t hstride, float2* G, float2* Out,
+                       int64_t items, int S, int I, int J, int K, int nX, int Hb, cudaStream_t st) {
+  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)items);
+  if (O == 2) tvbusin_mac_kernel<MODE, 2><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, K, nX, Hb);
+  else        tvbusin_mac_kernel<MODE, 1><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, K, nX, Hb);
+  DASP_LAUNCH_OK("tvbusin_mac_kernel");
+  return DASP_OK;
+}
+}  // extern "C++"
+
+struct TvBusInOp {
+  static constexpr const char* kFwd = "tvbus in fwd";
+  static constexpr const char* kBwd = "tvbus in bwd";
+  static constexpr bool kOddSelf = false;
+  int S, O, K, Hb, ir_rows;                          // sources, outputs, anchors, hop / kB, IR rows K S O
+  int nx() const { return (K - 1) * Hb; }            // crossfaded blocks (< ib)
+  int fwd_chunk(const ConvGeom& g, const Plans&, bool own, const float* tw, const float* x, const float*, float2* xs,
+                float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    // dasp_tvbus_*'s bits, and bit 3: the source-side crossfade
+    g_tvbus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (K > 1 ? 4 : 0) | 8;
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    if (h_stride != 0 && (rc = ir_partition_spectra(g, tw, hs, items, st)) != DASP_OK) return rc;
+    float2* ys = (float2*)(ws + w.ys);
+    const int I = (int)g.ib, J = (int)g.jb, nwin = (int)(items * g.xw), nblk = (int)(items * I);
+    const int64_t hop = (int64_t)Hb * kB;
+    tvbusin_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, S, I, nx(), Hb, hop, g.n,
+                                                                         nwin);
+    DASP_LAUNCH_OK("tvbusin_fft_kernel");
+    if ((rc = launch_tvbusin_mac<TVI_FWD>(O, xs, hs, h_stride, nullptr, ys, items, S, I, J, K, nx(), Hb, st)) != DASP_OK)
+      return rc;
+    // no crossfaded slots: every inverse is one output block, rows 0 and 1 as re and im
+    tvbus_ifft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y,
+                                                                        item0, I, 0, Hb, hop, g.n, O, nblk);
+    DASP_LAUNCH_OK("tvbus_ifft_kernel");
+    return DASP_OK;
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans&, bool own, IrGrad e, const float* tw, const float* gy, const float*,
+                const float*, const float2* xs, const float2* hs, int64_t h_stride, float* gx, unsigned char* ws,
+                const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    // dasp_tvbus_*'s bits, and bit 4: the source-side crossfade
+    g_tvbus_last_path[1] = (own ? 1 : 0) | (K > 1 ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) | (g.shared ? 8 : 0) | 16;
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* gs = (float2*)(ws + w.gs);
+    float2* ds = (float2*)(ws + w.ds);
+    const int I = (int)g.ib, J = (int)g.jb, nwin = (int)(items * g.xw), nblk = (int)(items * I);
+    const int64_t hop = (int64_t)Hb * kB;
+    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, O, 1, I, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    if ((rc = launch_tvbusin_mac<TVI_DX>(O, xs, hs, h_stride, gs, ds, items, S, I, J, K, nx(), Hb, st)) != DASP_OK)
+      return rc;
+    tvbusin_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx,
+                                                                          item0, S, I, nx(), Hb, hop, g.n, nwin);
+    DASP_LAUNCH_OK("tvbusin_ifft_kernel");
+    if (e == IrGrad::kNone) return DASP_OK;          // a fixed trajectory set: no dL/dIR work at all
+    return launch_tvbusin_mac<TVI_DIR>(O, xs, hs, 0, gs, (float2*)(ws + w.es), items, S, I, J, K, nx(), Hb, st);
+  }
+  // dL/dIR taps [0, leff) of items [item0, item0 + items): the first half of the inverse of each partition
+  int ir_taps(const ConvGeom& g, bool, const float* tw, const float2* es, const float*, float* gir, int64_t item0,
+              int64_t items, cudaStream_t st) const {
+    const int J = (int)g.jb, nparts = (int)(items * g.sets * J);
+    bus_ifft_kernel<<<runs(nparts), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(es), tw, gir,
+                                                                        item0, ir_rows, g.sets, J, g.L, g.leff, 0,
+                                                                        nparts);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    return DASP_OK;
+  }
+};
+
+// dasp_tvbus_*'s argument checks; the source-side windows: S per crossfaded block, ceil(S / 2) per later block, and one
+// product and gradient spectrum per block
+int make_tvbusin_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t K, int64_t S, int64_t O, int64_t hop,
+                      int64_t chunk, ConvGeom& g) {
+  int rc = make_tvbus_geom(shared, bs, n, L, K, S, O, hop, chunk, g);
+  if (rc != DASP_OK) return rc;
+  const int64_t nX = (K - 1) * (hop / kB);
+  g.ex = 0;
+  g.xw = nX * S + (g.ib - nX) * g.p;
+  return DASP_OK;
+}
+TvBusInOp tvbusin_op(int64_t K, int64_t S, int64_t O, int64_t hop) {
+  return TvBusInOp{(int)S, (int)O, (int)K, (int)(hop / kB), (int)(K * S * O)};
+}
+
+int tvbusin_fwd(bool shared, const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
+                int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_tvbusin_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return caller_ir_fwd(tvbusin_op(K, S, O, hop), g, x, ir, nullptr, y, xspec_save, irspec_save, workspace,
+                       workspace_bytes, stream);
+}
+
+int tvbusin_bwd(bool shared, const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
+                int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = make_tvbusin_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return caller_ir_bwd(tvbusin_op(K, S, O, hop), g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir, nullptr,
+                       workspace, workspace_bytes, stream);
+}
+}  // namespace
+
+int dasp_tvbus_in_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs,
+                           int64_t hop, int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "tvbus in geometry: null out");
+  ConvGeom g;
+  int rc = make_tvbusin_geom(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
+}
+
+int dasp_tvbus_in_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                      int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                      int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvbusin_fwd(false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                     outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvbus_in_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                      void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                      int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvbusin_bwd(false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                     outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvbus_in_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                             int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                             void* stream) {
+  return tvbusin_fwd(true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                     outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvbus_in_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                             int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                             void* stream) {
+  return tvbusin_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
+                     outputs, hop, chunk_items, stream);
 }
 
 // ------------------------------------------------------------------ noise_shaped_impulse_response

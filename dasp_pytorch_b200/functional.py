@@ -1610,7 +1610,8 @@ def time_varying_convolution_reverberation(x: torch.Tensor, sample_rate: float, 
     without splitting the audio windows: every output block lies inside one anchor interval, so it needs the products
     of two IRs with the same window spectra a static convolution uses, and the crossfade is applied to the inverse
     transform's output.  Input-side weighting, ``sum_k (w_k x) * h_k``, would need zero-padded transforms per block
-    and IR, because an overlap-save window straddles anchor boundaries.
+    and IR, because an overlap-save window straddles anchor boundaries.  A moving mono source (input-side weighting) is
+    ``time_varying_convolution_bus`` with ``S = 1`` and ``crossfade="input"``.
 
     Args:
         x: audio ``(bs, 1|2, n)``; mono is used for both channels.
@@ -1674,38 +1675,39 @@ def time_varying_convolution_reverberation(x: torch.Tensor, sample_rate: float, 
 
 class _TvBusFn(torch.autograd.Function):
     """x (bs, S, n), ir (bs | 1, K, S, O, L) -> y (bs, O, n).  n % 4 == 0 and 16-byte aligned rows
-    (time_varying_convolution_bus pads).  An ir of batch 1 with bs > 1 runs the dasp_tvbus_shared_* entry points; its
-    gradient is the sum over the items."""
+    (time_varying_convolution_bus pads).  entry "tvbus" crossfades on the output side, "tvbus_in" on the source side.
+    An ir of batch 1 with bs > 1 runs the dasp_<entry>_shared_* entry points; its gradient is the sum over the
+    items."""
 
     @staticmethod
-    def forward(ctx, x, ir, hop, chunk):
+    def forward(ctx, x, ir, hop, chunk, entry="tvbus"):
         lib = _abi.lib()
         bs, S, n = x.shape
         ir_bs, K, _, O, ir_len = ir.shape
         shared = ir_bs == 1 and bs > 1
-        kind = "tvbus_shared" if shared else "tvbus"
+        kind = f"{entry}_shared" if shared else entry
         dev = x.device
         y = torch.empty(bs, O, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:2])
         with torch.cuda.device(dev):
             ws, (xspec, irspec), bwd_bytes = _geom_buffers(
-                _abi.ConvGeom(), "dasp_tvbus_geometry", (bs, n, ir_len, K, S, O, hop, int(shared), chunk), dev,
+                _abi.ConvGeom(), f"dasp_{entry}_geometry", (bs, n, ir_len, K, S, O, hop, int(shared), chunk), dev,
                 need_bwd)
-            with _timed("tvbus_fwd", dev):
+            with _timed(f"{entry}_fwd", dev):
                 check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), ptr(ir), ptr(y), ptr(xspec), ptr(irspec), ptr(ws),
                                                        ws.numel(), bs, n, ir_len, K, S, O, hop, chunk,
                                                        stream_ptr(dev)),
                       f"dasp_{kind}_fwd")
         if need_bwd:
             ctx.save_for_backward(xspec, irspec)
-        ctx.cfg = (kind, bs, S, O, n, ir.shape, hop, chunk, bwd_bytes)
+        ctx.cfg = (entry, kind, bs, S, O, n, ir.shape, hop, chunk, bwd_bytes)
         return y
 
     @staticmethod
     def backward(ctx, gy):
         lib = _abi.lib()
         xspec, irspec = ctx.saved_tensors
-        kind, bs, S, O, n, ir_shape, hop, chunk, bwd_bytes = ctx.cfg
+        entry, kind, bs, S, O, n, ir_shape, hop, chunk, bwd_bytes = ctx.cfg
         dev = gy.device
         gy = gy.contiguous()
         if gy.data_ptr() % 16:
@@ -1714,30 +1716,38 @@ class _TvBusFn(torch.autograd.Function):
         # a fixed trajectory set (measured or simulated rooms) skips every dL/dIR kernel
         gir = torch.empty(ir_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
         ws = _ws_bytes(bwd_bytes, dev)
-        with torch.cuda.device(dev), _timed("tvbus_bwd", dev):
+        with torch.cuda.device(dev), _timed(f"{entry}_bwd", dev):
             check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(xspec), ptr(irspec), ptr(gx), ptr(gir), ptr(ws),
                                                    ws.numel(), bs, n, ir_shape[4], ir_shape[1], S, O, hop, chunk,
                                                    stream_ptr(dev)),
                   f"dasp_{kind}_bwd")
-        return gx, gir, None, None
+        return gx, gir, None, None, None
 
 
-def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor, hop: int):
-    """Several moving sources, each through its own trajectory of impulse responses, crossfaded along the output and
-    summed into one mono or stereo bus: ``convolution_bus`` whose IR set changes over time, as
+def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor, hop: int, *,
+                                 crossfade: str = "output"):
+    """Several moving sources, each through its own trajectory of impulse responses, crossfaded and summed into one
+    mono or stereo bus: ``convolution_bus`` whose IR set changes over time, as
     ``time_varying_convolution_reverberation``'s IR does.  Set ``k`` of the trajectory, ``h[:, k]``, is a complete
-    ``convolution_bus`` IR set, the scene at the anchor time ``t_k = k * hop``::
+    ``convolution_bus`` IR set, the scene at the anchor time ``t_k = k * hop``.  ``crossfade`` chooses where the
+    weights apply::
 
-        y[:, o](t) = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, o])(t)
+        "output":  y[:, o](t) = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, o])(t)
+        "input":   y[:, o](t) = sum_k sum_s ((w_k x[:, s]) * h[:, k, s, o])(t)
 
         k hop <= t < (k+1) hop, k < K - 1:   a = (t - k hop) / hop,   w_k = 1 - a,   w_{k+1} = a,   other w = 0
         t >= (K - 1) hop:                    w_{K-1} = 1
 
     (``*`` the causal convolution cropped to ``n``, exactly as ``convolution_reverberation`` defines its wet signal;
-    ``w_k`` are ``time_varying_convolution_reverberation``'s crossfade weights).  Uses: reverberant multi-talker
-    mixtures with moving speakers for separation and enhancement training, binaural or stereo scenes with several
-    moving objects, a stereo source moving through a room (``S = 2, O = 2`` is a time-varying true-stereo rendering),
-    and a learnable time-varying S-input FIR.
+    ``w_k`` are ``time_varying_convolution_reverberation``'s crossfade weights).  The output-side crossfade weights the
+    time a sample is heard: it models a moving listener (or a static source heard through a changing room).  The
+    input-side (source-side) crossfade weights the time a sample is emitted: a sample emitted at ``tau`` between anchors
+    ``k`` and ``k + 1`` keeps ``(1 - a) h_k + a h_{k+1}`` over its whole reverb tail, also the part heard after later
+    anchors, which is the model of a moving point source (propagation delay and Doppler aside).  The two agree when
+    ``L = 1`` or all sets are equal; they differ most when ``L`` is long against ``hop``.  Uses: reverberant
+    multi-talker mixtures with moving speakers for separation and enhancement training, binaural or stereo scenes with
+    several moving objects, a stereo source moving through a room (``S = 2, O = 2`` is a time-varying true-stereo
+    rendering), and a learnable time-varying S-input FIR.
 
     Args:
         x: audio ``(bs, S, n)``, ``1 <= S <= CONV_BUS_MAX_INPUTS`` sources.
@@ -1748,23 +1758,32 @@ def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_re
         hop: the anchor spacing in samples, a positive multiple of ``CONV_PARTITION_SAMPLES`` (4096), so that every
             output block and every gradient block lies inside one anchor interval; ``(K - 1) * hop < n``.  All
             sources share the one anchor grid.
+        crossfade: ``"output"`` (the default: a moving listener) or ``"input"`` (a moving source), keyword only.
 
     Returns ``(bs, O, n)`` in x's dtype, computed in fp32.  There is no dry/wet mix, as in ``convolution_bus``.
 
-    Identities (held to fp32 rounding):
+    Identities (held to fp32 rounding), for ``crossfade="output"``:
 
     1. ``K = 1``: ``convolution_bus(x, sr, h[:, 0])``; K equal sets: ``convolution_bus`` with that set.
     2. ``S = 1, O = 2``: ``time_varying_convolution_reverberation(x, sr, h[:, :, 0], hop, mix=1)``.
     3. Any ``S``: the sum over ``s`` of ``time_varying_convolution_bus(x[:, s:s+1], sr, h[:, :, s:s+1], hop)``.
     4. From the last anchor on (``t >= (K - 1) hop``): ``convolution_bus(x, sr, h[:, K - 1])``.
 
+    and for ``crossfade="input"``:
+
+    1. ``K = 1``: ``convolution_bus(x, sr, h[:, 0])``; K equal sets: ``convolution_bus`` with that set.
+    2. Any ``S``: the sum over ``s`` of the single-source calls, as above.
+    3. ``sum_k convolution_bus(w_k x, sr, h[:, k])``, the segment composition, with ``w_k`` broadcast over the sources.
+    4. Emission time: a unit impulse at ``tau`` between anchors ``k`` and ``k + 1`` (weight ``a``) gives
+       ``(1 - a) h[:, k] + a h[:, k + 1]`` starting at ``tau``, over its whole tail.
+
     Gradients flow to ``x`` (every source) and to every IR row; taps at or beyond ``min(L, n)`` reach no output and
     get exactly 0.  The gradient of a shared ``(1, K, S, O, L)`` set has that shape and is the sum over the items,
     accumulated in fp64 in item order, so it does not depend on ``REVERB_CHUNK_ITEMS``.  When the IRs do not require a
-    gradient, the backward skips all dL/dIR work.
+    gradient, the backward skips all dL/dIR work.  This holds for both crossfades.
 
-    Cost: the rows of every signal are packed two per transform, as in ``convolution_bus``: ceil(S / 2) window
-    transforms per block, transformed and kept for the backward once for all K sets; the K S O IR rows' partitions in
+    Cost of ``"output"``: the rows of every signal are packed two per transform, as in ``convolution_bus``: ceil(S / 2)
+    window transforms per block, transformed and kept for the backward once for all K sets; the K S O IR rows' partitions in
     ceil(K S O / 2) transforms per partition; one product per IR set and block summed over the sources, and one inverse
     transform per output row and crossfaded block (a mono bus: per block).  S ``time_varying_convolution_reverberation``
     calls would transform and keep every window S times and take S sets of inverse transforms.  A source that does not
@@ -1772,7 +1791,18 @@ def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_re
     its windows by both copies, for the static convolution's result (a crossfade of two equal outputs).  Rows whose
     length is not a multiple of 4 are zero-padded to one (the transforms bulk-copy 16-byte rows); a padding sample
     reaches no output sample below ``n``.
+
+    Cost of ``"input"``: a block between two anchors is weighted per source and transformed zero-padded, one transform
+    per source carrying both weighted pieces (1 - a and a), so the window transforms and the spectra kept for the
+    backward are S per crossfaded block instead of ceil(S / 2); after the last anchor two sources share a transform.
+    The partitions are those of ``"output"``.  Each output block takes one product (both IR sets of every input block it
+    reaches, summed over the sources, the overlap-add of the zero-padded blocks done on the spectra) and one inverse
+    transform for both bus rows.  The backward transforms the gradient once per block for both rows, and takes one dL/dx
+    inverse per source and crossfaded block (ceil(S / 2) per later block).  The segment composition above would
+    transform every block of every source once per segment it falls in, and its segments' tails again.
     """
+    if crossfade not in ("output", "input"):
+        raise ValueError(f'crossfade must be "output" or "input", got {crossfade!r}')
     if not torch.is_tensor(x) or x.dim() != 3:
         raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
     if not torch.is_tensor(impulse_response) or impulse_response.dim() != 5:
@@ -1801,5 +1831,8 @@ def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_re
             irf = irf[..., :n].contiguous()
     elif xf.data_ptr() % 16:
         xf = xf.clone()
-    y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device))
+    if crossfade == "output":
+        y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device))
+    else:
+        y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device), "tvbus_in")
     return (y[..., :n] if n4 != n else y).to(dt)

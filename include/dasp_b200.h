@@ -421,9 +421,32 @@ int dasp_tvbus_shared_bwd(const float* gy, const void* xspec_save, const void* i
                           float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
                           int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
                           void* stream);
-/* test hook: dispatch of the most recent call.  which = 0 (forward): bit 0 = own in-shared-memory FFT (always),
-   bit 1 = shared trajectory set, bit 2 = crossfaded blocks (K > 1).  which = 1 (backward): bit 0 = own FFT (always),
-   bit 1 = crossfaded blocks, bit 2 = dL/dIR computed, bit 3 = shared trajectory set */
+/* ---- the same bus with a source-side crossfade: every emitted sample keeps the IR set of its emission time --------
+ *   y[:, o](t) = sum_k sum_s ((w_k x[:, s]) * h[:, k, s, o])(t)
+ * The arguments, shapes, rules and rejections are dasp_tvbus_*'s.  The window spectra are zero-padded transforms of
+ * each source's weighted blocks: S per crossfaded block ((K - 1) hop / conv_block blocks), ceil(S / 2) per later block,
+ * so geom.xspec_c64 comes from dasp_tvbus_in_geometry; one product and one inverse transform per output block. */
+int dasp_tvbus_in_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs,
+                           int64_t hop, int64_t shared, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_tvbus_in_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                      int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                      int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvbus_in_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                      float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                      int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                      void* stream);
+int dasp_tvbus_in_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                             int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                             void* stream);
+int dasp_tvbus_in_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                             float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
+                             int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                             int64_t chunk_items, void* stream);
+/* test hook: dispatch of the most recent dasp_tvbus_* or dasp_tvbus_in_* call.  which = 0 (forward): bit 0 = own
+   in-shared-memory FFT (always), bit 1 = shared trajectory set, bit 2 = crossfaded blocks (K > 1), bit 3 = source-side
+   crossfade (dasp_tvbus_in_*).  which = 1 (backward): bit 0 = own FFT (always), bit 1 = crossfaded blocks, bit 2 =
+   dL/dIR computed, bit 3 = shared trajectory set, bit 4 = source-side crossfade */
 int dasp_debug_tvbus_last_path(int which);
 
 #ifdef __cplusplus

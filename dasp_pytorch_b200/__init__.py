@@ -13,11 +13,14 @@ number of input channels, each through its own impulse responses, summed into a 
 ``time_varying_convolution_reverberation`` (a trajectory of impulse responses crossfaded along the output, for moving
 sources and listeners) and ``time_varying_convolution_bus`` (several moving sources, each with its own trajectory of
 impulse responses, crossfaded and summed into a mono or stereo bus; ``crossfade="input"`` crossfades on the source side,
-so every emitted sample keeps the impulse response of its emission time).
+so every emitted sample keeps the impulse response of its emission time) and ``multichannel_convolution`` (S sources
+through an S x M matrix of impulse responses into up to 32 output channels: microphone arrays, ambisonics, multichannel
+beds).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
     CONV_BUS_MAX_INPUTS,
+    CONV_MC_MAX_OUTPUTS,
     CONV_PARTITION_SAMPLES,
     compressor,
     compressor_gain,
@@ -27,6 +30,7 @@ from dasp_pytorch_b200.functional import (  # noqa: F401
     expander,
     expander_gain,
     gain,
+    multichannel_convolution,
     noise_shaped_impulse_response,
     noise_shaped_impulse_response_packed,
     noise_shaped_reverberation,

@@ -98,6 +98,11 @@ _SIGNATURES = {
     "dasp_conv_bus_shared_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_conv_bus_shared_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_debug_conv_bus_last_path": (c_int, [c_int]),
+    "dasp_conv_mc_geometry": (c_int, [I64, I64, I64, I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
+    "dasp_conv_mc_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_conv_mc_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_conv_mc_shared_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_conv_mc_shared_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_tvconv_geometry": (c_int, [I64, I64, I64, I64, I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
     "dasp_tvconv_fwd": (c_int, [P, I64, P, I64, I64, I64, I64, P, P, P, P, P, I64, I64, I64, I64, P]),
     "dasp_tvconv_bwd": (c_int, [P, P, I64, I64, I64, I64, I64, P, P, P, P, P, P, P, I64, I64, I64, I64, P]),

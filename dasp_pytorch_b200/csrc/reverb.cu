@@ -38,6 +38,8 @@
 // convolution_bus (dasp_conv_bus_*) is the same partitioned convolution for S inputs summed into O = 1 or 2 outputs:
 // every signal's rows are packed two per transform (bus_fft_kernel, ir_pack_kernel + x_fft_kernel's partition units),
 // bus_mac_kernel sums the untangled products over the inputs, and bus_ifft_kernel writes the outputs, dL/dx and dL/dIR.
+// multichannel_convolution (dasp_conv_mc_*) is the bus with up to 32 outputs: the outputs and their gradients in
+// ceil(M / 2) row pairs per block, and busmc_mac_kernel for the products when M >= 3.
 //
 // time_varying_convolution_reverberation (dasp_tvconv_*) is the same convolution with K IRs crossfaded along the
 // output: the audio windows of a static convolution, the products of the two IRs of each block (tv_mac_kernel), and
@@ -1986,6 +1988,18 @@ bus_fft_kernel(const float* __restrict__ src, float2* __restrict__ out, const fl
 // MAXB > 0 caches the block operands of one input in registers (I, J <= MAXB) and loops over the inputs with the
 // accumulators held; MAXB == 0 reads every operand from L2.
 enum BusMac { BUS_FWD, BUS_DX, BUS_DIR };
+// bus_mac_kernel's emit and axpy as functions, for busmc_mac_kernel, at bins (f, fm = kNbA - f) of one thread: real
+// rows (a, b) packed planar into block `slot` of Out, scaled; and acc + (-1)^f v (sgn = (-1)^f).  bus_mac_kernel keeps
+// its lambdas: calling these from them changes the code nvcc generates for its dL/dx instantiations.
+__device__ __forceinline__ void bus_emit(float2* Out, int64_t slot, int f, int fm, float scale, float2 a, float2 b) {
+  a.x *= scale; a.y *= scale; b.x *= scale; b.y *= scale;
+  float* pl = reinterpret_cast<float*>(Out + slot * kNbA);
+  pl[f] = a.x - b.y; pl[kNbA + f] = a.y + b.x;
+  if (fm != f) { pl[fm] = a.x + b.y; pl[kNbA + fm] = b.x - a.y; }
+}
+__device__ __forceinline__ float2 bus_axpy(float sgn, float2 acc, float2 v) {
+  return make_float2(fmaf(sgn, v.x, acc.x), fmaf(sgn, v.y, acc.y));
+}
 template <int MAXB, int MODE, int O>
 __global__ void __launch_bounds__(128) bus_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
                                                       int64_t hstride, const float2* __restrict__ G,
@@ -2191,6 +2205,211 @@ __global__ void __launch_bounds__(128) bus_mac_kernel(const float2* __restrict__
             emit(ob + (int64_t)p * J + j, e00, two ? e10 : zero);
           }
         }
+      }
+    }
+  }
+}
+
+// bus_emit's second row: adds real row b to a block bus_emit stored with b = 0 (the same thread, the same bins), which
+// leaves the bits of bus_emit(a, b)
+__device__ __forceinline__ void bus_emit_add(float2* Out, int64_t slot, int f, int fm, float scale, float2 b) {
+  b.x *= scale; b.y *= scale;
+  float* pl = reinterpret_cast<float*>(Out + slot * kNbA);
+  pl[f] -= b.y; pl[kNbA + f] += b.x;
+  if (fm != f) { pl[fm] += b.y; pl[kNbA + fm] += b.x; }
+}
+
+// The bus products for M >= 3 outputs (multichannel_convolution), the operands and results of bus_mac_kernel with the
+// outputs in Q = ceil(M / 2) packed pairs: IR row s M + m is row (s M + m) & 1 of partition set (s M + m) >> 1, and
+// output / gradient pair q of block i is block q I + i of the item.  One slice of an item per blockIdx.y, the items
+// along blockIdx.z, so the slices of an item run next to each other and re-read its spectra from L2:
+//   BUS_FWD: slice q < Q:   Y_2q[i], Y_2q+1[i], as the O = 2 body                      out: Q I blocks (Y_2q + i Y_2q+1)
+//   BUS_DX:  slice p < P:   W_2p[i], W_2p+1[i] (bus_mac_kernel's), D_s summed over the Q output pairs; source 2p + 1
+//                           is added to the stored source 2p (bus_emit_add)            out: P I blocks
+//   BUS_DIR: slice k < NH:  E of rows 2k and 2k + 1, each an (s, m)                    out: NH J blocks
+// MAXB > 0 caches the blocks of one (input, output pair) in registers (I, J <= MAXB); MAXB == 0 reads from L2.
+template <int MAXB, int MODE>
+__global__ void __launch_bounds__(128) busmc_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                        int64_t hstride, const float2* __restrict__ G,
+                                                        float2* __restrict__ Out, int S, int M, int I, int J,
+                                                        float scale) {
+  constexpr int MB = MAXB > 0 ? MAXB : 1;
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int sl = blockIdx.y;
+  const int64_t il = blockIdx.z;
+  const int P = (S + 1) / 2, Q = (M + 1) / 2, NH = (S * M + 1) / 2;
+  const float2* x = X + il * (int64_t)P * I * kNbA;
+  const float2* h = H + il * hstride;
+  const float2* g = G + il * (int64_t)Q * I * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  auto pick = [&](const float2* base, int64_t set, int odd) -> float2 {
+    float2 a, b;
+    pair(base, set, a, b);
+    return odd ? b : a;
+  };
+  // input s at block i; IR row r at partition j; gradient row m at block i
+  auto xin = [&](int s, int i) { return pick(x, (int64_t)(s >> 1) * I + i, s & 1); };
+  auto hrow = [&](int r, int j) { return pick(h, (int64_t)(r >> 1) * J + j, r & 1); };
+  auto grow = [&](int m, int i) { return pick(g, (int64_t)(m >> 1) * I + i, m & 1); };
+  // IR rows (s, 2q) and (s, 2q + 1) at partition j, 0 past the last output; one set when s M + 2q is even
+  auto hin = [&](int s, int q, int j, float2& h0, float2& h1) {
+    const int r = s * M + 2 * q;
+    if (2 * q + 1 >= M) { h0 = hrow(r, j); h1 = zero; }
+    else if ((r & 1) == 0) pair(h, (int64_t)(r >> 1) * J + j, h0, h1);
+    else { h0 = hrow(r, j); h1 = hrow(r + 1, j); }
+  };
+  auto gin = [&](int q, int i, float2& g0, float2& g1) { pair(g, (int64_t)q * I + i, g0, g1); };
+  auto emit = [&](int64_t slot, float2 a, float2 b) { bus_emit(Out, slot, f, fm, scale, a, b); };
+  const float sgn = (f & 1) ? -1.f : 1.f;
+  auto axpy = [&](float2 acc, float2 v) { return bus_axpy(sgn, acc, v); };
+
+  if constexpr (MODE == BUS_FWD) {
+    const int q = sl;
+    const int64_t ob = (il * Q + q) * (int64_t)I;
+    if constexpr (MAXB > 0) {
+      float2 y0[MB], y1[MB];
+#pragma unroll
+      for (int o = 0; o < MB; ++o) y0[o] = y1[o] = zero;
+      for (int s = 0; s < S; ++s) {
+        float2 xv[MB], h0[MB], h1[MB];
+#pragma unroll
+        for (int i = 0; i < MB; ++i) {
+          xv[i] = h0[i] = h1[i] = zero;                // operands beyond I / J are zero
+          if (i < I) xv[i] = xin(s, i);
+          if (i < J) hin(s, q, i, h0[i], h1[i]);
+        }
+#pragma unroll
+        for (int o = 0; o < MB; ++o) {
+#pragma unroll
+          for (int j = 0; j <= o; ++j) {
+            cfma(y0[o], xv[o - j], h0[j]);
+            cfma(y1[o], xv[o - j], h1[j]);
+          }
+        }
+      }
+#pragma unroll
+      for (int o = 0; o < MB; ++o)
+        if (o < I) emit(ob + o, y0[o], y1[o]);
+    } else {
+      for (int o = 0; o < I; ++o) {
+        float2 y0 = zero, y1 = zero;
+        for (int s = 0; s < S; ++s) {
+          for (int j = 0; j <= o && j < J; ++j) {
+            float2 h0, h1;
+            hin(s, q, j, h0, h1);
+            const float2 xv = xin(s, o - j);
+            cfma(y0, xv, h0);
+            cfma(y1, xv, h1);
+          }
+        }
+        emit(ob + o, y0, y1);
+      }
+    }
+  } else if constexpr (MODE == BUS_DX) {
+    const int p = sl;
+    const int64_t ob = (il * P + p) * (int64_t)I;
+    if constexpr (MAXB > 0) {
+      for (int c = 0; c < 2 && 2 * p + c < S; ++c) {
+        const int s = 2 * p + c;
+        float2 d[MB];                                  // D_s, then W_s folded in place (ascending)
+#pragma unroll
+        for (int i = 0; i < MB; ++i) d[i] = zero;
+        for (int q = 0; q < Q; ++q) {
+          float2 g0[MB], g1[MB], h0[MB], h1[MB];
+#pragma unroll
+          for (int i = 0; i < MB; ++i) {
+            g0[i] = g1[i] = h0[i] = h1[i] = zero;
+            if (i < I) gin(q, i, g0[i], g1[i]);
+            if (i < J) hin(s, q, i, h0[i], h1[i]);
+          }
+#pragma unroll
+          for (int i = 0; i < MB; ++i) {
+#pragma unroll
+            for (int j = 0; i + j < MB; ++j) {
+              cfma_conj(d[i], g0[i + j], h0[j]);
+              cfma_conj(d[i], g1[i + j], h1[j]);
+            }
+          }
+        }
+#pragma unroll
+        for (int i = 0; i + 1 < MB; ++i) d[i] = axpy(d[i], d[i + 1]);
+#pragma unroll
+        for (int i = 0; i < MB; ++i) {
+          if (i < I) {
+            if (c == 0) emit(ob + i, d[i], zero);
+            else bus_emit_add(Out, ob + i, f, fm, scale, d[i]);
+          }
+        }
+      }
+    } else {
+      for (int i = 0; i < I; ++i) {
+        float2 w[2] = {zero, zero};
+        for (int c = 0; c < 2 && 2 * p + c < S; ++c) {
+          for (int b = i; b < i + 2 && b < I; ++b) {   // D_s[i] + (-1)^f D_s[i + 1]
+            float2 d = zero;
+            for (int q = 0; q < Q; ++q) {
+              for (int j = 0; j < J && b + j < I; ++j) {
+                float2 g0, g1, h0, h1;
+                gin(q, b + j, g0, g1);
+                hin(2 * p + c, q, j, h0, h1);
+                cfma_conj(d, g0, h0);
+                cfma_conj(d, g1, h1);
+              }
+            }
+            w[c] = b == i ? d : axpy(w[c], d);
+          }
+        }
+        emit(ob + i, w[0], w[1]);
+      }
+    }
+  } else {
+    static_assert(MODE == BUS_DIR, "busmc_mac_kernel: unknown mode");
+    const int k = sl;
+    const int r0 = 2 * k, r1 = 2 * k + 1;
+    const bool two = r1 < S * M;
+    const int s0 = r0 / M, m0 = r0 - s0 * M, s1 = r1 / M, m1 = r1 - s1 * M;
+    const int64_t ob = (il * NH + k) * (int64_t)J;
+    if constexpr (MAXB > 0) {
+      // row 2k into ea, then row 2k + 1 with the operands of row 2k out of registers, emitted with ea
+      float2 ea[MB], gv[MB], xv[MB];
+#pragma unroll
+      for (int i = 0; i < MB; ++i) {
+        gv[i] = xv[i] = zero;
+        if (i < I) { gv[i] = grow(m0, i); xv[i] = xin(s0, i); }
+      }
+#pragma unroll
+      for (int j = 0; j < MB; ++j) {
+        ea[j] = zero;
+#pragma unroll
+        for (int i = 0; i + j < MB; ++i) cfma_conj(ea[j], gv[j + i], xv[i]);
+      }
+#pragma unroll
+      for (int i = 0; i < MB; ++i) {
+        gv[i] = xv[i] = zero;
+        if (two && i < I) { gv[i] = grow(m1, i); xv[i] = xin(s1, i); }
+      }
+#pragma unroll
+      for (int j = 0; j < MB; ++j) {
+        if (j < J) {
+          float2 eb = zero;
+#pragma unroll
+          for (int i = 0; i + j < MB; ++i) cfma_conj(eb, gv[j + i], xv[i]);
+          emit(ob + j, ea[j], eb);
+        }
+      }
+    } else {
+      for (int j = 0; j < J; ++j) {
+        float2 ea = zero, eb = zero;
+        for (int i = 0; i + j < I; ++i) {
+          cfma_conj(ea, grow(m0, j + i), xin(s0, i));
+          if (two) cfma_conj(eb, grow(m1, j + i), xin(s1, i));
+        }
+        emit(ob + j, ea, eb);
       }
     }
   }
@@ -4146,11 +4365,24 @@ void launch_bus_mac_o(const ConvGeom& g, int S, const float2* X, const float2* H
   else if (m <= 16) bus_mac_kernel<16, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, inv);
   else              bus_mac_kernel<0, MODE, O><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, I, J, inv);
 }
+// O >= 3 outputs: one slice per output pair (forward), input pair (dL/dx) or partition set (dL/dIR) of each item
+template <int MODE>
+void launch_busmc_mac(const ConvGeom& g, int S, int O, const float2* X, const float2* H, int64_t hstride,
+                      const float2* G, float2* Out, int64_t items, cudaStream_t st) {
+  const int slices = MODE == BUS_FWD ? (O + 1) / 2 : (MODE == BUS_DX ? g.p : g.sets);
+  dim3 grid((kNbA / 2 + 1 + 127) / 128, (unsigned)slices, (unsigned)items);
+  const int I = (int)g.ib, J = (int)g.jb, m = I > J ? I : J;
+  const float inv = 1.0f / (float)kNbA;
+  if (m <= 12)      busmc_mac_kernel<12, MODE><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, O, I, J, inv);
+  else if (m <= 16) busmc_mac_kernel<16, MODE><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, O, I, J, inv);
+  else              busmc_mac_kernel<0, MODE><<<grid, 128, 0, st>>>(X, H, hstride, G, Out, S, O, I, J, inv);
+}
 template <int MODE>
 int launch_bus_mac(const ConvGeom& g, int S, int O, const float2* X, const float2* H, int64_t hstride, const float2* G,
                    float2* Out, int64_t items, cudaStream_t st) {
-  if (O == 2) launch_bus_mac_o<MODE, 2>(g, S, X, H, hstride, G, Out, items, st);
-  else        launch_bus_mac_o<MODE, 1>(g, S, X, H, hstride, G, Out, items, st);
+  if (O == 2)      launch_bus_mac_o<MODE, 2>(g, S, X, H, hstride, G, Out, items, st);
+  else if (O == 1) launch_bus_mac_o<MODE, 1>(g, S, X, H, hstride, G, Out, items, st);
+  else             launch_busmc_mac<MODE>(g, S, O, X, H, hstride, G, Out, items, st);
   DASP_LAUNCH_OK("bus_mac_kernel");
   return DASP_OK;
 }
@@ -4165,32 +4397,34 @@ struct BusOp {
   int fwd_chunk(const ConvGeom& g, const Plans&, bool own, const float* tw, const float* x, const float*, float2* xs,
                 float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
                 int64_t items, cudaStream_t st) const {
-    g_bus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (bus_mac_cached(g) ? 4 : 0);
+    // bit 0: own FFT, bit 1: one IR shared by the batch, bit 2: register-cached products, bit 3: O >= 3 outputs
+    g_bus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (bus_mac_cached(g) ? 4 : 0) | (O > 2 ? 8 : 0);
     int rc = configure_fft_kernels();
     if (rc != DASP_OK) return rc;
     if (h_stride != 0 && (rc = ir_partition_spectra(g, tw, hs, items, st)) != DASP_OK) return rc;
     float2* ys = (float2*)(ws + w.ys);
-    const int I = (int)g.ib, nwin = (int)(items * g.p * I), nblk = (int)(items * I);
+    const int I = (int)g.ib, Q = (O + 1) / 2, nwin = (int)(items * g.p * I), nblk = (int)(items * Q * I);
     bus_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, S, g.p, I, g.n, 0, nwin);
     DASP_LAUNCH_OK("bus_fft_kernel");
     if ((rc = launch_bus_mac<BUS_FWD>(g, S, O, xs, hs, h_stride, nullptr, ys, items, st)) != DASP_OK) return rc;
     bus_ifft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y, item0,
-                                                                      O, 1, I, g.n, g.n, 1, nblk);
+                                                                      O, Q, I, g.n, g.n, 1, nblk);
     DASP_LAUNCH_OK("bus_ifft_kernel");
     return DASP_OK;
   }
   int bwd_chunk(const ConvGeom& g, const Plans&, bool own, IrGrad e, const float* tw, const float* gy, const float*,
                 const float*, const float2* xs, const float2* hs, int64_t h_stride, float* gx, unsigned char* ws,
                 const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
-    // bit 0: own FFT, bit 1: register-cached products, bit 2: dL/dIR computed, bit 3: one IR shared by the batch
+    // bit 0: own FFT, bit 1: register-cached products, bit 2: dL/dIR computed, bit 3: one IR shared by the batch,
+    // bit 4: O >= 3 outputs
     g_bus_last_path[1] = (own ? 1 : 0) | (bus_mac_cached(g) ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) |
-                         (g.shared ? 8 : 0);
+                         (g.shared ? 8 : 0) | (O > 2 ? 16 : 0);
     int rc = configure_fft_kernels();
     if (rc != DASP_OK) return rc;
     float2* gs = (float2*)(ws + w.gs);
     float2* ds = (float2*)(ws + w.ds);
-    const int I = (int)g.ib, nblk = (int)(items * I), nwin = (int)(items * g.p * I);
-    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, O, 1, I, g.n, 1, nblk);
+    const int I = (int)g.ib, Q = (O + 1) / 2, nblk = (int)(items * Q * I), nwin = (int)(items * g.p * I);
+    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, O, Q, I, g.n, 1, nblk);
     DASP_LAUNCH_OK("bus_fft_kernel");
     if ((rc = launch_bus_mac<BUS_DX>(g, S, O, xs, hs, h_stride, gs, ds, items, st)) != DASP_OK) return rc;
     bus_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx, item0,
@@ -4211,11 +4445,24 @@ struct BusOp {
   }
 };
 
-// the bus's argument checks, filling its geometry
-int make_bus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t S, int64_t O, int64_t chunk, ConvGeom& g) {
-  DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "conv bus: 1 to %d inputs are supported, got %lld",
+// multichannel_convolution: the bus with up to DASP_CONV_MC_MAX_OUTPUTS outputs, and its own messages
+struct McOp : BusOp {
+  static constexpr const char* kFwd = "conv mc fwd";
+  static constexpr const char* kBwd = "conv mc bwd";
+};
+
+// the argument checks of the bus (max_out 2, dasp_conv_bus_*) and of multichannel_convolution (max_out
+// DASP_CONV_MC_MAX_OUTPUTS, dasp_conv_mc_*), filling their geometry.  Q = ceil(O / 2) output and gradient spectra per
+// block: the Q - 1 beyond the first are g.ex
+int make_bus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t S, int64_t O, int max_out, int64_t chunk,
+                  ConvGeom& g) {
+  const char* what = max_out == 2 ? "conv bus" : "conv mc";
+  DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "%s: 1 to %d inputs are supported, got %lld", what,
                DASP_CONV_BUS_MAX_INPUTS, (long long)S);
-  DASP_REQUIRE(O == 1 || O == 2, "conv bus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
+  if (max_out == 2)
+    DASP_REQUIRE(O == 1 || O == 2, "conv bus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
+  else
+    DASP_REQUIRE(O >= 1 && O <= max_out, "%s: 1 to %d outputs are supported, got %lld", what, max_out, (long long)O);
   int rc = make_conv_geom(bs, n, L, chunk, g);
   if (rc != DASP_OK) return rc;
   g.shared = shared;
@@ -4223,27 +4470,44 @@ int make_bus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t S, int6
   g.sets = (int)(S * O + 1) / 2;
   g.has_mix = false;
   g.own_only = true;
+  g.ex = ((O + 1) / 2 - 1) * g.ib;
   return DASP_OK;
 }
 
-int conv_bus_fwd(bool shared, const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
-                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O,
-                 int64_t chunk_items, void* stream) {
+extern "C++" {
+template <class Op>
+int conv_bus_fwd(int max_out, bool shared, const float* x, const float* ir, float* y, void* xspec_save,
+                 void* irspec_save, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                 int64_t S, int64_t O, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
+  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, max_out, chunk_items, g);
   if (rc != DASP_OK) return rc;
-  return caller_ir_fwd(BusOp{(int)S, (int)O, (int)(S * O)}, g, x, ir, nullptr, y, xspec_save, irspec_save, workspace,
-                       workspace_bytes, stream);
+  Op op{};
+  op.S = (int)S; op.O = (int)O; op.ir_rows = (int)(S * O);
+  return caller_ir_fwd(op, g, x, ir, nullptr, y, xspec_save, irspec_save, workspace, workspace_bytes, stream);
 }
 
-int conv_bus_bwd(bool shared, const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
-                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t S, int64_t O,
-                 int64_t chunk_items, void* stream) {
+template <class Op>
+int conv_bus_bwd(int max_out, bool shared, const float* gy, const void* xspec_save, const void* irspec_save,
+                 float* gx, float* gir, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                 int64_t ir_len, int64_t S, int64_t O, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, chunk_items, g);
+  int rc = make_bus_geom(shared, bs, n, ir_len, S, O, max_out, chunk_items, g);
   if (rc != DASP_OK) return rc;
-  return caller_ir_bwd(BusOp{(int)S, (int)O, (int)(S * O)}, g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir,
-                       nullptr, workspace, workspace_bytes, stream);
+  Op op{};
+  op.S = (int)S; op.O = (int)O; op.ir_rows = (int)(S * O);
+  return caller_ir_bwd(op, g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir, nullptr, workspace,
+                       workspace_bytes, stream);
+}
+}  // extern "C++"
+
+int conv_bus_geometry(int max_out, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs,
+                      int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "%s geometry: null out", max_out == 2 ? "conv bus" : "conv mc");
+  ConvGeom g;
+  int rc = make_bus_geom(shared != 0, bs, n, ir_len, inputs, outputs, max_out, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
 }
 }  // namespace
 
@@ -4251,39 +4515,71 @@ int dasp_debug_conv_bus_last_path(int which) { return g_bus_last_path[which ? 1 
 
 int dasp_conv_bus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t shared,
                            int64_t chunk_items, dasp_conv_geom* out) {
-  DASP_REQUIRE(out != nullptr, "conv bus geometry: null out");
-  ConvGeom g;
-  int rc = make_bus_geom(shared != 0, bs, n, ir_len, inputs, outputs, chunk_items, g);
-  if (rc != DASP_OK) return rc;
-  return put_conv_geometry(g, nullptr, out);
+  return conv_bus_geometry(2, bs, n, ir_len, inputs, outputs, shared, chunk_items, out);
 }
 
 int dasp_conv_bus_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
                       int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs,
                       int64_t chunk_items, void* stream) {
-  return conv_bus_fwd(false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, inputs,
-                      outputs, chunk_items, stream);
+  return conv_bus_fwd<BusOp>(2, false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len,
+                             inputs, outputs, chunk_items, stream);
 }
 
 int dasp_conv_bus_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
                       void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs,
                       int64_t outputs, int64_t chunk_items, void* stream) {
-  return conv_bus_bwd(false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, inputs,
-                      outputs, chunk_items, stream);
+  return conv_bus_bwd<BusOp>(2, false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len,
+                             inputs, outputs, chunk_items, stream);
 }
 
 int dasp_conv_bus_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
                              void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
                              int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
-  return conv_bus_fwd(true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, inputs,
-                      outputs, chunk_items, stream);
+  return conv_bus_fwd<BusOp>(2, true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len,
+                             inputs, outputs, chunk_items, stream);
 }
 
 int dasp_conv_bus_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
                              void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
                              int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
-  return conv_bus_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, inputs,
-                      outputs, chunk_items, stream);
+  return conv_bus_bwd<BusOp>(2, true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len,
+                             inputs, outputs, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ multichannel_convolution
+// y[:, m] = sum_s x[:, s] * h[:, s, m] for 1 <= M <= DASP_CONV_MC_MAX_OUTPUTS outputs: BusOp with O = M.  M <= 2 runs
+// the bus's own products (the same bits as dasp_conv_bus_*), M >= 3 busmc_mac_kernel.
+int dasp_conv_mc_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t shared,
+                          int64_t chunk_items, dasp_conv_geom* out) {
+  return conv_bus_geometry(DASP_CONV_MC_MAX_OUTPUTS, bs, n, ir_len, inputs, outputs, shared, chunk_items, out);
+}
+
+int dasp_conv_mc_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                     int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs,
+                     int64_t chunk_items, void* stream) {
+  return conv_bus_fwd<McOp>(DASP_CONV_MC_MAX_OUTPUTS, false, x, ir, y, xspec_save, irspec_save, workspace,
+                            workspace_bytes, bs, n, ir_len, inputs, outputs, chunk_items, stream);
+}
+
+int dasp_conv_mc_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                     void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs,
+                     int64_t outputs, int64_t chunk_items, void* stream) {
+  return conv_bus_bwd<McOp>(DASP_CONV_MC_MAX_OUTPUTS, false, gy, xspec_save, irspec_save, gx, gir, workspace,
+                            workspace_bytes, bs, n, ir_len, inputs, outputs, chunk_items, stream);
+}
+
+int dasp_conv_mc_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                            void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                            int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
+  return conv_bus_fwd<McOp>(DASP_CONV_MC_MAX_OUTPUTS, true, x, ir, y, xspec_save, irspec_save, workspace,
+                            workspace_bytes, bs, n, ir_len, inputs, outputs, chunk_items, stream);
+}
+
+int dasp_conv_mc_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                            void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                            int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream) {
+  return conv_bus_bwd<McOp>(DASP_CONV_MC_MAX_OUTPUTS, true, gy, xspec_save, irspec_save, gx, gir, workspace,
+                            workspace_bytes, bs, n, ir_len, inputs, outputs, chunk_items, stream);
 }
 
 // ------------------------------------------------------------------ time_varying_convolution_reverberation

@@ -37,6 +37,7 @@ __all__ = [
     "noise_shaped_reverberation",
     "convolution_reverberation",
     "convolution_bus",
+    "multichannel_convolution",
     "time_varying_convolution_reverberation",
     "time_varying_convolution_bus",
     "noise_shaped_impulse_response",
@@ -1405,39 +1406,41 @@ def convolution_reverberation(x: torch.Tensor, sample_rate: float, impulse_respo
 # --------------------------------------------------------------------------------------
 
 CONV_BUS_MAX_INPUTS = 32      # DASP_CONV_BUS_MAX_INPUTS in include/dasp_b200.h
+CONV_MC_MAX_OUTPUTS = 32      # DASP_CONV_MC_MAX_OUTPUTS in include/dasp_b200.h
 
 
 class _ConvBusFn(torch.autograd.Function):
-    """x (bs, S, n), ir (bs | 1, S, O, L) -> y (bs, O, n).  n % 4 == 0 and 16-byte aligned rows (convolution_bus pads).
-    An ir of batch 1 with bs > 1 runs the dasp_conv_bus_shared_* entry points; its gradient is the sum over the items."""
+    """x (bs, S, n), ir (bs | 1, S, O, L) -> y (bs, O, n).  n % 4 == 0 and 16-byte aligned rows (_bus_inputs pads).
+    entry "conv_bus" runs the bus (O <= 2), "conv_mc" multichannel_convolution (O <= CONV_MC_MAX_OUTPUTS).  An ir of
+    batch 1 with bs > 1 runs the dasp_<entry>_shared_* entry points; its gradient is the sum over the items."""
 
     @staticmethod
-    def forward(ctx, x, ir, chunk):
+    def forward(ctx, x, ir, chunk, entry="conv_bus"):
         lib = _abi.lib()
         bs, S, n = x.shape
         ir_bs, _, O, ir_len = ir.shape
         shared = ir_bs == 1 and bs > 1
-        kind = "conv_bus_shared" if shared else "conv_bus"
+        kind = f"{entry}_shared" if shared else entry
         dev = x.device
         y = torch.empty(bs, O, n, dtype=torch.float32, device=dev)
         need_bwd = any(ctx.needs_input_grad[:2])
         with torch.cuda.device(dev):
-            ws, (xspec, irspec), bwd_bytes = _geom_buffers(_abi.ConvGeom(), "dasp_conv_bus_geometry",
+            ws, (xspec, irspec), bwd_bytes = _geom_buffers(_abi.ConvGeom(), f"dasp_{entry}_geometry",
                                                            (bs, n, ir_len, S, O, int(shared), chunk), dev, need_bwd)
-            with _timed("conv_bus_fwd", dev):
+            with _timed(f"{entry}_fwd", dev):
                 check(getattr(lib, f"dasp_{kind}_fwd")(ptr(x), ptr(ir), ptr(y), ptr(xspec), ptr(irspec), ptr(ws),
                                                        ws.numel(), bs, n, ir_len, S, O, chunk, stream_ptr(dev)),
                       f"dasp_{kind}_fwd")
         if need_bwd:
             ctx.save_for_backward(xspec, irspec)
-        ctx.cfg = (kind, bs, S, O, n, ir.shape, chunk, bwd_bytes)
+        ctx.cfg = (entry, kind, bs, S, O, n, ir.shape, chunk, bwd_bytes)
         return y
 
     @staticmethod
     def backward(ctx, gy):
         lib = _abi.lib()
         xspec, irspec = ctx.saved_tensors
-        kind, bs, S, O, n, ir_shape, chunk, bwd_bytes = ctx.cfg
+        entry, kind, bs, S, O, n, ir_shape, chunk, bwd_bytes = ctx.cfg
         dev = gy.device
         gy = gy.contiguous()
         if gy.data_ptr() % 16:
@@ -1446,11 +1449,44 @@ class _ConvBusFn(torch.autograd.Function):
         # a fixed IR (measured rooms, a fixed downmix) skips every dL/dIR kernel
         gir = torch.empty(ir_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
         ws = _ws_bytes(bwd_bytes, dev)
-        with torch.cuda.device(dev), _timed("conv_bus_bwd", dev):
+        with torch.cuda.device(dev), _timed(f"{entry}_bwd", dev):
             check(getattr(lib, f"dasp_{kind}_bwd")(ptr(gy), ptr(xspec), ptr(irspec), ptr(gx), ptr(gir), ptr(ws),
                                                    ws.numel(), bs, n, ir_shape[3], S, O, chunk, stream_ptr(dev)),
                   f"dasp_{kind}_bwd")
-        return gx, gir, None
+        return gx, gir, None, None
+
+
+def _bus_inputs(x, impulse_response, name: str, max_outputs: int):
+    """The checks and the padding of convolution_bus (max_outputs 2) and multichannel_convolution: x (bs, S, n) and
+    the IR (bs | 1, S, O, L) as fp32, rows padded to n % 4 == 0 and 16-byte aligned, the taps that would reach only
+    the padding dropped.  `name` heads the input-count message.  Returns (x, ir, n, x's dtype)."""
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
+    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 4:
+        raise ValueError("impulse_response must be a tensor of shape (batch, inputs, outputs, taps)")
+    bs, S, n = x.shape
+    if not 1 <= S <= CONV_BUS_MAX_INPUTS:
+        raise ValueError(f"{name}: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, got {S}")
+    _, ir_s, O, L = impulse_response.shape
+    if ir_s != S:
+        raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
+    if max_outputs == 2 and O not in (1, 2):
+        raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
+    if not 1 <= O <= max_outputs:
+        raise ValueError(f"impulse_response: 1 to {max_outputs} output channels are supported, got {O}")
+    _caller_ir_shape(impulse_response, bs)
+    if n < 1:
+        raise ValueError("x needs at least one sample")
+    xf, dt = _audio(x)
+    irf = _caller_ir(impulse_response, xf, 4)
+    n4 = (n + 3) // 4 * 4
+    if n4 != n:
+        xf = torch.nn.functional.pad(xf, (0, n4 - n))
+        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
+            irf = irf[..., :n].contiguous()
+    elif xf.data_ptr() % 16:
+        xf = xf.clone()
+    return xf, irf, n, dt
 
 
 def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor):
@@ -1490,32 +1526,50 @@ def convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch
     multiple of 4 are zero-padded to one (the transforms bulk-copy 16-byte rows); a padding sample reaches no output
     sample below ``n``.
     """
-    if not torch.is_tensor(x) or x.dim() != 3:
-        raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
-    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 4:
-        raise ValueError("impulse_response must be a tensor of shape (batch, inputs, outputs, taps)")
-    bs, S, n = x.shape
-    if not 1 <= S <= CONV_BUS_MAX_INPUTS:
-        raise ValueError(f"convolution_bus: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, got {S}")
-    _, ir_s, O, L = impulse_response.shape
-    if ir_s != S:
-        raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
-    if O not in (1, 2):
-        raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
-    _caller_ir_shape(impulse_response, bs)
-    if n < 1:
-        raise ValueError("x needs at least one sample")
-    xf, dt = _audio(x)
-    irf = _caller_ir(impulse_response, xf, 4)
-    n4 = (n + 3) // 4 * 4
-    if n4 != n:
-        xf = torch.nn.functional.pad(xf, (0, n4 - n))
-        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
-            irf = irf[..., :n].contiguous()
-    elif xf.data_ptr() % 16:
-        xf = xf.clone()
+    xf, irf, n, dt = _bus_inputs(x, impulse_response, "convolution_bus", 2)
     y = _ConvBusFn.apply(xf, irf, reverb_chunk_items(xf.device))
-    return (y[..., :n] if n4 != n else y).to(dt)
+    return (y[..., :n] if xf.shape[-1] != n else y).to(dt)
+
+
+def multichannel_convolution(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor):
+    """S input channels through an S x M matrix of impulse responses into M output channels::
+
+        y[:, m] = sum_s (x[:, s] * h[:, s, m])[:n]
+
+    (``*`` the causal convolution cropped to ``n``, as ``convolution_bus`` defines it; this is ``convolution_bus``
+    with up to ``CONV_MC_MAX_OUTPUTS`` output rows).  Uses: microphone-array simulation for multichannel separation,
+    enhancement, beamforming and direction-of-arrival training (S talkers or noise sources through the room impulse
+    responses of an M-microphone array), ambisonic rendering (first order is 4 channels, third order 16, fourth order
+    25) and multichannel reproduction such as 5.1 / 7.1 beds and upmixes through a room.
+
+    Args:
+        x: audio ``(bs, S, n)``, ``1 <= S <= CONV_BUS_MAX_INPUTS`` input channels (sources).
+        sample_rate: unused (kept for the common processor signature).
+        impulse_response: ``(bs, S, M, L)``, one matrix per item, or ``(1, S, M, L)``, one matrix shared by the batch;
+            ``1 <= M <= CONV_MC_MAX_OUTPUTS``, any ``L >= 1``.  Row ``(s, m)`` is the path from input ``s`` to output
+            ``m`` (microphone, ambisonic channel or speaker feed).
+
+    Returns ``(bs, M, n)`` in x's dtype, computed in fp32.  There is no dry/wet mix, as in ``convolution_bus``.
+
+    Identities (held to fp32 rounding):
+
+    1. ``M <= 2``: ``convolution_bus(x, sr, h)``, bit for bit.
+    2. Any ``M``: the concatenation over the output pairs ``q`` of ``convolution_bus(x, sr, h[:, :, 2q:2q+2])``.
+    3. Any ``S``: the sum over ``s`` of ``multichannel_convolution(x[:, s:s+1], sr, h[:, s:s+1])``.
+
+    Gradients flow to ``x`` (every input) and to every IR row; taps at or beyond ``n`` reach no output and get exactly
+    0.  The gradient of a shared ``(1, S, M, L)`` matrix has that shape and is the sum over the items, accumulated in
+    fp64 in item order, so it does not depend on ``REVERB_CHUNK_ITEMS``.  When the IR does not require a gradient, the
+    backward skips all dL/dIR work.  The convolution is ``convolution_bus``'s: every input's windows are transformed
+    (two inputs per transform) and kept for the backward once for all M outputs, the S M IR rows go two per partition
+    transform, and the outputs, their gradients and dL/dx are transformed two rows per transform.  The ceil(M / 2)
+    ``convolution_bus`` calls of identity 2 would transform and keep every window, and transform dL/dx, once per call.
+    Rows whose length is not a multiple of 4 are zero-padded to one; a padding sample reaches no output sample below
+    ``n``.
+    """
+    xf, irf, n, dt = _bus_inputs(x, impulse_response, "multichannel_convolution", CONV_MC_MAX_OUTPUTS)
+    y = _ConvBusFn.apply(xf, irf, reverb_chunk_items(xf.device), "conv_mc")
+    return (y[..., :n] if xf.shape[-1] != n else y).to(dt)
 
 
 # --------------------------------------------------------------------------------------

@@ -349,9 +349,34 @@ int dasp_conv_bus_shared_bwd(const float* gy, const void* xspec_save, const void
                              float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
                              int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t chunk_items,
                              void* stream);
-/* test hook: dispatch of the most recent bus call.  which = 0 (forward): bit 0 = own in-shared-memory FFT (always),
-   bit 1 = shared IR, bit 2 = register-cached products.  which = 1 (backward): bit 0 = own FFT (always), bit 1 =
-   register-cached products, bit 2 = dL/dIR computed, bit 3 = shared IR */
+/* ---- multichannel_convolution: S input rows through an S x M impulse-response matrix into M output rows -----------
+ * The bus with 1 <= M <= DASP_CONV_MC_MAX_OUTPUTS outputs (microphone arrays, ambisonics, multichannel beds):
+ *   y[b, m] = sum_s (x[b, s] * ir[b, s, m])[:n]
+ * The arguments, shapes, rules and rejections are dasp_conv_bus_*'s with outputs = M.  The IR rows s M + m are packed two
+ * per partition set (ceil(S M / 2) sets), the outputs and their gradients two per transform (ceil(M / 2) spectra per
+ * block), so xspec_c64 and irspec_c64 come from dasp_conv_mc_geometry, which needs no GPU.  M <= 2 gives the bits of
+ * dasp_conv_bus_*. */
+#define DASP_CONV_MC_MAX_OUTPUTS 32
+int dasp_conv_mc_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t shared,
+                          int64_t chunk_items, dasp_conv_geom* out);
+int dasp_conv_mc_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                     int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs,
+                     int64_t chunk_items, void* stream);
+int dasp_conv_mc_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                     float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                     int64_t ir_len, int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream);
+int dasp_conv_mc_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                            void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len,
+                            int64_t inputs, int64_t outputs, int64_t chunk_items, void* stream);
+int dasp_conv_mc_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                            float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
+                            int64_t n, int64_t ir_len, int64_t inputs, int64_t outputs, int64_t chunk_items,
+                            void* stream);
+
+/* test hook: dispatch of the most recent dasp_conv_bus_* or dasp_conv_mc_* call.  which = 0 (forward): bit 0 = own
+   in-shared-memory FFT (always), bit 1 = shared IR, bit 2 = register-cached products, bit 3 = M >= 3 outputs
+   (dasp_conv_mc_*).  which = 1 (backward): bit 0 = own FFT (always), bit 1 = register-cached products, bit 2 = dL/dIR
+   computed, bit 3 = shared IR, bit 4 = M >= 3 outputs */
 int dasp_debug_conv_bus_last_path(int which);
 
 /* ---- time_varying_convolution_reverberation: a trajectory of K impulse responses crossfaded along the output -------

@@ -15,7 +15,8 @@ sources and listeners) and ``time_varying_convolution_bus`` (several moving sour
 impulse responses, crossfaded and summed into a mono or stereo bus; ``crossfade="input"`` crossfades on the source side,
 so every emitted sample keeps the impulse response of its emission time) and ``multichannel_convolution`` (S sources
 through an S x M matrix of impulse responses into up to 32 output channels: microphone arrays, ambisonics, multichannel
-beds).
+beds) and ``time_varying_multichannel_convolution`` (moving sources through a trajectory of such matrices, crossfaded on
+the output or the source side: moving talkers at a microphone array, moving objects in ambisonic or 5.1 / 7.1 scenes).
 """
 from dasp_pytorch_b200 import functional  # noqa: F401
 from dasp_pytorch_b200.functional import (  # noqa: F401
@@ -44,6 +45,7 @@ from dasp_pytorch_b200.functional import (  # noqa: F401
     stereo_widener,
     time_varying_convolution_bus,
     time_varying_convolution_reverberation,
+    time_varying_multichannel_convolution,
 )
 from dasp_pytorch_b200.modules import (  # noqa: F401
     Compressor,

@@ -119,6 +119,16 @@ _SIGNATURES = {
     "dasp_tvbus_in_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_tvbus_in_shared_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_tvbus_in_shared_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_geometry": (c_int, [I64, I64, I64, I64, I64, I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
+    "dasp_tvmc_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_shared_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_shared_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_in_geometry": (c_int, [I64, I64, I64, I64, I64, I64, I64, I64, I64, ctypes.POINTER(ConvGeom)]),
+    "dasp_tvmc_in_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_in_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_in_shared_fwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
+    "dasp_tvmc_in_shared_bwd": (c_int, [P, P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I64, P]),
     "dasp_debug_tvbus_last_path": (c_int, [c_int]),
     "dasp_dynamics_tile_len": (I64, [I64, I64]),
     "dasp_dynamics_fwd": (c_int, [c_int, P, P, P, P, P, P, P, P, I64, I64, I64, c_float, c_float, I64, P]),

@@ -52,6 +52,9 @@
 // the input instead, so every sample keeps the IR sets of its emission time: zero-padded transforms of each source's
 // weighted blocks (tvbusin_fft_kernel), the products with the IR sets of each input block's interval, overlap-added on
 // the spectra (tvbusin_mac_kernel), and the crossfade of dL/dx in the epilogue of its inverse (tvbusin_ifft_kernel).
+// time_varying_multichannel_convolution (dasp_tvmc_*, dasp_tvmc_in_*) is that bus with up to 32 outputs: for M >= 3 its
+// products are tvmc_mac_kernel's / tvmcin_mac_kernel's, one slice per output pair, input pair or partition set, and
+// every transform is an existing kernel's.
 //
 // The ops whose IR the caller supplies run one host stage per direction (caller_ir_fwd / caller_ir_bwd: checks,
 // workspace, IR packing, chunk loop, zeros of the unreachable dL/dIR taps).  One IR for the whole batch
@@ -75,6 +78,7 @@
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -3293,6 +3297,303 @@ __global__ void __launch_bounds__(128) tvbusin_mac_kernel(const float2* __restri
   }
 }
 
+// ---- time_varying_multichannel_convolution: the time-varying bus with M >= 3 outputs (Q = ceil(M / 2) output pairs) --
+// The IR layout is the bus's: row r = (k S + s) M + m, two rows per partition set (NH = ceil(K S M / 2) sets).
+// Output side (tvmc_mac_kernel): the product and gradient slots of an item are tvin_block's layout with (S, P) ->
+// (M, Q), U = M nX + Q (I - nX) slots:
+//   slot i M + m (i < nX):                (Y_k,m[i], Y_k+1,m[i]); gradient FFT of [0 | (1 - a) g_m,i + i a g_m,i]
+//   slot M nX + (i - nX) Q + q (i >= nX): (Y_K-1,2q[i], Y_K-1,2q+1[i]); gradient FFT of [0 | g_2q,i + i g_2q+1,i]
+// which are the source-side window spectra of M rows: tvbusin_fft_kernel transforms the gradient into them and
+// tvbusin_ifft_kernel gives (1 - a) re + a im on a crossfaded slot, rows 2q and 2q + 1 on a later one.
+// Source side (tvmcin_mac_kernel): the windows are tvbusin_fft_kernel's (XW per item), the products and gradients one
+// spectrum per block and output pair, pair q of block i at block q I + i of the item (bus_ifft_kernel /
+// bus_fft_kernel with rows M, groups Q).
+// Both kernels run one slice of an item per blockIdx.y and the items along blockIdx.z, so the slices of an item run
+// next to each other and re-read its spectra from L2; all operands from L2, results packed two real rows per block,
+// planar, scaled by 1 / kNbA.
+//   TVM_FWD: slice q < Q:  Y_k,2q / 2q+1[i] = sum_s sum_j X_s[i - j] H_k,s,m[j] for the IR sets of block i
+//                                                                                    out: U slots
+//   TVM_DX:  slice p < P:  D_s[i] (s = 2p, 2p + 1) = sum_m sum_j Ga_m[i+j] conj(H_k,s,m[j]) + Gb_m[i+j]
+//            conj(H_k+1,s,m[j]), stored as W_s[i] = D_s[i] + (-1)^f D_s[i + 1]   out: P I blocks (bus_ifft_kernel)
+//   TVM_DIR: slice h < NH: E_r[j] of rows r = 2h, 2h + 1, each an (k, s, m):
+//            sum_{i in interval k} Ga_m[i] conj(X_s[i-j]) + sum_{i in interval k-1} Gb_m[i] conj(X_s[i-j])
+//                                                                                    out: NH J blocks
+// X: P I blocks per item; H: NH J partitions per trajectory set at item stride hstride (0: one set for the batch);
+// G: U slots per item.
+enum TvMcMac { TVM_FWD, TVM_DX, TVM_DIR };
+template <int MODE>
+__global__ void __launch_bounds__(128) tvmc_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                       int64_t hstride, const float2* __restrict__ G,
+                                                       float2* __restrict__ Out, int S, int M, int I, int J, int K,
+                                                       int nX, int Hb) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int sl = blockIdx.y;
+  const int64_t il = blockIdx.z;
+  const int P = (S + 1) / 2, Q = (M + 1) / 2, U = M * nX + Q * (I - nX), NH = (K * S * M + 1) / 2;
+  const float2* x = X + il * (int64_t)P * I * kNbA;
+  const float2* h = H + il * hstride;
+  const float2* g = G + il * (int64_t)U * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  auto pick = [&](const float2* base, int64_t slot, int odd) -> float2 {
+    float2 a, b;
+    pair(base, slot, a, b);
+    return odd ? b : a;
+  };
+  // IR rows (k, s, 2q) and (k, s, 2q + 1) at partition j, 0 past the last output; one set when the first row is even
+  auto hin = [&](int k, int s, int q, int j, float2& h0, float2& h1) {
+    const int r = (k * S + s) * M + 2 * q;
+    if (2 * q + 1 >= M) { h0 = pick(h, (int64_t)(r >> 1) * J + j, r & 1); h1 = zero; }
+    else if ((r & 1) == 0) pair(h, (int64_t)(r >> 1) * J + j, h0, h1);
+    else { h0 = pick(h, (int64_t)(r >> 1) * J + j, 1); h1 = pick(h, (int64_t)((r + 1) >> 1) * J + j, 0); }
+  };
+  // the gradient of outputs 2q, 2q + 1 at block i: IR set k(i) (ga) and k(i) + 1 (gb, 0 after the last anchor)
+  auto gin = [&](int i, int q, float2 (&ga)[2], float2 (&gb)[2]) {
+    if (i < nX) {
+      pair(g, (int64_t)i * M + 2 * q, ga[0], gb[0]);
+      if (2 * q + 1 < M) pair(g, (int64_t)i * M + 2 * q + 1, ga[1], gb[1]);
+      else ga[1] = gb[1] = zero;
+    } else {
+      pair(g, (int64_t)M * nX + (int64_t)(i - nX) * Q + q, ga[0], ga[1]);
+      gb[0] = gb[1] = zero;
+    }
+  };
+  auto emit = [&](int64_t slot, float2 a, float2 b) { bus_emit(Out, slot, f, fm, 1.0f / (float)kNbA, a, b); };
+  auto ival = [&](int i) { const int k = i / Hb; return k < K - 1 ? k : K - 1; };   // anchor interval of block i
+
+  if constexpr (MODE == TVM_FWD) {
+    const int q = sl;
+    const int64_t ob = il * (int64_t)U;
+    for (int o = 0; o < I; ++o) {
+      const int k = ival(o);
+      const bool cross = o < nX;
+      float2 y0 = zero, y1 = zero, z0 = zero, z1 = zero;    // IR set k: outputs 2q, 2q + 1; IR set k + 1: the same
+      for (int p = 0; p < P; ++p) {
+        const int nc = 2 * p + 1 < S ? 2 : 1;
+        for (int j = 0; j <= o && j < J; ++j) {
+          float2 xv[2], h0, h1;
+          pair(x, (int64_t)p * I + o - j, xv[0], xv[1]);
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            if (c >= nc) break;
+            hin(k, 2 * p + c, q, j, h0, h1);
+            cfma(y0, xv[c], h0);
+            cfma(y1, xv[c], h1);
+            if (cross) {
+              hin(k + 1, 2 * p + c, q, j, h0, h1);
+              cfma(z0, xv[c], h0);
+              cfma(z1, xv[c], h1);
+            }
+          }
+        }
+      }
+      if (cross) {
+        emit(ob + (int64_t)o * M + 2 * q, y0, z0);
+        if (2 * q + 1 < M) emit(ob + (int64_t)o * M + 2 * q + 1, y1, z1);
+      } else {
+        emit(ob + (int64_t)M * nX + (int64_t)(o - nX) * Q + q, y0, y1);
+      }
+    }
+  } else if constexpr (MODE == TVM_DX) {
+    const int p = sl;
+    const int nc = 2 * p + 1 < S ? 2 : 1;
+    const float sgn = (f & 1) ? -1.f : 1.f;
+    const int64_t ob = (il * P + p) * (int64_t)I;
+    float2 next[2] = {zero, zero};                 // D[m + 1]
+    for (int m = I - 1; m >= 0; --m) {
+      float2 d[2] = {zero, zero};                  // D_2p+c[m] (d[1] stays 0 for an odd last source)
+      for (int j = 0; j < J && m + j < I; ++j) {
+        const int i = m + j, k = ival(i);
+        for (int q = 0; q < Q; ++q) {
+          float2 ga[2], gb[2], h0, h1;
+          gin(i, q, ga, gb);
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            if (c >= nc) break;
+            hin(k, 2 * p + c, q, j, h0, h1);
+            cfma_conj(d[c], ga[0], h0);
+            cfma_conj(d[c], ga[1], h1);
+            if (i < nX) {
+              hin(k + 1, 2 * p + c, q, j, h0, h1);
+              cfma_conj(d[c], gb[0], h0);
+              cfma_conj(d[c], gb[1], h1);
+            }
+          }
+        }
+      }
+      emit(ob + m, bus_axpy(sgn, d[0], next[0]), bus_axpy(sgn, d[1], next[1]));
+      next[0] = d[0]; next[1] = d[1];
+    }
+  } else {
+    static_assert(MODE == TVM_DIR, "tvmc_mac_kernel: unknown mode");
+    // E_r[j] of row r = (k S + s) M + m over both intervals that carry IR set k
+    auto ecorr = [&](int r, int j) -> float2 {
+      const int k = r / (S * M), sm = r - k * S * M, s = sm / M, m = sm - s * M;
+      float2 e = zero;
+      for (int part = 0; part < 2; ++part) {       // 0: Ga (G) of interval k, 1: Gb of interval k - 1
+        const int kk = k - part;
+        if (kk < 0) continue;
+        const int lo = kk * Hb, hi = kk == K - 1 ? I : ((kk + 1) * Hb < I ? (kk + 1) * Hb : I);
+        for (int i = lo > j ? lo : j; i < hi; ++i) {
+          const float2 gv = i < nX ? pick(g, (int64_t)i * M + m, part)
+                                   : pick(g, (int64_t)M * nX + (int64_t)(i - nX) * Q + (m >> 1), m & 1);
+          cfma_conj(e, gv, pick(x, (int64_t)(s >> 1) * I + i - j, s & 1));
+        }
+      }
+      return e;
+    };
+    const int r0 = 2 * sl;
+    const bool two = r0 + 1 < K * S * M;
+    const int64_t ob = (il * NH + sl) * (int64_t)J;
+    for (int j = 0; j < J; ++j) emit(ob + j, ecorr(r0, j), two ? ecorr(r0 + 1, j) : zero);
+  }
+}
+
+// The source-side products with M >= 3 outputs, operands as tvbusin_mac_kernel's (Za_s / Zb_s / Z_s: the window
+// slots of source s; G_m: FFT of [0 | g_m block], rows 2q, 2q + 1 in block q I + i of the item), one slice per
+// blockIdx.y as tvmc_mac_kernel:
+//   TVJ_FOLD: slice q < Q:  folds G of pair q in place, G[i] <- Gt[i] = G[i] + (-1)^f G[i + 1] (tvbusin_mac_kernel's
+//                           TVI_DX prologue; each slice and thread owns its blocks and bins)
+//   TVJ_FWD:  slice q < Q:  Y_m[i] (m = 2q, 2q + 1) = sum_s sum_j Za_s[i-j] H_k(i-j),s,m[j] + Zb_s[i-j]
+//                           H_k(i-j)+1,s,m[j], stored as W_m[i] = Y_m[i] + (-1)^f Y_m[i - 1]   out: Q I blocks
+//   TVJ_DX:   slice p < P:  Da_s[i] = sum_m sum_j Gt_m[i+j] conj(H_k(i),s,m[j]), Db_s[i] with IR set k(i) + 1
+//                           (i < nX)                                      out: XW slots (tvbusin_ifft_kernel's)
+//   TVJ_DIR:  slice h < NH: E_r[j] of rows r = 2h, 2h + 1, each an (k, s, m): sum_{i in interval k} Gt_m[i+j]
+//                           conj(Za_s[i]) + sum_{i in interval k-1} Gt_m[i+j] conj(Zb_s[i])     out: NH J blocks
+// X: XW slots per item; H: NH J partitions per trajectory set at item stride hstride; G: Q I blocks per item.
+enum TvMcInMac { TVJ_FOLD, TVJ_FWD, TVJ_DX, TVJ_DIR };
+template <int MODE>
+__global__ void __launch_bounds__(128) tvmcin_mac_kernel(const float2* __restrict__ X, const float2* __restrict__ H,
+                                                         int64_t hstride, float2* G, float2* __restrict__ Out, int S,
+                                                         int M, int I, int J, int K, int nX, int Hb) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > kNbA / 2) return;
+  const int fm = (kNbA - f) & (kNbA - 1);
+  const int sl = blockIdx.y;
+  const int64_t il = blockIdx.z;
+  const int P = (S + 1) / 2, Q = (M + 1) / 2, XW = nX * S + (I - nX) * P, NH = (K * S * M + 1) / 2;
+  const float2* x = X + il * (int64_t)XW * kNbA;
+  const float2* h = H + il * hstride;
+  float2* g = G + il * (int64_t)Q * I * kNbA;
+  const float2 zero = make_float2(0.f, 0.f);
+  auto pair = [&](const float2* base, int64_t slot, float2& a, float2& b) {
+    untangle(base[slot * kNbA + f], base[slot * kNbA + fm], a, b);
+  };
+  auto pick = [&](const float2* base, int64_t slot, int odd) -> float2 {
+    float2 a, b;
+    pair(base, slot, a, b);
+    return odd ? b : a;
+  };
+  // source s of block i: (Za, Zb), or (Z, 0) after the last anchor
+  auto xin = [&](int i, int s, float2& za, float2& zb) {
+    if (i < nX) { pair(x, (int64_t)i * S + s, za, zb); return; }
+    za = pick(x, (int64_t)nX * S + (int64_t)(i - nX) * P + (s >> 1), s & 1);
+    zb = zero;
+  };
+  auto hin = [&](int k, int s, int q, int j, float2& h0, float2& h1) {   // as tvmc_mac_kernel's
+    const int r = (k * S + s) * M + 2 * q;
+    if (2 * q + 1 >= M) { h0 = pick(h, (int64_t)(r >> 1) * J + j, r & 1); h1 = zero; }
+    else if ((r & 1) == 0) pair(h, (int64_t)(r >> 1) * J + j, h0, h1);
+    else { h0 = pick(h, (int64_t)(r >> 1) * J + j, 1); h1 = pick(h, (int64_t)((r + 1) >> 1) * J + j, 0); }
+  };
+  auto emit = [&](int64_t slot, float2 a, float2 b) { bus_emit(Out, slot, f, fm, 1.0f / (float)kNbA, a, b); };
+  const float sgn = (f & 1) ? -1.f : 1.f;          // (-1)^f, and (-1)^fm: kNbA is even
+  auto ival = [&](int i) { const int k = i / Hb; return k < K - 1 ? k : K - 1; };   // anchor interval of block i
+
+  if constexpr (MODE == TVJ_FOLD) {
+    float2* gq = g + (int64_t)sl * I * kNbA;
+    for (int q = 0; q + 1 < I; ++q) {
+      float2* a = gq + (int64_t)q * kNbA;
+      const float2* b = a + kNbA;
+      a[f] = bus_axpy(sgn, a[f], b[f]);
+      if (fm != f) a[fm] = bus_axpy(sgn, a[fm], b[fm]);
+    }
+  } else if constexpr (MODE == TVJ_FWD) {
+    const int q = sl;
+    const int64_t ob = (il * Q + q) * (int64_t)I;
+    float2 p0 = zero, p1 = zero;                   // Y_2q[m - 1], Y_2q+1[m - 1]
+    for (int m = 0; m < I; ++m) {
+      float2 y0 = zero, y1 = zero;
+      for (int j = 0; j <= m && j < J; ++j) {
+        const int i = m - j, k = ival(i);
+        for (int s = 0; s < S; ++s) {
+          float2 za, zb, h0, h1;
+          xin(i, s, za, zb);
+          hin(k, s, q, j, h0, h1);
+          cfma(y0, za, h0);
+          cfma(y1, za, h1);
+          if (i < nX) {
+            hin(k + 1, s, q, j, h0, h1);
+            cfma(y0, zb, h0);
+            cfma(y1, zb, h1);
+          }
+        }
+      }
+      emit(ob + m, bus_axpy(sgn, y0, p0), bus_axpy(sgn, y1, p1));
+      p0 = y0; p1 = y1;
+    }
+  } else if constexpr (MODE == TVJ_DX) {
+    const int p = sl;
+    const int nc = 2 * p + 1 < S ? 2 : 1;
+    const int64_t ob = il * (int64_t)XW;
+    for (int i = 0; i < I; ++i) {
+      const int k = ival(i);
+      const bool cross = i < nX;
+      float2 da[2] = {zero, zero}, db[2] = {zero, zero};
+      for (int j = 0; j < J && i + j < I; ++j) {
+        for (int q = 0; q < Q; ++q) {
+          float2 g0, g1, h0, h1;
+          pair(g, (int64_t)q * I + i + j, g0, g1);
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            if (c >= nc) break;
+            hin(k, 2 * p + c, q, j, h0, h1);
+            cfma_conj(da[c], g0, h0);
+            cfma_conj(da[c], g1, h1);
+            if (cross) {
+              hin(k + 1, 2 * p + c, q, j, h0, h1);
+              cfma_conj(db[c], g0, h0);
+              cfma_conj(db[c], g1, h1);
+            }
+          }
+        }
+      }
+      if (cross) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) if (c < nc) emit(ob + (int64_t)i * S + 2 * p + c, da[c], db[c]);
+      } else {
+        emit(ob + (int64_t)nX * S + (int64_t)(i - nX) * P + p, da[0], da[1]);
+      }
+    }
+  } else {
+    static_assert(MODE == TVJ_DIR, "tvmcin_mac_kernel: unknown mode");
+    // E_r[j] of row r = (k S + s) M + m over both intervals that carry IR set k
+    auto ecorr = [&](int r, int j) -> float2 {
+      const int k = r / (S * M), sm = r - k * S * M, s = sm / M, m = sm - s * M;
+      float2 e = zero;
+      for (int part = 0; part < 2; ++part) {       // 0: Za (Z) of interval k, 1: Zb of interval k - 1
+        const int kk = k - part;
+        if (kk < 0) continue;
+        const int lo = kk * Hb, hi = kk == K - 1 ? I : ((kk + 1) * Hb < I ? (kk + 1) * Hb : I);
+        for (int i = lo; i < hi && i + j < I; ++i) {
+          float2 za, zb;
+          xin(i, s, za, zb);
+          cfma_conj(e, pick(g, (int64_t)(m >> 1) * I + i + j, m & 1), part ? zb : za);
+        }
+      }
+      return e;
+    };
+    const int r0 = 2 * sl;
+    const bool two = r0 + 1 < K * S * M;
+    const int64_t ob = (il * NH + sl) * (int64_t)J;
+    for (int j = 0; j < J; ++j) emit(ob + j, ecorr(r0, j), two ? ecorr(r0 + 1, j) : zero);
+  }
+}
+
 // Device-resident band spectra H_k, built once per (device, taps, sr, grid).  half (the spectral synthesis): the half
 // spectrum of the taps on its n1-point grid, 12 x (n1/2+1) complex, scaled sqrt(n1/2)/n1 -- the 1/n1 of the inverse
 // transform and the sqrt(n1/2) of the bins' complex Gaussians (Z ~ CN(0, n1)) folded in.  Otherwise the full spectrum on
@@ -4845,25 +5146,34 @@ struct TvBusOp {
   }
 };
 
-// the argument checks of dasp_tvbus_*, filling the geometry
+// the argument checks of dasp_tvbus_* (max_out 2) and of time_varying_multichannel_convolution (max_out
+// DASP_CONV_MC_MAX_OUTPUTS, dasp_tvmc_*), filling the geometry of the output-side crossfade: U = O nX + Q (I - nX)
+// product / gradient slots per item (Q = ceil(O / 2)), the U - I beyond the first I in g.ex.  That is I + nX for a
+// stereo bus and I for a mono bus, which packs both IR sets of a block into one slot.
 int make_tvbus_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t K, int64_t S, int64_t O, int64_t hop,
-                    int64_t chunk, ConvGeom& g) {
-  DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "tvbus: 1 to %d inputs are supported, got %lld",
+                    int max_out, int64_t chunk, ConvGeom& g) {
+  const char* what = max_out == 2 ? "tvbus" : "tvmc";
+  DASP_REQUIRE(S >= 1 && S <= DASP_CONV_BUS_MAX_INPUTS, "%s: 1 to %d inputs are supported, got %lld", what,
                DASP_CONV_BUS_MAX_INPUTS, (long long)S);
-  DASP_REQUIRE(O == 1 || O == 2, "tvbus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
-  DASP_REQUIRE(K >= 1, "tvbus: K >= 1 impulse-response sets are needed, got %lld", (long long)K);
-  DASP_REQUIRE(hop > 0 && hop % kB == 0, "tvbus: hop must be a positive multiple of %d, got %lld", kB, (long long)hop);
+  if (max_out == 2)
+    DASP_REQUIRE(O == 1 || O == 2, "tvbus: a mono (1) or stereo (2) bus, got %lld outputs", (long long)O);
+  else
+    DASP_REQUIRE(O >= 1 && O <= max_out, "%s: 1 to %d outputs are supported, got %lld", what, max_out, (long long)O);
+  DASP_REQUIRE(K >= 1, "%s: K >= 1 impulse-response sets are needed, got %lld", what, (long long)K);
+  DASP_REQUIRE(hop > 0 && hop % kB == 0, "%s: hop must be a positive multiple of %d, got %lld", what, kB,
+               (long long)hop);
   int rc = make_conv_geom(bs, n, L, chunk, g);
   if (rc != DASP_OK) return rc;
-  DASP_REQUIRE(K - 1 <= (n - 1) / hop, "tvbus: anchor %lld at (K - 1) hop is at or after the end of x (n=%lld)",
+  DASP_REQUIRE(K - 1 <= (n - 1) / hop, "%s: anchor %lld at (K - 1) hop is at or after the end of x (n=%lld)", what,
                (long long)(K - 1), (long long)n);
   const int64_t sets = (K * S * O + 1) / 2;
-  DASP_REQUIRE(sets <= 65535, "tvbus: at most 65535 partition sets (K S O / 2) per trajectory set, got %lld",
+  DASP_REQUIRE(sets <= 65535, "%s: at most 65535 partition sets (K S O / 2) per trajectory set, got %lld", what,
                (long long)sets);
   g.shared = shared;
   g.p = (int)(S + 1) / 2;
   g.sets = (int)sets;
-  g.ex = O == 2 ? (K - 1) * (hop / kB) : 0;        // a mono bus packs both IR sets of a block into one slot
+  const int64_t nX = (K - 1) * (hop / kB);
+  g.ex = O * nX + (O + 1) / 2 * (g.ib - nX) - g.ib;
   g.has_mix = false;
   g.own_only = true;
   return DASP_OK;
@@ -4876,7 +5186,7 @@ int tvbus_fwd(bool shared, const float* x, const float* ir, float* y, void* xspe
               void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
               int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_tvbus_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  int rc = make_tvbus_geom(shared, bs, n, ir_len, K, S, O, hop, 2, chunk_items, g);
   if (rc != DASP_OK) return rc;
   return caller_ir_fwd(tvbus_op(K, S, O, hop), g, x, ir, nullptr, y, xspec_save, irspec_save, workspace,
                        workspace_bytes, stream);
@@ -4886,7 +5196,7 @@ int tvbus_bwd(bool shared, const float* gy, const void* xspec_save, const void* 
               void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
               int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_tvbus_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  int rc = make_tvbus_geom(shared, bs, n, ir_len, K, S, O, hop, 2, chunk_items, g);
   if (rc != DASP_OK) return rc;
   return caller_ir_bwd(tvbus_op(K, S, O, hop), g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir, nullptr,
                        workspace, workspace_bytes, stream);
@@ -4899,7 +5209,7 @@ int dasp_tvbus_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_
                         int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
   DASP_REQUIRE(out != nullptr, "tvbus geometry: null out");
   ConvGeom g;
-  int rc = make_tvbus_geom(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, chunk_items, g);
+  int rc = make_tvbus_geom(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, 2, chunk_items, g);
   if (rc != DASP_OK) return rc;
   return put_conv_geometry(g, nullptr, out);
 }
@@ -5011,14 +5321,15 @@ struct TvBusInOp {
   }
 };
 
-// dasp_tvbus_*'s argument checks; the source-side windows: S per crossfaded block, ceil(S / 2) per later block, and one
-// product and gradient spectrum per block
+// make_tvbus_geom's argument checks; the source-side windows: S per crossfaded block, ceil(S / 2) per later block, and
+// one product and gradient spectrum per block and output pair (Q = ceil(O / 2) per block, the Q - 1 beyond the first
+// in g.ex)
 int make_tvbusin_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t K, int64_t S, int64_t O, int64_t hop,
-                      int64_t chunk, ConvGeom& g) {
-  int rc = make_tvbus_geom(shared, bs, n, L, K, S, O, hop, chunk, g);
+                      int max_out, int64_t chunk, ConvGeom& g) {
+  int rc = make_tvbus_geom(shared, bs, n, L, K, S, O, hop, max_out, chunk, g);
   if (rc != DASP_OK) return rc;
   const int64_t nX = (K - 1) * (hop / kB);
-  g.ex = 0;
+  g.ex = ((O + 1) / 2 - 1) * g.ib;
   g.xw = nX * S + (g.ib - nX) * g.p;
   return DASP_OK;
 }
@@ -5030,7 +5341,7 @@ int tvbusin_fwd(bool shared, const float* x, const float* ir, float* y, void* xs
                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
                 int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_tvbusin_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  int rc = make_tvbusin_geom(shared, bs, n, ir_len, K, S, O, hop, 2, chunk_items, g);
   if (rc != DASP_OK) return rc;
   return caller_ir_fwd(tvbusin_op(K, S, O, hop), g, x, ir, nullptr, y, xspec_save, irspec_save, workspace,
                        workspace_bytes, stream);
@@ -5040,7 +5351,7 @@ int tvbusin_bwd(bool shared, const float* gy, const void* xspec_save, const void
                 void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
                 int64_t O, int64_t hop, int64_t chunk_items, void* stream) {
   ConvGeom g;
-  int rc = make_tvbusin_geom(shared, bs, n, ir_len, K, S, O, hop, chunk_items, g);
+  int rc = make_tvbusin_geom(shared, bs, n, ir_len, K, S, O, hop, 2, chunk_items, g);
   if (rc != DASP_OK) return rc;
   return caller_ir_bwd(tvbusin_op(K, S, O, hop), g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir, nullptr,
                        workspace, workspace_bytes, stream);
@@ -5051,7 +5362,7 @@ int dasp_tvbus_in_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int
                            int64_t hop, int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
   DASP_REQUIRE(out != nullptr, "tvbus in geometry: null out");
   ConvGeom g;
-  int rc = make_tvbusin_geom(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, chunk_items, g);
+  int rc = make_tvbusin_geom(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, 2, chunk_items, g);
   if (rc != DASP_OK) return rc;
   return put_conv_geometry(g, nullptr, out);
 }
@@ -5084,6 +5395,245 @@ int dasp_tvbus_in_shared_bwd(const float* gy, const void* xspec_save, const void
                              void* stream) {
   return tvbusin_bwd(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K, inputs,
                      outputs, hop, chunk_items, stream);
+}
+
+// ------------------------------------------------------------------ time_varying_multichannel_convolution
+// The time-varying bus with 1 <= M <= DASP_CONV_MC_MAX_OUTPUTS outputs, both crossfades.  M <= 2 runs TvBusOp /
+// TvBusInOp unchanged (the bits of dasp_tvbus_* / dasp_tvbus_in_*).  M >= 3, output side: the bus's windows, the
+// products of tvmc_mac_kernel in U = M nX + Q (I - nX) slots, whose inverse (tvbusin_ifft_kernel with M rows) crossfades
+// each output row of a crossfaded block, and whose gradient slots are tvbusin_fft_kernel's transforms of the M gradient
+// rows; dL/dx through bus_ifft_kernel.  Source side: tvbusin_fft_kernel's windows, the products of tvmcin_mac_kernel in
+// Q I blocks (inverse bus_ifft_kernel, gradient bus_fft_kernel, rows M, groups Q), dL/dx through tvbusin_ifft_kernel.
+// The IR packing, partition transforms, shared-gradient sum and dL/dIR taps are the tv bus's.
+namespace {
+// the products' grid: `slices` slices (output pairs, input pairs or partition sets) of each item
+dim3 tvmc_grid(int slices, int64_t items) {
+  return dim3((kNbA / 2 + 1 + 127) / 128, (unsigned)slices, (unsigned)items);
+}
+
+struct TvMcOp : TvBusOp {
+  static constexpr const char* kFwd = "tvmc fwd";
+  static constexpr const char* kBwd = "tvmc bwd";
+  int fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, const float* mix,
+                float2* xs, float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    if (O <= 2) return TvBusOp::fwd_chunk(g, pl, own, tw, x, mix, xs, hs, h_stride, y, ws, w, item0, items, st);
+    // dasp_tvbus_*'s bits, and bit 4: M >= 3 outputs
+    g_tvbus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (K > 1 ? 4 : 0) | 16;
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    if (h_stride != 0 && (rc = ir_partition_spectra(g, tw, hs, items, st)) != DASP_OK) return rc;
+    float2* ys = (float2*)(ws + w.ys);
+    const int I = (int)g.ib, J = (int)g.jb, nwin = (int)(items * g.p * I), nout = (int)(items * slots(g));
+    const int64_t hop = (int64_t)Hb * kB;
+    bus_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, S, g.p, I, g.n, 0, nwin);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    tvmc_mac_kernel<TVM_FWD><<<tvmc_grid((O + 1) / 2, items), 128, 0, st>>>(xs, hs, h_stride, nullptr, ys, S,
+                                                                                     O, I, J, K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmc_mac_kernel");
+    tvbusin_ifft_kernel<<<runs(nout), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y,
+                                                                          item0, O, I, nx(), Hb, hop, g.n, nout);
+    DASP_LAUNCH_OK("tvbusin_ifft_kernel");
+    return DASP_OK;
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const float* tw, const float* gy,
+                const float* x, const float* mix, const float2* xs, const float2* hs, int64_t h_stride, float* gx,
+                unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    if (O <= 2)
+      return TvBusOp::bwd_chunk(g, pl, own, e, tw, gy, x, mix, xs, hs, h_stride, gx, ws, w, item0, items, st);
+    // dasp_tvbus_*'s bits, and bit 5: M >= 3 outputs
+    g_tvbus_last_path[1] = (own ? 1 : 0) | (K > 1 ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) | (g.shared ? 8 : 0) | 32;
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* gs = (float2*)(ws + w.gs);
+    float2* ds = (float2*)(ws + w.ds);
+    const int I = (int)g.ib, J = (int)g.jb, nwin = (int)(items * g.p * I), ng = (int)(items * slots(g));
+    const int64_t hop = (int64_t)Hb * kB;
+    tvbusin_fft_kernel<<<runs(ng), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, O, I, nx(), Hb, hop, g.n, ng);
+    DASP_LAUNCH_OK("tvbusin_fft_kernel");
+    tvmc_mac_kernel<TVM_DX><<<tvmc_grid(g.p, items), 128, 0, st>>>(xs, hs, h_stride, gs, ds, S, O, I, J,
+                                                                                  K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmc_mac_kernel");
+    bus_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx, item0,
+                                                                      S, g.p, I, g.n, g.n, 1, nwin);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    if (e == IrGrad::kNone) return DASP_OK;          // a fixed trajectory: no dL/dIR work at all
+    tvmc_mac_kernel<TVM_DIR><<<tvmc_grid(g.sets, items), 128, 0, st>>>(
+        xs, hs, 0, gs, (float2*)(ws + w.es), S, O, I, J, K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmc_mac_kernel");
+    return DASP_OK;
+  }
+};
+
+struct TvMcInOp : TvBusInOp {
+  static constexpr const char* kFwd = "tvmc in fwd";
+  static constexpr const char* kBwd = "tvmc in bwd";
+  int fwd_chunk(const ConvGeom& g, const Plans& pl, bool own, const float* tw, const float* x, const float* mix,
+                float2* xs, float2* hs, int64_t h_stride, float* y, unsigned char* ws, const FwdWs& w, int64_t item0,
+                int64_t items, cudaStream_t st) const {
+    if (O <= 2) return TvBusInOp::fwd_chunk(g, pl, own, tw, x, mix, xs, hs, h_stride, y, ws, w, item0, items, st);
+    // dasp_tvbus_in_*'s bits, and bit 4: M >= 3 outputs
+    g_tvbus_last_path[0] = (own ? 1 : 0) | (g.shared ? 2 : 0) | (K > 1 ? 4 : 0) | 8 | 16;
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    if (h_stride != 0 && (rc = ir_partition_spectra(g, tw, hs, items, st)) != DASP_OK) return rc;
+    float2* ys = (float2*)(ws + w.ys);
+    const int I = (int)g.ib, J = (int)g.jb, Q = (O + 1) / 2, nwin = (int)(items * g.xw), nblk = (int)(items * Q * I);
+    const int64_t hop = (int64_t)Hb * kB;
+    tvbusin_fft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(x, xs, tw, item0, S, I, nx(), Hb, hop, g.n,
+                                                                         nwin);
+    DASP_LAUNCH_OK("tvbusin_fft_kernel");
+    tvmcin_mac_kernel<TVJ_FWD><<<tvmc_grid(Q, items), 128, 0, st>>>(xs, hs, h_stride, nullptr, ys,
+                                                                                       S, O, I, J, K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmcin_mac_kernel");
+    bus_ifft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ys), tw, y, item0,
+                                                                      O, Q, I, g.n, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_ifft_kernel");
+    return DASP_OK;
+  }
+  int bwd_chunk(const ConvGeom& g, const Plans& pl, bool own, IrGrad e, const float* tw, const float* gy,
+                const float* x, const float* mix, const float2* xs, const float2* hs, int64_t h_stride, float* gx,
+                unsigned char* ws, const BwdWs& w, int64_t item0, int64_t items, cudaStream_t st) const {
+    if (O <= 2)
+      return TvBusInOp::bwd_chunk(g, pl, own, e, tw, gy, x, mix, xs, hs, h_stride, gx, ws, w, item0, items, st);
+    // dasp_tvbus_in_*'s bits, and bit 5: M >= 3 outputs
+    g_tvbus_last_path[1] =
+        (own ? 1 : 0) | (K > 1 ? 2 : 0) | (e != IrGrad::kNone ? 4 : 0) | (g.shared ? 8 : 0) | 16 | 32;
+    int rc = configure_fft_kernels();
+    if (rc != DASP_OK) return rc;
+    float2* gs = (float2*)(ws + w.gs);
+    float2* ds = (float2*)(ws + w.ds);
+    const int I = (int)g.ib, J = (int)g.jb, Q = (O + 1) / 2, nwin = (int)(items * g.xw), nblk = (int)(items * Q * I);
+    const int64_t hop = (int64_t)Hb * kB;
+    bus_fft_kernel<<<runs(nblk), kFusedThreads, kFftSmemBytes, st>>>(gy, gs, tw, item0, O, Q, I, g.n, 1, nblk);
+    DASP_LAUNCH_OK("bus_fft_kernel");
+    tvmcin_mac_kernel<TVJ_FOLD><<<tvmc_grid(Q, items), 128, 0, st>>>(xs, hs, h_stride, gs, nullptr,
+                                                                                         S, O, I, J, K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmcin_mac_kernel");
+    tvmcin_mac_kernel<TVJ_DX><<<tvmc_grid(g.p, items), 128, 0, st>>>(xs, hs, h_stride, gs, ds, S, O, I,
+                                                                                    J, K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmcin_mac_kernel");
+    tvbusin_ifft_kernel<<<runs(nwin), kFusedThreads, kFftSmemBytes, st>>>(reinterpret_cast<const float*>(ds), tw, gx,
+                                                                          item0, S, I, nx(), Hb, hop, g.n, nwin);
+    DASP_LAUNCH_OK("tvbusin_ifft_kernel");
+    if (e == IrGrad::kNone) return DASP_OK;          // a fixed trajectory: no dL/dIR work at all
+    tvmcin_mac_kernel<TVJ_DIR><<<tvmc_grid(g.sets, items), 128, 0, st>>>(
+        xs, hs, 0, gs, (float2*)(ws + w.es), S, O, I, J, K, nx(), Hb);
+    DASP_LAUNCH_OK("tvmcin_mac_kernel");
+    return DASP_OK;
+  }
+};
+
+extern "C++" {
+// input: the source-side crossfade (TvMcInOp), else the output side (TvMcOp)
+template <bool INPUT>
+int tvmc_geom(bool shared, int64_t bs, int64_t n, int64_t L, int64_t K, int64_t S, int64_t M, int64_t hop,
+              int64_t chunk, ConvGeom& g) {
+  return INPUT ? make_tvbusin_geom(shared, bs, n, L, K, S, M, hop, DASP_CONV_MC_MAX_OUTPUTS, chunk, g)
+               : make_tvbus_geom(shared, bs, n, L, K, S, M, hop, DASP_CONV_MC_MAX_OUTPUTS, chunk, g);
+}
+
+template <bool INPUT>
+int tvmc_fwd(bool shared, const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
+             int64_t M, int64_t hop, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = tvmc_geom<INPUT>(shared, bs, n, ir_len, K, S, M, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  typename std::conditional<INPUT, TvMcInOp, TvMcOp>::type op{};
+  op.S = (int)S; op.O = (int)M; op.K = (int)K; op.Hb = (int)(hop / kB); op.ir_rows = (int)(K * S * M);
+  return caller_ir_fwd(op, g, x, ir, nullptr, y, xspec_save, irspec_save, workspace, workspace_bytes, stream);
+}
+
+template <bool INPUT>
+int tvmc_bwd(bool shared, const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+             void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t S,
+             int64_t M, int64_t hop, int64_t chunk_items, void* stream) {
+  ConvGeom g;
+  int rc = tvmc_geom<INPUT>(shared, bs, n, ir_len, K, S, M, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  typename std::conditional<INPUT, TvMcInOp, TvMcOp>::type op{};
+  op.S = (int)S; op.O = (int)M; op.K = (int)K; op.Hb = (int)(hop / kB); op.ir_rows = (int)(K * S * M);
+  return caller_ir_bwd(op, g, gy, nullptr, nullptr, xspec_save, irspec_save, gx, gir, nullptr, workspace,
+                       workspace_bytes, stream);
+}
+
+template <bool INPUT>
+int tvmc_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                  int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
+  DASP_REQUIRE(out != nullptr, "%s geometry: null out", INPUT ? "tvmc in" : "tvmc");
+  ConvGeom g;
+  int rc = tvmc_geom<INPUT>(shared != 0, bs, n, ir_len, K, inputs, outputs, hop, chunk_items, g);
+  if (rc != DASP_OK) return rc;
+  return put_conv_geometry(g, nullptr, out);
+}
+}  // extern "C++"
+}  // namespace
+
+int dasp_tvmc_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                       int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
+  return tvmc_geometry<false>(bs, n, ir_len, K, inputs, outputs, hop, shared, chunk_items, out);
+}
+
+int dasp_tvmc_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                  int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                  int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_fwd<false>(false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K,
+                         inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                  void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                  int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_bwd<false>(false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K,
+                         inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                         void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                         int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_fwd<false>(true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K,
+                         inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                         void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                         int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_bwd<false>(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K,
+                         inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_in_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs,
+                          int64_t hop, int64_t shared, int64_t chunk_items, dasp_conv_geom* out) {
+  return tvmc_geometry<true>(bs, n, ir_len, K, inputs, outputs, hop, shared, chunk_items, out);
+}
+
+int dasp_tvmc_in_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                     int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                     int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_fwd<true>(false, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K,
+                        inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_in_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                     void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                     int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_bwd<true>(false, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K,
+                        inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_in_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                            void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                            int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_fwd<true>(true, x, ir, y, xspec_save, irspec_save, workspace, workspace_bytes, bs, n, ir_len, K,
+                        inputs, outputs, hop, chunk_items, stream);
+}
+
+int dasp_tvmc_in_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx, float* gir,
+                            void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                            int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream) {
+  return tvmc_bwd<true>(true, gy, xspec_save, irspec_save, gx, gir, workspace, workspace_bytes, bs, n, ir_len, K,
+                        inputs, outputs, hop, chunk_items, stream);
 }
 
 // ------------------------------------------------------------------ noise_shaped_impulse_response

@@ -40,6 +40,7 @@ __all__ = [
     "multichannel_convolution",
     "time_varying_convolution_reverberation",
     "time_varying_convolution_bus",
+    "time_varying_multichannel_convolution",
     "noise_shaped_impulse_response",
     "noise_shaped_impulse_response_packed",
     "parametric_eq_frequency_response",
@@ -1729,9 +1730,9 @@ def time_varying_convolution_reverberation(x: torch.Tensor, sample_rate: float, 
 
 class _TvBusFn(torch.autograd.Function):
     """x (bs, S, n), ir (bs | 1, K, S, O, L) -> y (bs, O, n).  n % 4 == 0 and 16-byte aligned rows
-    (time_varying_convolution_bus pads).  entry "tvbus" crossfades on the output side, "tvbus_in" on the source side.
-    An ir of batch 1 with bs > 1 runs the dasp_<entry>_shared_* entry points; its gradient is the sum over the
-    items."""
+    (_tv_bus_inputs pads).  entry "tvbus" crossfades on the output side, "tvbus_in" on the source side (O <= 2);
+    "tvmc" and "tvmc_in" are the same for time_varying_multichannel_convolution (O <= CONV_MC_MAX_OUTPUTS).  An ir of
+    batch 1 with bs > 1 runs the dasp_<entry>_shared_* entry points; its gradient is the sum over the items."""
 
     @staticmethod
     def forward(ctx, x, ir, hop, chunk, entry="tvbus"):
@@ -1776,6 +1777,45 @@ class _TvBusFn(torch.autograd.Function):
                                                    stream_ptr(dev)),
                   f"dasp_{kind}_bwd")
         return gx, gir, None, None, None
+
+
+def _tv_bus_inputs(x, impulse_response, hop, crossfade, name: str, max_outputs: int):
+    """The checks and the padding of time_varying_convolution_bus (max_outputs 2) and
+    time_varying_multichannel_convolution: x (bs, S, n) and the trajectory (bs | 1, K, S, O, L) as fp32, rows padded to
+    n % 4 == 0 and 16-byte aligned, the taps that would reach only the padding dropped.  `name` heads the input-count
+    message.  Returns (x, ir, n, x's dtype, hop)."""
+    if crossfade not in ("output", "input"):
+        raise ValueError(f'crossfade must be "output" or "input", got {crossfade!r}')
+    if not torch.is_tensor(x) or x.dim() != 3:
+        raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
+    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 5:
+        raise ValueError("impulse_response must be a tensor of shape (batch, K, inputs, outputs, taps)")
+    bs, S, n = x.shape
+    if not 1 <= S <= CONV_BUS_MAX_INPUTS:
+        raise ValueError(f"{name}: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, got {S}")
+    _, K, ir_s, O, L = impulse_response.shape
+    if ir_s != S:
+        raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
+    if max_outputs == 2 and O not in (1, 2):
+        raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
+    if not 1 <= O <= max_outputs:
+        raise ValueError(f"impulse_response: 1 to {max_outputs} output channels are supported, got {O}")
+    if K < 1:
+        raise ValueError("impulse_response needs at least one impulse-response set (K >= 1)")
+    _caller_ir_shape(impulse_response, bs)
+    if n < 1:
+        raise ValueError("x needs at least one sample")
+    hop = _anchor_hop(hop, K, n)
+    xf, dt = _audio(x)
+    irf = _caller_ir(impulse_response, xf, 5)
+    n4 = (n + 3) // 4 * 4
+    if n4 != n:
+        xf = torch.nn.functional.pad(xf, (0, n4 - n))
+        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
+            irf = irf[..., :n].contiguous()
+    elif xf.data_ptr() % 16:
+        xf = xf.clone()
+    return xf, irf, n, dt, hop
 
 
 def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor, hop: int, *,
@@ -1855,38 +1895,79 @@ def time_varying_convolution_bus(x: torch.Tensor, sample_rate: float, impulse_re
     inverse per source and crossfaded block (ceil(S / 2) per later block).  The segment composition above would
     transform every block of every source once per segment it falls in, and its segments' tails again.
     """
-    if crossfade not in ("output", "input"):
-        raise ValueError(f'crossfade must be "output" or "input", got {crossfade!r}')
-    if not torch.is_tensor(x) or x.dim() != 3:
-        raise ValueError("x must be a tensor of shape (batch, inputs, samples)")
-    if not torch.is_tensor(impulse_response) or impulse_response.dim() != 5:
-        raise ValueError("impulse_response must be a tensor of shape (batch, K, inputs, outputs, taps)")
-    bs, S, n = x.shape
-    if not 1 <= S <= CONV_BUS_MAX_INPUTS:
-        raise ValueError(f"time_varying_convolution_bus: 1 to {CONV_BUS_MAX_INPUTS} input channels are supported, "
-                         f"got {S}")
-    _, K, ir_s, O, L = impulse_response.shape
-    if ir_s != S:
-        raise ValueError(f"impulse_response has {ir_s} input rows, x has {S} channels")
-    if O not in (1, 2):
-        raise ValueError(f"impulse_response: a mono (1) or stereo (2) bus is supported, got {O} outputs")
-    if K < 1:
-        raise ValueError("impulse_response needs at least one impulse-response set (K >= 1)")
-    _caller_ir_shape(impulse_response, bs)
-    if n < 1:
-        raise ValueError("x needs at least one sample")
-    hop = _anchor_hop(hop, K, n)
-    xf, dt = _audio(x)
-    irf = _caller_ir(impulse_response, xf, 5)
-    n4 = (n + 3) // 4 * 4
-    if n4 != n:
-        xf = torch.nn.functional.pad(xf, (0, n4 - n))
-        if L > n:                        # taps n .. n4 - 1 would reach the padding; their gradient is exactly 0
-            irf = irf[..., :n].contiguous()
-    elif xf.data_ptr() % 16:
-        xf = xf.clone()
-    if crossfade == "output":
-        y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device))
-    else:
-        y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device), "tvbus_in")
-    return (y[..., :n] if n4 != n else y).to(dt)
+    xf, irf, n, dt, hop = _tv_bus_inputs(x, impulse_response, hop, crossfade, "time_varying_convolution_bus", 2)
+    entry = "tvbus" if crossfade == "output" else "tvbus_in"
+    y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device), entry)
+    return (y[..., :n] if xf.shape[-1] != n else y).to(dt)
+
+
+def time_varying_multichannel_convolution(x: torch.Tensor, sample_rate: float, impulse_response: torch.Tensor,
+                                          hop: int, *, crossfade: str = "output"):
+    """Moving sources through a trajectory of S x M impulse-response matrices into M output channels:
+    ``multichannel_convolution`` whose matrix changes over time, as ``time_varying_convolution_bus``'s IR sets do.
+    Matrix ``k`` of the trajectory, ``h[:, k]``, is a complete ``multichannel_convolution`` matrix, the scene at the
+    anchor time ``t_k = k * hop``.  ``crossfade`` chooses where the weights apply::
+
+        "output":  y[:, m](t) = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, m])(t)
+        "input":   y[:, m](t) = sum_k sum_s ((w_k x[:, s]) * h[:, k, s, m])(t)
+
+    with ``time_varying_convolution_bus``'s crossfade weights ``w_k`` and ``*``.  This is that op with up to
+    ``CONV_MC_MAX_OUTPUTS`` output rows.  ``"input"`` is the model of moving point sources: every emitted sample keeps
+    the matrix of its emission time over its whole tail.  ``"output"`` models a moving array or listener.  Uses: moving
+    talkers recorded by a 4- to 32-microphone array, to train direction-of-arrival tracking, multichannel separation and
+    enhancement; ambisonic scenes with moving objects (4, 16 or 25 channels); 5.1 / 7.1 renders of moving sources.
+
+    Args:
+        x: audio ``(bs, S, n)``, ``1 <= S <= CONV_BUS_MAX_INPUTS`` sources.
+        sample_rate: unused (kept for the common processor signature).
+        impulse_response: ``(bs, K, S, M, L)``, one trajectory per item, or ``(1, K, S, M, L)``, one trajectory shared
+            by the batch; ``K >= 1``, ``1 <= M <= CONV_MC_MAX_OUTPUTS``, any ``L >= 1``.  Row ``(k, s, m)`` is the
+            path from source ``s`` to output ``m`` (microphone, ambisonic channel or speaker feed) at anchor ``k``.
+        hop: the anchor spacing in samples, a positive multiple of ``CONV_PARTITION_SAMPLES`` (4096);
+            ``(K - 1) * hop < n``.  All sources share the one anchor grid.
+        crossfade: ``"output"`` (the default) or ``"input"``, keyword only.
+
+    Returns ``(bs, M, n)`` in x's dtype, computed in fp32.  There is no dry/wet mix, as in ``convolution_bus``.
+
+    Identities (held to fp32 rounding), for both crossfades:
+
+    1. ``M <= 2``: ``time_varying_convolution_bus(x, sr, h, hop, crossfade=...)``, bit for bit.
+    2. Any ``M``: the concatenation over the output pairs ``q`` of
+       ``time_varying_convolution_bus(x, sr, h[:, :, :, 2q:2q+2], hop, crossfade=...)``.
+    3. ``K = 1`` or K equal matrices: ``multichannel_convolution`` with that matrix.
+    4. Any ``S``: the sum over ``s`` of the single-source calls ``x[:, s:s+1]``, ``h[:, :, s:s+1]``.
+    5. ``"output"``: from the last anchor on (``t >= (K - 1) hop``), ``multichannel_convolution(x, sr, h[:, K - 1])``.
+    6. ``"input"``: ``sum_k multichannel_convolution(w_k x, sr, h[:, k])``, and a unit impulse at ``tau`` between
+       anchors ``k`` and ``k + 1`` (weight ``a``) gives ``(1 - a) h[:, k] + a h[:, k + 1]`` from ``tau`` on.
+
+    Gradients flow to ``x`` (every source) and to every IR row; taps at or beyond ``min(L, n)`` reach no output and
+    get exactly 0.  The gradient of a shared ``(1, K, S, M, L)`` trajectory has that shape and is the sum over the
+    items, accumulated in fp64 in item order, so it does not depend on ``REVERB_CHUNK_ITEMS``.  When the IRs do not
+    require a gradient, the backward skips all dL/dIR work.  Rows whose length is not a multiple of 4 are zero-padded
+    to one; a padding sample reaches no output sample below ``n``.
+
+    Cost, in 8192-point transforms per item, with ``I = ceil(n / 4096)`` blocks, ``nX = (K - 1) hop / 4096``
+    crossfaded blocks, ``J = ceil(min(L, n) / 4096)`` partitions, ``P = ceil(S / 2)``, ``Q = ceil(M / 2)`` and
+    ``NH = ceil(K S M / 2)``:
+
+    ============================  ===========================  ===========================
+    transforms                    ``"output"``                 ``"input"``
+    ============================  ===========================  ===========================
+    window (forward)              ``P I``                      ``S nX + P (I - nX)``
+    partition (forward)           ``NH J``                     ``NH J``
+    output inverse                ``M nX + Q (I - nX)``        ``Q I``
+    gradient (backward)           ``M nX + Q (I - nX)``        ``Q I``
+    dL/dx inverse                 ``P I``                      ``S nX + P (I - nX)``
+    dL/dIR inverse                ``NH J``                     ``NH J``
+    spectra kept for backward     ``P I + NH J``               ``S nX + P (I - nX) + NH J``
+    ============================  ===========================  ===========================
+
+    Identity 2's Q calls would take the window and dL/dx transforms, and keep the window spectra, Q times over, and
+    autograd would sum their Q copies of dL/dx.  A crossfaded block takes one output inverse per output row
+    (``"output"``: both IR sets of the row in one spectrum); ``"input"`` takes one per output pair and block.
+    """
+    xf, irf, n, dt, hop = _tv_bus_inputs(x, impulse_response, hop, crossfade, "time_varying_multichannel_convolution",
+                                         CONV_MC_MAX_OUTPUTS)
+    entry = "tvmc" if crossfade == "output" else "tvmc_in"
+    y = _TvBusFn.apply(xf, irf, hop, reverb_chunk_items(xf.device), entry)
+    return (y[..., :n] if xf.shape[-1] != n else y).to(dt)

@@ -468,10 +468,57 @@ int dasp_tvbus_in_shared_bwd(const float* gy, const void* xspec_save, const void
                              float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
                              int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
                              int64_t chunk_items, void* stream);
-/* test hook: dispatch of the most recent dasp_tvbus_* or dasp_tvbus_in_* call.  which = 0 (forward): bit 0 = own
-   in-shared-memory FFT (always), bit 1 = shared trajectory set, bit 2 = crossfaded blocks (K > 1), bit 3 = source-side
-   crossfade (dasp_tvbus_in_*).  which = 1 (backward): bit 0 = own FFT (always), bit 1 = crossfaded blocks, bit 2 =
-   dL/dIR computed, bit 3 = shared trajectory set, bit 4 = source-side crossfade */
+/* ---- time_varying_multichannel_convolution: the time-varying bus with up to 32 outputs ----------------------------
+ * dasp_tvbus_* and dasp_tvbus_in_* with 1 <= outputs (M) <= DASP_CONV_MC_MAX_OUTPUTS (moving talkers recorded by a
+ * microphone array, ambisonic scenes and multichannel beds with moving objects):
+ *   dasp_tvmc_*:     y[:, m](t) = sum_k w_k(t) sum_s (x[:, s] * h[:, k, s, m])(t)
+ *   dasp_tvmc_in_*:  y[:, m](t) = sum_k sum_s ((w_k x[:, s]) * h[:, k, s, m])(t)
+ * The arguments, shapes, rules and rejections are dasp_tvbus_*'s with outputs = M; at most 65535 partition sets
+ * ceil(K S M / 2) per trajectory set (K <= 127 at S = M = 32).  M <= 2 gives the bits of dasp_tvbus_* /
+ * dasp_tvbus_in_*.  With nX = (K - 1) hop / conv_block crossfaded blocks, I = ceil(n / conv_block) blocks,
+ * J = ceil(min(ir_len, n) / conv_block) partitions, P = ceil(S / 2) and Q = ceil(M / 2), per item:
+ *   dasp_tvmc_*:     xspec_c64 = P I 8192, product / gradient slots U = M nX + Q (I - nX)
+ *   dasp_tvmc_in_*:  xspec_c64 = (S nX + P (I - nX)) 8192, product / gradient spectra Q I
+ *   both:            irspec_c64 = ceil(K S M / 2) J 8192 (one trajectory set for the shared entry points)
+ * The geometry queries return these sizes and the workspaces and need no GPU. */
+int dasp_tvmc_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                       int64_t shared, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_tvmc_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                  int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                  int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvmc_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                  float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                  int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                  void* stream);
+int dasp_tvmc_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                         void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                         int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvmc_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                         float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                         int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                         void* stream);
+int dasp_tvmc_in_geometry(int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs,
+                          int64_t hop, int64_t shared, int64_t chunk_items, dasp_conv_geom* out);
+int dasp_tvmc_in_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save, void* workspace,
+                     int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K, int64_t inputs,
+                     int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvmc_in_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                     float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n,
+                     int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items,
+                     void* stream);
+int dasp_tvmc_in_shared_fwd(const float* x, const float* ir, float* y, void* xspec_save, void* irspec_save,
+                            void* workspace, int64_t workspace_bytes, int64_t bs, int64_t n, int64_t ir_len, int64_t K,
+                            int64_t inputs, int64_t outputs, int64_t hop, int64_t chunk_items, void* stream);
+int dasp_tvmc_in_shared_bwd(const float* gy, const void* xspec_save, const void* irspec_save, float* gx,
+                            float* gir /* may be NULL */, void* workspace, int64_t workspace_bytes, int64_t bs,
+                            int64_t n, int64_t ir_len, int64_t K, int64_t inputs, int64_t outputs, int64_t hop,
+                            int64_t chunk_items, void* stream);
+
+/* test hook: dispatch of the most recent dasp_tvbus_*, dasp_tvbus_in_*, dasp_tvmc_* or dasp_tvmc_in_* call.  which = 0
+   (forward): bit 0 = own in-shared-memory FFT (always), bit 1 = shared trajectory set, bit 2 = crossfaded blocks
+   (K > 1), bit 3 = source-side crossfade (dasp_tvbus_in_*, dasp_tvmc_in_*), bit 4 = M >= 3 outputs.  which = 1
+   (backward): bit 0 = own FFT (always), bit 1 = crossfaded blocks, bit 2 = dL/dIR computed, bit 3 = shared trajectory
+   set, bit 4 = source-side crossfade, bit 5 = M >= 3 outputs */
 int dasp_debug_tvbus_last_path(int which);
 
 #ifdef __cplusplus
